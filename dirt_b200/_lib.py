@@ -22,6 +22,8 @@ ERR_STALE_WORKSPACE = -8
 BWD_SHARED_GEOMETRY = 1
 BWD_SKIP_POSITION = 2
 BWD_SKIP_COLOUR = 4
+TEXTURE_BILINEAR = 0
+TEXTURE_NEAREST = 1
 
 
 def lib():
@@ -68,13 +70,18 @@ def load(path):
     L.dirt_kernel_timer_enable.restype = i
     L.dirt_kernel_timer_enable.argtypes = [i]
     L.dirt_kernel_timer_elapsed_ms.restype = ctypes.c_float
+    L.dirt_texture_sample.restype = i
+    L.dirt_texture_sample.argtypes = [vp] * 3 + [i] * 5 + [ctypes.c_longlong, i, vp]
+    L.dirt_texture_sample_backward.restype = i
+    L.dirt_texture_sample_backward.argtypes = [vp] * 5 + [i] * 5 + [ctypes.c_longlong, i, vp]
     return L
 
 
 EXPORTED_SYMBOLS = ['dirt_error_string', 'dirt_abi_version', 'dirt_workspace_bytes', 'dirt_workspace_bytes_min', 'dirt_rasterise_forward',
                     'dirt_rasterise_backward', 'dirt_rasterise_backward_ex', 'dirt_workspace_status',
                     'dirt_rasterise_visibility', 'dirt_peer_exchange_bytes', 'dirt_peer_exchange', 'dirt_last_launch_count',
-                    'dirt_kernel_timer_enable', 'dirt_kernel_timer_elapsed_ms']
+                    'dirt_kernel_timer_enable', 'dirt_kernel_timer_elapsed_ms', 'dirt_texture_sample',
+                    'dirt_texture_sample_backward']
 
 
 def error_string(code):

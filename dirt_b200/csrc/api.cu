@@ -250,6 +250,62 @@ extern "C" int dirt_rasterise_backward_ex(const float* vertices, const int32_t* 
                          W, C, V, F, channel_groups, n_groups, workspace_holds_setup, flags, workspace, workspace_bytes, cuda_stream);
 }
 
+// texel indices (and the warp keys built from them) stay below 2^62, element offsets of every buffer below 2^62
+static bool texture_shape_ok(int TB, int TH, int TW, int C, int B, long long N, int mode)
+{
+    if (B < 0 || N < 0 || TH <= 0 || TW <= 0 || C <= 0) return false;
+    if (TB != 1 && TB != B) return false;
+    if (mode != DIRT_TEXTURE_BILINEAR && mode != DIRT_TEXTURE_NEAREST) return false;
+    const double limit = 4.0e18;
+    if ((double)TB * TH * TW * C > limit || (double)B * N * (C > 2 ? C : 2) > limit) return false;
+    return true;
+}
+
+static TexDims make_tex_dims(int TB, int TH, int TW, int C, int B, long long N, int mode)
+{
+    TexDims d;
+    d.total = (long long)B * N; d.N = N; d.texels = (long long)TH * TW;
+    d.TB = TB; d.TH = TH; d.TW = TW; d.C = C; d.mode = mode;
+    return d;
+}
+
+extern "C" int dirt_texture_sample(const float* texture, const float* indices, float* out, int TB, int TH, int TW, int C,
+                                   int B, long long N, int mode, void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (!texture_shape_ok(TB, TH, TW, C, B, N, mode)) return DIRT_ERR_BAD_SHAPE;
+    if (B == 0 || N == 0) return DIRT_OK;
+    if (!texture || !indices || !out) return DIRT_ERR_NULL_POINTER;
+    if ((uintptr_t)texture % 4 || (uintptr_t)indices % 4 || (uintptr_t)out % 4) return DIRT_ERR_MISALIGNED;
+    CUDA_TRY(launch_texture_forward(texture, indices, out, make_tex_dims(TB, TH, TW, C, B, N, mode), (cudaStream_t)cuda_stream,
+                                    &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
+extern "C" int dirt_texture_sample_backward(const float* texture, const float* indices, const float* grad_out,
+                                            float* grad_texture, float* grad_indices, int TB, int TH, int TW, int C, int B,
+                                            long long N, int mode, void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (!texture_shape_ok(TB, TH, TW, C, B, N, mode)) return DIRT_ERR_BAD_SHAPE;
+    const TexDims d = make_tex_dims(TB, TH, TW, C, B, N, mode);
+    if (d.total > 0) {
+        if (!indices || !grad_out) return DIRT_ERR_NULL_POINTER;
+        if (grad_indices && mode == DIRT_TEXTURE_BILINEAR && !texture) return DIRT_ERR_NULL_POINTER;
+    }
+    if ((uintptr_t)texture % 4 || (uintptr_t)indices % 4 || (uintptr_t)grad_out % 4 || (uintptr_t)grad_texture % 4 ||
+        (uintptr_t)grad_indices % 4)
+        return DIRT_ERR_MISALIGNED;
+    // with no lookups only the memset of grad_texture is enqueued
+    CUDA_TRY(launch_texture_backward(texture, indices, grad_out, grad_texture, grad_indices, d, (cudaStream_t)cuda_stream,
+                                     &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
 extern "C" int dirt_workspace_status(const void* workspace, size_t workspace_bytes, int B, int H, int W, int C, int V, int F,
                                      void* cuda_stream)
 {

@@ -4,9 +4,11 @@ torch in place of TensorFlow and a procedural texture in place of the photograph
 
     python examples/textured.py [out.png]
 
-`uvs_to_pixel_indices` and `sample_texture` are plain torch and run on any device (tests/test_helpers_cpu.py checks them on
-the CPU); only `main()` needs the GPU.
+`main()` shades with the package's CUDA lookup, `dirt_b200.sample_texture`.  `sample_texture` below is its restatement in
+plain torch: it runs on any device (tests/test_helpers_cpu.py checks it on the CPU) and the GPU tests compare the CUDA op
+with it bit for bit.  `uvs_to_pixel_indices` is the package's (plain torch as well).  Only `main()` needs the GPU.
 """
+import functools
 import os
 import sys
 
@@ -14,19 +16,9 @@ import torch
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), '..'))
 
+from dirt_b200.texture import uvs_to_pixel_indices  # noqa: E402  (plain torch, any device)
+
 frame_width, frame_height = 640, 480
-
-
-def uvs_to_pixel_indices(uvs, texture_shape, mode='repeat'):
-    """uv coordinates [..., 2] -> fractional (row, column) texel indices [..., 2]; u = 0, v = 0 is the TOP-left texel
-    corner (as in samples/textured.py:15-27, unlike OpenGL)."""
-    uvs = uvs.flip(-1)   # (u, v) = (x, y) -> (row, column)
-    shape = torch.as_tensor(texture_shape, dtype=uvs.dtype, device=uvs.device)
-    if mode == 'repeat':
-        return uvs % 1. * shape
-    if mode == 'clamp':
-        return uvs.clamp(0., 1.) * shape
-    raise NotImplementedError(mode)
 
 
 def sample_texture(texture, indices, mode='bilinear'):
@@ -74,11 +66,12 @@ def build_cube():
     return vertices, uvs, faces
 
 
-def shader_fn(gbuffer, texture, light_direction):
-    """G-buffer [H, W, 6] = (mask, u, v, nx, ny, nz) -> shaded pixels [H, W, 3] (samples/textured.py:117-143)."""
+def shader_fn(gbuffer, texture, light_direction, sample=sample_texture):
+    """G-buffer [H, W, 6] = (mask, u, v, nx, ny, nz) -> shaded pixels [H, W, 3] (samples/textured.py:117-143).
+    `sample`: the texture lookup, the torch restatement by default, `dirt_b200.sample_texture` on the GPU."""
     from dirt_b200 import lighting
     mask, uvs, normals = gbuffer[..., :1], gbuffer[..., 1:3], gbuffer[..., 3:]
-    unlit = sample_texture(texture, uvs_to_pixel_indices(uvs, texture.shape[:2]))
+    unlit = sample(texture, uvs_to_pixel_indices(uvs, texture.shape[:2]))
     ambient = unlit * 0.4
     diffuse = lighting.diffuse_directional(normals.reshape(-1, 3), unlit.reshape(-1, 3), light_direction,
                                            light_color=torch.full((3,), 0.6, device=gbuffer.device), double_sided=True)
@@ -110,7 +103,7 @@ def main():
     pixels = dirt.rasterise_deferred(
         background_attributes=torch.zeros([frame_height, frame_width, 6], device=device),
         vertices=vertices_clip, vertex_attributes=attributes, faces=faces,
-        shader_fn=shader_fn, shader_additional_inputs=[texture, light_direction])
+        shader_fn=functools.partial(shader_fn, sample=dirt.sample_texture), shader_additional_inputs=[texture, light_direction])
 
     loss = -pixels.mean()   # a toy loss: gradients reach the geometry, the texture and the light
     loss.backward()

@@ -151,6 +151,33 @@ size_t dirt_peer_exchange_bytes(int world, long long count);
 int dirt_peer_exchange(const float* local, float* out, void* const* peer_slots, void* const* peer_flags,
                        int world, int rank, long long count, unsigned int sequence, void* cuda_stream);
 
+/* Differentiable texture lookup: the bilinear / nearest lookup of the reference's textured sample
+ * (samples/textured.py:30-60), with the four bilinear texels wrapping around the texture edge.
+ *   texture          float32 [TB, TH, TW, C]: TB = 1 (one texture shared by every lookup) or TB = B (one per batch item)
+ *   indices          float32 [B, N, 2]: fractional (row, column) texel indices; (0, 0) is the top-left texel corner
+ *   out, grad_out    float32 [B, N, C]
+ *   grad_texture     float32 [TB, TH, TW, C]; grad_indices float32 [B, N, 2]
+ *   mode DIRT_TEXTURE_BILINEAR: r0 = floor(row) mod TH, c0 = floor(col) mod TW, r1 = (r0+1) mod TH, c1 = (c0+1) mod TW
+ *        (mod with the sign of the divisor), fr / fc = index - floor(index), and
+ *        out = t00*(1-fc)*(1-fr) + t01*fc*(1-fr) + t10*(1-fc)*fr + t11*fc*fr, each operation rounded as written, left to
+ *        right, in fp32: bit-identical to the same expression evaluated by torch.
+ *   mode DIRT_TEXTURE_NEAREST: the texel at (trunc(row), trunc(col)), each clamped to the texture; no index gradient.
+ * A lookup with a non-finite index returns 0 in every channel, reads no texel and contributes no gradient.
+ * Backward: grad_texture is zeroed by the library before it accumulates into it; grad_indices is written once per
+ * lookup (through the fractions only; zero for nearest).  Either may be NULL, and that half of the work is skipped;
+ * texture may then be NULL unless grad_indices of a bilinear lookup is wanted.
+ * B = 0 or N = 0: nothing is launched (the backward call still zeroes grad_texture).  All pointers 4-byte aligned;
+ * 8- / 16-byte alignment enables the vector paths. */
+enum {
+    DIRT_TEXTURE_BILINEAR = 0,
+    DIRT_TEXTURE_NEAREST = 1
+};
+int dirt_texture_sample(const float* texture, const float* indices, float* out,
+                        int TB, int TH, int TW, int C, int B, long long N, int mode, void* cuda_stream);
+int dirt_texture_sample_backward(const float* texture, const float* indices, const float* grad_out,
+                                 float* grad_texture, float* grad_indices,
+                                 int TB, int TH, int TW, int C, int B, long long N, int mode, void* cuda_stream);
+
 /* Number of kernels the last call on this thread launched (bench.py's gpu_launches). */
 int dirt_last_launch_count(void);
 
