@@ -24,6 +24,9 @@ BWD_SKIP_POSITION = 2
 BWD_SKIP_COLOUR = 4
 TEXTURE_BILINEAR = 0
 TEXTURE_NEAREST = 1
+LIGHT_DIFFUSE_DIRECTIONAL = 0
+LIGHT_SPECULAR_DIRECTIONAL = 1
+LIGHT_DIFFUSE_POINT = 2
 
 
 def lib():
@@ -74,6 +77,14 @@ def load(path):
     L.dirt_texture_sample.argtypes = [vp] * 3 + [i] * 5 + [ctypes.c_longlong, i, vp]
     L.dirt_texture_sample_backward.restype = i
     L.dirt_texture_sample_backward.argtypes = [vp] * 5 + [i] * 5 + [ctypes.c_longlong, i, vp]
+    ll = ctypes.c_longlong
+    light_inputs = [i, i, vp, ll, vp, ll, vp, ll] + [vp, i] * 4
+    L.dirt_lighting_workspace_bytes.restype = sz
+    L.dirt_lighting_workspace_bytes.argtypes = [i, ll, i]
+    L.dirt_lighting_forward.restype = i
+    L.dirt_lighting_forward.argtypes = light_inputs + [vp, i, ll, i, vp]
+    L.dirt_lighting_backward.restype = i
+    L.dirt_lighting_backward.argtypes = light_inputs + [vp] * 9 + [sz, i, ll, i, vp]
     return L
 
 
@@ -81,7 +92,8 @@ EXPORTED_SYMBOLS = ['dirt_error_string', 'dirt_abi_version', 'dirt_workspace_byt
                     'dirt_rasterise_backward', 'dirt_rasterise_backward_ex', 'dirt_workspace_status',
                     'dirt_rasterise_visibility', 'dirt_peer_exchange_bytes', 'dirt_peer_exchange', 'dirt_last_launch_count',
                     'dirt_kernel_timer_enable', 'dirt_kernel_timer_elapsed_ms', 'dirt_texture_sample',
-                    'dirt_texture_sample_backward']
+                    'dirt_texture_sample_backward', 'dirt_lighting_workspace_bytes', 'dirt_lighting_forward',
+                    'dirt_lighting_backward']
 
 
 def error_string(code):

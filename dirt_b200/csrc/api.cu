@@ -306,6 +306,123 @@ extern "C" int dirt_texture_sample_backward(const float* texture, const float* i
     return DIRT_OK;
 }
 
+// element offsets of every per-point buffer stay below 2^62, the chunk count within the grid's x limit
+static bool lighting_shape_ok(int model, int B, long long V, int C, long long sn, long long sp, long long sc)
+{
+    if (model != DIRT_LIGHT_DIFFUSE_DIRECTIONAL && model != DIRT_LIGHT_SPECULAR_DIRECTIONAL &&
+        model != DIRT_LIGHT_DIFFUSE_POINT)
+        return false;
+    if (B < 0 || V < 0 || C <= 0 || sn < 0 || sp < 0 || sc < 0) return false;
+    const double limit = 4.0e18, rows = (double)B * V;
+    const double widest = (double)(C > 3 ? C : 3) + sn + sp + sc;
+    if (rows * widest > limit || light_chunks(V) > 0x7fffffffll) return false;
+    if ((double)B * light_chunks(V) * (LIGHT_FIXED_PARAMS + (double)C) * sizeof(float) > limit) return false;
+    return true;
+}
+
+extern "C" size_t dirt_lighting_workspace_bytes(int B, long long V, int C)
+{
+    if (B <= 0 || V <= 0 || C <= 0) return 0;
+    return sizeof(float) * (size_t)B * (size_t)light_chunks(V) * (size_t)(LIGHT_FIXED_PARAMS + C);
+}
+
+static LightArgs make_light_args(int model, int double_sided, const float* normals, long long sn, const float* positions,
+                                 long long sp, const float* colors, long long sc, const float* light, int light_per_item,
+                                 const float* light_color, int light_color_per_item, const float* camera,
+                                 int camera_per_item, const float* shininess, int shininess_per_item, int B, long long V,
+                                 int C)
+{
+    LightArgs a = {};
+    a.normals = normals; a.positions = positions; a.colors = colors;
+    a.sn = sn; a.sp = sp; a.sc = sc;
+    a.light = light; a.light_color = light_color; a.camera = camera; a.shininess = shininess;
+    a.item_light = light_per_item != 0; a.item_color = light_color_per_item != 0;
+    a.item_camera = camera_per_item != 0; a.item_shininess = shininess_per_item != 0;
+    a.V = V; a.B = B; a.C = C; a.chunks = (int)light_chunks(V);
+    a.model = model; a.double_sided = double_sided != 0;
+    return a;
+}
+
+// the inputs a model reads are required, the others ignored
+static int lighting_inputs_check(const LightArgs& a)
+{
+    const bool pos = a.model != DIRT_LIGHT_DIFFUSE_DIRECTIONAL, sp = a.model == DIRT_LIGHT_SPECULAR_DIRECTIONAL;
+    if (!a.normals || !a.colors || !a.light || !a.light_color || (pos && !a.positions) || (sp && (!a.camera || !a.shininess)))
+        return DIRT_ERR_NULL_POINTER;
+    if ((uintptr_t)a.normals % 4 || (uintptr_t)a.colors % 4 || (uintptr_t)a.light % 4 || (uintptr_t)a.light_color % 4 ||
+        (pos && (uintptr_t)a.positions % 4) || (sp && ((uintptr_t)a.camera % 4 || (uintptr_t)a.shininess % 4)))
+        return DIRT_ERR_MISALIGNED;
+    return DIRT_OK;
+}
+
+extern "C" int dirt_lighting_forward(int model, int double_sided, const float* normals, long long normals_stride,
+                                     const float* positions, long long positions_stride, const float* colors,
+                                     long long colors_stride, const float* light, int light_per_item,
+                                     const float* light_color, int light_color_per_item, const float* camera,
+                                     int camera_per_item, const float* shininess, int shininess_per_item, float* out,
+                                     int B, long long V, int C, void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (!lighting_shape_ok(model, B, V, C, normals_stride, positions_stride, colors_stride)) return DIRT_ERR_BAD_SHAPE;
+    if ((long long)B * V == 0) return DIRT_OK;
+    LightArgs a = make_light_args(model, double_sided, normals, normals_stride, positions, positions_stride, colors,
+                                  colors_stride, light, light_per_item, light_color, light_color_per_item, camera,
+                                  camera_per_item, shininess, shininess_per_item, B, V, C);
+    a.out = out;
+    const int rc = lighting_inputs_check(a);
+    if (rc != DIRT_OK) return rc;
+    if (!out) return DIRT_ERR_NULL_POINTER;
+    if ((uintptr_t)out % 4) return DIRT_ERR_MISALIGNED;
+    CUDA_TRY(launch_lighting_forward(a, (cudaStream_t)cuda_stream, &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
+extern "C" int dirt_lighting_backward(int model, int double_sided, const float* normals, long long normals_stride,
+                                      const float* positions, long long positions_stride, const float* colors,
+                                      long long colors_stride, const float* light, int light_per_item,
+                                      const float* light_color, int light_color_per_item, const float* camera,
+                                      int camera_per_item, const float* shininess, int shininess_per_item,
+                                      const float* grad_out, float* grad_normals, float* grad_positions,
+                                      float* grad_colors, float* grad_light, float* grad_light_color, float* grad_camera,
+                                      float* grad_shininess, void* workspace, size_t workspace_bytes, int B, long long V,
+                                      int C, void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (!lighting_shape_ok(model, B, V, C, normals_stride, positions_stride, colors_stride)) return DIRT_ERR_BAD_SHAPE;
+    LightArgs a = make_light_args(model, double_sided, normals, normals_stride, positions, positions_stride, colors,
+                                  colors_stride, light, light_per_item, light_color, light_color_per_item, camera,
+                                  camera_per_item, shininess, shininess_per_item, B, V, C);
+    const bool sp = model == DIRT_LIGHT_SPECULAR_DIRECTIONAL;
+    a.grad_out = grad_out;
+    a.g_normals = grad_normals; a.g_colors = grad_colors; a.g_light = grad_light; a.g_light_color = grad_light_color;
+    a.g_positions = model != DIRT_LIGHT_DIFFUSE_DIRECTIONAL ? grad_positions : nullptr;
+    a.g_camera = sp ? grad_camera : nullptr;
+    a.g_shininess = sp ? grad_shininess : nullptr;
+    float* outs[] = {a.g_normals, a.g_positions, a.g_colors, a.g_light, a.g_light_color, a.g_camera, a.g_shininess};
+    for (float* p : outs)
+        if ((uintptr_t)p % 4) return DIRT_ERR_MISALIGNED;
+    const bool params = a.g_light || a.g_light_color || a.g_camera || a.g_shininess;
+    if ((long long)B * V > 0 && (params || a.g_normals || a.g_positions || a.g_colors)) {
+        int rc = lighting_inputs_check(a);
+        if (rc != DIRT_OK) return rc;
+        if (!grad_out) return DIRT_ERR_NULL_POINTER;
+        if ((uintptr_t)grad_out % 4) return DIRT_ERR_MISALIGNED;
+        if (params) {
+            if (!workspace) return DIRT_ERR_NULL_POINTER;
+            if ((uintptr_t)workspace % 4) return DIRT_ERR_MISALIGNED;
+            if (workspace_bytes < dirt_lighting_workspace_bytes(B, V, C)) return DIRT_ERR_WORKSPACE_TOO_SMALL;
+            a.partial = static_cast<float*>(workspace);
+        }
+    }
+    // with no points only the memsets of the wanted parameter gradients are enqueued
+    CUDA_TRY(launch_lighting_backward(a, (cudaStream_t)cuda_stream, &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
 extern "C" int dirt_workspace_status(const void* workspace, size_t workspace_bytes, int B, int H, int W, int C, int V, int F,
                                      void* cuda_stream)
 {

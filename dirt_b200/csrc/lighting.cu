@@ -1,0 +1,464 @@
+// lighting.cu -- the reflectance models of dirt_b200/lighting.py (dirt_lighting_forward / dirt_lighting_backward):
+// Lambert under a directional light, Phong under a directional light, Lambert under a point light, each as one pass over
+// the points (DESIGN.md §7.2).
+//
+// One thread per point; a CTA holds 256 points of one item (blockIdx.x = chunk of the item, blockIdx.y = item, looping
+// past the grid limit).  The 12-byte rows (normals, positions, and colours / grad_out / outputs when C = 3) are staged
+// through the warp's slice of shared memory, so that each global access of the warp covers consecutive floats.
+// Backward recomputes the forward from the inputs.  Gradients of parameters shared by many points (light, light colour,
+// camera, shininess) are summed without atomics: each CTA writes its sums to its own row of the partials, then one
+// small kernel adds the rows of each item (or of all items, for a shared parameter) in a fixed order.  Two calls on the
+// same inputs therefore give bit-identical parameter gradients.
+#include "../../include/dirt_b200.h"
+#include "common.cuh"
+
+namespace dirt {
+
+namespace {
+
+constexpr int WARPS = LIGHT_THREADS / 32;
+constexpr int RED_SLOTS = 4;                 // values per reduction round (light, camera: 3; shininess, one channel: 1)
+constexpr unsigned FULL = 0xffffffffu;
+constexpr int DD = DIRT_LIGHT_DIFFUSE_DIRECTIONAL, SP = DIRT_LIGHT_SPECULAR_DIRECTIONAL, DP = DIRT_LIGHT_DIFFUSE_POINT;
+constexpr int REDUCE_THREADS = 256;
+constexpr unsigned MAX_ITEMS_PER_GRID = 65535;   // gridDim.y
+
+// The warp's rows row0 .. row0+n-1 of a [rows, K] tensor with row stride rs: loaded as 32*K consecutive-in-the-row
+// floats per warp (coalesced for rs == K), passed through the warp's slice s of shared memory, K values per lane.
+// Lanes >= n get unspecified values.  Warp-collective.
+template <int K>
+__device__ __forceinline__ void stage_load(const float* __restrict__ src, long long rs, long long row0, int n, float* s,
+                                           int lane, float v[K])
+{
+#pragma unroll
+    for (int j = 0; j < K; ++j) {
+        const int idx = j * 32 + lane, r = idx / K, c = idx - r * K;
+        if (r < n) s[idx] = __ldg(src + (row0 + r) * rs + c);
+    }
+    __syncwarp();
+#pragma unroll
+    for (int c = 0; c < K; ++c) v[c] = s[lane * K + c];
+    __syncwarp();
+}
+
+// The reverse: lanes < n write their K values to rows row0 .. row0+n-1 of a contiguous [rows, K] tensor.
+template <int K>
+__device__ __forceinline__ void stage_store(float* __restrict__ dst, long long row0, int n, float* s, int lane,
+                                            const float v[K])
+{
+#pragma unroll
+    for (int c = 0; c < K; ++c) s[lane * K + c] = v[c];
+    __syncwarp();
+#pragma unroll
+    for (int j = 0; j < K; ++j) {
+        const int idx = j * 32 + lane;
+        if (idx < n * K) dst[row0 * K + idx] = s[idx];
+    }
+    __syncwarp();
+}
+
+// dot product in a fixed order: fma(a2, b2, fma(a1, b1, a0 * b0))
+__device__ __forceinline__ float dot3(const float a[3], const float b[3])
+{
+    return __fmaf_rn(a[2], b[2], __fmaf_rn(a[1], b[1], __fmul_rn(a[0], b[0])));
+}
+
+// abs(cos) (double-sided) or clamp(cos, min=0), NaN passing through as in torch
+template <bool DS>
+__device__ __forceinline__ float cos_term(float c)
+{
+    return DS ? fabsf(c) : (c < 0.f ? 0.f : c);
+}
+// torch's derivative of cos_term: sgn (0 at 0 and at NaN) or the mask cos >= 0 (1 at exactly 0, 0 at NaN)
+template <bool DS>
+__device__ __forceinline__ float cos_term_grad(float c)
+{
+    return DS ? (c > 0.f ? 1.f : (c < 0.f ? -1.f : 0.f)) : (c >= 0.f ? 1.f : 0.f);
+}
+
+// The forward's intermediates of one point.  f multiplies every channel: out_c = (light_color_c * color_c) * f.
+struct Shade {
+    float L[3];                  // light direction (directional models) or position (point light)
+    float cos, t, f;             // cosine, its term, the channel factor (t, or pow(t, s) for Phong)
+    float s;                     // Phong: shininess
+    float two_dot, r[3];         // Phong: 2 (n . -L), reflected = L + two_dot * n
+    float tc[3], norm, u[3];     // Phong: to_camera = camera - p, |to_camera|, to_camera / norm + 1e-12
+    float rel[3], nr, d, inc[3]; // point light: p - light, |rel|, |rel| + 1e-12, rel / d
+};
+
+__device__ __forceinline__ const float* item_row(const float* p, bool per_item, long long b, int k)
+{
+    return p + (per_item ? b * k : 0);
+}
+
+template <int MODEL, bool DS>
+__device__ __forceinline__ Shade shade(const LightArgs& a, long long b, const float n[3], const float p[3])
+{
+    Shade h;
+    const float* L = item_row(a.light, a.item_light, b, 3);
+#pragma unroll
+    for (int i = 0; i < 3; ++i) h.L[i] = __ldg(L + i);
+    if (MODEL == DD) {
+        const float m[3] = {-h.L[0], -h.L[1], -h.L[2]};
+        h.cos = dot3(n, m);
+        h.t = h.f = cos_term<DS>(h.cos);
+    } else if (MODEL == SP) {
+        const float m[3] = {-h.L[0], -h.L[1], -h.L[2]};
+        h.two_dot = __fmul_rn(2.f, dot3(n, m));
+        const float* cam = item_row(a.camera, a.item_camera, b, 3);
+#pragma unroll
+        for (int i = 0; i < 3; ++i) {
+            h.r[i] = __fadd_rn(h.L[i], __fmul_rn(h.two_dot, n[i]));
+            h.tc[i] = __fsub_rn(__ldg(cam + i), p[i]);
+        }
+        h.norm = __fsqrt_rn(dot3(h.tc, h.tc));
+#pragma unroll
+        for (int i = 0; i < 3; ++i) h.u[i] = __fadd_rn(__fdiv_rn(h.tc[i], h.norm), 1.e-12f);
+        h.cos = dot3(h.u, h.r);
+        h.t = cos_term<DS>(h.cos);
+        h.s = __ldg(item_row(a.shininess, a.item_shininess, b, 1));
+        h.f = powf(h.t, h.s);
+    } else {
+#pragma unroll
+        for (int i = 0; i < 3; ++i) h.rel[i] = __fsub_rn(p[i], h.L[i]);
+        h.nr = __fsqrt_rn(dot3(h.rel, h.rel));
+        h.d = __fadd_rn(h.nr, 1.e-12f);
+#pragma unroll
+        for (int i = 0; i < 3; ++i) h.inc[i] = __fdiv_rn(h.rel[i], h.d);
+        h.cos = dot3(n, h.inc);
+        h.t = h.f = cos_term<DS>(h.cos);
+    }
+    return h;
+}
+
+// ---- forward --------------------------------------------------------------------------------------------------------
+
+// CT = 3 (colours and outputs staged like the other rows) or 0 (any C, one channel at a time)
+template <int MODEL, bool DS, int CT>
+__global__ void __launch_bounds__(LIGHT_THREADS) lighting_forward_kernel(LightArgs a)
+{
+    __shared__ float stage[LIGHT_THREADS * 3];
+    const int lane = threadIdx.x & 31;
+    float* s = stage + (threadIdx.x & ~31) * 3;
+    const long long v0 = (long long)blockIdx.x * LIGHT_THREADS + (threadIdx.x & ~31);
+    if (v0 >= a.V) return;   // the whole warp
+    const int n = (int)(a.V - v0 < 32 ? a.V - v0 : 32);
+    const int C = CT ? CT : a.C;
+    for (long long b = blockIdx.y; b < a.B; b += gridDim.y) {
+        const long long row0 = b * a.V + v0, row = row0 + lane;
+        float nrm[3], pos[3] = {0.f, 0.f, 0.f};
+        stage_load<3>(a.normals, a.sn, row0, n, s, lane, nrm);
+        if (MODEL != DD) stage_load<3>(a.positions, a.sp, row0, n, s, lane, pos);
+        const Shade h = shade<MODEL, DS>(a, b, nrm, pos);
+        const float* lc = item_row(a.light_color, a.item_color, b, C);
+        if (CT == 3) {
+            float k[3], o[3];
+            stage_load<3>(a.colors, a.sc, row0, n, s, lane, k);
+#pragma unroll
+            for (int c = 0; c < 3; ++c) o[c] = __fmul_rn(__fmul_rn(__ldg(lc + c), k[c]), h.f);
+            stage_store<3>(a.out, row0, n, s, lane, o);
+        } else if (lane < n) {
+            for (int c = 0; c < C; ++c)
+                a.out[row * C + c] = __fmul_rn(__fmul_rn(__ldg(lc + c), __ldg(a.colors + row * a.sc + c)), h.f);
+        }
+    }
+}
+
+// ---- backward -------------------------------------------------------------------------------------------------------
+
+// Sums NV values over the CTA in a fixed order (a butterfly in each warp, then the warps in order) and has thread j write
+// the j-th sum to dst[j].  Block-collective.
+template <int NV>
+__device__ __forceinline__ void cta_partial(const float v[NV], float* red, float* dst)
+{
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int j = 0; j < NV; ++j) {
+        float x = v[j];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(FULL, x, o);
+        if (lane == 0) red[warp * RED_SLOTS + j] = x;
+    }
+    __syncthreads();
+    if (threadIdx.x < NV) {
+        float x = red[threadIdx.x];
+#pragma unroll
+        for (int w = 1; w < WARPS; ++w) x += red[w * RED_SLOTS + threadIdx.x];
+        dst[threadIdx.x] = x;
+    }
+    __syncthreads();
+}
+
+template <int MODEL, bool DS, int CT>
+__global__ void __launch_bounds__(LIGHT_THREADS) lighting_backward_kernel(LightArgs a)
+{
+    __shared__ float stage[LIGHT_THREADS * 3];
+    __shared__ float red[WARPS * RED_SLOTS];
+    const int lane = threadIdx.x & 31;
+    float* s = stage + (threadIdx.x & ~31) * 3;
+    const long long v0 = (long long)blockIdx.x * LIGHT_THREADS + (threadIdx.x & ~31);
+    const int n = v0 >= a.V ? 0 : (int)(a.V - v0 < 32 ? a.V - v0 : 32);   // warp-uniform; 0: the warp only helps reduce
+    const bool live = lane < n;
+    const int C = CT ? CT : a.C;
+    const int P = LIGHT_FIXED_PARAMS + a.C;
+    for (long long b = blockIdx.y; b < a.B; b += gridDim.y) {
+        const long long row0 = b * a.V + v0, row = row0 + lane;
+        float nrm[3] = {0.f, 0.f, 0.f}, pos[3] = {0.f, 0.f, 0.f};
+        if (n) {
+            stage_load<3>(a.normals, a.sn, row0, n, s, lane, nrm);
+            if (MODEL != DD) stage_load<3>(a.positions, a.sp, row0, n, s, lane, pos);
+        }
+        const Shade h = shade<MODEL, DS>(a, b, nrm, pos);
+        const float* lc = item_row(a.light_color, a.item_color, b, C);
+
+        // out_c = q_c * f with q_c = light_color_c * color_c:  d/df = sum_c g_c q_c, d/dq_c = g_c f
+        float gf = 0.f, glc3[3] = {0.f, 0.f, 0.f};
+        if (CT == 3) {
+            float g[3] = {0.f, 0.f, 0.f}, k[3] = {0.f, 0.f, 0.f}, gk[3];
+            if (n) {
+                stage_load<3>(a.grad_out, 3, row0, n, s, lane, g);
+                stage_load<3>(a.colors, a.sc, row0, n, s, lane, k);
+            }
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                const float l = __ldg(lc + c), gq = g[c] * h.f;
+                gf += g[c] * (l * k[c]);
+                gk[c] = gq * l;
+                glc3[c] = live ? gq * k[c] : 0.f;
+            }
+            if (a.g_colors && n) stage_store<3>(a.g_colors, row0, n, s, lane, gk);
+        } else if (live) {
+            for (int c = 0; c < C; ++c) {
+                const float l = __ldg(lc + c), g = __ldg(a.grad_out + row * C + c);
+                gf += g * (l * __ldg(a.colors + row * a.sc + c));
+                if (a.g_colors) a.g_colors[row * C + c] = (g * h.f) * l;
+            }
+        }
+
+        // the scalar chain down to the cosine, then to the per-point inputs and the parameters
+        float gn[3], gp[3] = {0.f, 0.f, 0.f}, gL[3], gcam[3] = {0.f, 0.f, 0.f}, gs = 0.f;
+        float gt = gf;
+        if (MODEL == SP) {
+            // torch's pow backward: no gradient through an exponent of 0, none to the exponent at base 0 (exponent >= 0)
+            gt = h.s == 0.f ? 0.f : gf * (h.s * powf(h.t, h.s - 1.f));
+            gs = gf * ((h.t == 0.f && h.s >= 0.f) ? 0.f : h.f * logf(h.t));
+        }
+        const float gc = gt * cos_term_grad<DS>(h.cos);
+        if (MODEL == DD) {
+#pragma unroll
+            for (int i = 0; i < 3; ++i) {
+                gn[i] = gc * -h.L[i];
+                gL[i] = -(gc * nrm[i]);
+            }
+        } else if (MODEL == SP) {
+            float gu[3], gnorm = 0.f, g2d = 0.f;
+#pragma unroll
+            for (int i = 0; i < 3; ++i) {
+                gu[i] = gc * h.r[i];
+                const float gr = gc * h.u[i];
+                gL[i] = gr;
+                g2d += gr * nrm[i];
+                gn[i] = gr * h.two_dot;
+                gnorm -= gu[i] * h.tc[i] / (h.norm * h.norm);
+            }
+            const float gdot = 2.f * g2d;
+#pragma unroll
+            for (int i = 0; i < 3; ++i) {
+                gn[i] += gdot * -h.L[i];
+                gL[i] -= gdot * nrm[i];
+                // torch's norm backward has no gradient at a zero vector
+                const float gtc = gu[i] / h.norm + (h.norm == 0.f ? 0.f : h.tc[i] * (gnorm / h.norm));
+                gcam[i] = gtc;
+                gp[i] = -gtc;
+            }
+        } else {
+            float gd = 0.f, grel[3];
+#pragma unroll
+            for (int i = 0; i < 3; ++i) {
+                gn[i] = gc * h.inc[i];
+                const float ginc = gc * nrm[i];
+                grel[i] = ginc / h.d;
+                gd -= ginc * h.rel[i] / (h.d * h.d);
+            }
+#pragma unroll
+            for (int i = 0; i < 3; ++i) {
+                gp[i] = grel[i] + (h.nr == 0.f ? 0.f : h.rel[i] * (gd / h.nr));
+                gL[i] = -gp[i];
+            }
+        }
+        if (n) {
+            if (a.g_normals) stage_store<3>(a.g_normals, row0, n, s, lane, gn);
+            if (MODEL != DD && a.g_positions) stage_store<3>(a.g_positions, row0, n, s, lane, gp);
+        }
+
+        // this CTA's sums of the parameter gradients (lanes without a point add zeros)
+        if (a.partial) {
+            float* dst = a.partial + ((long long)b * a.chunks + blockIdx.x) * P;
+            if (a.g_light) {
+                const float v[3] = {live ? gL[0] : 0.f, live ? gL[1] : 0.f, live ? gL[2] : 0.f};
+                cta_partial<3>(v, red, dst);
+            }
+            if (a.g_light_color) {
+                if (CT == 3) {
+                    cta_partial<3>(glc3, red, dst + 3);
+                } else {
+                    for (int c = 0; c < C; ++c) {
+                        const float v[1] = {live ? (__ldg(a.grad_out + row * C + c) * h.f) *
+                                                       __ldg(a.colors + row * a.sc + c) : 0.f};
+                        cta_partial<1>(v, red, dst + 3 + c);
+                    }
+                }
+            }
+            if (MODEL == SP && a.g_camera) {
+                const float v[3] = {live ? gcam[0] : 0.f, live ? gcam[1] : 0.f, live ? gcam[2] : 0.f};
+                cta_partial<3>(v, red, dst + 3 + C);
+            }
+            if (MODEL == SP && a.g_shininess) {
+                const float v[1] = {live ? gs : 0.f};
+                cta_partial<1>(v, red, dst + 6 + C);
+            }
+        }
+    }
+}
+
+// One CTA per element of a wanted parameter gradient: the sum of its column of the partials over the rows of its item
+// (per-item parameter) or of every item (shared parameter), each thread taking a fixed stride of rows and the CTA
+// adding the threads' sums as a fixed tree.
+struct ReduceJobs {
+    float* out[4];
+    int offset[4];           // column of the partials
+    int width[4];
+    bool per_item[4];
+    long long first[5];      // first output element of each job; first[count] = total
+    int count;
+};
+
+__global__ void __launch_bounds__(REDUCE_THREADS) lighting_reduce_kernel(const float* __restrict__ partial, ReduceJobs jobs,
+                                                                         long long total, long long chunks, int B, int P)
+{
+    __shared__ float sum[REDUCE_THREADS];
+    for (long long e = blockIdx.x; e < total; e += gridDim.x) {
+        // the job of element e, selected without indexing the parameter struct dynamically (which needs a stack copy)
+        float* out = jobs.out[0];
+        long long first = 0;
+        int offset = jobs.offset[0], width = jobs.width[0];
+        bool per_item = jobs.per_item[0];
+#pragma unroll
+        for (int j = 1; j < 4; ++j)
+            if (j < jobs.count && e >= jobs.first[j]) {
+                out = jobs.out[j]; first = jobs.first[j]; offset = jobs.offset[j]; width = jobs.width[j];
+                per_item = jobs.per_item[j];
+            }
+        const long long local = e - first;
+        const long long item = per_item ? local / width : 0;
+        const int col = offset + (int)(local - item * width);
+        const long long r0 = per_item ? item * chunks : 0, rows = per_item ? chunks : B * chunks;
+        float x = 0.f;
+        for (long long i = threadIdx.x; i < rows; i += REDUCE_THREADS) x += partial[(r0 + i) * P + col];
+        sum[threadIdx.x] = x;
+        __syncthreads();
+#pragma unroll
+        for (int h = REDUCE_THREADS / 2; h > 0; h >>= 1) {
+            if (threadIdx.x < h) sum[threadIdx.x] += sum[threadIdx.x + h];
+            __syncthreads();
+        }
+        if (threadIdx.x == 0) out[local] = sum[0];
+        __syncthreads();
+    }
+}
+
+inline dim3 point_grid(const LightArgs& a)
+{
+    return dim3((unsigned)a.chunks, (unsigned)(a.B < (int)MAX_ITEMS_PER_GRID ? a.B : (int)MAX_ITEMS_PER_GRID));
+}
+
+template <int MODEL, bool DS>
+void forward_md(const LightArgs& a, cudaStream_t stream)
+{
+    if (a.C == 3) lighting_forward_kernel<MODEL, DS, 3><<<point_grid(a), LIGHT_THREADS, 0, stream>>>(a);
+    else lighting_forward_kernel<MODEL, DS, 0><<<point_grid(a), LIGHT_THREADS, 0, stream>>>(a);
+}
+
+template <int MODEL, bool DS>
+void backward_md(const LightArgs& a, cudaStream_t stream)
+{
+    if (a.C == 3) lighting_backward_kernel<MODEL, DS, 3><<<point_grid(a), LIGHT_THREADS, 0, stream>>>(a);
+    else lighting_backward_kernel<MODEL, DS, 0><<<point_grid(a), LIGHT_THREADS, 0, stream>>>(a);
+}
+
+template <int MODEL>
+void forward_m(const LightArgs& a, cudaStream_t stream)
+{
+    if (a.double_sided) forward_md<MODEL, true>(a, stream);
+    else forward_md<MODEL, false>(a, stream);
+}
+
+template <int MODEL>
+void backward_m(const LightArgs& a, cudaStream_t stream)
+{
+    if (a.double_sided) backward_md<MODEL, true>(a, stream);
+    else backward_md<MODEL, false>(a, stream);
+}
+
+}  // namespace
+
+cudaError_t launch_lighting_forward(const LightArgs& a, cudaStream_t stream, int* launches)
+{
+    if ((long long)a.B * a.V == 0) return cudaSuccess;
+    switch (a.model) {
+        case DD: forward_m<DD>(a, stream); break;
+        case SP: forward_m<SP>(a, stream); break;
+        default: forward_m<DP>(a, stream);
+    }
+    const cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) ++*launches;
+    return e;
+}
+
+cudaError_t launch_lighting_backward(const LightArgs& a, cudaStream_t stream, int* launches)
+{
+    const bool sp = a.model == SP;
+    ReduceJobs jobs;
+    jobs.count = 0;
+    jobs.first[0] = 0;
+    auto add = [&](float* out, int offset, int width, bool per_item) {
+        if (!out) return;
+        const int k = jobs.count++;
+        jobs.out[k] = out; jobs.offset[k] = offset; jobs.width[k] = width; jobs.per_item[k] = per_item;
+        jobs.first[k + 1] = jobs.first[k] + (per_item ? (long long)a.B : 1ll) * width;
+    };
+    add(a.g_light, 0, 3, a.item_light);
+    add(a.g_light_color, 3, a.C, a.item_color);
+    if (sp) add(a.g_camera, 3 + a.C, 3, a.item_camera);
+    if (sp) add(a.g_shininess, 6 + a.C, 1, a.item_shininess);
+    cudaError_t e;
+    if ((long long)a.B * a.V == 0) {
+        for (int k = 0; k < jobs.count; ++k) {
+            const size_t bytes = sizeof(float) * (size_t)(jobs.first[k + 1] - jobs.first[k]);
+            if (bytes && (e = cudaMemsetAsync(jobs.out[k], 0, bytes, stream)) != cudaSuccess) return e;
+        }
+        return cudaSuccess;
+    }
+    const bool per_point = a.g_normals || a.g_colors || (a.model != DD && a.g_positions);
+    if (!per_point && !jobs.count) return cudaSuccess;
+    LightArgs b = a;
+    if (!jobs.count) b.partial = nullptr;
+    switch (a.model) {
+        case DD: backward_m<DD>(b, stream); break;
+        case SP: backward_m<SP>(b, stream); break;
+        default: backward_m<DP>(b, stream);
+    }
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    ++*launches;
+    if (jobs.count) {
+        const long long total = jobs.first[jobs.count];
+        const unsigned blocks = (unsigned)(total < (1ll << 20) ? total : (1ll << 20));
+        lighting_reduce_kernel<<<blocks, REDUCE_THREADS, 0, stream>>>(b.partial, jobs, total, a.chunks, a.B,
+                                                                      LIGHT_FIXED_PARAMS + a.C);
+        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+        ++*launches;
+    }
+    return cudaSuccess;
+}
+
+}  // namespace dirt

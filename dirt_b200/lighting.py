@@ -1,5 +1,15 @@
-"""Mesh normals and simple reflectance models (torch); mirrors the API of dirt/lighting.py."""
+"""Mesh normals and simple reflectance models; mirrors the API of dirt/lighting.py.
+
+The normals are torch code.  The three reflectance models run CUDA kernels (dirt_lighting_forward / _backward of
+include/dirt_b200.h) when their inputs are on one CUDA device in the shapes `cuda_route` accepts, and their torch
+restatements (`_diffuse_directional`, `_specular_directional`, `_diffuse_point`) otherwise; see DESIGN.md §7.2.
+"""
+import math
+from collections import namedtuple
+
 import torch
+
+from . import _lib
 
 
 def _prepare(vertices, faces):
@@ -51,28 +61,17 @@ def _cosine_term(cosines, double_sided):
     return cosines.abs() if double_sided else cosines.clamp(min=0.)
 
 
-def diffuse_directional(vertex_normals, vertex_colors, light_direction, light_color, double_sided=True, name=None):
-    """Lambertian reflectance under one directional light (dirt/lighting.py:182-225)."""
-    vertex_normals = torch.as_tensor(vertex_normals, dtype=torch.float32)
-    dev = vertex_normals.device
-    vertex_colors = torch.as_tensor(vertex_colors, dtype=torch.float32, device=dev)
-    light_direction = torch.as_tensor(light_direction, dtype=torch.float32, device=dev)
-    light_color = torch.as_tensor(light_color, dtype=torch.float32, device=dev)
+def _diffuse_directional(vertex_normals, vertex_colors, light_direction, light_color, double_sided=True):
+    """The torch restatement of `diffuse_directional`: its CPU implementation and its specification.
+    Takes tensors of one dtype and device, and keeps that dtype (the tests evaluate it in float64)."""
     cosines = torch.matmul(vertex_normals, -light_direction[..., None])  # [*, V, 1]
     return light_color[..., None, :] * vertex_colors * _cosine_term(cosines, double_sided)
 
 
-def specular_directional(vertex_positions, vertex_normals, vertex_reflectivities, light_direction, light_color,
-                         camera_position, shininess, double_sided=True, name=None):
-    """Phong reflectance under one directional light (dirt/lighting.py:228-288)."""
-    vertex_positions = torch.as_tensor(vertex_positions, dtype=torch.float32)
-    dev = vertex_positions.device
-    vertex_normals = torch.as_tensor(vertex_normals, dtype=torch.float32, device=dev)
-    vertex_reflectivities = torch.as_tensor(vertex_reflectivities, dtype=torch.float32, device=dev)
-    light_direction = torch.as_tensor(light_direction, dtype=torch.float32, device=dev)
-    light_color = torch.as_tensor(light_color, dtype=torch.float32, device=dev)
-    camera_position = torch.as_tensor(camera_position, dtype=torch.float32, device=dev)
-    shininess = torch.as_tensor(shininess, dtype=torch.float32, device=dev)
+def _specular_directional(vertex_positions, vertex_normals, vertex_reflectivities, light_direction, light_color,
+                          camera_position, shininess, double_sided=True):
+    """The torch restatement of `specular_directional`: its CPU implementation and its specification.
+    Takes tensors of one dtype and device, and keeps that dtype (the tests evaluate it in float64)."""
     to_light = -light_direction
     # (the reference adds `-to_light` of shape [*,3] to a [*,V,3] tensor, which only broadcasts without batch dimensions,
     # dirt/lighting.py:272; the vertex axis is inserted here so that batches work as its docstring promises)
@@ -84,15 +83,227 @@ def specular_directional(vertex_positions, vertex_normals, vertex_reflectivities
                                                                          shininess[..., None, None])
 
 
+def _diffuse_point(vertex_positions, vertex_normals, vertex_colors, light_position, light_color, double_sided=True):
+    """The torch restatement of `diffuse_point`: its CPU implementation and its specification.
+    Takes tensors of one dtype and device, and keeps that dtype (the tests evaluate it in float64)."""
+    relative = vertex_positions - light_position[..., None, :]
+    incident = relative / (torch.linalg.norm(relative, dim=-1, keepdim=True) + 1.e-12)
+    cosines = (vertex_normals * incident).sum(-1)
+    return light_color[..., None, :] * vertex_colors * _cosine_term(cosines, double_sided)[..., None]
+
+
+# ---- the CUDA path --------------------------------------------------------------------------------------------------
+
+Route = namedtuple('Route', 'lead B V C per_item')
+
+
+def cuda_route(point_shapes, item_shapes, devices):
+    """Whether a reflectance call runs the CUDA kernels, decided from shapes and devices alone.
+
+    point_shapes: the shapes of the per-point tensors, colours (or reflectivities) last: [*, V, 3], ..., [*, V, C].
+    item_shapes: (shape, width) of each per-item tensor, width 3 (a direction or position), 'C' (the light colour) or 0
+        (the shininess, a scalar per item); each must have leading shape exactly `*` (one value per item) or none
+        (shared by all points).
+    devices: the devices of all the tensors; they must be one CUDA device.
+
+    Returns a Route (lead = `*`, B = its product, V, C, per_item flags in the order of item_shapes) or None."""
+    devices = list(devices)
+    if not devices or any(d.type != 'cuda' for d in devices) or any(d != devices[0] for d in devices):
+        return None
+    first = tuple(point_shapes[0])
+    if len(first) < 2:
+        return None
+    lead, V, C = first[:-2], first[-2], tuple(point_shapes[-1])[-1] if len(point_shapes[-1]) else 0
+    if C < 1:
+        return None
+    for k, shape in enumerate(point_shapes):
+        shape = tuple(shape)
+        if len(shape) != len(first) or shape[:-1] != first[:-1] or shape[-1] != (C if k == len(point_shapes) - 1 else 3):
+            return None
+    per_item = []
+    for shape, width in item_shapes:
+        width = C if width == 'C' else width
+        tail = (width,) if width else ()
+        shape = tuple(shape)
+        if shape == tail:
+            per_item.append(False)
+        elif shape == lead + tail:
+            per_item.append(True)
+        else:
+            return None
+    B = math.prod(lead)
+    if B >= 1 << 31:
+        return None
+    return Route(lead, B, V, C, tuple(per_item))
+
+
+def _route(points, items):
+    tensors = list(points) + [t for t, _ in items]
+    return cuda_route([t.shape for t in points], [(t.shape, w) for t, w in items], [t.device for t in tensors])
+
+
+def _rows(t, k):
+    """A per-point tensor [*, V, k] as [rows, k] with unit stride along k: a view when one exists (for example the
+    normals of a G-buffer, gbuffer[..., 7:].reshape(-1, 3)), else a contiguous copy."""
+    try:
+        r = t.view(-1, k)
+    except RuntimeError:
+        return t.reshape(-1, k).contiguous()
+    return r if k == 1 or r.stride(1) == 1 else r.contiguous()
+
+
+def _ptr(t):
+    return t.data_ptr() if t is not None else None
+
+
+_MODEL_NAMES = {_lib.LIGHT_DIFFUSE_DIRECTIONAL: 'DiffuseDirectional', _lib.LIGHT_SPECULAR_DIRECTIONAL: 'SpecularDirectional',
+                _lib.LIGHT_DIFFUSE_POINT: 'DiffusePoint'}
+
+
+def _restate(model, double_sided, route, normals, positions, colors, light, light_color, camera, shininess):
+    """The restatement on the op's own inputs (flattened per-point rows, per-item rows): its value has the op's output
+    shape, and autograd through it gives differentiable gradients (double backward)."""
+    lead, V, C = route.lead, route.V, route.C
+    point = lambda t, w: t.reshape(lead + (V, w))
+    item = lambda t, per_item, tail: t.reshape(lead + tail) if per_item else t
+    p_light, p_color, *p_rest = route.per_item
+    n, k = point(normals, 3), point(colors, C)
+    L, lc = item(light, p_light, (3,)), item(light_color, p_color, (C,))
+    if model == _lib.LIGHT_DIFFUSE_DIRECTIONAL:
+        return _diffuse_directional(n, k, L, lc, double_sided)
+    if model == _lib.LIGHT_DIFFUSE_POINT:
+        return _diffuse_point(point(positions, 3), n, k, L, lc, double_sided)
+    return _specular_directional(point(positions, 3), n, k, L, lc, item(camera, p_rest[0], (3,)),
+                                 item(shininess, p_rest[1], ()), double_sided)
+
+
+class _Reflectance(torch.autograd.Function):
+    """dirt_lighting_forward with its gradient.  Per-point inputs are [rows, k] with unit stride along k; per-item inputs
+    contiguous [B, k] or shared [k] (shininess [B] or []).  The node keeps only its inputs: the backward kernel
+    recomputes the forward from them."""
+
+    @staticmethod
+    def forward(ctx, model, double_sided, route, normals, positions, colors, light, light_color, camera, shininess):
+        out = torch.empty(route.lead + (route.V, route.C), dtype=torch.float32, device=normals.device)
+        with torch.cuda.device(normals.device):
+            rc = _lib.lib().dirt_lighting_forward(*_inputs(model, double_sided, route, normals, positions, colors, light,
+                                                           light_color, camera, shininess), _ptr(out), route.B, route.V,
+                                                  route.C, _stream(normals.device))
+        _lib.check(rc, _MODEL_NAMES[model])
+        ctx.save_for_backward(normals, positions, colors, light, light_color, camera, shininess)
+        ctx.model, ctx.double_sided, ctx.route = model, double_sided, route
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        want = ctx.needs_input_grad[3:]
+        if not any(want):
+            return (None,) * 10
+        inputs = ctx.saved_tensors
+        if torch.is_grad_enabled():
+            # create_graph=True: differentiable gradients through the restatement
+            out = _restate(ctx.model, ctx.double_sided, ctx.route, *inputs)
+            wanted = [t for t, w in zip(inputs, want) if w]
+            grads = iter(torch.autograd.grad(out, wanted, grad_out, create_graph=True))
+            return (None,) * 3 + tuple(next(grads) if w else None for w in want)
+        route = ctx.route
+        dev = inputs[0].device
+        grads = [torch.empty(t.shape, dtype=torch.float32, device=dev) if w and t is not None else None
+                 for t, w in zip(inputs, want)]
+        lib = _lib.lib()
+        ws_bytes = int(lib.dirt_lighting_workspace_bytes(route.B, route.V, route.C)) if any(
+            g is not None for g in grads[3:]) else 0
+        workspace = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev) if ws_bytes else None
+        grad_out = grad_out.to(torch.float32).contiguous()
+        with torch.cuda.device(dev):
+            rc = lib.dirt_lighting_backward(*_inputs(ctx.model, ctx.double_sided, route, *inputs), _ptr(grad_out),
+                                            *[_ptr(g) for g in grads], _ptr(workspace), ws_bytes, route.B, route.V,
+                                            route.C, _stream(dev))
+        _lib.check(rc, _MODEL_NAMES[ctx.model] + 'Grad')
+        return (None,) * 3 + tuple(grads)
+
+
+def _stream(device):
+    return torch.cuda.current_stream(device).cuda_stream
+
+
+def _inputs(model, double_sided, route, normals, positions, colors, light, light_color, camera, shininess):
+    """The input arguments of dirt_lighting_forward / _backward, in their order."""
+    stride = lambda t: t.stride(0) if t is not None and t.shape[0] > 1 else 0
+    per_item = list(route.per_item) + [False] * (4 - len(route.per_item))
+    return [model, int(bool(double_sided)), _ptr(normals), stride(normals), _ptr(positions), stride(positions),
+            _ptr(colors), stride(colors), _ptr(light), int(per_item[0]), _ptr(light_color), int(per_item[1]),
+            _ptr(camera), int(per_item[2]), _ptr(shininess), int(per_item[3])]
+
+
+def _reflectance(model, double_sided, route, normals, colors, light, light_color, positions=None, camera=None,
+                 shininess=None):
+    """The CUDA path of a call that `cuda_route` accepted."""
+    C = route.C
+    item = lambda t, per_item: (t.reshape((route.B,) + t.shape[len(route.lead):]) if per_item else t).contiguous()
+    flags = list(route.per_item) + [False] * (4 - len(route.per_item))
+    return _Reflectance.apply(model, double_sided, route, _rows(normals, 3),
+                              _rows(positions, 3) if positions is not None else None, _rows(colors, C),
+                              item(light, flags[0]), item(light_color, flags[1]),
+                              item(camera, flags[2]) if camera is not None else None,
+                              item(shininess, flags[3]) if shininess is not None else None)
+
+
+def diffuse_directional(vertex_normals, vertex_colors, light_direction, light_color, double_sided=True, name=None):
+    """Lambertian reflectance under one directional light (dirt/lighting.py:182-225).
+
+    vertex_normals [*, V, 3], vertex_colors [*, V, C], light_direction [*, 3] or [3], light_color [*, C] or [C]
+    -> [*, V, C].  On CUDA in these shapes a fused kernel computes it; any other call runs the torch restatement."""
+    vertex_normals = torch.as_tensor(vertex_normals, dtype=torch.float32)
+    dev = vertex_normals.device
+    vertex_colors = torch.as_tensor(vertex_colors, dtype=torch.float32, device=dev)
+    light_direction = torch.as_tensor(light_direction, dtype=torch.float32, device=dev)
+    light_color = torch.as_tensor(light_color, dtype=torch.float32, device=dev)
+    route = _route([vertex_normals, vertex_colors], [(light_direction, 3), (light_color, 'C')])
+    if route is None:
+        return _diffuse_directional(vertex_normals, vertex_colors, light_direction, light_color, double_sided)
+    return _reflectance(_lib.LIGHT_DIFFUSE_DIRECTIONAL, double_sided, route, vertex_normals, vertex_colors,
+                        light_direction, light_color)
+
+
+def specular_directional(vertex_positions, vertex_normals, vertex_reflectivities, light_direction, light_color,
+                         camera_position, shininess, double_sided=True, name=None):
+    """Phong reflectance under one directional light (dirt/lighting.py:228-288).
+
+    vertex_positions, vertex_normals [*, V, 3], vertex_reflectivities [*, V, C], light_direction and camera_position
+    [*, 3] or [3], light_color [*, C] or [C], shininess [*] or [] -> [*, V, C].  On CUDA in these shapes a fused kernel
+    computes it; any other call runs the torch restatement."""
+    vertex_positions = torch.as_tensor(vertex_positions, dtype=torch.float32)
+    dev = vertex_positions.device
+    vertex_normals = torch.as_tensor(vertex_normals, dtype=torch.float32, device=dev)
+    vertex_reflectivities = torch.as_tensor(vertex_reflectivities, dtype=torch.float32, device=dev)
+    light_direction = torch.as_tensor(light_direction, dtype=torch.float32, device=dev)
+    light_color = torch.as_tensor(light_color, dtype=torch.float32, device=dev)
+    camera_position = torch.as_tensor(camera_position, dtype=torch.float32, device=dev)
+    shininess = torch.as_tensor(shininess, dtype=torch.float32, device=dev)
+    route = _route([vertex_positions, vertex_normals, vertex_reflectivities],
+                   [(light_direction, 3), (light_color, 'C'), (camera_position, 3), (shininess, 0)])
+    if route is None:
+        return _specular_directional(vertex_positions, vertex_normals, vertex_reflectivities, light_direction,
+                                     light_color, camera_position, shininess, double_sided)
+    return _reflectance(_lib.LIGHT_SPECULAR_DIRECTIONAL, double_sided, route, vertex_normals, vertex_reflectivities,
+                        light_direction, light_color, vertex_positions, camera_position, shininess)
+
+
 def diffuse_point(vertex_positions, vertex_normals, vertex_colors, light_position, light_color, double_sided=True, name=None):
-    """Lambertian reflectance under one point light (dirt/lighting.py:291-343)."""
+    """Lambertian reflectance under one point light (dirt/lighting.py:291-343).
+
+    vertex_positions, vertex_normals [*, V, 3], vertex_colors [*, V, C], light_position [*, 3] or [3], light_color
+    [*, C] or [C] -> [*, V, C].  On CUDA in these shapes a fused kernel computes it; any other call runs the torch
+    restatement."""
     vertex_positions = torch.as_tensor(vertex_positions, dtype=torch.float32)
     dev = vertex_positions.device
     vertex_normals = torch.as_tensor(vertex_normals, dtype=torch.float32, device=dev)
     vertex_colors = torch.as_tensor(vertex_colors, dtype=torch.float32, device=dev)
     light_position = torch.as_tensor(light_position, dtype=torch.float32, device=dev)
     light_color = torch.as_tensor(light_color, dtype=torch.float32, device=dev)
-    relative = vertex_positions - light_position[..., None, :]
-    incident = relative / (torch.linalg.norm(relative, dim=-1, keepdim=True) + 1.e-12)
-    cosines = (vertex_normals * incident).sum(-1)
-    return light_color[..., None, :] * vertex_colors * _cosine_term(cosines, double_sided)[..., None]
+    route = _route([vertex_positions, vertex_normals, vertex_colors], [(light_position, 3), (light_color, 'C')])
+    if route is None:
+        return _diffuse_point(vertex_positions, vertex_normals, vertex_colors, light_position, light_color, double_sided)
+    return _reflectance(_lib.LIGHT_DIFFUSE_POINT, double_sided, route, vertex_normals, vertex_colors, light_position,
+                        light_color, vertex_positions)

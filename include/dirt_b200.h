@@ -178,6 +178,52 @@ int dirt_texture_sample_backward(const float* texture, const float* indices, con
                                  float* grad_texture, float* grad_indices,
                                  int TB, int TH, int TW, int C, int B, long long N, int mode, void* cuda_stream);
 
+/* Reflectance models of the reference's lighting module (dirt/lighting.py:182-343), one value per point and channel.
+ * B items of V points each, C channels:
+ *   normals, positions   float32 [B*V, 3], row stride normals_stride / positions_stride floats, unit stride along the row
+ *   colors               float32 [B*V, C] (vertex colours or reflectivities), row stride colors_stride
+ *   light                float32 [B, 3] (light_per_item != 0) or [3] (shared): direction, or position for the point light
+ *   light_color          float32 [B, C] or [C];  camera float32 [B, 3] or [3];  shininess float32 [B] or [1]
+ *   out, grad_out        float32 [B*V, C], contiguous
+ * Per point, with m = -light, term(x) = double_sided ? |x| : max(x, 0), and out_c = (light_color_c * color_c) * f:
+ *   DIRT_LIGHT_DIFFUSE_DIRECTIONAL   f = term(n . m)                                  (positions, camera, shininess unused)
+ *   DIRT_LIGHT_SPECULAR_DIRECTIONAL  r = light + (2 (n . m)) n,  tc = camera - p,
+ *                                    f = pow(term((tc / |tc| + 1e-12) . r), shininess)   (NaN when p == camera)
+ *   DIRT_LIGHT_DIFFUSE_POINT         q = p - light,  f = term(n . (q / (|q| + 1e-12)))  (camera, shininess unused)
+ * Dot products are fma(a2, b2, fma(a1, b1, a0 * b0)); every other operation is one IEEE-rounded fp32 operation in the
+ * order written (pow is powf).
+ * Backward: the gradients torch autograd gives for the same expressions (at kinks too: no gradient through |x| at 0,
+ * the full gradient through max(x, 0) at 0, none through a zero vector's norm, pow's masks for exponent 0 and base 0).
+ * Each gradient output may be NULL, and its work is skipped; the per-point ones are contiguous [B*V, k], the
+ * parameter ones have the shape of their input.  Parameter gradients are summed in a fixed order (per-CTA partials in
+ * the workspace, then one reduction kernel): repeated calls give bit-identical results.  The workspace, of at least
+ * dirt_lighting_workspace_bytes(B, V, C) bytes, is needed only when a parameter gradient is wanted.
+ * B = 0 or V = 0: nothing is launched (the backward call still zeroes the wanted parameter gradients).
+ * All pointers 4-byte aligned; row strides >= 0. */
+enum {
+    DIRT_LIGHT_DIFFUSE_DIRECTIONAL = 0,
+    DIRT_LIGHT_SPECULAR_DIRECTIONAL = 1,
+    DIRT_LIGHT_DIFFUSE_POINT = 2
+};
+size_t dirt_lighting_workspace_bytes(int B, long long V, int C);
+int dirt_lighting_forward(int model, int double_sided,
+                          const float* normals, long long normals_stride,
+                          const float* positions, long long positions_stride,
+                          const float* colors, long long colors_stride,
+                          const float* light, int light_per_item, const float* light_color, int light_color_per_item,
+                          const float* camera, int camera_per_item, const float* shininess, int shininess_per_item,
+                          float* out, int B, long long V, int C, void* cuda_stream);
+int dirt_lighting_backward(int model, int double_sided,
+                           const float* normals, long long normals_stride,
+                           const float* positions, long long positions_stride,
+                           const float* colors, long long colors_stride,
+                           const float* light, int light_per_item, const float* light_color, int light_color_per_item,
+                           const float* camera, int camera_per_item, const float* shininess, int shininess_per_item,
+                           const float* grad_out,
+                           float* grad_normals, float* grad_positions, float* grad_colors,
+                           float* grad_light, float* grad_light_color, float* grad_camera, float* grad_shininess,
+                           void* workspace, size_t workspace_bytes, int B, long long V, int C, void* cuda_stream);
+
 /* Number of kernels the last call on this thread launched (bench.py's gpu_launches). */
 int dirt_last_launch_count(void);
 
