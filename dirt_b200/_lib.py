@@ -27,6 +27,8 @@ TEXTURE_NEAREST = 1
 LIGHT_DIFFUSE_DIRECTIONAL = 0
 LIGHT_SPECULAR_DIRECTIONAL = 1
 LIGHT_DIFFUSE_POINT = 2
+NORMALS_AVERAGE = 0
+NORMALS_PRE_SPLIT = 1
 
 
 def lib():
@@ -85,6 +87,12 @@ def load(path):
     L.dirt_lighting_forward.argtypes = light_inputs + [vp, i, ll, i, vp]
     L.dirt_lighting_backward.restype = i
     L.dirt_lighting_backward.argtypes = light_inputs + [vp] * 9 + [sz, i, ll, i, vp]
+    L.dirt_normals_workspace_bytes.restype = sz
+    L.dirt_normals_workspace_bytes.argtypes = [i, ll, ll]
+    L.dirt_normals_forward.restype = i
+    L.dirt_normals_forward.argtypes = [i, vp, ll, vp, vp, vp, sz, i, ll, ll, vp]
+    L.dirt_normals_backward.restype = i
+    L.dirt_normals_backward.argtypes = [i, vp, ll, vp, vp, vp, vp, sz, i, ll, ll, vp]
     return L
 
 
@@ -93,7 +101,8 @@ EXPORTED_SYMBOLS = ['dirt_error_string', 'dirt_abi_version', 'dirt_workspace_byt
                     'dirt_rasterise_visibility', 'dirt_peer_exchange_bytes', 'dirt_peer_exchange', 'dirt_last_launch_count',
                     'dirt_kernel_timer_enable', 'dirt_kernel_timer_elapsed_ms', 'dirt_texture_sample',
                     'dirt_texture_sample_backward', 'dirt_lighting_workspace_bytes', 'dirt_lighting_forward',
-                    'dirt_lighting_backward']
+                    'dirt_lighting_backward', 'dirt_normals_workspace_bytes', 'dirt_normals_forward',
+                    'dirt_normals_backward']
 
 
 def error_string(code):

@@ -423,6 +423,80 @@ extern "C" int dirt_lighting_backward(int model, int double_sided, const float* 
     return DIRT_OK;
 }
 
+// element offsets of the vertex rows stay below 2^62; vertex ids and incidence ids (k*F + f) are int32
+static bool normals_shape_ok(int mode, int B, long long V, long long F, long long stride)
+{
+    if (mode != DIRT_NORMALS_AVERAGE && mode != DIRT_NORMALS_PRE_SPLIT) return false;
+    if (B < 0 || V < 0 || F < 0 || stride < 3) return false;
+    if (V >= (1ll << 31) || 3 * F >= (1ll << 31)) return false;
+    return (double)B * V * stride <= 4.0e18;
+}
+
+extern "C" size_t dirt_normals_workspace_bytes(int B, long long V, long long F)
+{
+    if (!normals_shape_ok(DIRT_NORMALS_AVERAGE, B, V, F, 3) || B == 0 || V == 0 || F == 0) return 0;
+    return carve_normals_workspace(nullptr, B, V, F).bytes;
+}
+
+static int normals_check(const float* vertices, const int32_t* faces, const void* workspace, size_t workspace_bytes,
+                         int B, long long V, long long F)
+{
+    if (!vertices || (F > 0 && (!faces || !workspace))) return DIRT_ERR_NULL_POINTER;
+    if ((uintptr_t)vertices % 4 || (uintptr_t)faces % 4 || (uintptr_t)workspace % 4) return DIRT_ERR_MISALIGNED;
+    if (workspace_bytes < dirt_normals_workspace_bytes(B, V, F)) return DIRT_ERR_WORKSPACE_TOO_SMALL;
+    return DIRT_OK;
+}
+
+static NormalsArgs make_normals_args(int mode, const float* vertices, long long stride, const int32_t* faces, int B,
+                                     long long V, long long F)
+{
+    NormalsArgs a = {};
+    a.vertices = vertices; a.stride = stride; a.faces = faces;
+    a.total = (long long)B * V; a.V = (int)V; a.F = (int)F; a.mode = mode;
+    return a;
+}
+
+extern "C" int dirt_normals_forward(int mode, const float* vertices, long long vertex_stride, const int32_t* faces,
+                                    float* normals, void* workspace, size_t workspace_bytes, int B, long long V, long long F,
+                                    void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (!normals_shape_ok(mode, B, V, F, vertex_stride)) return DIRT_ERR_BAD_SHAPE;
+    if ((long long)B * V == 0) return DIRT_OK;
+    const int rc = normals_check(vertices, faces, workspace, workspace_bytes, B, V, F);
+    if (rc != DIRT_OK) return rc;
+    if (!normals) return DIRT_ERR_NULL_POINTER;
+    if ((uintptr_t)normals % 4) return DIRT_ERR_MISALIGNED;
+    NormalsArgs a = make_normals_args(mode, vertices, vertex_stride, faces, B, V, F);
+    a.out = normals;
+    CUDA_TRY(launch_normals_forward(a, carve_normals_workspace(F > 0 ? workspace : nullptr, B, V, F),
+                                    (cudaStream_t)cuda_stream, &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
+extern "C" int dirt_normals_backward(int mode, const float* vertices, long long vertex_stride, const int32_t* faces,
+                                     const float* grad_normals, float* grad_vertices, void* workspace,
+                                     size_t workspace_bytes, int B, long long V, long long F, void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (!normals_shape_ok(mode, B, V, F, vertex_stride)) return DIRT_ERR_BAD_SHAPE;
+    if ((long long)B * V == 0) return DIRT_OK;
+    const int rc = normals_check(vertices, faces, workspace, workspace_bytes, B, V, F);
+    if (rc != DIRT_OK) return rc;
+    if (!grad_normals || !grad_vertices) return DIRT_ERR_NULL_POINTER;
+    if ((uintptr_t)grad_normals % 4 || (uintptr_t)grad_vertices % 4) return DIRT_ERR_MISALIGNED;
+    NormalsArgs a = make_normals_args(mode, vertices, vertex_stride, faces, B, V, F);
+    a.grad = grad_normals;
+    a.g_vertices = grad_vertices;
+    CUDA_TRY(launch_normals_backward(a, carve_normals_workspace(F > 0 ? workspace : nullptr, B, V, F),
+                                     (cudaStream_t)cuda_stream, &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
 extern "C" int dirt_workspace_status(const void* workspace, size_t workspace_bytes, int B, int H, int W, int C, int V, int F,
                                      void* cuda_stream)
 {

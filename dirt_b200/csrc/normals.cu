@@ -1,0 +1,366 @@
+// normals.cu -- the vertex normals of dirt_b200/lighting.py (dirt_normals_forward / dirt_normals_backward,
+// DESIGN.md §7.3): per vertex, the normalised sum of the unit normals of the faces using it, or, for pre-split meshes,
+// the unit normal of its last face.
+//
+// The faces [F, 3] are shared by the batch, so the vertex -> incidence adjacency is built once per call, as CSR, from the
+// faces alone: offsets[V + 1] and the incidence ids i = k*F + f (corner k of face f) of each vertex in ascending order,
+// the order in which the restatement's three index_add calls visit them.  Faces with an index outside [0, V) are left
+// out.  The build counts the incidences per vertex (integer atomics), scans the counts, drops the ids into their rows
+// (integer atomics, in no fixed order) and then puts each id at its rank within its row, so the rows do not depend on
+// scheduling.
+//
+// Every other pass is one thread per (item, vertex) that gathers over its row and recomputes what it needs of each face
+// (its unit normal, or its corner gradients) from the positions: no per-face buffer, and no float atomics.  A row longer
+// than LONG_ROW is summed by the whole warp instead (lane-strided partial sums, then a butterfly), so that a high-valence
+// vertex does not hold up its warp's other 31 lanes.  Either way each sum has one fixed order for given faces, and two
+// calls give bit-identical results.
+#include <cub/block/block_scan.cuh>
+
+#include "../../include/dirt_b200.h"
+#include "common.cuh"
+
+namespace dirt {
+
+namespace {
+
+constexpr unsigned FULL = 0xffffffffu;
+constexpr int SCAN_THREADS = 1024;
+constexpr long long MAX_BLOCKS = 1ll << 20;
+
+__device__ __forceinline__ float3 ld3(const float* p) { return make_float3(__ldg(p), __ldg(p + 1), __ldg(p + 2)); }
+__device__ __forceinline__ void st3(float* p, float3 a) { p[0] = a.x; p[1] = a.y; p[2] = a.z; }
+__device__ __forceinline__ float3 add3(float3 a, float3 b)
+{
+    return make_float3(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y), __fadd_rn(a.z, b.z));
+}
+__device__ __forceinline__ float3 sub3(float3 a, float3 b)
+{
+    return make_float3(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y), __fsub_rn(a.z, b.z));
+}
+__device__ __forceinline__ float dot3(float3 a, float3 b)
+{
+    return __fmaf_rn(a.z, b.z, __fmaf_rn(a.y, b.y, __fmul_rn(a.x, b.x)));
+}
+// torch.linalg.cross: (a1 b2 - a2 b1, a2 b0 - a0 b2, a0 b1 - a1 b0)
+__device__ __forceinline__ float3 cross3(float3 a, float3 b)
+{
+    return make_float3(__fsub_rn(__fmul_rn(a.y, b.z), __fmul_rn(a.z, b.y)),
+                       __fsub_rn(__fmul_rn(a.z, b.x), __fmul_rn(a.x, b.z)),
+                       __fsub_rn(__fmul_rn(a.x, b.y), __fmul_rn(a.y, b.x)));
+}
+
+// x / (|x| + 1e-12)
+__device__ __forceinline__ float3 normalise(float3 x)
+{
+    const float d = __fadd_rn(__fsqrt_rn(dot3(x, x)), 1.e-12f);
+    return make_float3(__fdiv_rn(x.x, d), __fdiv_rn(x.y, d), __fdiv_rn(x.z, d));
+}
+
+// The gradient torch autograd gives `normalise` at x for the output gradient g: g / d through the numerator, and
+// -(g . x) / d^2 through d = |x| + 1e-12 on to x, except through the norm of a zero vector.
+__device__ __forceinline__ float3 normalise_grad(float3 x, float3 g)
+{
+    const float nr = __fsqrt_rn(dot3(x, x)), d = __fadd_rn(nr, 1.e-12f);
+    const float gd = -__fdiv_rn(dot3(g, x), __fmul_rn(d, d));
+    const float k = nr == 0.f ? 0.f : __fdiv_rn(gd, nr);
+    return make_float3(__fmaf_rn(x.x, k, __fdiv_rn(g.x, d)), __fmaf_rn(x.y, k, __fdiv_rn(g.y, d)),
+                       __fmaf_rn(x.z, k, __fdiv_rn(g.z, d)));
+}
+
+__device__ __forceinline__ bool load_face(const int* __restrict__ faces, long long f, int V, int v[3])
+{
+#pragma unroll
+    for (int k = 0; k < 3; ++k) v[k] = __ldg(faces + 3 * f + k);
+    return v[0] >= 0 && v[0] < V && v[1] >= 0 && v[1] < V && v[2] >= 0 && v[2] < V;
+}
+
+// The positions of the corners of face f of item b, and its edges from corner 0.
+struct Corners {
+    int v[3];
+    float3 e1, e2;
+};
+
+__device__ __forceinline__ Corners corners(const NormalsArgs& a, long long b, int f)
+{
+    Corners c;
+    load_face(a.faces, f, a.V, c.v);
+    const float* base = a.vertices + b * a.V * a.stride;
+    const float3 p0 = ld3(base + c.v[0] * a.stride);
+    c.e1 = sub3(ld3(base + c.v[1] * a.stride), p0);
+    c.e2 = sub3(ld3(base + c.v[2] * a.stride), p0);
+    return c;
+}
+
+// ---- the adjacency ----------------------------------------------------------------------------------------------------
+
+__global__ void __launch_bounds__(NORMALS_THREADS) count_kernel(const int* __restrict__ faces, int F, int V,
+                                                                int* __restrict__ counts)
+{
+    for (long long f = (long long)blockIdx.x * NORMALS_THREADS + threadIdx.x; f < F; f += (long long)gridDim.x * NORMALS_THREADS) {
+        int v[3];
+        if (!load_face(faces, f, V, v)) continue;
+#pragma unroll
+        for (int k = 0; k < 3; ++k) atomicAdd(counts + v[k], 1);
+    }
+}
+
+// offsets[v] = sum of counts[0 .. v), for v in [0, V]: one CTA, each thread scanning a contiguous chunk
+__global__ void __launch_bounds__(SCAN_THREADS) scan_kernel(const int* __restrict__ counts, int V, int* __restrict__ offsets)
+{
+    using Scan = cub::BlockScan<int, SCAN_THREADS>;
+    __shared__ typename Scan::TempStorage tmp;
+    const long long chunk = ((long long)V + SCAN_THREADS - 1) / SCAN_THREADS;
+    const long long lo = threadIdx.x * chunk, hi = lo + chunk < V ? lo + chunk : V;
+    int sum = 0;
+    for (long long v = lo; v < hi; ++v) sum += counts[v];
+    int run, total;
+    Scan(tmp).ExclusiveSum(sum, run, total);
+    for (long long v = lo; v < hi; ++v) {
+        offsets[v] = run;
+        run += counts[v];
+    }
+    if (threadIdx.x == 0) offsets[V] = total;
+}
+
+// Drops every incidence id into its vertex's row, at a place the atomics choose; counts[v] runs back down to 0.
+__global__ void __launch_bounds__(NORMALS_THREADS) fill_kernel(const int* __restrict__ faces, int F, int V,
+                                                               const int* __restrict__ offsets, int* __restrict__ counts,
+                                                               int* __restrict__ unsorted)
+{
+    for (long long f = (long long)blockIdx.x * NORMALS_THREADS + threadIdx.x; f < F; f += (long long)gridDim.x * NORMALS_THREADS) {
+        int v[3];
+        if (!load_face(faces, f, V, v)) continue;
+#pragma unroll
+        for (int k = 0; k < 3; ++k) unsorted[offsets[v[k]] + atomicSub(counts + v[k], 1) - 1] = k * F + (int)f;
+    }
+}
+
+// Moves every id to its rank among the ids of its row: the rows in ascending order.
+__global__ void __launch_bounds__(NORMALS_THREADS) rank_kernel(const int* __restrict__ faces, int F,
+                                                               const int* __restrict__ offsets,
+                                                               const int* __restrict__ unsorted, int* __restrict__ inc,
+                                                               int V)
+{
+    const long long n = offsets[V];
+    for (long long p = (long long)blockIdx.x * NORMALS_THREADS + threadIdx.x; p < n; p += (long long)gridDim.x * NORMALS_THREADS) {
+        const int i = unsorted[p], k = i / F, v = __ldg(faces + 3ll * (i - k * F) + k);
+        const int lo = offsets[v], hi = offsets[v + 1];
+        int rank = 0;
+        for (int j = lo; j < hi; ++j) rank += unsorted[j] < i;
+        inc[lo + rank] = i;
+    }
+}
+
+// ---- the per-vertex passes --------------------------------------------------------------------------------------------
+
+// The sum over the row [lo, hi) of item b of term(b, i) for its incidence ids i.  Rows of up to LONG_ROW ids are summed by
+// their own lane in row order; longer rows by the whole warp, one after another, each lane summing every 32nd id and the
+// warp adding the lanes' sums as a butterfly.  Warp-collective: every lane calls it, inactive ones with an empty row.
+template <class Term>
+__device__ __forceinline__ float3 row_sum(const int* __restrict__ inc, int lo, int hi, long long b, const Term& term)
+{
+    const int lane = threadIdx.x & 31;
+    float3 s = make_float3(0.f, 0.f, 0.f);
+    const bool long_row = hi - lo > NORMALS_LONG_ROW;
+    if (!long_row)
+        for (int j = lo; j < hi; ++j) s = add3(s, term(b, __ldg(inc + j)));
+    unsigned pending = __ballot_sync(FULL, long_row);
+    while (pending) {
+        const int src = __ffs(pending) - 1;
+        pending &= pending - 1;
+        const int l = __shfl_sync(FULL, lo, src), h = __shfl_sync(FULL, hi, src);
+        const long long bb = __shfl_sync(FULL, b, src);
+        float3 p = make_float3(0.f, 0.f, 0.f);
+        for (int j = l + lane; j < h; j += 32) p = add3(p, term(bb, __ldg(inc + j)));
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            p.x = __fadd_rn(p.x, __shfl_xor_sync(FULL, p.x, o));
+            p.y = __fadd_rn(p.y, __shfl_xor_sync(FULL, p.y, o));
+            p.z = __fadd_rn(p.z, __shfl_xor_sync(FULL, p.z, o));
+        }
+        if (lane == src) s = p;
+    }
+    return s;
+}
+
+// u_f of the face of incidence i
+struct FaceUnit {
+    const NormalsArgs& a;
+    __device__ __forceinline__ float3 operator()(long long b, int i) const
+    {
+        const int f = i % a.F;
+        const Corners c = corners(a, b, f);
+        return normalise(cross3(c.e1, c.e2));
+    }
+};
+
+// The gradient of corner k of the face of incidence i = k*F + f.  g_u of the face is the sum over its corners k' of
+// the gradient of the vertex they feed: gs (average), or, pre-split, grad_normals where the incidence k'*F + f is the
+// last of its vertex's row.
+template <int MODE>
+struct CornerGrad {
+    const NormalsArgs& a;
+    __device__ __forceinline__ float3 operator()(long long b, int i) const
+    {
+        const int k = i / a.F, f = i - k * a.F;
+        const Corners c = corners(a, b, f);
+        float3 gu = make_float3(0.f, 0.f, 0.f);
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+            const long long row = b * a.V + c.v[j];
+            if (MODE == DIRT_NORMALS_AVERAGE) gu = add3(gu, ld3(a.gs + 3 * row));
+            else if (__ldg(a.inc + __ldg(a.offsets + c.v[j] + 1) - 1) == j * a.F + f)
+                gu = add3(gu, ld3(a.grad + 3 * row));
+        }
+        const float3 gn = normalise_grad(cross3(c.e1, c.e2), gu);
+        const float3 g1 = cross3(c.e2, gn), g2 = cross3(gn, c.e1);   // d/d e1, d/d e2
+        if (k == 1) return g1;
+        if (k == 2) return g2;
+        return make_float3(-__fadd_rn(g1.x, g2.x), -__fadd_rn(g1.y, g2.y), -__fadd_rn(g1.z, g2.z));
+    }
+};
+
+// The threads of a warp take consecutive (item, vertex) rows t = b*V + v; the loop is warp-uniform.
+#define FOR_EACH_ROW(a)                                                                                                \
+    for (long long t0 = (long long)blockIdx.x * NORMALS_THREADS + (threadIdx.x & ~31); t0 < (a).total;               \
+         t0 += (long long)gridDim.x * NORMALS_THREADS)
+
+struct Row {
+    long long t, b;
+    int lo, hi;
+    bool active;
+};
+
+__device__ __forceinline__ Row row_of(const NormalsArgs& a, long long t0)
+{
+    Row r;
+    r.t = t0 + (threadIdx.x & 31);
+    r.active = r.t < a.total;
+    r.b = r.active ? r.t / a.V : 0;
+    const long long v = r.t - r.b * a.V;
+    r.lo = r.hi = 0;
+    if (r.active) {
+        r.lo = __ldg(a.offsets + v);
+        r.hi = __ldg(a.offsets + v + 1);
+    }
+    return r;
+}
+
+template <int MODE>
+__global__ void __launch_bounds__(NORMALS_THREADS) normals_forward_kernel(NormalsArgs a)
+{
+    FOR_EACH_ROW(a) {
+        const Row r = row_of(a, t0);
+        float3 n;
+        if (MODE == DIRT_NORMALS_AVERAGE) {
+            n = normalise(row_sum(a.inc, r.lo, r.hi, r.b, FaceUnit{a}));
+        } else {
+            n = r.hi > r.lo ? FaceUnit{a}(r.b, __ldg(a.inc + r.hi - 1)) : make_float3(0.f, 0.f, 0.f);
+        }
+        if (r.active) st3(a.out + 3 * r.t, n);
+    }
+}
+
+// average mode: gs = the gradient of the vertex's sum of face normals
+__global__ void __launch_bounds__(NORMALS_THREADS) normals_sum_grad_kernel(NormalsArgs a)
+{
+    FOR_EACH_ROW(a) {
+        const Row r = row_of(a, t0);
+        const float3 s = row_sum(a.inc, r.lo, r.hi, r.b, FaceUnit{a});
+        if (r.active) st3(a.gs + 3 * r.t, normalise_grad(s, ld3(a.grad + 3 * r.t)));
+    }
+}
+
+template <int MODE>
+__global__ void __launch_bounds__(NORMALS_THREADS) normals_position_grad_kernel(NormalsArgs a)
+{
+    FOR_EACH_ROW(a) {
+        const Row r = row_of(a, t0);
+        const float3 g = row_sum(a.inc, r.lo, r.hi, r.b, CornerGrad<MODE>{a});
+        if (r.active) st3(a.g_vertices + 3 * r.t, g);
+    }
+}
+
+inline unsigned blocks_for(long long n)
+{
+    const long long b = (n + NORMALS_THREADS - 1) / NORMALS_THREADS;
+    return (unsigned)(b < 1 ? 1 : (b < MAX_BLOCKS ? b : MAX_BLOCKS));
+}
+
+}  // namespace
+
+NormalsWorkspace carve_normals_workspace(void* base, int B, long long V, long long F)
+{
+    NormalsWorkspace w = {};
+    char* p = static_cast<char*>(base);
+    size_t off = 0;
+    auto take = [&](size_t bytes) {
+        char* q = p ? p + off : nullptr;
+        off += (bytes + 255) & ~size_t(255);
+        return q;
+    };
+    w.offsets = reinterpret_cast<int*>(take(sizeof(int) * (size_t)(V + 1)));
+    w.inc = reinterpret_cast<int*>(take(sizeof(int) * (size_t)(3 * F)));
+    // the build's scratch (counts, unsorted ids) and the backward's per-vertex gradients share one region
+    const size_t build = ((sizeof(int) * (size_t)V + 255) & ~size_t(255)) + sizeof(int) * (size_t)(3 * F);
+    const size_t grads = sizeof(float) * 3 * (size_t)B * (size_t)V;
+    char* scratch = take(build > grads ? build : grads);
+    w.counts = reinterpret_cast<int*>(scratch);
+    w.unsorted = scratch ? reinterpret_cast<int*>(scratch + ((sizeof(int) * (size_t)V + 255) & ~size_t(255))) : nullptr;
+    w.gs = reinterpret_cast<float*>(scratch);
+    w.bytes = off;
+    return w;
+}
+
+cudaError_t launch_normals_forward(NormalsArgs a, const NormalsWorkspace& w, cudaStream_t stream, int* launches)
+{
+    cudaError_t e;
+    if (a.total == 0) return cudaSuccess;
+    if (a.F == 0) return cudaMemsetAsync(a.out, 0, sizeof(float) * 3 * (size_t)a.total, stream);
+    const int V = a.V, F = a.F;
+    if ((e = cudaMemsetAsync(w.counts, 0, sizeof(int) * (size_t)V, stream)) != cudaSuccess) return e;
+    count_kernel<<<blocks_for(F), NORMALS_THREADS, 0, stream>>>(a.faces, F, V, w.counts);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    ++*launches;
+    scan_kernel<<<1, SCAN_THREADS, 0, stream>>>(w.counts, V, w.offsets);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    ++*launches;
+    fill_kernel<<<blocks_for(F), NORMALS_THREADS, 0, stream>>>(a.faces, F, V, w.offsets, w.counts, w.unsorted);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    ++*launches;
+    rank_kernel<<<blocks_for(3ll * F), NORMALS_THREADS, 0, stream>>>(a.faces, F, w.offsets, w.unsorted, w.inc, V);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    ++*launches;
+    a.offsets = w.offsets;
+    a.inc = w.inc;
+    if (a.mode == DIRT_NORMALS_AVERAGE)
+        normals_forward_kernel<DIRT_NORMALS_AVERAGE><<<blocks_for(a.total), NORMALS_THREADS, 0, stream>>>(a);
+    else
+        normals_forward_kernel<DIRT_NORMALS_PRE_SPLIT><<<blocks_for(a.total), NORMALS_THREADS, 0, stream>>>(a);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    ++*launches;
+    return cudaSuccess;
+}
+
+cudaError_t launch_normals_backward(NormalsArgs a, const NormalsWorkspace& w, cudaStream_t stream, int* launches)
+{
+    cudaError_t e;
+    if (a.total == 0) return cudaSuccess;
+    if (a.F == 0) return cudaMemsetAsync(a.g_vertices, 0, sizeof(float) * 3 * (size_t)a.total, stream);
+    a.offsets = w.offsets;
+    a.inc = w.inc;
+    a.gs = w.gs;
+    if (a.mode == DIRT_NORMALS_AVERAGE) {
+        normals_sum_grad_kernel<<<blocks_for(a.total), NORMALS_THREADS, 0, stream>>>(a);
+        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+        ++*launches;
+        normals_position_grad_kernel<DIRT_NORMALS_AVERAGE><<<blocks_for(a.total), NORMALS_THREADS, 0, stream>>>(a);
+    } else {
+        normals_position_grad_kernel<DIRT_NORMALS_PRE_SPLIT><<<blocks_for(a.total), NORMALS_THREADS, 0, stream>>>(a);
+    }
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    ++*launches;
+    return cudaSuccess;
+}
+
+}  // namespace dirt

@@ -1,8 +1,11 @@
 """Mesh normals and simple reflectance models; mirrors the API of dirt/lighting.py.
 
-The normals are torch code.  The three reflectance models run CUDA kernels (dirt_lighting_forward / _backward of
-include/dirt_b200.h) when their inputs are on one CUDA device in the shapes `cuda_route` accepts, and their torch
-restatements (`_diffuse_directional`, `_specular_directional`, `_diffuse_point`) otherwise; see DESIGN.md §7.2.
+`vertex_normals` and `vertex_normals_pre_split` run CUDA kernels (dirt_normals_forward / _backward of
+include/dirt_b200.h) when their vertices are float32 on a CUDA device in the shapes `normals_route` accepts, and their
+torch restatements (`_vertex_normals`, `_vertex_normals_pre_split`) otherwise; see DESIGN.md §7.3.  The three
+reflectance models run CUDA kernels (dirt_lighting_forward / _backward) when their inputs are on one CUDA device in the
+shapes `cuda_route` accepts, and their torch restatements (`_diffuse_directional`, `_specular_directional`,
+`_diffuse_point`) otherwise; see DESIGN.md §7.2.  `split_vertices_by_face` is torch code.
 """
 import math
 from collections import namedtuple
@@ -24,9 +27,8 @@ def _face_normals(vertices, faces):
     return n / (torch.linalg.norm(n, dim=-1, keepdim=True) + 1.e-12)
 
 
-def vertex_normals(vertices, faces, name=None):
-    """Per-vertex normals: normalised sum of the unit normals of the faces using each vertex
-    (dirt/lighting.py:34-93).  vertices [*,V,3|4], faces [F,3] -> [*,V,3]."""
+def _vertex_normals(vertices, faces):
+    """The torch restatement of `vertex_normals`: its CPU implementation and its specification."""
     vertices, faces = _prepare(vertices, faces)
     vertices = vertices[..., :3]
     normals_by_face = _face_normals(vertices, faces)  # [*, F, 3]
@@ -36,9 +38,8 @@ def vertex_normals(vertices, faces, name=None):
     return summed / (torch.linalg.norm(summed, dim=-1, keepdim=True) + 1.e-12)
 
 
-def vertex_normals_pre_split(vertices, faces, name=None, static=False):
-    """As `vertex_normals` for meshes where every vertex belongs to exactly one face
-    (dirt/lighting.py:101-133)."""
+def _vertex_normals_pre_split(vertices, faces):
+    """The torch restatement of `vertex_normals_pre_split`: its CPU implementation and its specification."""
     vertices, faces = _prepare(vertices, faces)
     vertices = vertices[..., :3]
     normals_by_face = _face_normals(vertices, faces)
@@ -46,6 +47,27 @@ def vertex_normals_pre_split(vertices, faces, name=None, static=False):
     for corner in range(3):
         out = out.index_copy(-2, faces[:, corner], normals_by_face)
     return out
+
+
+def vertex_normals(vertices, faces, name=None):
+    """Per-vertex normals: normalised sum of the unit normals of the faces using each vertex
+    (dirt/lighting.py:34-93).  vertices [*,V,3|4], faces [F,3] -> [*,V,3].  On CUDA in the shapes `normals_route`
+    accepts, kernels compute it (a face with an index outside [0, V) is then left out); any other call runs the torch
+    restatement."""
+    route = _normals_route(vertices, faces)
+    if route is None:
+        return _vertex_normals(vertices, faces)
+    return _normals(_lib.NORMALS_AVERAGE, route, vertices, faces)
+
+
+def vertex_normals_pre_split(vertices, faces, name=None, static=False):
+    """As `vertex_normals` for meshes where every vertex belongs to exactly one face
+    (dirt/lighting.py:101-133): each vertex takes the unit normal of its face (of its last face corner, corner-major,
+    when there are several).  Routed as `vertex_normals`."""
+    route = _normals_route(vertices, faces)
+    if route is None:
+        return _vertex_normals_pre_split(vertices, faces)
+    return _normals(_lib.NORMALS_PRE_SPLIT, route, vertices, faces)
 
 
 def split_vertices_by_face(vertices, faces, name=None):
@@ -307,3 +329,96 @@ def diffuse_point(vertex_positions, vertex_normals, vertex_colors, light_positio
         return _diffuse_point(vertex_positions, vertex_normals, vertex_colors, light_position, light_color, double_sided)
     return _reflectance(_lib.LIGHT_DIFFUSE_POINT, double_sided, route, vertex_normals, vertex_colors, light_position,
                         light_color, vertex_positions)
+
+
+# ---- the CUDA path of the normals -----------------------------------------------------------------------------------
+
+NormalsRoute = namedtuple('NormalsRoute', 'lead B V F')
+
+
+def normals_route(vertex_shape, vertex_dtype, vertex_device, face_shape, face_dtype):
+    """Whether a normals call runs the CUDA kernels, decided from shapes, dtypes and devices alone: float32 vertices
+    [*, V, 3] or [*, V, 4] on a CUDA device, with prod(*) < 2^31 and V < 2^31, and int32 or int64 faces [F, 3] on any
+    device, with 3F < 2^31.  Returns a NormalsRoute (lead = `*`, B = its product, V, F) or None."""
+    vertex_shape, face_shape = tuple(vertex_shape), tuple(face_shape)
+    if vertex_device.type != 'cuda' or vertex_dtype != torch.float32 or face_dtype not in (torch.int32, torch.int64):
+        return None
+    if len(vertex_shape) < 2 or vertex_shape[-1] not in (3, 4) or len(face_shape) != 2 or face_shape[1] != 3:
+        return None
+    lead, V, F = vertex_shape[:-2], vertex_shape[-2], face_shape[0]
+    B = math.prod(lead)
+    if B >= 1 << 31 or V >= 1 << 31 or 3 * F >= 1 << 31:
+        return None
+    return NormalsRoute(lead, B, V, F)
+
+
+def _normals_route(vertices, faces):
+    if not isinstance(vertices, torch.Tensor):
+        return None
+    faces = faces if isinstance(faces, torch.Tensor) else torch.as_tensor(faces)
+    return normals_route(vertices.shape, vertices.dtype, vertices.device, faces.shape, faces.dtype)
+
+
+_NORMALS_NAMES = {_lib.NORMALS_AVERAGE: 'VertexNormals', _lib.NORMALS_PRE_SPLIT: 'VertexNormalsPreSplit'}
+
+
+class _Normals(torch.autograd.Function):
+    """dirt_normals_forward with its gradient.  rows: the vertices' positions as [B*V, 3] with unit stride along the row
+    and one row stride >= 3; faces: int32 [F, 3] on their device.  The node keeps its inputs and the forward's
+    workspace, whose adjacency the backward kernels read."""
+
+    @staticmethod
+    def forward(ctx, mode, route, rows, faces):
+        dev = rows.device
+        lib = _lib.lib()
+        out = torch.empty((route.B * route.V, 3), dtype=torch.float32, device=dev)
+        ws_bytes = int(lib.dirt_normals_workspace_bytes(route.B, route.V, route.F))
+        workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=dev) if ws_bytes else None
+        with torch.cuda.device(dev):
+            rc = lib.dirt_normals_forward(mode, _ptr(rows), _row_stride(rows), _ptr(faces), _ptr(out), _ptr(workspace),
+                                          ws_bytes, route.B, route.V, route.F, _stream(dev))
+        _lib.check(rc, _NORMALS_NAMES[mode])
+        ctx.save_for_backward(rows, faces)
+        ctx.mode, ctx.route, ctx.workspace, ctx.ws_bytes = mode, route, workspace, ws_bytes
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        if not ctx.needs_input_grad[2]:
+            return None, None, None, None
+        rows, faces = ctx.saved_tensors
+        route = ctx.route
+        if torch.is_grad_enabled():
+            # create_graph=True: differentiable gradients through the restatement, on the faces the kernels used
+            valid = faces[((faces >= 0) & (faces < route.V)).all(1)]
+            restate = _vertex_normals if ctx.mode == _lib.NORMALS_AVERAGE else _vertex_normals_pre_split
+            out = restate(rows.reshape(route.lead + (route.V, 3)), valid)
+            grad, = torch.autograd.grad(out, rows, grad_out.reshape(out.shape), create_graph=True)
+            return None, None, grad, None
+        dev = rows.device
+        grad_out = grad_out.to(torch.float32).contiguous()
+        grad = torch.empty((route.B * route.V, 3), dtype=torch.float32, device=dev)
+        lib = _lib.lib()
+        with torch.cuda.device(dev):
+            rc = lib.dirt_normals_backward(ctx.mode, _ptr(rows), _row_stride(rows), _ptr(faces), _ptr(grad_out),
+                                           _ptr(grad), _ptr(ctx.workspace), ctx.ws_bytes, route.B, route.V, route.F,
+                                           _stream(dev))
+        _lib.check(rc, _NORMALS_NAMES[ctx.mode] + 'Grad')
+        return None, None, grad, None
+
+
+def _row_stride(rows):
+    return rows.stride(0) if rows.shape[0] > 1 else 3
+
+
+def _normals(mode, route, vertices, faces):
+    """The CUDA path of a call that `normals_route` accepted."""
+    faces = torch.as_tensor(faces).to(device=vertices.device)
+    if faces.dtype == torch.int64:
+        faces = faces.clamp(-1, (1 << 31) - 1)   # above int32: >= V, so left out like any other invalid index
+    faces = faces.to(torch.int32).contiguous()
+    rows = _rows(vertices[..., :3], 3)
+    if rows.shape[0] > 1 and rows.stride(0) < 3:
+        rows = rows.contiguous()
+    out = _Normals.apply(mode, route, rows, faces)
+    return out.reshape(route.lead + (route.V, 3))

@@ -224,6 +224,39 @@ int dirt_lighting_backward(int model, int double_sided,
                            float* grad_light, float* grad_light_color, float* grad_camera, float* grad_shininess,
                            void* workspace, size_t workspace_bytes, int B, long long V, int C, void* cuda_stream);
 
+/* Vertex normals of the reference's lighting module (dirt/lighting.py:34-133) for B items of V vertices sharing the
+ * faces:
+ *   vertices             float32 [B*V, 3], row stride vertex_stride >= 3 floats, unit stride along the row (the first
+ *                        three columns of a [B, V, 4] tensor go in as they are, with vertex_stride 4)
+ *   faces                int32 [F, 3], shared by the batch
+ *   normals, grad_normals, grad_vertices   float32 [B*V, 3], contiguous
+ * With u_f = n_f / (|n_f| + 1e-12), n_f = (p1 - p0) x (p2 - p0) for the corners p0, p1, p2 of face f:
+ *   DIRT_NORMALS_AVERAGE    normal_v = s_v / (|s_v| + 1e-12), s_v = sum of u_f over every corner of every face that
+ *                           is v (a face naming v twice adds twice)
+ *   DIRT_NORMALS_PRE_SPLIT  normal_v = u_f of the last face corner naming v, corner-major then by face (0 if none)
+ * A face with an index outside [0, V) is left out: it adds nothing and receives no gradient.
+ * Backward: grad_vertices = the gradient torch autograd gives the same expressions (no gradient through the norm of a
+ * zero vector; the division by |x| + 1e-12 passes its full 1e12).  Pre-split, grad_normals of v reaches only the face
+ * corner whose normal v took, and the positions of every face reach all three of its vertices.
+ * Workspace: at least dirt_normals_workspace_bytes(B, V, F) bytes (0 when B, V or F is 0), a function of the sizes
+ * alone.  The forward call writes the vertex -> face-corner adjacency into it, and the backward call reads it there:
+ * pass the backward call the workspace of the forward call on the same faces and V, with nothing written to it since.
+ * The backward call also uses the rest of the workspace as scratch.
+ * Every sum has one fixed order (no float atomics): repeated calls give bit-identical normals and gradients.
+ * B = 0 or V = 0: nothing is launched; F = 0: the outputs are zeroed.  V < 2^31, 3F < 2^31; all pointers 4-byte
+ * aligned. */
+enum {
+    DIRT_NORMALS_AVERAGE = 0,
+    DIRT_NORMALS_PRE_SPLIT = 1
+};
+size_t dirt_normals_workspace_bytes(int B, long long V, long long F);
+int dirt_normals_forward(int mode, const float* vertices, long long vertex_stride, const int32_t* faces,
+                         float* normals, void* workspace, size_t workspace_bytes,
+                         int B, long long V, long long F, void* cuda_stream);
+int dirt_normals_backward(int mode, const float* vertices, long long vertex_stride, const int32_t* faces,
+                          const float* grad_normals, float* grad_vertices, void* workspace, size_t workspace_bytes,
+                          int B, long long V, long long F, void* cuda_stream);
+
 /* Number of kernels the last call on this thread launched (bench.py's gpu_launches). */
 int dirt_last_launch_count(void);
 
