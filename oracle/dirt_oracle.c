@@ -533,9 +533,11 @@ static inline float scharr_comp(float nn, float np, float pn, float pp, float mn
 
 static void backward_image_group(const float* verts, const Tri* tris, const int32_t* ids_rows, int rb,
                                  const float* pixels, const float* grad_pixels,
-                                 double* gverts /*[V,4]*/, int b, int B, int H, int W, int C, int c0, int n, int r0, int r1)
+                                 double* gverts /*[V,4]*/, int b, int B, int H, int W, int C, int c0, int n, int r0, int r1,
+                                 uint8_t* dilated /*[B,H,W] of this group, or NULL*/)
 {
-    /* rows [r0, r1) of the image; ids_rows holds the visibility buffer from row rb on (rb <= r0 - 1 unless r0 == 0) */
+    /* rows [r0, r1) of the image; ids_rows holds the visibility buffer from row rb on (rb <= r0 - 1 unless r0 == 0).
+     * `dilated` marks the pixels that take a neighbour's face (the reference's debug_thingy[..., 0] = 1e-2, :172) */
 #define IDS(r_, c_) ids_rows[((r_) - rb) * W + (c_)]
     for (int r = r0; r < r1; ++r)
         for (int c = 0; c < W; ++c) {
@@ -576,6 +578,7 @@ static void backward_image_group(const float* verts, const Tri* tris, const int3
                         if (differs && g[3] > gn[3]) {
                             g[0] = gn[0]; g[1] = gn[1]; g[2] = gn[2]; g[3] = gn[3];
                             f = fn;
+                            if (dilated) dilated[((size_t)b * H + r) * W + c] = 1;
                             break;
                         }
                     }
@@ -611,10 +614,12 @@ static void backward_image_group(const float* verts, const Tri* tris, const int3
 #undef IDS
 }
 
-int dirt_oracle_backward(const float* vertices, const int32_t* faces, const float* pixels,
-                         const float* grad_pixels, float* grad_background, float* grad_vertices,
-                         float* grad_vertex_colors, int B, int H, int W, int C, int V, int F,
-                         const int* channel_groups, int n_groups)
+/* dirt_oracle_backward with the dilation decisions: `dilated` (NULL, or zeroed uint8 [n_groups, B, H, W] with one
+ * plane per channel group in call order) gets 1 where a pixel takes a neighbour's face */
+int dirt_oracle_backward_ex(const float* vertices, const int32_t* faces, const float* pixels,
+                            const float* grad_pixels, float* grad_background, float* grad_vertices,
+                            float* grad_vertex_colors, int B, int H, int W, int C, int V, int F,
+                            const int* channel_groups, int n_groups, uint8_t* dilated)
 {
     if (B < 0 || H <= 0 || W <= 0 || C <= 0 || V < 0 || F < 0) return -1;
     int* groups = (int*)malloc(sizeof(int) * (size_t)(C + 1));
@@ -675,7 +680,8 @@ int dirt_oracle_backward(const float* vertices, const int32_t* faces, const floa
             }
         int c0 = 0;
         for (int gi = 0; gi < ng; ++gi) {
-            backward_image_group(verts, tris, ids, rb, pixels, grad_pixels, gv, b, B, H, W, C, c0, groups[gi], r0, r1);
+            backward_image_group(verts, tris, ids, rb, pixels, grad_pixels, gv, b, B, H, W, C, c0, groups[gi], r0, r1,
+                                 dilated ? dilated + (size_t)gi * B * H * W : NULL);
             c0 += groups[gi];
         }
         free(ids); free(keys);
@@ -697,6 +703,15 @@ int dirt_oracle_backward(const float* vertices, const int32_t* faces, const floa
     free(gv_all); free(gc_all);
     free(groups);
     return fail ? -2 : 0;
+}
+
+int dirt_oracle_backward(const float* vertices, const int32_t* faces, const float* pixels,
+                         const float* grad_pixels, float* grad_background, float* grad_vertices,
+                         float* grad_vertex_colors, int B, int H, int W, int C, int V, int F,
+                         const int* channel_groups, int n_groups)
+{
+    return dirt_oracle_backward_ex(vertices, faces, pixels, grad_pixels, grad_background, grad_vertices,
+                                   grad_vertex_colors, B, H, W, C, V, F, channel_groups, n_groups, NULL);
 }
 
 /* debug: per-face setup records of one image, for comparing the CUDA setup kernel bit for bit */

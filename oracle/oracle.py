@@ -106,8 +106,11 @@ def forward(background, vertices, vertex_colors, faces, return_face_ids=False):
     return (pixels, ids) if return_face_ids else pixels
 
 
-def backward(vertices, faces, pixels, grad_pixels, channel_groups=None):
-    """RasteriseGrad: -> grad_background [B,H,W,C], grad_vertices [B,V,4], grad_vertex_colors [B,V,C]."""
+def backward(vertices, faces, pixels, grad_pixels, channel_groups=None, return_dilation=False):
+    """RasteriseGrad: -> grad_background [B,H,W,C], grad_vertices [B,V,4], grad_vertex_colors [B,V,C].
+    With return_dilation, also a list with one bool [B,H,W] mask per channel group (the given groups, or the greedy
+    split): the pixels whose position gradient goes to a neighbour's face, as oracle/ref.py backward returns them from
+    the reference kernel."""
     vertices, faces = _f32(vertices), _i32(faces)
     pixels, grad_pixels = _f32(pixels), _f32(grad_pixels)
     B, H, W, C = pixels.shape
@@ -121,11 +124,14 @@ def backward(vertices, faces, pixels, grad_pixels, channel_groups=None):
     else:
         arr = (ctypes.c_int * len(channel_groups))(*channel_groups)
         groups_ptr, ng = arr, len(channel_groups)
-    rc = lib().dirt_oracle_backward(_ptr(vertices), _ptr(faces), _ptr(pixels), _ptr(grad_pixels),
-                                    _ptr(gb), _ptr(gv), _ptr(gc), B, H, W, C, V, F, groups_ptr, ng)
+    n_masks = len(channel_groups) if channel_groups is not None else len(default_groups(C))
+    dilated = np.zeros((n_masks, B, H, W), np.uint8) if return_dilation else None
+    rc = lib().dirt_oracle_backward_ex(_ptr(vertices), _ptr(faces), _ptr(pixels), _ptr(grad_pixels),
+                                       _ptr(gb), _ptr(gv), _ptr(gc), B, H, W, C, V, F, groups_ptr, ng,
+                                       _ptr(dilated) if return_dilation else None)
     if rc != 0:
         raise RuntimeError('dirt_oracle_backward failed: %d' % rc)
-    return gb, gv, gc
+    return (gb, gv, gc, list(dilated.astype(bool))) if return_dilation else (gb, gv, gc)
 
 
 class TriExport(ctypes.Structure):

@@ -10,13 +10,12 @@ Comparisons are those of test_gpu_parity._check_scene: face ids and grad_backgro
 (1e-4 relative), with the worst ratios in the end-of-run summary under names starting with 'paths:'.
 """
 import ctypes
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
 import kernel_paths as kp
+import variant_builds
 from conftest import rel_close
 
 pytestmark = pytest.mark.gpu
@@ -298,14 +297,8 @@ def test_pixels_against_fp64_truth_extreme_w_is_logged(cuda_lib):
 
 @pytest.fixture(scope='session')
 def four_slot_lib(cuda_lib, tmp_path_factory):
-    """libdirt_b200 built with DIRT_BWD_SLOTS_C4 = DIRT_BWD_SLOTS_C3 = 4, outside the tree."""
-    from dirt_b200 import _lib, build
-    out = str(tmp_path_factory.mktemp('variant') / 'libdirt_b200_slots4.so')
-    srcs = [os.path.join(os.path.dirname(build.SO_PATH), 'csrc', s) for s in build.SOURCES]
-    cmd = [build._nvcc()] + build.NVCC_FLAGS + ['-DDIRT_BWD_SLOTS_C4=4', '-DDIRT_BWD_SLOTS_C3=4', '-o', out] + srcs
-    proc = subprocess.run(cmd, capture_output=True, text=True)
-    assert proc.returncode == 0, proc.stdout + proc.stderr
-    return _lib.load(out)
+    """libdirt_b200 built with DIRT_BWD_SLOTS_C4 = DIRT_BWD_SLOTS_C3 = 4, outside the tree (variant_builds.py)."""
+    return variant_builds.four_slot_library(tmp_path_factory)
 
 
 @pytest.mark.parametrize('channels,groups', kp.OVERFLOW_CHANNELS)

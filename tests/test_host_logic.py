@@ -147,3 +147,43 @@ def test_bench_reference_arm_prints_one_json_line():
                 'cpu_baseline', 'e2e'):
         assert key in out, key
     assert out['value'] > 0 and out['cpu_baseline']['kind'] == 'port' and out['e2e']['h2d_bytes_per_step'] == 0
+
+
+def test_reference_gradient_library_is_built():
+    """Where a reference checkout can be found, __graft_entry__.build() compiles the reference's gradient kernel into
+    oracle/_ref/libdirt_ref_grad.so, which tests/test_gpu_ref_live.py runs against the CUDA path; a build() that quietly
+    stopped producing it would turn those tests into skips."""
+    from oracle import ref
+    if not ref.can_build():
+        pytest.skip('no reference checkout (neither $DIRT_REFERENCE nor a `reference` directory beside the repository)')
+    so = os.path.join(ROOT, 'oracle', '_ref', 'libdirt_ref_grad.so')
+    assert os.path.exists(so), '%s is missing although a reference checkout is at %s' % (so, ref.reference_checkout())
+    lib = ctypes.CDLL(so)
+    for name in ('dirt_ref_assemble_grads', 'dirt_ref_upload_vertices', 'dirt_ref_sizeof_vertex'):
+        assert hasattr(lib, name), name
+
+
+def test_reference_inputs_and_oracle_dilation_masks():
+    """The host side of the live reference comparison: the vertex-index image the reference's fragment shader would
+    write, and the oracle's dilation masks (one per channel group, the same gradients as without them)."""
+    from dirt_b200 import scenes
+    from oracle import oracle, ref
+    s = scenes.random_soup(batch=3, width=33, height=27, n_faces=40, channels=4, seed=4)
+    ids, _ = oracle.visibility(s['vertices'], s['faces'], 27, 33)
+    vids = ref.vertex_ids_image(s['faces'], ids)
+    for b in range(3):
+        for r, c in zip(*np.nonzero(ids[b] >= 0)):
+            assert (vids[b, r, c] == s['faces'][b, ids[b, r, c]]).all()
+        assert (vids[b][ids[b] < 0] == -1).all()
+    pixels = oracle.forward(**s)
+    gp = np.random.default_rng(2).standard_normal(pixels.shape).astype(np.float32)
+    plain = oracle.backward(s['vertices'], s['faces'], pixels, gp, [1, 3])
+    gb, gv, gc, masks = oracle.backward(s['vertices'], s['faces'], pixels, gp, [1, 3], return_dilation=True)
+    for a, b in zip(plain, (gb, gv, gc)):
+        np.testing.assert_array_equal(a, b)
+    assert len(masks) == 2 and all(m.shape == ids.shape and m.dtype == bool for m in masks)
+    for m in masks:
+        assert m.any()
+        # dilation happens at interior pixels only (csrc/rasterise_grad_egl.cu:155)
+        assert not (m[:, 0].any() or m[:, -1].any() or m[:, :, 0].any() or m[:, :, -1].any())
+    assert len(oracle.backward(s['vertices'], s['faces'], pixels, gp, return_dilation=True)[3]) == 2   # greedy [3, 1]
