@@ -64,6 +64,11 @@ def load(path):
     L.dirt_rasterise_backward.argtypes = [vp] * 8 + [i] * 6 + [ctypes.POINTER(ctypes.c_int), i, i, vp, sz, vp]
     L.dirt_rasterise_backward_ex.restype = i
     L.dirt_rasterise_backward_ex.argtypes = [vp] * 8 + [i] * 6 + [ctypes.POINTER(ctypes.c_int), i, i, i, vp, sz, vp]
+    L.dirt_rasterise_backward_deterministic_bytes.restype = sz
+    L.dirt_rasterise_backward_deterministic_bytes.argtypes = [i] * 6
+    L.dirt_rasterise_backward_deterministic.restype = i
+    L.dirt_rasterise_backward_deterministic.argtypes = ([vp] * 8 + [i] * 6 + [ctypes.POINTER(ctypes.c_int), i, i, i, vp, sz, vp, sz,
+                                                        vp])
     L.dirt_workspace_status.restype = i
     L.dirt_workspace_status.argtypes = [vp, sz] + [i] * 6 + [vp]
     L.dirt_rasterise_visibility.restype = i
@@ -102,7 +107,8 @@ EXPORTED_SYMBOLS = ['dirt_error_string', 'dirt_abi_version', 'dirt_workspace_byt
                     'dirt_kernel_timer_enable', 'dirt_kernel_timer_elapsed_ms', 'dirt_texture_sample',
                     'dirt_texture_sample_backward', 'dirt_lighting_workspace_bytes', 'dirt_lighting_forward',
                     'dirt_lighting_backward', 'dirt_normals_workspace_bytes', 'dirt_normals_forward',
-                    'dirt_normals_backward']
+                    'dirt_normals_backward', 'dirt_rasterise_backward_deterministic_bytes',
+                    'dirt_rasterise_backward_deterministic']
 
 
 def error_string(code):

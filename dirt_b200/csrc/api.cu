@@ -185,7 +185,8 @@ extern "C" int dirt_rasterise_visibility(const float* vertices, const int32_t* f
 static int backward_impl(const float* vertices, const int32_t* faces, const float* pixels, const float* grad_pixels,
                          const int32_t* face_ids, float* grad_background, float* grad_vertices, float* grad_vertex_colors,
                          int B, int H, int W, int C, int V, int F, const int* channel_groups, int n_groups,
-                         int workspace_holds_setup, int flags, void* workspace, size_t workspace_bytes, void* cuda_stream)
+                         int workspace_holds_setup, int flags, void* workspace, size_t workspace_bytes, void* cuda_stream,
+                         bool deterministic = false, void* scratch = nullptr, size_t scratch_bytes = 0)
 {
     int launches = 0;
     t_last_launches = 0;
@@ -206,6 +207,11 @@ static int backward_impl(const float* vertices, const int32_t* faces, const floa
         return DIRT_ERR_MISALIGNED;
     rc = check_workspace(workspace, workspace_bytes, B, H, W, C, V, F, face_ids == nullptr);
     if (rc != DIRT_OK) return rc;
+    if (deterministic) {
+        if (!scratch) return DIRT_ERR_NULL_POINTER;
+        if ((uintptr_t)scratch % 256 != 0) return DIRT_ERR_MISALIGNED;
+        if (scratch_bytes < dirt_rasterise_backward_deterministic_bytes(B, H, W, C, V, F)) return DIRT_ERR_WORKSPACE_TOO_SMALL;
+    }
     cudaStream_t stream = (cudaStream_t)cuda_stream;
     const Workspace ws = carve_workspace(workspace, B, H, W, C, V, F);
     const Dims d = make_dims(B, H, W, C, V, F);
@@ -224,8 +230,13 @@ static int backward_impl(const float* vertices, const int32_t* faces, const floa
         // a promise: checked on the device against the tag the setup pass left in the workspace
         expect_tag = workspace_tag(vertices, faces, B, H, W, V, F);
     }
-    CUDA_TRY(launch_backward(vertices, pixels, grad_pixels, ids, grad_background, grad_vertices, grad_vertex_colors, ws, d,
-                             groups, flags_valid, flags, expect_tag, stream, &launches));
+    if (deterministic)
+        CUDA_TRY(launch_backward_deterministic(vertices, faces, pixels, grad_pixels, ids, grad_background, grad_vertices,
+                                               grad_vertex_colors, ws, d, groups, flags, expect_tag,
+                                               carve_det_scratch(scratch, B, H, W, C, V, F), stream, &launches));
+    else
+        CUDA_TRY(launch_backward(vertices, pixels, grad_pixels, ids, grad_background, grad_vertices, grad_vertex_colors, ws, d,
+                                 groups, flags_valid, flags, expect_tag, stream, &launches));
     t_last_launches = launches;
     return DIRT_OK;
 }
@@ -248,6 +259,33 @@ extern "C" int dirt_rasterise_backward_ex(const float* vertices, const int32_t* 
 {
     return backward_impl(vertices, faces, pixels, grad_pixels, face_ids, grad_background, grad_vertices, grad_vertex_colors, B, H,
                          W, C, V, F, channel_groups, n_groups, workspace_holds_setup, flags, workspace, workspace_bytes, cuda_stream);
+}
+
+// the adjacency's corner ids b*3F + k*F + f are int32
+static bool deterministic_shape_ok(int B, int H, int W, int C, int V, int F)
+{
+    return shape_ok(B, H, W, C, V, F) && 3ll * B * F <= (1ll << 31) - 1;
+}
+
+extern "C" size_t dirt_rasterise_backward_deterministic_bytes(int B, int H, int W, int C, int V, int F)
+{
+    if (!shape_ok(B, H, W, C > 0 ? C : 1, V, F) || B == 0) return 0;
+    return carve_det_scratch(nullptr, B, H, W, C, V, F).bytes;
+}
+
+extern "C" int dirt_rasterise_backward_deterministic(const float* vertices, const int32_t* faces, const float* pixels,
+                                                     const float* grad_pixels, const int32_t* face_ids, float* grad_background,
+                                                     float* grad_vertices, float* grad_vertex_colors, int B, int H, int W,
+                                                     int C, int V, int F, const int* channel_groups, int n_groups,
+                                                     int workspace_holds_setup, int flags, void* workspace,
+                                                     size_t workspace_bytes, void* scratch, size_t scratch_bytes,
+                                                     void* cuda_stream)
+{
+    t_last_launches = 0;
+    if (!deterministic_shape_ok(B, H, W, C, V, F)) return DIRT_ERR_BAD_SHAPE;
+    return backward_impl(vertices, faces, pixels, grad_pixels, face_ids, grad_background, grad_vertices, grad_vertex_colors, B, H,
+                         W, C, V, F, channel_groups, n_groups, workspace_holds_setup, flags, workspace, workspace_bytes,
+                         cuda_stream, true, scratch, scratch_bytes);
 }
 
 // texel indices (and the warp keys built from them) stay below 2^62, element offsets of every buffer below 2^62

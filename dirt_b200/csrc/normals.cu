@@ -93,24 +93,29 @@ __device__ __forceinline__ Corners corners(const NormalsArgs& a, long long b, in
 
 // ---- the adjacency ----------------------------------------------------------------------------------------------------
 
-__global__ void __launch_bounds__(NORMALS_THREADS) count_kernel(const int* __restrict__ faces, int F, int V,
-                                                                int* __restrict__ counts)
+// The adjacency builder serves `items` face tables of F faces each, `face_stride` ints apart (0: one table shared by the
+// batch).  Row b*V + v holds the incidences of vertex v in table b, as ids b*3F + k*F + f.
+
+__global__ void __launch_bounds__(NORMALS_THREADS) count_kernel(const int* __restrict__ faces, long long face_stride, int items,
+                                                                int F, int V, int* __restrict__ counts)
 {
-    for (long long f = (long long)blockIdx.x * NORMALS_THREADS + threadIdx.x; f < F; f += (long long)gridDim.x * NORMALS_THREADS) {
+    const long long n = (long long)items * F;
+    for (long long t = (long long)blockIdx.x * NORMALS_THREADS + threadIdx.x; t < n; t += (long long)gridDim.x * NORMALS_THREADS) {
+        const long long b = t / F, f = t - b * F;
         int v[3];
-        if (!load_face(faces, f, V, v)) continue;
+        if (!load_face(faces + b * face_stride, f, V, v)) continue;
 #pragma unroll
-        for (int k = 0; k < 3; ++k) atomicAdd(counts + v[k], 1);
+        for (int k = 0; k < 3; ++k) atomicAdd(counts + b * V + v[k], 1);
     }
 }
 
-// offsets[v] = sum of counts[0 .. v), for v in [0, V]: one CTA, each thread scanning a contiguous chunk
-__global__ void __launch_bounds__(SCAN_THREADS) scan_kernel(const int* __restrict__ counts, int V, int* __restrict__ offsets)
+// offsets[r] = sum of counts[0 .. r), for r in [0, n]: one CTA, each thread scanning a contiguous chunk
+__global__ void __launch_bounds__(SCAN_THREADS) scan_kernel(const int* __restrict__ counts, long long n, int* __restrict__ offsets)
 {
     using Scan = cub::BlockScan<int, SCAN_THREADS>;
     __shared__ typename Scan::TempStorage tmp;
-    const long long chunk = ((long long)V + SCAN_THREADS - 1) / SCAN_THREADS;
-    const long long lo = threadIdx.x * chunk, hi = lo + chunk < V ? lo + chunk : V;
+    const long long chunk = (n + SCAN_THREADS - 1) / SCAN_THREADS;
+    const long long lo = threadIdx.x * chunk, hi = lo + chunk < n ? lo + chunk : n;
     int sum = 0;
     for (long long v = lo; v < hi; ++v) sum += counts[v];
     int run, total;
@@ -119,32 +124,38 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_kernel(const int* __restric
         offsets[v] = run;
         run += counts[v];
     }
-    if (threadIdx.x == 0) offsets[V] = total;
+    if (threadIdx.x == 0) offsets[n] = total;
 }
 
-// Drops every incidence id into its vertex's row, at a place the atomics choose; counts[v] runs back down to 0.
-__global__ void __launch_bounds__(NORMALS_THREADS) fill_kernel(const int* __restrict__ faces, int F, int V,
-                                                               const int* __restrict__ offsets, int* __restrict__ counts,
-                                                               int* __restrict__ unsorted)
+// Drops every incidence id into its vertex's row, at a place the atomics choose; counts[r] runs back down to 0.
+__global__ void __launch_bounds__(NORMALS_THREADS) fill_kernel(const int* __restrict__ faces, long long face_stride, int items,
+                                                               int F, int V, const int* __restrict__ offsets,
+                                                               int* __restrict__ counts, int* __restrict__ unsorted)
 {
-    for (long long f = (long long)blockIdx.x * NORMALS_THREADS + threadIdx.x; f < F; f += (long long)gridDim.x * NORMALS_THREADS) {
+    const long long n = (long long)items * F;
+    for (long long t = (long long)blockIdx.x * NORMALS_THREADS + threadIdx.x; t < n; t += (long long)gridDim.x * NORMALS_THREADS) {
+        const long long b = t / F, f = t - b * F;
         int v[3];
-        if (!load_face(faces, f, V, v)) continue;
+        if (!load_face(faces + b * face_stride, f, V, v)) continue;
 #pragma unroll
-        for (int k = 0; k < 3; ++k) unsorted[offsets[v[k]] + atomicSub(counts + v[k], 1) - 1] = k * F + (int)f;
+        for (int k = 0; k < 3; ++k) {
+            const long long r = b * V + v[k];
+            unsorted[offsets[r] + atomicSub(counts + r, 1) - 1] = (int)(b * 3 * F + k * F + f);
+        }
     }
 }
 
 // Moves every id to its rank among the ids of its row: the rows in ascending order.
-__global__ void __launch_bounds__(NORMALS_THREADS) rank_kernel(const int* __restrict__ faces, int F,
-                                                               const int* __restrict__ offsets,
+__global__ void __launch_bounds__(NORMALS_THREADS) rank_kernel(const int* __restrict__ faces, long long face_stride, int items,
+                                                               int F, const int* __restrict__ offsets,
                                                                const int* __restrict__ unsorted, int* __restrict__ inc,
                                                                int V)
 {
-    const long long n = offsets[V];
+    const long long n = offsets[(long long)items * V];
     for (long long p = (long long)blockIdx.x * NORMALS_THREADS + threadIdx.x; p < n; p += (long long)gridDim.x * NORMALS_THREADS) {
-        const int i = unsorted[p], k = i / F, v = __ldg(faces + 3ll * (i - k * F) + k);
-        const int lo = offsets[v], hi = offsets[v + 1];
+        const int i = unsorted[p], b = i / (3 * F), local = i - b * 3 * F, k = local / F;
+        const long long r = (long long)b * V + __ldg(faces + b * face_stride + 3ll * (local - k * F) + k);
+        const int lo = offsets[r], hi = offsets[r + 1];
         int rank = 0;
         for (int j = lo; j < hi; ++j) rank += unsorted[j] < i;
         inc[lo + rank] = i;
@@ -312,25 +323,34 @@ NormalsWorkspace carve_normals_workspace(void* base, int B, long long V, long lo
     return w;
 }
 
+cudaError_t launch_corner_adjacency(const int* faces, long long face_stride, int items, int V, int F, int* counts, int* offsets,
+                                    int* unsorted, int* inc, cudaStream_t stream, int* launches)
+{
+    cudaError_t e;
+    const long long rows = (long long)items * V, corners = 3ll * items * F;
+    if ((e = cudaMemsetAsync(counts, 0, sizeof(int) * (size_t)rows, stream)) != cudaSuccess) return e;
+    count_kernel<<<blocks_for(corners / 3), NORMALS_THREADS, 0, stream>>>(faces, face_stride, items, F, V, counts);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    ++*launches;
+    scan_kernel<<<1, SCAN_THREADS, 0, stream>>>(counts, rows, offsets);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    ++*launches;
+    fill_kernel<<<blocks_for(corners / 3), NORMALS_THREADS, 0, stream>>>(faces, face_stride, items, F, V, offsets, counts, unsorted);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    ++*launches;
+    rank_kernel<<<blocks_for(corners), NORMALS_THREADS, 0, stream>>>(faces, face_stride, items, F, offsets, unsorted, inc, V);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    ++*launches;
+    return cudaSuccess;
+}
+
 cudaError_t launch_normals_forward(NormalsArgs a, const NormalsWorkspace& w, cudaStream_t stream, int* launches)
 {
     cudaError_t e;
     if (a.total == 0) return cudaSuccess;
     if (a.F == 0) return cudaMemsetAsync(a.out, 0, sizeof(float) * 3 * (size_t)a.total, stream);
-    const int V = a.V, F = a.F;
-    if ((e = cudaMemsetAsync(w.counts, 0, sizeof(int) * (size_t)V, stream)) != cudaSuccess) return e;
-    count_kernel<<<blocks_for(F), NORMALS_THREADS, 0, stream>>>(a.faces, F, V, w.counts);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    ++*launches;
-    scan_kernel<<<1, SCAN_THREADS, 0, stream>>>(w.counts, V, w.offsets);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    ++*launches;
-    fill_kernel<<<blocks_for(F), NORMALS_THREADS, 0, stream>>>(a.faces, F, V, w.offsets, w.counts, w.unsorted);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    ++*launches;
-    rank_kernel<<<blocks_for(3ll * F), NORMALS_THREADS, 0, stream>>>(a.faces, F, w.offsets, w.unsorted, w.inc, V);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    ++*launches;
+    if ((e = launch_corner_adjacency(a.faces, 0, 1, a.V, a.F, w.counts, w.offsets, w.unsorted, w.inc, stream, launches)) != cudaSuccess)
+        return e;
     a.offsets = w.offsets;
     a.inc = w.inc;
     if (a.mode == DIRT_NORMALS_AVERAGE)

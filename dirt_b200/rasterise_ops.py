@@ -103,13 +103,16 @@ def _geometry_identity(vertices, faces, H, W):
 
 
 def rasterise_backward_raw(vertices, faces, pixels, grad_pixels, face_ids=None, channel_groups=None, setup_workspace=None,
-                           shared_geometry=False, want_position=True, want_colour=True):
+                           shared_geometry=False, want_position=True, want_colour=True, deterministic=None):
     """One call of dirt_rasterise_backward (the RasteriseGrad op, csrc/rasterise_grad_egl.cpp:33-53).
     `setup_workspace`: the workspace tensor of the forward call on the same (vertices, faces); its setup records are
     reused only if it still describes exactly these tensors (storage, version counters, sizes), otherwise they are
     recomputed.  `shared_geometry`: accumulate the vertex gradients over the batch (DIRT_BWD_SHARED_GEOMETRY):
     grad_vertices [V,4] and grad_vertex_colors [V,C] instead of [B,V,.].  want_position / want_colour = False skip
     the position terms (grad_vertices comes back zero) / the colour terms (grad_vertex_colors zero, grad_background None).
+    `deterministic`: run dirt_rasterise_backward_deterministic, whose outputs are bit-reproducible (float64 sums in a
+    fixed order, no float atomics); None follows torch.are_deterministic_algorithms_enabled().  Its scratch is allocated
+    per call.
     Returns (grad_background, grad_vertices, grad_vertex_colors)."""
     B, H, W, C = pixels.shape
     V, F = vertices.shape[1], faces.shape[1]
@@ -139,11 +142,22 @@ def rasterise_backward_raw(vertices, faces, pixels, grad_pixels, face_ids=None, 
     nbytes = int(ws.numel())
     flags = ((_lib.BWD_SHARED_GEOMETRY if shared_geometry else 0) | (0 if want_position else _lib.BWD_SKIP_POSITION) |
              (0 if want_colour else _lib.BWD_SKIP_COLOUR))
+    if deterministic is None:
+        deterministic = torch.are_deterministic_algorithms_enabled()
     with torch.cuda.device(device):
-        rc = _lib.lib().dirt_rasterise_backward_ex(
-            _ptr(vertices), _ptr(faces), _ptr(pixels), _ptr(grad_pixels), _ptr(face_ids),
-            _ptr(grad_background), _ptr(grad_vertices), _ptr(grad_vertex_colors),
-            B, H, W, C, V, F, groups_ptr, n_groups, reuse, flags, _ptr(ws), nbytes, _stream_ptr(device))
+        if deterministic:
+            scratch_bytes = max(int(_lib.lib().dirt_rasterise_backward_deterministic_bytes(B, H, W, C, V, F)), 256)
+            scratch = torch.empty(scratch_bytes, dtype=torch.uint8, device=device)
+            rc = _lib.lib().dirt_rasterise_backward_deterministic(
+                _ptr(vertices), _ptr(faces), _ptr(pixels), _ptr(grad_pixels), _ptr(face_ids),
+                _ptr(grad_background), _ptr(grad_vertices), _ptr(grad_vertex_colors),
+                B, H, W, C, V, F, groups_ptr, n_groups, reuse, flags, _ptr(ws), nbytes, _ptr(scratch), scratch_bytes,
+                _stream_ptr(device))
+        else:
+            rc = _lib.lib().dirt_rasterise_backward_ex(
+                _ptr(vertices), _ptr(faces), _ptr(pixels), _ptr(grad_pixels), _ptr(face_ids),
+                _ptr(grad_background), _ptr(grad_vertices), _ptr(grad_vertex_colors),
+                B, H, W, C, V, F, groups_ptr, n_groups, reuse, flags, _ptr(ws), nbytes, _stream_ptr(device))
     _lib.check(rc, 'RasteriseGrad')
     return grad_background, grad_vertices, grad_vertex_colors
 

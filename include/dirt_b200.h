@@ -124,6 +124,33 @@ int dirt_rasterise_backward_ex(const float* vertices, const int32_t* faces,
                                const int* channel_groups, int n_groups, int workspace_holds_setup, int flags,
                                void* workspace, size_t workspace_bytes, void* cuda_stream);
 
+/* dirt_rasterise_backward_ex with reproducible results (DESIGN.md §7.4): the same arguments, flags, channel groups and
+ * outputs, the same per-pixel terms and dilation decisions, but no float atomics.  Each vertex gradient is one float64
+ * sum in a fixed order (pixels of a face in raster order, then the face corners of the vertex in ascending id k*F + f,
+ * then the items in order under DIRT_BWD_SHARED_GEOMETRY), rounded once to fp32.  Two calls on the same inputs give
+ * bit-identical outputs.  An item's gradients do not depend on the other items of the batch, except where a 1-wide
+ * channel group's Scharr taps at the end of an image read the next image's first pixels in flat order (the reference's
+ * semantics, as in dirt_rasterise_backward_ex); with groups of width 3 only they never do.  Needs 3*B*F < 2^31.
+ *
+ * scratch: at least dirt_rasterise_backward_deterministic_bytes(B, H, W, C, V, F) bytes, 256-byte aligned, owned by the
+ * caller and separate from the workspace (which means what it means for dirt_rasterise_backward_ex).  Nothing in it needs
+ * to be initialised.  After the call it starts with the dilation codes: C planes of B*H*W bytes, plane g (g < the number
+ * of channel groups) holding group g's code per pixel, in [B][H][W] order:
+ *   bits 0-1  0: no position term, 1: the pixel's own face takes it, 2: the neighbour one step along the preferred
+ *             direction does (the dilation took it), 3: the neighbour one step against it does;
+ *   bit 2     the preferred step runs along the row (the Scharr x sum dominates); meaningful for codes 2 and 3.
+ * The step is +1 along the axis (column + 1, or the row above) on pixels whose col + row is even, -1 on odd ones.
+ * Returns 0 for B == 0; the size is a function of the shapes alone (SIZE_MAX if it does not fit a size_t). */
+size_t dirt_rasterise_backward_deterministic_bytes(int B, int H, int W, int C, int V, int F);
+int dirt_rasterise_backward_deterministic(const float* vertices, const int32_t* faces,
+                                          const float* pixels, const float* grad_pixels,
+                                          const int32_t* face_ids,
+                                          float* grad_background, float* grad_vertices, float* grad_vertex_colors,
+                                          int B, int H, int W, int C, int V, int F,
+                                          const int* channel_groups, int n_groups, int workspace_holds_setup, int flags,
+                                          void* workspace, size_t workspace_bytes, void* scratch, size_t scratch_bytes,
+                                          void* cuda_stream);
+
 /* Waits for the stream and reports whether a backward call found the workspace not to hold the setup records it was
  * promised (DIRT_ERR_STALE_WORKSPACE), else DIRT_OK.  The only entry point that synchronises the host. */
 int dirt_workspace_status(const void* workspace, size_t workspace_bytes,
