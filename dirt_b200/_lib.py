@@ -84,6 +84,10 @@ def load(path):
     L.dirt_texture_sample.argtypes = [vp] * 3 + [i] * 5 + [ctypes.c_longlong, i, vp]
     L.dirt_texture_sample_backward.restype = i
     L.dirt_texture_sample_backward.argtypes = [vp] * 5 + [i] * 5 + [ctypes.c_longlong, i, vp]
+    L.dirt_texture_sample_backward_deterministic_bytes.restype = sz
+    L.dirt_texture_sample_backward_deterministic_bytes.argtypes = [i] * 5 + [ctypes.c_longlong, i]
+    L.dirt_texture_sample_backward_deterministic.restype = i
+    L.dirt_texture_sample_backward_deterministic.argtypes = [vp] * 5 + [i] * 5 + [ctypes.c_longlong, i, vp, sz, vp]
     ll = ctypes.c_longlong
     light_inputs = [i, i, vp, ll, vp, ll, vp, ll] + [vp, i] * 4
     L.dirt_lighting_workspace_bytes.restype = sz
@@ -108,7 +112,8 @@ EXPORTED_SYMBOLS = ['dirt_error_string', 'dirt_abi_version', 'dirt_workspace_byt
                     'dirt_texture_sample_backward', 'dirt_lighting_workspace_bytes', 'dirt_lighting_forward',
                     'dirt_lighting_backward', 'dirt_normals_workspace_bytes', 'dirt_normals_forward',
                     'dirt_normals_backward', 'dirt_rasterise_backward_deterministic_bytes',
-                    'dirt_rasterise_backward_deterministic']
+                    'dirt_rasterise_backward_deterministic', 'dirt_texture_sample_backward_deterministic_bytes',
+                    'dirt_texture_sample_backward_deterministic']
 
 
 def error_string(code):

@@ -344,6 +344,50 @@ extern "C" int dirt_texture_sample_backward(const float* texture, const float* i
     return DIRT_OK;
 }
 
+// the deterministic path's lookup ids and sort keys (texel ids plus one sentinel) are 32-bit
+static bool texture_det_shape_ok(int TB, int TH, int TW, int C, int B, long long N, int mode)
+{
+    return texture_shape_ok(TB, TH, TW, C, B, N, mode) && (long long)B * N < (1ll << 31) &&
+           (long long)TB * TH * TW < (1ll << 31) - 1;
+}
+
+extern "C" size_t dirt_texture_sample_backward_deterministic_bytes(int TB, int TH, int TW, int C, int B, long long N, int mode)
+{
+    if (!texture_det_shape_ok(TB, TH, TW, C, B, N, mode) || (long long)B * N == 0) return 0;
+    return carve_texture_det_scratch(nullptr, make_tex_dims(TB, TH, TW, C, B, N, mode)).bytes;
+}
+
+extern "C" int dirt_texture_sample_backward_deterministic(const float* texture, const float* indices, const float* grad_out,
+                                                          float* grad_texture, float* grad_indices, int TB, int TH, int TW,
+                                                          int C, int B, long long N, int mode, void* scratch,
+                                                          size_t scratch_bytes, void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (!texture_det_shape_ok(TB, TH, TW, C, B, N, mode)) return DIRT_ERR_BAD_SHAPE;
+    const TexDims d = make_tex_dims(TB, TH, TW, C, B, N, mode);
+    if (d.total > 0) {
+        if (!indices || !grad_out) return DIRT_ERR_NULL_POINTER;
+        if (grad_indices && mode == DIRT_TEXTURE_BILINEAR && !texture) return DIRT_ERR_NULL_POINTER;
+    }
+    if ((uintptr_t)texture % 4 || (uintptr_t)indices % 4 || (uintptr_t)grad_out % 4 || (uintptr_t)grad_texture % 4 ||
+        (uintptr_t)grad_indices % 4)
+        return DIRT_ERR_MISALIGNED;
+    // only the texture gradient of a call with lookups sorts them
+    const bool sorts = grad_texture && d.total > 0;
+    if (sorts) {
+        if (!scratch) return DIRT_ERR_NULL_POINTER;
+        if ((uintptr_t)scratch % 256) return DIRT_ERR_MISALIGNED;
+        if (scratch_bytes < dirt_texture_sample_backward_deterministic_bytes(TB, TH, TW, C, B, N, mode))
+            return DIRT_ERR_WORKSPACE_TOO_SMALL;
+    }
+    CUDA_TRY(launch_texture_backward_deterministic(texture, indices, grad_out, grad_texture, grad_indices, d,
+                                                   carve_texture_det_scratch(sorts ? scratch : nullptr, d),
+                                                   (cudaStream_t)cuda_stream, &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
 // element offsets of every per-point buffer stay below 2^62, the chunk count within the grid's x limit
 static bool lighting_shape_ok(int model, int B, long long V, int C, long long sn, long long sp, long long sc)
 {

@@ -8,6 +8,8 @@
 // Backward: one thread per lookup.  grad_indices comes from the same four texels.  grad_texture is aggregated inside the
 // warp before it touches global memory: lanes that hit the same texel (MATCH.ANY on its linear index) sum their
 // contributions and the lowest of them issues one reduction (a vector RED for C = 2 / 4).
+// Deterministic backward (dirt_texture_sample_backward_deterministic): a radix sort of the lookups by base texel, then
+// fixed-order float64 sums per texel; see the section below and DESIGN.md §7.5.
 #include "../../include/dirt_b200.h"
 #include "common.cuh"
 
@@ -396,7 +398,422 @@ cudaError_t backward_ct(const float* texture, const float* indices, const float*
     return cudaGetLastError();
 }
 
+// ---- deterministic backward (DESIGN.md §7.5) ------------------------------------------------------------------------
+//
+// grad_texture with no float atomics: each (texel, channel) is one float64 sum in a fixed order, rounded once to fp32.
+//  (1) A stable LSD radix sort of (key, id) over the lookups, 8 bits per pass and only as many passes as the largest key
+//      needs.  A valid lookup's key is its base texel tb*TH*TW + r0*TW + c0, an invalid one's the sentinel TB*TH*TW; the
+//      ids are the lookup ids g = b*N + n.  The first pass computes the keys from the indices (taps_of) and takes the
+//      ids from the positions.  Per pass: a histogram per tile of RS_TILE lookups, an exclusive scan of each digit's
+//      row of the [digit][tile] count matrix (one CTA per digit), and a scatter in which a lookup's rank in its tile
+//      comes from MATCH.ANY on the digit and the warps' digit counts taken in warp order.  The output is unique.
+//  (2) offsets[k] = the first sorted position whose key is >= k, k = 0 .. sentinel + 1, by binary search: the lookups
+//      whose base is texel x are the segment [offsets[x], offsets[x + 1]).
+//  (3) Texel x = (tb, r, c) receives the terms of four segments, in this order: corner 00 of base (r, c), corner 01 of
+//      base (r, c-1), corner 10 of base (r-1, c), corner 11 of base (r-1, c-1), modulo the texture (nearest: corner 00
+//      only).  A term is the fp32 product grad_out[g][ch] * w of the default kernel, w the corner's bilinear weight (a
+//      zero weight gives +0.0), widened to float64.  The sequence's L terms are cut into chunks of DET_CHUNK; in chunk q
+//      lane t of a warp sums the terms q*DET_CHUNK + t, + t + 32, ... in order from +0.0, the lanes meet in the xor
+//      butterfly 16, 8, 4, 2, 1, and the chunk sums are added in chunk order from +0.0.  The tree depends on L alone.
+//      A texel of at most DET_CHUNK terms is summed by one warp; a longer one is listed, each of its chunks is summed by
+//      a warp of its own into the scratch, and one thread per (texel, channel) adds its chunks.
+constexpr int RS_THREADS = 256;             // sort CTA: one thread per digit value
+constexpr int RS_RADIX = 256;
+constexpr int RS_WARPS = RS_THREADS / 32;
+constexpr int RS_TILE = 4096;               // lookups per sort tile, 16 per thread
+constexpr long long DET_CHUNK = 4096;       // terms per chunk of a texel's sum
+constexpr unsigned DET_GRID = 8192;         // CTAs of the grid-stride passes
+
+__device__ __forceinline__ unsigned lookup_key(const float* indices, const TexDims& d, long long g, unsigned sentinel)
+{
+    const Taps t = taps_of(__ldg(indices + 2 * g), __ldg(indices + 2 * g + 1), d, g);
+    return t.valid ? (unsigned)(t.base + (long long)t.r0 * d.TW + t.c0) : sentinel;
+}
+
+// Exclusive scan of one value per thread over the RS_THREADS threads of the CTA; *total gets the sum.  Contains
+// __syncthreads(); warp_sums is RS_WARPS words of shared memory.
+__device__ __forceinline__ unsigned block_exclusive_scan(unsigned v, unsigned* warp_sums, unsigned* total)
+{
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    unsigned x = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const unsigned y = __shfl_up_sync(FULL, x, o);
+        if (lane >= o) x += y;
+    }
+    if (lane == 31) warp_sums[warp] = x;
+    __syncthreads();
+    unsigned before = 0, all = 0;
+#pragma unroll
+    for (int w = 0; w < RS_WARPS; ++w) {
+        const unsigned s = warp_sums[w];
+        before += w < warp ? s : 0u;
+        all += s;
+    }
+    __syncthreads();
+    *total = all;
+    return before + x - v;
+}
+
+// counts[digit][tile]: how many lookups of the tile have the digit (key >> shift) & 255
+template <bool FIRST>
+__global__ void __launch_bounds__(RS_THREADS) tex_sort_hist_kernel(const unsigned* __restrict__ keys,
+                                                                   const float* __restrict__ indices, TexDims d,
+                                                                   unsigned sentinel, int shift,
+                                                                   unsigned* __restrict__ counts, int tiles)
+{
+    __shared__ unsigned hist[RS_RADIX];
+    hist[threadIdx.x] = 0;
+    __syncthreads();
+    const long long first = (long long)blockIdx.x * RS_TILE;
+    for (int j = 0; j < RS_TILE / RS_THREADS; ++j) {
+        const long long i = first + j * RS_THREADS + threadIdx.x;
+        if (i < d.total) {
+            const unsigned key = FIRST ? lookup_key(indices, d, i, sentinel) : __ldg(keys + i);
+            atomicAdd(&hist[(key >> shift) & 255u], 1u);
+        }
+    }
+    __syncthreads();
+    counts[(size_t)threadIdx.x * tiles + blockIdx.x] = hist[threadIdx.x];
+}
+
+// one CTA per digit: its row of tile counts becomes the exclusive prefix, in place; the row's sum goes to digit_total
+__global__ void __launch_bounds__(RS_THREADS) tex_sort_scan_kernel(unsigned* __restrict__ counts,
+                                                                   unsigned* __restrict__ digit_total, int tiles)
+{
+    __shared__ unsigned warp_sums[RS_WARPS];
+    unsigned* row = counts + (size_t)blockIdx.x * tiles;
+    unsigned carry = 0;
+    for (int base = 0; base < tiles; base += RS_THREADS) {
+        const int i = base + threadIdx.x;
+        const unsigned v = i < tiles ? row[i] : 0u;
+        unsigned total;
+        const unsigned ex = block_exclusive_scan(v, warp_sums, &total);
+        if (i < tiles) row[i] = carry + ex;
+        carry += total;
+    }
+    if (threadIdx.x == 0) digit_total[blockIdx.x] = carry;
+}
+
+// Stable scatter of one tile.  Its lookups go in 16 rounds of RS_THREADS consecutive ones; in a round a lookup's slot is
+// the tile's running slot of its digit, plus the lookups of the lower warps with that digit, plus its rank among its
+// warp's lanes with that digit.  Thread dgt keeps the running slot of digit dgt.
+template <bool FIRST>
+__global__ void __launch_bounds__(RS_THREADS) tex_sort_scatter_kernel(const unsigned* __restrict__ keys_in,
+                                                                      const int* __restrict__ ids_in,
+                                                                      const float* __restrict__ indices, TexDims d,
+                                                                      unsigned sentinel, int shift,
+                                                                      const unsigned* __restrict__ counts,
+                                                                      const unsigned* __restrict__ digit_total, int tiles,
+                                                                      unsigned* __restrict__ keys_out,
+                                                                      int* __restrict__ ids_out)
+{
+    __shared__ unsigned warp_sums[RS_WARPS];
+    __shared__ unsigned wcount[RS_WARPS][RS_RADIX];
+    __shared__ unsigned woff[RS_WARPS][RS_RADIX];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, dgt = threadIdx.x;
+    unsigned all;
+    // the lookups of the smaller digits, then those of digit dgt in the earlier tiles
+    unsigned run = block_exclusive_scan(digit_total[dgt], warp_sums, &all) + counts[(size_t)dgt * tiles + blockIdx.x];
+#pragma unroll
+    for (int w = 0; w < RS_WARPS; ++w) wcount[w][dgt] = 0;
+    __syncthreads();
+    const long long first = (long long)blockIdx.x * RS_TILE;
+    for (int j = 0; j < RS_TILE / RS_THREADS; ++j) {
+        const long long i = first + j * RS_THREADS + threadIdx.x;
+        const bool live = i < d.total;
+        unsigned key = 0;
+        int id = 0;
+        if (live) {
+            key = FIRST ? lookup_key(indices, d, i, sentinel) : __ldg(keys_in + i);
+            id = FIRST ? (int)i : __ldg(ids_in + i);
+        }
+        const unsigned digit = live ? (key >> shift) & 255u : (unsigned)RS_RADIX;
+        const unsigned peers = __match_any_sync(FULL, digit);
+        const unsigned rank = __popc(peers & ((1u << lane) - 1u));
+        if (live && rank == 0) wcount[warp][digit] = __popc(peers);
+        __syncthreads();
+#pragma unroll
+        for (int w = 0; w < RS_WARPS; ++w) {
+            woff[w][dgt] = run;
+            run += wcount[w][dgt];
+            wcount[w][dgt] = 0;
+        }
+        __syncthreads();
+        if (live) {
+            const unsigned pos = woff[warp][digit] + rank;
+            keys_out[pos] = key;
+            ids_out[pos] = id;
+        }
+    }
+}
+
+// offsets[k] = the first position of the sorted keys that is >= k, k = 0 .. sentinel + 1
+__global__ void __launch_bounds__(TEX_THREADS) tex_segment_bounds_kernel(const unsigned* __restrict__ keys, long long n,
+                                                                         unsigned sentinel, int* __restrict__ offsets)
+{
+    const long long stride = (long long)gridDim.x * TEX_THREADS;
+    for (long long k = (long long)blockIdx.x * TEX_THREADS + threadIdx.x; k <= (long long)sentinel + 1; k += stride) {
+        long long lo = 0, hi = n;
+        while (lo < hi) {
+            const long long mid = (lo + hi) >> 1;
+            if (__ldg(keys + mid) < (unsigned)k) lo = mid + 1;
+            else hi = mid;
+        }
+        offsets[k] = (int)lo;
+    }
+}
+
+// The term sequence of one texel: segment k (corner k) starts at sorted position s_k and holds terms [e_k, e_{k+1}) of
+// the sequence (e_0 = 0, e_4 = L).  Scalars, not arrays, so that nothing is indexed dynamically.
+struct TexSeq {
+    int s0, s1, s2, s3;
+    long long e1, e2, e3, L;
+};
+
+__device__ __forceinline__ TexSeq texel_sequence(const int* __restrict__ offsets, const TexDims& d, int x)
+{
+    const long long tb = x / d.texels, rc = x - tb * d.texels;
+    const int r = (int)(rc / d.TW), c = (int)(rc - (long long)r * d.TW);
+    const int rm = r == 0 ? d.TH - 1 : r - 1, cm = c == 0 ? d.TW - 1 : c - 1;
+    const long long t0 = tb * d.texels;
+    TexSeq q;
+    const long long k0 = t0 + (long long)r * d.TW + c;
+    q.s0 = __ldg(offsets + k0);
+    q.e1 = __ldg(offsets + k0 + 1) - q.s0;
+    if (d.mode == DIRT_TEXTURE_NEAREST) {
+        q.s1 = q.s2 = q.s3 = 0;
+        q.e2 = q.e3 = q.L = q.e1;
+        return q;
+    }
+    const long long k1 = t0 + (long long)r * d.TW + cm, k2 = t0 + (long long)rm * d.TW + c, k3 = t0 + (long long)rm * d.TW + cm;
+    q.s1 = __ldg(offsets + k1);
+    q.e2 = q.e1 + (__ldg(offsets + k1 + 1) - q.s1);
+    q.s2 = __ldg(offsets + k2);
+    q.e3 = q.e2 + (__ldg(offsets + k2 + 1) - q.s2);
+    q.s3 = __ldg(offsets + k3);
+    q.L = q.e3 + (__ldg(offsets + k3 + 1) - q.s3);
+    return q;
+}
+
+// Lane `lane`'s sums of terms i0 + lane, i0 + lane + 32, ... < i1 of the sequence, channels c0 .. c0 + NV - 1, then
+// the warp's xor butterfly: every lane returns the chunk's sums.  Warp-uniform.
+template <int NV>
+__device__ __forceinline__ void chunk_sums(const TexSeq& q, long long i0, long long i1, int c0, const int* __restrict__ ids,
+                                           const float* __restrict__ indices, const float* __restrict__ grad_out,
+                                           const TexDims& d, int C, double acc[NV])
+{
+    const int lane = threadIdx.x & 31;
+#pragma unroll
+    for (int j = 0; j < NV; ++j) acc[j] = 0.0;
+    for (long long i = i0 + lane; i < i1; i += 32) {
+        const int k = i < q.e1 ? 0 : i < q.e2 ? 1 : i < q.e3 ? 2 : 3;
+        const long long pos = k == 0 ? q.s0 + i : k == 1 ? q.s1 + (i - q.e1) : k == 2 ? q.s2 + (i - q.e2) : q.s3 + (i - q.e3);
+        const long long g = __ldg(ids + pos);
+        const Taps t = taps_of(__ldg(indices + 2 * g), __ldg(indices + 2 * g + 1), d, g);
+        const float w = __fmul_rn((k & 1) ? t.fc : __fsub_rn(1.0f, t.fc), (k & 2) ? t.fr : __fsub_rn(1.0f, t.fr));
+        const float* go = grad_out + g * C + c0;
+#pragma unroll
+        for (int j = 0; j < NV; ++j) acc[j] = __dadd_rn(acc[j], w != 0.f ? (double)__fmul_rn(__ldg(go + j), w) : 0.0);
+    }
+#pragma unroll
+    for (int j = 0; j < NV; ++j)
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) acc[j] = __dadd_rn(acc[j], __shfl_xor_sync(FULL, acc[j], o));
+}
+
+struct TexDetArgs {
+    const float *indices, *grad_out;
+    const int *ids, *offsets;
+    float* grad_texture;
+    int* counters;        // [0] chunk slots taken, [1] long texels listed
+    int4* long_list;      // (texel, first slot, chunks)
+    int2* owner;          // per slot: (texel, chunk)
+    double* partial;      // per slot: C chunk sums
+    TexDims d;
+};
+
+// One warp per texel (CT = C in 1..4, or 0: any C, one channel at a time): a texel of at most DET_CHUNK terms is summed
+// and written; a longer one takes slots for its chunks and is listed.
+// (__maxnreg__ instead of __launch_bounds__: under the latter ptxas keeps the CT = 0 instance at 32 registers and spills)
+template <int CT>
+__global__ void __maxnreg__(64) tex_det_gather_kernel(TexDetArgs a)
+{
+    constexpr int NV = CT ? CT : 1;
+    const int C = CT ? CT : a.d.C;
+    const int lane = threadIdx.x & 31;
+    const long long texels = (long long)a.d.TB * a.d.texels, warps = (long long)gridDim.x * (TEX_THREADS / 32);
+    for (long long x = (long long)blockIdx.x * (TEX_THREADS / 32) + (threadIdx.x >> 5); x < texels; x += warps) {
+        const TexSeq q = texel_sequence(a.offsets, a.d, (int)x);
+        if (q.L > DET_CHUNK) {
+            const int n = (int)((q.L + DET_CHUNK - 1) / DET_CHUNK);
+            int slot = 0;
+            if (lane == 0) {
+                slot = atomicAdd(a.counters, n);
+                a.long_list[atomicAdd(a.counters + 1, 1)] = make_int4((int)x, slot, n, 0);
+            }
+            slot = __shfl_sync(FULL, slot, 0);
+            for (int c = lane; c < n; c += 32) a.owner[slot + c] = make_int2((int)x, c);
+            continue;
+        }
+#pragma unroll 1
+        for (int c0 = 0; c0 < C; c0 += NV) {
+            double acc[NV];
+            chunk_sums<NV>(q, 0, q.L, c0, a.ids, a.indices, a.grad_out, a.d, C, acc);
+            if (lane == 0)
+#pragma unroll
+                for (int j = 0; j < NV; ++j) a.grad_texture[x * C + c0 + j] = __double2float_rn(__dadd_rn(0.0, acc[j]));
+        }
+    }
+}
+
+// one warp per chunk of a listed texel: its sums go to the chunk's slot
+template <int CT>
+__global__ void __launch_bounds__(TEX_THREADS) tex_det_chunk_kernel(TexDetArgs a)
+{
+    constexpr int NV = CT ? CT : 1;
+    const int C = CT ? CT : a.d.C;
+    const int lane = threadIdx.x & 31, slots = a.counters[0];
+    const int warps = gridDim.x * (TEX_THREADS / 32);
+    for (int s = blockIdx.x * (TEX_THREADS / 32) + (threadIdx.x >> 5); s < slots; s += warps) {
+        const int2 o = a.owner[s];
+        const TexSeq q = texel_sequence(a.offsets, a.d, o.x);
+        const long long i0 = o.y * DET_CHUNK, i1 = i0 + DET_CHUNK < q.L ? i0 + DET_CHUNK : q.L;
+        for (int c0 = 0; c0 < C; c0 += NV) {
+            double acc[NV];
+            chunk_sums<NV>(q, i0, i1, c0, a.ids, a.indices, a.grad_out, a.d, C, acc);
+            if (lane == 0)
+#pragma unroll
+                for (int j = 0; j < NV; ++j) a.partial[(size_t)s * C + c0 + j] = acc[j];
+        }
+    }
+}
+
+// one thread per (listed texel, channel): the chunk sums in chunk order
+__global__ void __launch_bounds__(TEX_THREADS) tex_det_finish_kernel(TexDetArgs a)
+{
+    const int C = a.d.C;
+    const long long n = (long long)a.counters[1] * C, stride = (long long)gridDim.x * TEX_THREADS;
+    for (long long e = (long long)blockIdx.x * TEX_THREADS + threadIdx.x; e < n; e += stride) {
+        const int j = (int)(e / C), ch = (int)(e - (long long)j * C);
+        const int4 t = a.long_list[j];
+        double s = 0.0;
+        for (int c = 0; c < t.z; ++c) s = __dadd_rn(s, a.partial[(size_t)(t.y + c) * C + ch]);
+        a.grad_texture[(long long)t.x * C + ch] = __double2float_rn(s);
+    }
+}
+
+template <int CT>
+cudaError_t det_gather_ct(const TexDetArgs& a, unsigned gather_blocks, unsigned chunk_blocks, cudaStream_t stream)
+{
+    tex_det_gather_kernel<CT><<<gather_blocks, TEX_THREADS, 0, stream>>>(a);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+    tex_det_chunk_kernel<CT><<<chunk_blocks, TEX_THREADS, 0, stream>>>(a);
+    return cudaGetLastError();
+}
+
+inline unsigned det_blocks(long long work, long long per_block)
+{
+    const long long b = (work + per_block - 1) / per_block;
+    return (unsigned)(b < 1 ? 1 : (b < DET_GRID ? b : DET_GRID));
+}
+
+// sort passes: one per 8 bits of the largest key, the sentinel
+inline int sort_passes(unsigned sentinel)
+{
+    int bits = 0;
+    while (bits < 32 && (sentinel >> bits) != 0) ++bits;
+    return (bits + 7) / 8;
+}
+
 }  // namespace
+
+TexDetScratch carve_texture_det_scratch(void* base, const TexDims& d)
+{
+    TexDetScratch s = {};
+    char* p = static_cast<char*>(base);
+    size_t off = 0;
+    auto take = [&](size_t bytes) {
+        char* r = p ? p + off : nullptr;
+        off = align_up(off + bytes, 256);
+        return r;
+    };
+    const size_t n = (size_t)d.total, texels = (size_t)d.TB * d.texels;
+    const size_t tiles = (n + RS_TILE - 1) / RS_TILE;
+    // a listed texel has more than DET_CHUNK terms, and there are n terms per corner
+    const size_t terms = n * (d.mode == DIRT_TEXTURE_BILINEAR ? 4 : 1);
+    const size_t max_long = terms / (DET_CHUNK + 1), max_slots = (terms + DET_CHUNK - 1) / DET_CHUNK + max_long;
+    for (int k = 0; k < 2; ++k) s.keys[k] = reinterpret_cast<unsigned*>(take(n * sizeof(unsigned)));
+    for (int k = 0; k < 2; ++k) s.ids[k] = reinterpret_cast<int*>(take(n * sizeof(int)));
+    s.offsets = reinterpret_cast<int*>(take((texels + 2) * sizeof(int)));
+    s.counts = reinterpret_cast<unsigned*>(take((size_t)RS_RADIX * tiles * sizeof(unsigned)));
+    s.digit_total = reinterpret_cast<unsigned*>(take(RS_RADIX * sizeof(unsigned)));
+    s.counters = reinterpret_cast<int*>(take(2 * sizeof(int)));
+    s.long_list = reinterpret_cast<int4*>(take(max_long * sizeof(int4)));
+    s.owner = reinterpret_cast<int2*>(take(max_slots * sizeof(int2)));
+    s.partial = reinterpret_cast<double*>(take(max_slots * d.C * sizeof(double)));
+    s.bytes = off;
+    return s;
+}
+
+cudaError_t launch_texture_backward_deterministic(const float* texture, const float* indices, const float* grad_out,
+                                                  float* grad_texture, float* grad_indices, const TexDims& d,
+                                                  const TexDetScratch& s, cudaStream_t stream, int* launches)
+{
+    // grad_indices is per lookup and has no atomics: the default kernel writes it
+    if (!grad_texture || d.total == 0) return launch_texture_backward(texture, indices, grad_out, grad_texture, grad_indices, d,
+                                                                      stream, launches);
+    cudaError_t e;
+    if (grad_indices && (e = launch_texture_backward(texture, indices, grad_out, nullptr, grad_indices, d, stream, launches)) !=
+                            cudaSuccess)
+        return e;
+    if ((e = cudaMemsetAsync(s.counters, 0, 2 * sizeof(int), stream)) != cudaSuccess) return e;
+    const unsigned sentinel = (unsigned)(d.TB * d.texels);
+    const int tiles = (int)((d.total + RS_TILE - 1) / RS_TILE), passes = sort_passes(sentinel);
+    for (int p = 0; p < passes; ++p) {
+        const unsigned* kin = s.keys[(p + 1) & 1];
+        const int* iin = s.ids[(p + 1) & 1];
+        unsigned* kout = s.keys[p & 1];
+        int* iout = s.ids[p & 1];
+        if (p == 0) tex_sort_hist_kernel<true><<<tiles, RS_THREADS, 0, stream>>>(kin, indices, d, sentinel, 0, s.counts, tiles);
+        else tex_sort_hist_kernel<false><<<tiles, RS_THREADS, 0, stream>>>(kin, indices, d, sentinel, 8 * p, s.counts, tiles);
+        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+        tex_sort_scan_kernel<<<RS_RADIX, RS_THREADS, 0, stream>>>(s.counts, s.digit_total, tiles);
+        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+        if (p == 0)
+            tex_sort_scatter_kernel<true><<<tiles, RS_THREADS, 0, stream>>>(kin, iin, indices, d, sentinel, 0, s.counts,
+                                                                             s.digit_total, tiles, kout, iout);
+        else
+            tex_sort_scatter_kernel<false><<<tiles, RS_THREADS, 0, stream>>>(kin, iin, indices, d, sentinel, 8 * p, s.counts,
+                                                                              s.digit_total, tiles, kout, iout);
+        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+        *launches += 3;
+    }
+    const unsigned* keys = s.keys[(passes - 1) & 1];
+    tex_segment_bounds_kernel<<<det_blocks((long long)sentinel + 2, TEX_THREADS), TEX_THREADS, 0, stream>>>(keys, d.total,
+                                                                                                           sentinel, s.offsets);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    TexDetArgs a;
+    a.indices = indices; a.grad_out = grad_out; a.ids = s.ids[(passes - 1) & 1]; a.offsets = s.offsets;
+    a.grad_texture = grad_texture; a.counters = s.counters; a.long_list = s.long_list; a.owner = s.owner;
+    a.partial = s.partial; a.d = d;
+    const unsigned gather_blocks = det_blocks(sentinel, TEX_THREADS / 32);
+    const long long terms = d.total * (d.mode == DIRT_TEXTURE_BILINEAR ? 4 : 1);
+    const unsigned chunk_blocks = det_blocks(2 * ((terms + DET_CHUNK - 1) / DET_CHUNK), TEX_THREADS / 32);
+    switch (d.C) {
+        case 1: e = det_gather_ct<1>(a, gather_blocks, chunk_blocks, stream); break;
+        case 2: e = det_gather_ct<2>(a, gather_blocks, chunk_blocks, stream); break;
+        case 3: e = det_gather_ct<3>(a, gather_blocks, chunk_blocks, stream); break;
+        case 4: e = det_gather_ct<4>(a, gather_blocks, chunk_blocks, stream); break;
+        default: e = det_gather_ct<0>(a, gather_blocks, chunk_blocks, stream);
+    }
+    if (e != cudaSuccess) return e;
+    tex_det_finish_kernel<<<det_blocks((terms / (DET_CHUNK + 1) + 1) * d.C, TEX_THREADS), TEX_THREADS, 0, stream>>>(a);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    *launches += 4;
+    return cudaSuccess;
+}
 
 cudaError_t launch_texture_forward(const float* texture, const float* indices, float* out, const TexDims& d,
                                    cudaStream_t stream, int* launches)

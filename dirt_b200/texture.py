@@ -57,10 +57,26 @@ class _SampleTexture(torch.autograd.Function):
         grad_out = grad_out.contiguous().to(torch.float32)
         grad_texture = torch.empty_like(texture) if want_texture else None
         grad_indices = torch.empty_like(indices) if want_indices else None
+        # grad_indices alone is per lookup and already reproducible; grad_texture needs the sorted path
+        deterministic = want_texture and torch.are_deterministic_algorithms_enabled()
         with torch.cuda.device(indices.device):
-            rc = _lib.lib().dirt_texture_sample_backward(_ptr(texture), _ptr(indices), _ptr(grad_out), _ptr(grad_texture),
-                                                         _ptr(grad_indices), TB, TH, TW, C, B, N, ctx.mode,
-                                                         _stream_ptr(indices.device))
+            if deterministic:
+                L = _lib.lib()
+                scratch_bytes = max(int(L.dirt_texture_sample_backward_deterministic_bytes(TB, TH, TW, C, B, N, ctx.mode)), 256)
+                scratch = torch.empty(scratch_bytes, dtype=torch.uint8, device=indices.device)
+                rc = L.dirt_texture_sample_backward_deterministic(
+                    _ptr(texture), _ptr(indices), _ptr(grad_out), _ptr(grad_texture), _ptr(grad_indices), TB, TH, TW, C, B, N,
+                    ctx.mode, _ptr(scratch), scratch_bytes, _stream_ptr(indices.device))
+                if rc == _lib.ERR_BAD_SHAPE:
+                    # the shapes passed the forward call: what fails are the sorted path's 32-bit limits
+                    raise RuntimeError(
+                        'sample_texture backward: the texture gradient has no deterministic implementation for %d lookups '
+                        'into %d x %d x %d texels (it needs fewer than 2^31 of each), but '
+                        'torch.use_deterministic_algorithms(True) is set' % (B * N, TB, TH, TW))
+            else:
+                rc = _lib.lib().dirt_texture_sample_backward(_ptr(texture), _ptr(indices), _ptr(grad_out),
+                                                             _ptr(grad_texture), _ptr(grad_indices), TB, TH, TW, C, B, N,
+                                                             ctx.mode, _stream_ptr(indices.device))
         _lib.check(rc, 'SampleTextureGrad')
         return grad_texture, grad_indices, None, None
 

@@ -205,6 +205,27 @@ int dirt_texture_sample_backward(const float* texture, const float* indices, con
                                  float* grad_texture, float* grad_indices,
                                  int TB, int TH, int TW, int C, int B, long long N, int mode, void* cuda_stream);
 
+/* dirt_texture_sample_backward with a reproducible grad_texture (DESIGN.md §7.5): the same arguments, NULL and alignment
+ * rules and outputs; grad_indices is the same, bit for bit.  grad_texture has no float atomics: each (texel, channel) is
+ * one float64 sum, rounded once to fp32, of the terms grad_out[g][ch] * w (the fp32 product, w the corner's bilinear
+ * weight, 1 for nearest; a zero weight adds +0.0; a lookup with a non-finite index adds nothing).  Texel (r, c) of
+ * texture tb takes, in this order, the corner-00 terms of the lookups whose base texel (r0, c0) is (r, c), the corner-01
+ * terms of those based at (r, c-1), corner 10 from (r-1, c) and corner 11 from (r-1, c-1), modulo the texture size
+ * (nearest: the one texel read); within a corner, the lookups go in ascending id g = b*N + n.  The L terms of that
+ * sequence are cut into chunks of 4096: in each, lane t of 32 sums the terms t, t + 32, ... of the chunk in order from
+ * +0.0, the 32 sums meet in the xor butterfly over lane offsets 16, 8, 4, 2, 1, and the chunk sums are added in chunk
+ * order from +0.0.  Two calls on the same inputs give bit-identical outputs; with per-item textures (TB = B) an item's
+ * grad_texture does not depend on the other items.  Needs B*N < 2^31 and TB*TH*TW < 2^31 - 1 (else DIRT_ERR_BAD_SHAPE).
+ * scratch: at least dirt_texture_sample_backward_deterministic_bytes(...) bytes, 256-byte aligned, owned by the caller,
+ * needing no initialisation; it may be NULL when grad_texture is NULL or there are no lookups.  The size is a function of
+ * the shapes alone (0 for no lookups or shapes this entry rejects): 16 bytes per lookup for the sort, 4 per texel for the
+ * segment offsets, the sort's digit counts and the chunk sums of long sequences. */
+size_t dirt_texture_sample_backward_deterministic_bytes(int TB, int TH, int TW, int C, int B, long long N, int mode);
+int dirt_texture_sample_backward_deterministic(const float* texture, const float* indices, const float* grad_out,
+                                               float* grad_texture, float* grad_indices,
+                                               int TB, int TH, int TW, int C, int B, long long N, int mode,
+                                               void* scratch, size_t scratch_bytes, void* cuda_stream);
+
 /* Reflectance models of the reference's lighting module (dirt/lighting.py:182-343), one value per point and channel.
  * B items of V points each, C channels:
  *   normals, positions   float32 [B*V, 3], row stride normals_stride / positions_stride floats, unit stride along the row
