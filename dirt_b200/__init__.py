@@ -3,8 +3,8 @@
 `import dirt_b200 as dirt` is the drop-in for the reference package (dirt/__init__.py:1-3).
 """
 from .rasterise_ops import rasterise, rasterise_batch, rasterise_deferred, rasterise_batch_deferred
-from .texture import sample_texture, uvs_to_pixel_indices
+from .texture import index_derivatives, sample_texture, uvs_to_pixel_indices
 from . import matrices, lighting, projection
 
 __all__ = ['rasterise', 'rasterise_batch', 'rasterise_deferred', 'rasterise_batch_deferred',
-           'sample_texture', 'uvs_to_pixel_indices', 'matrices', 'lighting', 'projection']
+           'sample_texture', 'uvs_to_pixel_indices', 'index_derivatives', 'matrices', 'lighting', 'projection']

@@ -88,6 +88,18 @@ def load(path):
     L.dirt_texture_sample_backward_deterministic_bytes.argtypes = [i] * 5 + [ctypes.c_longlong, i]
     L.dirt_texture_sample_backward_deterministic.restype = i
     L.dirt_texture_sample_backward_deterministic.argtypes = [vp] * 5 + [i] * 5 + [ctypes.c_longlong, i, vp, sz, vp]
+    L.dirt_texture_mip_levels.restype = i
+    L.dirt_texture_mip_levels.argtypes = [i, i]
+    L.dirt_texture_mip_pyramid_bytes.restype = sz
+    L.dirt_texture_mip_pyramid_bytes.argtypes = [i] * 4
+    L.dirt_texture_mip_build.restype = i
+    L.dirt_texture_mip_build.argtypes = [vp] * 2 + [i] * 4 + [vp]
+    L.dirt_texture_sample_trilinear.restype = i
+    L.dirt_texture_sample_trilinear.argtypes = [vp] * 5 + [i] * 5 + [ctypes.c_longlong, vp]
+    L.dirt_texture_sample_trilinear_backward_bytes.restype = sz
+    L.dirt_texture_sample_trilinear_backward_bytes.argtypes = [i] * 5 + [ctypes.c_longlong, i]
+    L.dirt_texture_sample_trilinear_backward.restype = i
+    L.dirt_texture_sample_trilinear_backward.argtypes = [vp] * 7 + [i] * 5 + [ctypes.c_longlong, i, vp, sz, vp]
     ll = ctypes.c_longlong
     light_inputs = [i, i, vp, ll, vp, ll, vp, ll] + [vp, i] * 4
     L.dirt_lighting_workspace_bytes.restype = sz
@@ -113,7 +125,9 @@ EXPORTED_SYMBOLS = ['dirt_error_string', 'dirt_abi_version', 'dirt_workspace_byt
                     'dirt_lighting_backward', 'dirt_normals_workspace_bytes', 'dirt_normals_forward',
                     'dirt_normals_backward', 'dirt_rasterise_backward_deterministic_bytes',
                     'dirt_rasterise_backward_deterministic', 'dirt_texture_sample_backward_deterministic_bytes',
-                    'dirt_texture_sample_backward_deterministic']
+                    'dirt_texture_sample_backward_deterministic', 'dirt_texture_mip_levels',
+                    'dirt_texture_mip_pyramid_bytes', 'dirt_texture_mip_build', 'dirt_texture_sample_trilinear',
+                    'dirt_texture_sample_trilinear_backward_bytes', 'dirt_texture_sample_trilinear_backward']
 
 
 def error_string(code):

@@ -388,6 +388,101 @@ extern "C" int dirt_texture_sample_backward_deterministic(const float* texture, 
     return DIRT_OK;
 }
 
+// ---- mipmapped (trilinear) lookup ----
+
+// the bilinear lookup's limits, and the derivatives' 4 floats per lookup
+static bool mip_shape_ok(int TB, int TH, int TW, int C, int B, long long N)
+{
+    return texture_shape_ok(TB, TH, TW, C, B, N, DIRT_TEXTURE_BILINEAR) && (double)B * N * (C > 4 ? C : 4) <= 4.0e18;
+}
+
+extern "C" int dirt_texture_mip_levels(int TH, int TW) { return TH > 0 && TW > 0 ? mip_levels(TH, TW) : 0; }
+
+extern "C" size_t dirt_texture_mip_pyramid_bytes(int TB, int TH, int TW, int C)
+{
+    if (TB < 0 || !texture_shape_ok(TB, TH, TW, C, TB, 0, DIRT_TEXTURE_BILINEAR)) return 0;
+    const TexDims d = make_tex_dims(TB, TH, TW, C, TB, 0, DIRT_TEXTURE_BILINEAR);
+    return sizeof(float) * (size_t)mip_pyramid_texels(d, mip_levels(TH, TW)) * C;
+}
+
+extern "C" int dirt_texture_mip_build(const float* texture, float* pyramid, int TB, int TH, int TW, int C, void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (TB < 0 || !texture_shape_ok(TB, TH, TW, C, TB, 0, DIRT_TEXTURE_BILINEAR)) return DIRT_ERR_BAD_SHAPE;
+    if (TB == 0 || mip_levels(TH, TW) == 1) return DIRT_OK;
+    if (!texture || !pyramid) return DIRT_ERR_NULL_POINTER;
+    if ((uintptr_t)texture % 4 || (uintptr_t)pyramid % 4) return DIRT_ERR_MISALIGNED;
+    CUDA_TRY(launch_texture_mip_build(texture, pyramid, make_tex_dims(TB, TH, TW, C, TB, 0, DIRT_TEXTURE_BILINEAR),
+                                      (cudaStream_t)cuda_stream, &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
+extern "C" int dirt_texture_sample_trilinear(const float* texture, const float* pyramid, const float* indices,
+                                             const float* derivatives, float* out, int TB, int TH, int TW, int C, int B,
+                                             long long N, void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (!mip_shape_ok(TB, TH, TW, C, B, N)) return DIRT_ERR_BAD_SHAPE;
+    if (B == 0 || N == 0) return DIRT_OK;
+    if (!texture || !indices || !derivatives || !out || (!pyramid && mip_levels(TH, TW) > 1)) return DIRT_ERR_NULL_POINTER;
+    if ((uintptr_t)texture % 4 || (uintptr_t)pyramid % 4 || (uintptr_t)indices % 4 || (uintptr_t)derivatives % 4 ||
+        (uintptr_t)out % 4)
+        return DIRT_ERR_MISALIGNED;
+    CUDA_TRY(launch_texture_trilinear_forward(texture, pyramid, indices, derivatives, out,
+                                              make_tex_dims(TB, TH, TW, C, B, N, DIRT_TEXTURE_BILINEAR),
+                                              (cudaStream_t)cuda_stream, &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
+extern "C" size_t dirt_texture_sample_trilinear_backward_bytes(int TB, int TH, int TW, int C, int B, long long N,
+                                                               int deterministic)
+{
+    if (!mip_shape_ok(TB, TH, TW, C, B, N)) return 0;
+    if (deterministic && (!texture_det_shape_ok(TB, TH, TW, C, B, N, DIRT_TEXTURE_BILINEAR) || (long long)B * N == 0)) return 0;
+    const TexDims d = make_tex_dims(TB, TH, TW, C, B, N, DIRT_TEXTURE_BILINEAR);
+    if (!deterministic && mip_levels(TH, TW) == 1) return 0;
+    return carve_texture_mip_scratch(nullptr, d, deterministic != 0).bytes;
+}
+
+extern "C" int dirt_texture_sample_trilinear_backward(const float* texture, const float* pyramid, const float* indices,
+                                                      const float* derivatives, const float* grad_out, float* grad_texture,
+                                                      float* grad_indices, int TB, int TH, int TW, int C, int B, long long N,
+                                                      int deterministic, void* scratch, size_t scratch_bytes,
+                                                      void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (!mip_shape_ok(TB, TH, TW, C, B, N)) return DIRT_ERR_BAD_SHAPE;
+    if (deterministic && grad_texture && !texture_det_shape_ok(TB, TH, TW, C, B, N, DIRT_TEXTURE_BILINEAR))
+        return DIRT_ERR_BAD_SHAPE;
+    const TexDims d = make_tex_dims(TB, TH, TW, C, B, N, DIRT_TEXTURE_BILINEAR);
+    const int L = mip_levels(TH, TW);
+    if (d.total > 0) {
+        if (!indices || !derivatives || !grad_out) return DIRT_ERR_NULL_POINTER;
+        if (grad_indices && (!texture || (!pyramid && L > 1))) return DIRT_ERR_NULL_POINTER;
+    }
+    if ((uintptr_t)texture % 4 || (uintptr_t)pyramid % 4 || (uintptr_t)indices % 4 || (uintptr_t)derivatives % 4 ||
+        (uintptr_t)grad_out % 4 || (uintptr_t)grad_texture % 4 || (uintptr_t)grad_indices % 4)
+        return DIRT_ERR_MISALIGNED;
+    // the scratch holds the pyramid's gradients (default) or the per-level passes (deterministic)
+    const bool det = deterministic && grad_texture && d.total > 0;
+    const bool uses_scratch = grad_texture && d.total > 0 && (det || L > 1);
+    if (uses_scratch) {
+        if (!scratch) return DIRT_ERR_NULL_POINTER;
+        if ((uintptr_t)scratch % 256) return DIRT_ERR_MISALIGNED;
+        if (scratch_bytes < dirt_texture_sample_trilinear_backward_bytes(TB, TH, TW, C, B, N, det)) return DIRT_ERR_WORKSPACE_TOO_SMALL;
+    }
+    CUDA_TRY(launch_texture_trilinear_backward(texture, pyramid, indices, derivatives, grad_out, grad_texture, grad_indices, d,
+                                               det, carve_texture_mip_scratch(uses_scratch ? scratch : nullptr, d, det),
+                                               (cudaStream_t)cuda_stream, &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
 // element offsets of every per-point buffer stay below 2^62, the chunk count within the grid's x limit
 static bool lighting_shape_ok(int model, int B, long long V, int C, long long sn, long long sp, long long sc)
 {

@@ -855,4 +855,481 @@ cudaError_t launch_texture_backward(const float* texture, const float* indices, 
     return e;
 }
 
+// ---- mipmapped (trilinear) lookup (DESIGN.md §7.6) ------------------------------------------------------------------
+//
+// Level k of L is [TB, TH >> k, TW >> k, C]; levels 1 .. L-1 live in the caller's pyramid buffer (mip_offset).  Per
+// lookup: lambda from the screen-space derivatives, l = floor(lambda), f = lambda - l, and
+// out = (1-f) * bilinear_l + f * bilinear_{l+1}, with level l+1 not read when f == 0.  Level k >= 1 is read at
+// (index + 0.5) * 2^-k - 0.5, level 0 at the index itself, so that f == 0 at l == 0 is mode bilinear bit for bit.
+
+namespace {
+
+// level k's dims: the level-0 dims with TH, TW and texels scaled down
+__device__ __forceinline__ TexDims level_dims(const TexDims& d, int k)
+{
+    TexDims e = d;
+    e.TH = d.TH >> k;
+    e.TW = d.TW >> k;
+    e.texels = d.texels >> (2 * k);
+    return e;
+}
+
+// level k of the texture (k = 0) or of the pyramid
+template <typename T>
+__host__ __device__ __forceinline__ T* level_base(T* level0, T* pyramid, const TexDims& d, int k)
+{
+    return k == 0 ? level0 : pyramid + mip_offset(d, k) * d.C;
+}
+
+// (index + 0.5) * 2^-k - 0.5, each operation rounded in that order; the index itself at level 0
+__device__ __forceinline__ float level_index(float i, int k)
+{
+    if (k == 0) return i;
+    return __fsub_rn(__fmul_rn(__fadd_rn(i, 0.5f), __int_as_float((127 - k) << 23)), 0.5f);
+}
+
+struct Lod {
+    int l;      // the finer level read
+    float f;    // the weight of level l + 1; 0: level l alone
+};
+
+// rho^2 = max(d0^2 + d1^2, d2^2 + d3^2) (NaN if either is), lambda = 0.5 log2(rho^2), NaN -> 0, clamped to [0, L-1]
+__device__ __forceinline__ Lod lod_of(float4 v, int L)
+{
+    const float s0 = __fadd_rn(__fmul_rn(v.x, v.x), __fmul_rn(v.y, v.y));
+    const float s1 = __fadd_rn(__fmul_rn(v.z, v.z), __fmul_rn(v.w, v.w));
+    const float rho2 = isnan(s0) || isnan(s1) ? __int_as_float(0x7fc00000) : fmaxf(s0, s1);
+    float lam = __fmul_rn(0.5f, log2f(rho2));
+    lam = isnan(lam) ? 0.f : fminf(fmaxf(lam, 0.f), (float)(L - 1));
+    Lod o;
+    o.l = (int)floorf(lam);
+    o.f = __fsub_rn(lam, (float)o.l);
+    return o;
+}
+
+template <bool VEC>
+__device__ __forceinline__ float4 load_derivatives(const float* derivatives, long long g)
+{
+    if (VEC) return __ldg(reinterpret_cast<const float4*>(derivatives) + g);
+    const float* p = derivatives + 4 * g;
+    return make_float4(__ldg(p), __ldg(p + 1), __ldg(p + 2), __ldg(p + 3));
+}
+
+// the bilinear lookup of channels c0 .. c0 + NV - 1 at taps t of a texture of width TW and C channels
+template <int NV, bool VEC>
+__device__ __forceinline__ void bilinear_rows(const float* tex, const Taps& t, int TW, int C, int c0, float v[NV])
+{
+    float t00[NV], t01[NV], t10[NV], t11[NV];
+    load_row<NV, VEC>(tex + ((long long)t.r0 * TW + t.c0) * C + c0, t00);
+    load_row<NV, VEC>(tex + ((long long)t.r0 * TW + t.c1) * C + c0, t01);
+    load_row<NV, VEC>(tex + ((long long)t.r1 * TW + t.c0) * C + c0, t10);
+    load_row<NV, VEC>(tex + ((long long)t.r1 * TW + t.c1) * C + c0, t11);
+#pragma unroll
+    for (int j = 0; j < NV; ++j) v[j] = bilinear(t00[j], t01[j], t10[j], t11[j], t.fr, t.fc);
+}
+
+// One lookup's two levels: taps and pointers of level l (0) and l + 1 (1; unused when f == 0)
+struct Trilinear {
+    Taps t0, t1;
+    const float *p0, *p1;   // the lookup's texture at level l / l + 1
+    int w0, w1;             // their widths
+    Lod lod;
+};
+
+__device__ __forceinline__ Trilinear trilinear_of(float2 ix, float4 dv, const float* texture, const float* pyramid,
+                                                  const TexDims& d, int L, long long g)
+{
+    Trilinear q;
+    q.lod = lod_of(dv, L);
+    const int l = q.lod.l, l1 = l + 1 < L ? l + 1 : l;
+    const TexDims d0 = level_dims(d, l), d1 = level_dims(d, l1);
+    q.t0 = taps_of(level_index(ix.x, l), level_index(ix.y, l), d0, g);
+    q.t1 = taps_of(level_index(ix.x, l1), level_index(ix.y, l1), d1, g);
+    // a finite index can map to a non-finite one only past 3.4e38; such a lookup reads nothing, as a non-finite one
+    q.t0.valid = q.t0.valid && q.t1.valid;
+    q.p0 = level_base(texture, pyramid, d, l) + q.t0.base * d.C;
+    q.p1 = level_base(texture, pyramid, d, l1) + q.t1.base * d.C;
+    q.w0 = d0.TW;
+    q.w1 = d1.TW;
+    return q;
+}
+
+// one thread per element of the next level: ((a + b) + (c + e)) * 0.25 of the 2x2 block, in that order
+__global__ void __launch_bounds__(TEX_THREADS) mip_build_kernel(const float* __restrict__ src, float* __restrict__ dst,
+                                                                long long n, int H, int W, int C)
+{
+    const long long stride = (long long)gridDim.x * TEX_THREADS;
+    for (long long e = (long long)blockIdx.x * TEX_THREADS + threadIdx.x; e < n; e += stride) {
+        const long long x = e / C, row = x / W;   // row = tb * H + i
+        const int c = (int)(e - x * C), j = (int)(x - row * W);
+        const float* s = src + ((2 * row) * (2ll * W) + 2 * j) * C + c;
+        const long long down = 2ll * W * C;
+        const float a = __ldg(s), b = __ldg(s + C), cc = __ldg(s + down), ee = __ldg(s + down + C);
+        dst[e] = __fmul_rn(__fadd_rn(__fadd_rn(a, b), __fadd_rn(cc, ee)), 0.25f);
+    }
+}
+
+// One thread per lookup, CT = C in 1..4 or 0 (any C, one channel at a time).  VEC: indices 8-, derivatives 16-byte
+// aligned, out, texture and pyramid rows aligned for the vector loads and stores (the C = 3 store is staged as in
+// texture_forward_kernel).
+template <int CT, bool VEC>
+__global__ void __launch_bounds__(TEX_THREADS) texture_trilinear_forward_kernel(const float* __restrict__ texture,
+                                                                                const float* __restrict__ pyramid,
+                                                                                const float* __restrict__ indices,
+                                                                                const float* __restrict__ derivatives,
+                                                                                float* __restrict__ out, TexDims d, int L)
+{
+    constexpr int NV = CT ? CT : 1;
+    const int C = CT ? CT : d.C;
+    __shared__ __align__(16) float stage[CT == 3 ? TEX_THREADS * 3 : 1];
+    const int lane = threadIdx.x & 31;
+    const long long stride = (long long)gridDim.x * TEX_THREADS;
+    for (long long base = (long long)blockIdx.x * TEX_THREADS + (threadIdx.x & ~31); base < d.total; base += stride) {
+        const long long g = base + lane;
+        Trilinear q;
+        q.t0.valid = false;
+        if (g < d.total) q = trilinear_of(load_index<VEC>(indices, g), load_derivatives<VEC>(derivatives, g), texture, pyramid, d,
+                                          L, g);
+        for (int c0 = 0; c0 < C; c0 += NV) {
+            float v[NV];
+#pragma unroll
+            for (int j = 0; j < NV; ++j) v[j] = 0.f;
+            if (q.t0.valid) {
+                bilinear_rows<NV, VEC>(q.p0, q.t0, q.w0, C, c0, v);
+                if (q.lod.f != 0.f) {
+                    float u[NV];
+                    bilinear_rows<NV, VEC>(q.p1, q.t1, q.w1, C, c0, u);
+                    const float omf = __fsub_rn(1.0f, q.lod.f);
+#pragma unroll
+                    for (int j = 0; j < NV; ++j) v[j] = __fadd_rn(__fmul_rn(omf, v[j]), __fmul_rn(q.lod.f, u[j]));
+                }
+            }
+            float* o = out + g * C + c0;
+            if (VEC && CT == 4) {
+                if (g < d.total) *reinterpret_cast<float4*>(o) = make_float4(v[0], v[1 % NV], v[2 % NV], v[3 % NV]);
+            } else if (VEC && CT == 2) {
+                if (g < d.total) *reinterpret_cast<float2*>(o) = make_float2(v[0], v[1 % NV]);
+            } else if (VEC && CT == 3 && base + 32 <= d.total) {
+                float* s = stage + (threadIdx.x & ~31) * 3;
+#pragma unroll
+                for (int j = 0; j < NV; ++j) s[lane * 3 + j] = v[j];
+                __syncwarp();
+                if (lane < 24) *reinterpret_cast<float4*>(out + base * 3 + lane * 4) = reinterpret_cast<const float4*>(s)[lane];
+                __syncwarp();
+            } else if (g < d.total) {
+#pragma unroll
+                for (int j = 0; j < NV; ++j) o[j] = v[j];
+            }
+        }
+    }
+}
+
+// One thread per lookup, CT as in the forward kernel.  grad_indices per lookup, through both levels' fractions, each
+// scaled by 2^-k.  The texel gradients of level 0 go to grad_texture, those of level k >= 1 to level_grad (the pyramid's
+// layout), through the warp aggregation of texture_backward_kernel keyed on the packed texel index (level 0: its texel
+// index; level k: TB * texels + the pyramid's texel index).
+template <int CT, bool VEC>
+__global__ void __launch_bounds__(TEX_THREADS) texture_trilinear_backward_kernel(
+    const float* __restrict__ texture, const float* __restrict__ pyramid, const float* __restrict__ indices,
+    const float* __restrict__ derivatives, const float* __restrict__ grad_out, float* __restrict__ grad_texture,
+    float* __restrict__ level_grad, float* __restrict__ grad_indices, TexDims d, int L)
+{
+    constexpr int NV = CT ? CT : 1;
+    const int C = CT ? CT : d.C;
+    const int lane = threadIdx.x & 31;
+    const long long stride = (long long)gridDim.x * TEX_THREADS;
+    for (long long base = (long long)blockIdx.x * TEX_THREADS + (threadIdx.x & ~31); base < d.total; base += stride) {
+        const long long g = base + lane;
+        const bool live = g < d.total;
+        Trilinear q;
+        q.t0.valid = false;
+        q.lod.l = 0; q.lod.f = 0.f;
+        if (live) q = trilinear_of(load_index<VEC>(indices, g), load_derivatives<VEC>(derivatives, g), texture, pyramid, d, L, g);
+        if (!q.t0.valid) {
+            q.t0.r0 = q.t0.r1 = q.t0.c0 = q.t0.c1 = 0; q.t0.fr = q.t0.fc = 0.f; q.t0.base = 0;
+            q.t1 = q.t0;
+            q.lod.l = 0; q.lod.f = 0.f;
+        }
+        const bool both = q.t0.valid && q.lod.f != 0.f;
+        const float omf = __fsub_rn(1.0f, q.lod.f);
+        const float* gout = grad_out + g * C;
+        float go[NV];
+#pragma unroll
+        for (int j = 0; j < NV; ++j) go[j] = 0.f;
+        if (CT && q.t0.valid) load_row<NV, VEC>(gout, go);
+
+        if (grad_indices && live) {
+            float dr0 = 0.f, dc0 = 0.f, dr1 = 0.f, dc1 = 0.f;
+            if (q.t0.valid) {
+#pragma unroll
+                for (int s = 0; s < 2; ++s) {
+                    if (s == 1 && !both) break;
+                    const Taps t = s ? q.t1 : q.t0;
+                    const float* tex = s ? q.p1 : q.p0;
+                    const int TW = s ? q.w1 : q.w0;
+                    const float omr = __fsub_rn(1.0f, t.fr), omc = __fsub_rn(1.0f, t.fc);
+                    float dr = 0.f, dc = 0.f;
+                    for (int c0 = 0; c0 < C; c0 += NV) {
+                        float t00[NV], t01[NV], t10[NV], t11[NV];
+                        load_row<NV, VEC>(tex + ((long long)t.r0 * TW + t.c0) * C + c0, t00);
+                        load_row<NV, VEC>(tex + ((long long)t.r0 * TW + t.c1) * C + c0, t01);
+                        load_row<NV, VEC>(tex + ((long long)t.r1 * TW + t.c0) * C + c0, t10);
+                        load_row<NV, VEC>(tex + ((long long)t.r1 * TW + t.c1) * C + c0, t11);
+                        if (!CT) go[0] = __ldg(gout + c0);
+#pragma unroll
+                        for (int j = 0; j < NV; ++j) {
+                            dc += go[j] * ((t01[j] - t00[j]) * omr + (t11[j] - t10[j]) * t.fr);
+                            dr += go[j] * ((t10[j] - t00[j]) * omc + (t11[j] - t01[j]) * t.fc);
+                        }
+                    }
+                    if (s) { dr1 = dr; dc1 = dc; }
+                    else { dr0 = dr; dc0 = dc; }
+                }
+            }
+            // d index_k / d index = 2^-k
+            const float s0 = __int_as_float((127 - q.lod.l) << 23), s1 = 0.5f * s0;
+            float dr = dr0 * s0, dc = dc0 * s0;
+            if (both) {
+                dr = omf * dr + q.lod.f * (dr1 * s1);
+                dc = omf * dc + q.lod.f * (dc1 * s1);
+            }
+            if (VEC) reinterpret_cast<float2*>(grad_indices)[g] = make_float2(dr, dc);
+            else { grad_indices[2 * g] = dr; grad_indices[2 * g + 1] = dc; }
+        }
+
+        if (grad_texture) {
+#pragma unroll 1
+            for (int s = 0; s < 2; ++s) {   // warp-uniform: every lane takes part in agg_plan
+                const int k = q.lod.l + s;
+                const Taps t = s ? q.t1 : q.t0;
+                const float a = s ? q.lod.f : (both ? omf : 1.0f);
+                const bool level_on = s ? both : q.t0.valid;
+                const float omr = __fsub_rn(1.0f, t.fr), omc = __fsub_rn(1.0f, t.fc);
+                const int TW = s ? q.w1 : q.w0;
+                const long long first = k == 0 ? 0ll : (long long)d.TB * d.texels + mip_offset(d, k);
+                float* dst_level = k == 0 ? grad_texture : level_grad + mip_offset(d, k) * C;
+                for (int corner = 0; corner < 4; ++corner) {   // (r0,c0), (r0,c1), (r1,c0), (r1,c1)
+                    const int r = (corner & 2) ? t.r1 : t.r0, c = (corner & 1) ? t.c1 : t.c0;
+                    const float w = __fmul_rn(__fmul_rn((corner & 1) ? t.fc : omc, (corner & 2) ? t.fr : omr), a);
+                    const bool on = level_on && w != 0.f;
+                    const long long texel = t.base + (long long)r * TW + c;
+                    const Agg ag = agg_plan(on ? (unsigned long long)(first + texel) : (1ull << 63) | (unsigned)lane, lane);
+                    const bool leader = on && __ffs(ag.peers) - 1 == lane;
+                    float* dst = dst_level + texel * C;
+                    if (CT) {
+                        float v[NV];
+#pragma unroll
+                        for (int j = 0; j < NV; ++j) v[j] = on ? go[j] * w : 0.f;
+                        agg_sum<NV>(ag, v, lane);
+                        if (leader) red_row<NV, VEC>(dst, v);
+                    } else {
+                        for (int ch = 0; ch < C; ++ch) {
+                            float v[1] = {on ? __ldg(gout + ch) * w : 0.f};
+                            agg_sum<1>(ag, v, lane);
+                            if (leader) atomicAdd(dst + ch, v[0]);
+                        }
+                    }
+                }
+            }
+        }
+    }
+}
+
+// The pyramid's adjoint: each level-k texel passes 0.25 x its gradient to its four children.  One thread per element
+// (level-0 texel, channel): acc = g_{L-1}[ancestor], then acc = g_k[ancestor] + 0.25 * acc for k = L-2 .. 1, and
+// grad_texture += 0.25 * acc, each operation rounded in that order.  A gather: no atomics.
+__global__ void __launch_bounds__(TEX_THREADS) mip_collapse_kernel(float* __restrict__ grad_texture,
+                                                                   const float* __restrict__ level_grad, TexDims d, int L)
+{
+    const long long n = (long long)d.TB * d.texels * d.C, stride = (long long)gridDim.x * TEX_THREADS;
+    for (long long e = (long long)blockIdx.x * TEX_THREADS + threadIdx.x; e < n; e += stride) {
+        const long long x = e / d.C, tb = x / d.texels, rc = x - tb * d.texels;
+        const int ch = (int)(e - x * d.C), r = (int)(rc / d.TW), c = (int)(rc - (long long)r * d.TW);
+        float acc = 0.f;
+        for (int k = L - 1; k >= 1; --k) {
+            const long long tw = d.TW >> k, texels = d.texels >> (2 * k);
+            const float v = __ldg(level_grad + (mip_offset(d, k) + tb * texels + (long long)(r >> k) * tw + (c >> k)) * d.C + ch);
+            acc = k == L - 1 ? v : __fadd_rn(v, __fmul_rn(0.25f, acc));
+        }
+        grad_texture[e] = __fadd_rn(grad_texture[e], __fmul_rn(0.25f, acc));
+    }
+}
+
+// Deterministic path, per level k: the lookups' level-k index (NaN where level k is not read, which the §7.5 path
+// skips) and grad_out times their weight of level k, fp32
+__global__ void __launch_bounds__(TEX_THREADS) mip_level_terms_kernel(const float* __restrict__ indices,
+                                                                      const float* __restrict__ derivatives,
+                                                                      const float* __restrict__ grad_out, TexDims d, int L,
+                                                                      int k, float* __restrict__ level_indices,
+                                                                      float* __restrict__ level_grad_out)
+{
+    const long long stride = (long long)gridDim.x * TEX_THREADS;
+    for (long long g = (long long)blockIdx.x * TEX_THREADS + threadIdx.x; g < d.total; g += stride) {
+        const float ir = __ldg(indices + 2 * g), ic = __ldg(indices + 2 * g + 1);
+        const Lod lod = lod_of(load_derivatives<false>(derivatives, g), L);
+        const bool valid = isfinite(ir) && isfinite(ic);
+        const float a = lod.l == k ? (lod.f != 0.f ? __fsub_rn(1.0f, lod.f) : 1.0f) : lod.f;
+        const bool reads = valid && (lod.l == k || (lod.l + 1 == k && lod.f != 0.f));
+        const float nan = __int_as_float(0x7fc00000);
+        level_indices[2 * g] = reads ? level_index(ir, k) : nan;
+        level_indices[2 * g + 1] = reads ? level_index(ic, k) : nan;
+        for (int ch = 0; ch < d.C; ++ch) level_grad_out[g * d.C + ch] = reads ? __fmul_rn(__ldg(grad_out + g * d.C + ch), a) : 0.f;
+    }
+}
+
+template <int CT>
+cudaError_t trilinear_forward_ct(const float* texture, const float* pyramid, const float* indices, const float* derivatives,
+                                 float* out, const TexDims& d, int L, cudaStream_t stream)
+{
+    const int row = CT == 2 || CT == 4 ? 4 * CT : 4;
+    const int out_bytes = CT == 3 ? 16 : row;
+    const bool vec = CT && aligned(indices, 8) && aligned(derivatives, 16) && aligned(out, out_bytes) &&
+                     aligned(texture, row) && aligned(pyramid, row);
+    const unsigned blocks = blocks_for(d.total);
+    if constexpr (CT != 0) {   // any C has no vector path
+        if (vec) {
+            texture_trilinear_forward_kernel<CT, true><<<blocks, TEX_THREADS, 0, stream>>>(texture, pyramid, indices,
+                                                                                          derivatives, out, d, L);
+            return cudaGetLastError();
+        }
+    }
+    texture_trilinear_forward_kernel<CT, false><<<blocks, TEX_THREADS, 0, stream>>>(texture, pyramid, indices, derivatives,
+                                                                                       out, d, L);
+    return cudaGetLastError();
+}
+
+template <int CT>
+cudaError_t trilinear_backward_ct(const float* texture, const float* pyramid, const float* indices, const float* derivatives,
+                                  const float* grad_out, float* grad_texture, float* level_grad, float* grad_indices,
+                                  const TexDims& d, int L, cudaStream_t stream)
+{
+    const int row = CT == 2 || CT == 4 ? 4 * CT : 4;
+    const bool vec = CT && aligned(indices, 8) && aligned(derivatives, 16) && aligned(grad_indices, 8) &&
+                     aligned(grad_out, row) && aligned(texture, row) && aligned(pyramid, row) && aligned(grad_texture, row) &&
+                     aligned(level_grad, row);
+    const unsigned blocks = blocks_for(d.total);
+    if constexpr (CT != 0) {
+        if (vec) {
+            texture_trilinear_backward_kernel<CT, true><<<blocks, TEX_THREADS, 0, stream>>>(
+                texture, pyramid, indices, derivatives, grad_out, grad_texture, level_grad, grad_indices, d, L);
+            return cudaGetLastError();
+        }
+    }
+    texture_trilinear_backward_kernel<CT, false><<<blocks, TEX_THREADS, 0, stream>>>(
+            texture, pyramid, indices, derivatives, grad_out, grad_texture, level_grad, grad_indices, d, L);
+    return cudaGetLastError();
+}
+
+}  // namespace
+
+MipScratch carve_texture_mip_scratch(void* base, const TexDims& d, bool deterministic)
+{
+    MipScratch s = {};
+    char* p = static_cast<char*>(base);
+    size_t off = 0;
+    auto take = [&](size_t bytes) {
+        char* r = p && bytes ? p + off : nullptr;
+        off = align_up(off + bytes, 256);
+        return r;
+    };
+    const int L = mip_levels(d.TH, d.TW);
+    s.level_grad = reinterpret_cast<float*>(take((size_t)mip_pyramid_texels(d, L) * d.C * sizeof(float)));
+    if (deterministic) {
+        s.indices = reinterpret_cast<float*>(take((size_t)d.total * 2 * sizeof(float)));
+        s.grad_out = reinterpret_cast<float*>(take((size_t)d.total * d.C * sizeof(float)));
+        s.det = take(carve_texture_det_scratch(nullptr, d).bytes);
+    }
+    s.bytes = off;
+    return s;
+}
+
+cudaError_t launch_texture_mip_build(const float* texture, float* pyramid, const TexDims& d, cudaStream_t stream,
+                                     int* launches)
+{
+    const int L = mip_levels(d.TH, d.TW);
+    for (int k = 1; k < L; ++k) {
+        const long long n = (long long)d.TB * (d.texels >> (2 * k)) * d.C;
+        mip_build_kernel<<<blocks_for(n), TEX_THREADS, 0, stream>>>(level_base(texture, (const float*)pyramid, d, k - 1),
+                                                                    pyramid + mip_offset(d, k) * d.C, n, d.TH >> k,
+                                                                    d.TW >> k, d.C);
+        const cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) return e;
+        ++*launches;
+    }
+    return cudaSuccess;
+}
+
+cudaError_t launch_texture_trilinear_forward(const float* texture, const float* pyramid, const float* indices,
+                                             const float* derivatives, float* out, const TexDims& d, cudaStream_t stream,
+                                             int* launches)
+{
+    const int L = mip_levels(d.TH, d.TW);
+    cudaError_t e;
+    switch (d.C) {
+        case 1: e = trilinear_forward_ct<1>(texture, pyramid, indices, derivatives, out, d, L, stream); break;
+        case 2: e = trilinear_forward_ct<2>(texture, pyramid, indices, derivatives, out, d, L, stream); break;
+        case 3: e = trilinear_forward_ct<3>(texture, pyramid, indices, derivatives, out, d, L, stream); break;
+        case 4: e = trilinear_forward_ct<4>(texture, pyramid, indices, derivatives, out, d, L, stream); break;
+        default: e = trilinear_forward_ct<0>(texture, pyramid, indices, derivatives, out, d, L, stream);
+    }
+    if (e == cudaSuccess) ++*launches;
+    return e;
+}
+
+cudaError_t launch_texture_trilinear_backward(const float* texture, const float* pyramid, const float* indices,
+                                              const float* derivatives, const float* grad_out, float* grad_texture,
+                                              float* grad_indices, const TexDims& d, bool deterministic,
+                                              const MipScratch& s, cudaStream_t stream, int* launches)
+{
+    const int L = mip_levels(d.TH, d.TW);
+    const size_t texture_bytes = sizeof(float) * (size_t)d.TB * d.texels * d.C;
+    cudaError_t e;
+    if (d.total == 0 || !grad_texture) deterministic = false;
+    if (grad_texture && !deterministic) {
+        if ((e = cudaMemsetAsync(grad_texture, 0, texture_bytes, stream)) != cudaSuccess) return e;
+        if (L > 1 && d.total > 0 &&
+            (e = cudaMemsetAsync(s.level_grad, 0, sizeof(float) * (size_t)mip_pyramid_texels(d, L) * d.C, stream)) !=
+                cudaSuccess)
+            return e;
+    }
+    if (d.total == 0 || (!grad_texture && !grad_indices)) return cudaSuccess;
+    // the default kernel: both gradients, or under the deterministic flag grad_indices alone (it has no atomics)
+    float* gt = deterministic ? nullptr : grad_texture;
+    if (gt || grad_indices) {
+        switch (d.C) {
+            case 1: e = trilinear_backward_ct<1>(texture, pyramid, indices, derivatives, grad_out, gt, s.level_grad, grad_indices, d, L, stream); break;
+            case 2: e = trilinear_backward_ct<2>(texture, pyramid, indices, derivatives, grad_out, gt, s.level_grad, grad_indices, d, L, stream); break;
+            case 3: e = trilinear_backward_ct<3>(texture, pyramid, indices, derivatives, grad_out, gt, s.level_grad, grad_indices, d, L, stream); break;
+            case 4: e = trilinear_backward_ct<4>(texture, pyramid, indices, derivatives, grad_out, gt, s.level_grad, grad_indices, d, L, stream); break;
+            default: e = trilinear_backward_ct<0>(texture, pyramid, indices, derivatives, grad_out, gt, s.level_grad, grad_indices, d, L, stream);
+        }
+        if (e != cudaSuccess) return e;
+        ++*launches;
+    }
+    if (!grad_texture) return cudaSuccess;
+    if (deterministic) {
+        // level k's gradient, every texel written, by the §7.5 path over the lookups that read level k
+        for (int k = 0; k < L; ++k) {
+            mip_level_terms_kernel<<<blocks_for(d.total), TEX_THREADS, 0, stream>>>(indices, derivatives, grad_out, d, L, k,
+                                                                                     s.indices, s.grad_out);
+            if ((e = cudaGetLastError()) != cudaSuccess) return e;
+            ++*launches;
+            TexDims dk = d;
+            dk.TH = d.TH >> k; dk.TW = d.TW >> k; dk.texels = d.texels >> (2 * k);
+            float* gk = k == 0 ? grad_texture : s.level_grad + mip_offset(d, k) * d.C;
+            if ((e = launch_texture_backward_deterministic(nullptr, s.indices, s.grad_out, gk, nullptr, dk,
+                                                           carve_texture_det_scratch(s.det, dk), stream, launches)) !=
+                cudaSuccess)
+                return e;
+        }
+    }
+    if (L > 1) {
+        mip_collapse_kernel<<<blocks_for((long long)d.TB * d.texels * d.C), TEX_THREADS, 0, stream>>>(grad_texture, s.level_grad,
+                                                                                                      d, L);
+        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+        ++*launches;
+    }
+    return cudaSuccess;
+}
+
 }  // namespace dirt

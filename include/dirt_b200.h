@@ -226,6 +226,49 @@ int dirt_texture_sample_backward_deterministic(const float* texture, const float
                                                int TB, int TH, int TW, int C, int B, long long N, int mode,
                                                void* scratch, size_t scratch_bytes, void* cuda_stream);
 
+/* Mipmapped (trilinear) texture lookup (DESIGN.md §7.6), with gradients to the texels and to the indices.
+ * Levels: level 0 is the texture [TB, TH, TW, C]; level k+1 exists while level k has both dimensions even, and is its
+ * 2x2 box mean per channel, ((t[2i][2j] + t[2i][2j+1]) + (t[2i+1][2j] + t[2i+1][2j+1])) * 0.25, each operation rounded
+ * in that order in fp32.  Level k is [TB, TH >> k, TW >> k, C].  The pyramid buffer packs levels 1 .. L-1 in that order
+ * (level 0 is not copied); a texture with an odd dimension has L = 1 and an empty pyramid.
+ * Index mapping: texel j of a level has its full bilinear weight at index j, so level k >= 1 is read at
+ * (index + 0.5) * 2^-k - 0.5, each operation rounded in fp32 in that order, and level 0 at the index itself; each read
+ * is the bilinear lookup of DIRT_TEXTURE_BILINEAR at that level's size (wrapping around its edges).
+ * Level of detail: derivatives float32 [B, N, 4] = (d row / dx, d col / dx, d row / dy, d col / dy) in level-0 texels
+ * per pixel; rho^2 = max(d0^2 + d1^2, d2^2 + d3^2) (NaN if either sum is NaN), lambda = 0.5 * log2(rho^2), NaN -> 0,
+ * clamped to [0, L-1]; l = floor(lambda), f = lambda - l, and out = (1-f) * bilinear_l + f * bilinear_{l+1}, each
+ * operation rounded in that order.  f == 0 reads level l alone and returns it exactly: every lookup with rho <= 1 equals
+ * the bilinear lookup bit for bit.
+ * Gradients: to the texture through both levels' bilinear weights, then the pyramid's adjoint (a level-k texel passes
+ * 0.25 x its gradient to each of its four children); to the indices through both levels' fractions, scaled by 2^-k.
+ * The derivatives get none.  A lookup with a non-finite index returns 0, reads nothing and passes no gradient.
+ *   dirt_texture_mip_levels         L for a TH x TW texture (0 if either is not positive).
+ *   dirt_texture_mip_pyramid_bytes  size of the pyramid buffer (0 when L = 1 or for a bad shape).
+ *   dirt_texture_mip_build          writes the pyramid from the texture: one launch per level 1 .. L-1.
+ *   dirt_texture_sample_trilinear   the forward lookup; pyramid may be NULL when L = 1.
+ *   dirt_texture_sample_trilinear_backward  grad_texture is zeroed by the library before it accumulates; grad_indices
+ *       is written once per lookup.  Either may be NULL, and that half of the work is skipped; texture and pyramid are
+ *       read only for grad_indices.  deterministic != 0: grad_texture is bit-reproducible (each level's gradient by the
+ *       path of dirt_texture_sample_backward_deterministic, then the fixed-order adjoint; DESIGN.md §7.6), with that
+ *       path's limits (B*N < 2^31, TB*TH*TW < 2^31 - 1, else DIRT_ERR_BAD_SHAPE).  scratch: at least
+ *       dirt_texture_sample_trilinear_backward_bytes(...) bytes, 256-byte aligned, owned by the caller, needing no
+ *       initialisation; a function of the shapes alone, 0 (and scratch may be NULL) when grad_texture needs none.
+ *       scratch is read only when grad_texture is wanted and there are lookups.
+ * B = 0 or N = 0: nothing is launched (the backward call still zeroes grad_texture).  All pointers 4-byte aligned;
+ * 8-byte indices, 16-byte derivatives and row-aligned texture, pyramid, outputs enable the vector paths. */
+int dirt_texture_mip_levels(int TH, int TW);
+size_t dirt_texture_mip_pyramid_bytes(int TB, int TH, int TW, int C);
+int dirt_texture_mip_build(const float* texture, float* pyramid, int TB, int TH, int TW, int C, void* cuda_stream);
+int dirt_texture_sample_trilinear(const float* texture, const float* pyramid, const float* indices,
+                                  const float* derivatives, float* out,
+                                  int TB, int TH, int TW, int C, int B, long long N, void* cuda_stream);
+size_t dirt_texture_sample_trilinear_backward_bytes(int TB, int TH, int TW, int C, int B, long long N, int deterministic);
+int dirt_texture_sample_trilinear_backward(const float* texture, const float* pyramid, const float* indices,
+                                           const float* derivatives, const float* grad_out,
+                                           float* grad_texture, float* grad_indices,
+                                           int TB, int TH, int TW, int C, int B, long long N, int deterministic,
+                                           void* scratch, size_t scratch_bytes, void* cuda_stream);
+
 /* Reflectance models of the reference's lighting module (dirt/lighting.py:182-343), one value per point and channel.
  * B items of V points each, C channels:
  *   normals, positions   float32 [B*V, 3], row stride normals_stride / positions_stride floats, unit stride along the row
