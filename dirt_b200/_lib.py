@@ -69,6 +69,8 @@ def load(path):
     L.dirt_rasterise_backward_deterministic.restype = i
     L.dirt_rasterise_backward_deterministic.argtypes = ([vp] * 8 + [i] * 6 + [ctypes.POINTER(ctypes.c_int), i, i, i, vp, sz, vp, sz,
                                                         vp])
+    L.dirt_rasterise_derivatives.restype = i
+    L.dirt_rasterise_derivatives.argtypes = [vp] * 5 + [i] * 9 + [vp, sz, vp]
     L.dirt_workspace_status.restype = i
     L.dirt_workspace_status.argtypes = [vp, sz] + [i] * 6 + [vp]
     L.dirt_rasterise_visibility.restype = i
@@ -127,7 +129,8 @@ EXPORTED_SYMBOLS = ['dirt_error_string', 'dirt_abi_version', 'dirt_workspace_byt
                     'dirt_rasterise_backward_deterministic', 'dirt_texture_sample_backward_deterministic_bytes',
                     'dirt_texture_sample_backward_deterministic', 'dirt_texture_mip_levels',
                     'dirt_texture_mip_pyramid_bytes', 'dirt_texture_mip_build', 'dirt_texture_sample_trilinear',
-                    'dirt_texture_sample_trilinear_backward_bytes', 'dirt_texture_sample_trilinear_backward']
+                    'dirt_texture_sample_trilinear_backward_bytes', 'dirt_texture_sample_trilinear_backward',
+                    'dirt_rasterise_derivatives']
 
 
 def error_string(code):

@@ -261,6 +261,38 @@ extern "C" int dirt_rasterise_backward_ex(const float* vertices, const int32_t* 
                          W, C, V, F, channel_groups, n_groups, workspace_holds_setup, flags, workspace, workspace_bytes, cuda_stream);
 }
 
+extern "C" int dirt_rasterise_derivatives(const float* vertices, const int32_t* faces, const float* attributes,
+                                          const int32_t* face_ids, float* derivatives, int B, int H, int W, int C, int V,
+                                          int F, int first_channel, int channel_count, int workspace_holds_setup,
+                                          void* workspace, size_t workspace_bytes, void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (!shape_ok(B, H, W, C, V, F)) return DIRT_ERR_BAD_SHAPE;
+    if (first_channel < 0 || channel_count <= 0 || first_channel >= C || channel_count > C - first_channel)
+        return DIRT_ERR_BAD_SHAPE;
+    if (B == 0) return DIRT_OK;
+    if (!face_ids || !derivatives) return DIRT_ERR_NULL_POINTER;
+    if ((V > 0 && (!vertices || !attributes)) || (F > 0 && !faces)) return DIRT_ERR_NULL_POINTER;
+    if ((uintptr_t)vertices % 16 != 0) return DIRT_ERR_MISALIGNED;
+    if ((uintptr_t)attributes % 4 || (uintptr_t)faces % 4 || (uintptr_t)face_ids % 4 || (uintptr_t)derivatives % 4)
+        return DIRT_ERR_MISALIGNED;
+    int rc = check_workspace(workspace, workspace_bytes, B, H, W, C, V, F);
+    if (rc != DIRT_OK) return rc;
+    cudaStream_t stream = (cudaStream_t)cuda_stream;
+    const Workspace ws = carve_workspace(workspace, B, H, W, C, V, F);
+    const Dims d = make_dims(B, H, W, C, V, F);
+    unsigned long long expect_tag = 0;
+    if (!workspace_holds_setup)
+        CUDA_TRY(launch_setup_only(vertices, faces, ws, d, stream, &launches));
+    else
+        expect_tag = workspace_tag(vertices, faces, B, H, W, V, F);   // checked on the device, as backward_impl does
+    CUDA_TRY(launch_gbuffer_derivatives(face_ids, attributes, derivatives, ws, d, first_channel, channel_count, expect_tag,
+                                        stream, &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
 // the adjacency's corner ids b*3F + k*F + f are int32
 static bool deterministic_shape_ok(int B, int H, int W, int C, int V, int F)
 {

@@ -12,6 +12,7 @@ Differences that a caller can observe:
   csrc/rasterise_egl.cpp:410); there is no CPU fallback.
 """
 import ctypes
+import operator
 
 import torch
 
@@ -160,6 +161,28 @@ def rasterise_backward_raw(vertices, faces, pixels, grad_pixels, face_ids=None, 
                 B, H, W, C, V, F, groups_ptr, n_groups, reuse, flags, _ptr(ws), nbytes, _stream_ptr(device))
     _lib.check(rc, 'RasteriseGrad')
     return grad_background, grad_vertices, grad_vertex_colors
+
+
+def rasterise_derivatives_raw(vertices, faces, attributes, face_ids, first_channel, channel_count, setup_workspace=None):
+    """One call of dirt_rasterise_derivatives on contiguous CUDA tensors: the screen-space derivatives of attribute channels
+    [first_channel, first_channel + channel_count) at the pixels `face_ids` [B,H,W] shows, [B, H, W, 2, channel_count]
+    (index 0 of the `2` axis d/dx along W, index 1 d/dy down the rows; 0 on the background; DESIGN.md §7.7).
+    `setup_workspace`: the workspace of the forward call that produced `face_ids`, reused under the rule of
+    rasterise_backward_raw.  The result has no gradient."""
+    B, H, W = face_ids.shape
+    V, F, C = vertices.shape[1], faces.shape[1], attributes.shape[2]
+    device = face_ids.device
+    need = int(_lib.lib().dirt_workspace_bytes_min(B, H, W, C, V, F))
+    reuse = int(setup_workspace is not None and setup_workspace.numel() >= need and
+                getattr(setup_workspace, '_dirt_setup_of', None) == _geometry_identity(vertices, faces, H, W))
+    ws = setup_workspace if reuse else _workspace(B, H, W, C, V, F, device)[0]
+    out = torch.empty((B, H, W, 2, channel_count), dtype=torch.float32, device=device)
+    with torch.cuda.device(device):
+        rc = _lib.lib().dirt_rasterise_derivatives(_ptr(vertices), _ptr(faces), _ptr(attributes), _ptr(face_ids), _ptr(out),
+                                                   B, H, W, C, V, F, first_channel, channel_count, reuse, _ptr(ws),
+                                                   int(ws.numel()), _stream_ptr(device))
+    _lib.check(rc, 'RasteriseDerivatives')
+    return out
 
 
 def workspace_status(workspace, B, H, W, C, V, F):
@@ -365,7 +388,21 @@ class _InjectVertexGradient(torch.autograd.Function):
         return d_loss_by_pixels, d_loss_by_vertices, None, None, None
 
 
-def _rasterise_deferred_internal(background, vertices, attributes, faces, shader_fn, shader_additional_inputs, single_or_batch, name):
+def _channel_run(derivative_channels, channels):
+    """(first, count) of `derivative_channels`, which must be one ascending contiguous run of channel indices in
+    [0, channels), such as range(1, 3)."""
+    try:
+        run = [operator.index(c) for c in derivative_channels]
+    except TypeError:
+        run = None
+    if not run or run != list(range(run[0], run[0] + len(run))) or run[0] < 0 or run[-1] >= channels:
+        raise ValueError('derivative_channels must be one ascending run of consecutive attribute channels in [0, %d), '
+                         'such as range(1, 3); got %r' % (channels, derivative_channels))
+    return run[0], len(run)
+
+
+def _rasterise_deferred_internal(background, vertices, attributes, faces, shader_fn, shader_additional_inputs, single_or_batch, name,
+                                 derivative_channels=None):
     # dirt/rasterise_ops.py:180-257.  The reference wraps everything in one tf.custom_gradient; here the same
     # three gradient paths are expressed as two autograd nodes around an ordinary call of shader_fn, so tensors
     # and parameters that shader_fn uses receive their gradients from plain autograd.
@@ -381,32 +418,53 @@ def _rasterise_deferred_internal(background, vertices, attributes, faces, shader
         raise ValueError('Rasterise expects background_tensor to be 4D, and bgcolor.shape == [None, height, width, channels]')
     _check_shapes('Rasterise', background, vertices, attributes, faces, int(background.shape[1]), int(background.shape[2]),
                   int(background.shape[3]))
+    if derivative_channels is not None:
+        first, count = _channel_run(derivative_channels, int(attributes.shape[2]))
     _require_cuda(background, vertices, attributes, faces)
     background, vertices, attributes, faces = background.contiguous(), vertices.contiguous(), attributes.contiguous(), faces.contiguous()
     holder = _SetupHolder(None)
     gbuffer, face_ids = _RasteriseAttributes.apply(background, vertices, attributes, faces, holder)
+    extra = {}
+    if derivative_channels is not None:
+        with torch.no_grad():
+            derivatives = rasterise_derivatives_raw(vertices, faces, attributes, face_ids, first, count, holder.workspace)
+        extra['gbuffer_derivatives'] = derivatives[0] if single_or_batch == 'single' else derivatives
     if single_or_batch == 'single':
-        pixels = shader_fn(gbuffer[0], *shader_additional_inputs)[None]
+        pixels = shader_fn(gbuffer[0], *shader_additional_inputs, **extra)[None]
     else:
-        pixels = shader_fn(gbuffer, *shader_additional_inputs)
+        pixels = shader_fn(gbuffer, *shader_additional_inputs, **extra)
     if pixels.dim() != 4 or pixels.shape[:3] != gbuffer.shape[:3]:
         raise ValueError('shader_fn must return pixels of shape [height, width, channels] per image')
     pixels = _InjectVertexGradient.apply(pixels.to(torch.float32), vertices, faces, face_ids, holder)
     return pixels[0] if single_or_batch == 'single' else pixels
 
 
-def rasterise_deferred(background_attributes, vertices, vertex_attributes, faces, shader_fn, shader_additional_inputs=[], name=None):
+def rasterise_deferred(background_attributes, vertices, vertex_attributes, faces, shader_fn, shader_additional_inputs=[], name=None,
+                       derivative_channels=None):
     """Rasterises a G-buffer of vertex attributes and shades it with `shader_fn` (dirt/rasterise_ops.py:260-310).
 
     Equivalent to `shader_fn(rasterise(background_attributes, vertices, vertex_attributes, faces), *shader_additional_inputs)`
     in the forward direction; the gradient w.r.t. `vertices` is computed from the SHADED pixels, the gradients
     w.r.t. attributes / background from the G-buffer through `shader_fn`.
+
+    `derivative_channels`: optional, one ascending run of consecutive attribute channels, such as range(1, 3).  Then
+    `shader_fn` is called as `shader_fn(gbuffer, *shader_additional_inputs, gbuffer_derivatives=d)`, with d float32
+    [H, W, 2, K] (K channels) the screen-space derivatives of those G-buffer channels at each pixel centre: d[..., 0, k]
+    along x (the columns, to the right), d[..., 1, k] along y (the rows, downwards), in attribute units per pixel,
+    exactly those of the perspective-correct interpolant of the face the pixel shows (no neighbour differences, so no
+    error at silhouettes or uv seams); 0 on the background.  They carry no gradient (DESIGN.md §7.7).  For uv
+    channels u, u + 1 read with `uvs_to_pixel_indices(..., mode='repeat')` from a TH x TW texture, the derivatives
+    `sample_texture(..., mode='trilinear')` takes are
+        (d[..., :, u:u+2].flip(-1) * torch.tensor([TH, TW], device=d.device)).flatten(-2)
+    = (d row / dx, d col / dx, d row / dy, d col / dy).  Without it nothing else is computed or passed.
     """
     return _rasterise_deferred_internal(background_attributes, vertices, vertex_attributes, faces, shader_fn,
-                                        list(shader_additional_inputs), 'single', name)
+                                        list(shader_additional_inputs), 'single', name, derivative_channels)
 
 
-def rasterise_batch_deferred(background_attributes, vertices, vertex_attributes, faces, shader_fn, shader_additional_inputs=[], name=None):
-    """Batched `rasterise_deferred` (dirt/rasterise_ops.py:313-333)."""
+def rasterise_batch_deferred(background_attributes, vertices, vertex_attributes, faces, shader_fn, shader_additional_inputs=[], name=None,
+                             derivative_channels=None):
+    """Batched `rasterise_deferred` (dirt/rasterise_ops.py:313-333).  With `derivative_channels`, `gbuffer_derivatives`
+    is [B, H, W, 2, K]."""
     return _rasterise_deferred_internal(background_attributes, vertices, vertex_attributes, faces, shader_fn,
-                                        list(shader_additional_inputs), 'batch', name)
+                                        list(shader_additional_inputs), 'batch', name, derivative_channels)

@@ -162,6 +162,28 @@ int dirt_rasterise_visibility(const float* vertices, const int32_t* faces,
                               int B, int H, int W, int V, int F,
                               void* workspace, size_t workspace_bytes, void* cuda_stream);
 
+/* Screen-space derivatives of G-buffer attributes (DESIGN.md §7.7), e.g. uv footprints for a trilinear texture lookup.
+ *   attributes   float32 [B, V, C]: the vertex attributes of a forward call (its vertex_colors)
+ *   face_ids     int32 [B, H, W]: that call's face_ids_out (required)
+ *   derivatives  float32 [B, H, W, 2, channel_count]: for channels c in [first_channel, first_channel + channel_count),
+ *                index 0 of the `2` axis is d a_c / dx (x along W, to the right), index 1 d a_c / dy (y along H,
+ *                downwards), in attribute units per pixel at the pixel centre, a_c being the perspective-correct
+ *                interpolant of the attributes of the face the pixel shows.  A pixel whose id is not in [0, F) gets 0.
+ * The values come from the face's interpolation planes in the workspace (the G-buffer's own), with b_k = q_k / S:
+ *   d a / dx = ((a0 - a2) (q0A - b0 sA) + (a1 - a2) (q1A - b1 sA)) / S, and the same with the B coefficients for y.
+ * No gradient, no atomics: two calls on the same inputs give bit-identical outputs.
+ * workspace_holds_setup means what it means for dirt_rasterise_backward: != 0 reuses the setup records of the forward
+ * call on the same (vertices, faces, H, W) in `workspace` (checked on the device; a workspace of other geometry sets the
+ * error dirt_workspace_status reports and every output is NaN); 0 recomputes them there first.
+ * An empty channel range or one outside [0, C) is DIRT_ERR_BAD_SHAPE.  B = 0: nothing is launched.  All pointers 4-byte
+ * aligned (vertices 16); derivatives 8- (one channel) or 16-byte aligned (two or four) enable the vector stores.  Only
+ * enqueues work on cuda_stream. */
+int dirt_rasterise_derivatives(const float* vertices, const int32_t* faces, const float* attributes,
+                               const int32_t* face_ids, float* derivatives,
+                               int B, int H, int W, int C, int V, int F,
+                               int first_channel, int channel_count,
+                               int workspace_holds_setup, void* workspace, size_t workspace_bytes, void* cuda_stream);
+
 /* Multi-GPU (one process per GPU, one node): sum over the ranks of the batch-shared vertex gradient -- the [V,4 | V,C] buffer
  * a DIRT_BWD_SHARED_GEOMETRY call fills -- over peer memory, as ONE kernel of `world` CTAs per rank and step: every rank
  * pushes its buffer into its slot of every peer's exchange area (stores through the NVLink peer mapping), releases a flag
