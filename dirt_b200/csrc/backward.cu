@@ -28,8 +28,7 @@
 //      of the fragment) keyed by the possibly dilated face.  The warp loops over the occupied slots and reduces the
 //      3*(C+3) sums of each face over its 32 lanes with a transposed butterfly (every lane ends up owning one finished
 //      sum): ONE warp-wide RED per (face, tile) instead of the reference's atomicAdd per pixel per term
-//      (csrc/rasterise_grad_egl.cu:139,227-229).  Faces with only a few records in the tile skip the butterfly
-//      (vector REDs).
+//      (csrc/rasterise_grad_egl.cu:139,227-229).
 //  A tile with more distinct faces than the table holds takes the reference-shaped path (one atomic per term).
 #include "common.cuh"
 #include "grad_pixel.cuh"
@@ -43,10 +42,8 @@ namespace dirt {
 #define DIRT_BWD_WARPS 4
 #endif
 #ifndef DIRT_ABLATE
-#define DIRT_ABLATE 0   // timing experiments only: 1 = no per-face reduction, 2 = no Scharr/dilation, 3 = both
-#endif
-#ifndef DIRT_BWD_SMALL_FACE
-#define DIRT_BWD_SMALL_FACE 20  // faces owning at most this many records in a tile are added directly (0: always reduce)
+#define DIRT_ABLATE 0   // timing experiments only: 1 = no per-face reduction, 2 = no Scharr/dilation, 3 = both,
+                        // 4 = stop once the face table and the G-buffer tile are filled (the front end alone)
 #endif
 #ifndef DIRT_BWD_MIN_BLOCKS
 #define DIRT_BWD_MIN_BLOCKS 6   // x 4 warps: <= 80 registers; on H100 faster than 8 / 5 blocks at every workload (DESIGN.md section 5)
@@ -120,12 +117,6 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
     asm volatile(
         "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
         ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(x), "r"(y), "r"(z), "r"(smem_u32(bar)) : "memory");
-}
-
-// 16-byte vector reduction to global memory (sm_90+): four fp32 adds in one RED
-__device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d)
-{
-    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
 }
 
 // ---- the warp's slice of shared memory ----------------------------------------------------------------------------
@@ -637,6 +628,9 @@ __global__ void __launch_bounds__(NW * 32, DIRT_BWD_MIN_BLOCKS * DIRT_BWD_WARPS 
         gbuf[ring_r * GB_COLS + ring_c] = gr;
     }
     __syncwarp();
+#if DIRT_ABLATE == 4
+    return;
+#endif
 
     // ---- dilation and per-pixel terms ---------------------------------------------------------------------------------------
     const float halfW = 0.5f * (float)W, halfH = 0.5f * (float)H;
@@ -766,17 +760,17 @@ __global__ void __launch_bounds__(NW * 32, DIRT_BWD_MIN_BLOCKS * DIRT_BWD_WARPS 
 
     // ---- (4) per-face reduction -----------------------------------------------------------------------------------------
     // One iteration per occupied slot: the 3*(C+3) sums of the face are reduced over the 32 lanes with a transposed
-    // butterfly (each lane ends up owning one finished sum) and leave the SM as ONE warp-wide RED.  Faces that own only a
-    // few records in this tile skip the butterfly: their records are added directly, all such faces of the tile together,
-    // in one pass of vector REDs at the end.
-#if DIRT_ABLATE != 1
+    // butterfly (each lane ends up owning one finished sum) and leave the SM as ONE warp-wide RED, however few records
+    // the face owns in this tile.  (Adding the records of faces with at most 20 of them directly, as vector REDs, made
+    // the kernel 6-9 % slower on the H100 at cfg3, cfg4 and cfg5: those REDs, up to 12 per lane, cost more than the
+    // butterfly, DESIGN.md section 5.)
+#if DIRT_ABLATE != 1 && DIRT_ABLATE != 3
     {
         const int owner = owner_meta<C>(lane);
         // destination of this lane's finished sum: component (owner >> 2) & 3 of row `vid` of grad_vertices / grad_vertex_colors
         float* const owner_row = ((owner & 16) ? gverts : gcols) + ((owner >> 2) & 3);
         const int owner_stride = (owner & 16) ? 4 : (C == 4 ? 4 : gstride);
         const int kc0 = term[0].key_col, kc1 = term[1].key_col, kp0 = term[0].key_pos, kp1 = term[1].key_pos;
-        unsigned direct = 0;   // bit 0/1: colour record of pixel 0/1, bit 2/3: position record of pixel 0/1
         // slots that own at least one record of this tile (faces of the ring that nothing dilates from own none)
         unsigned occupied = __reduce_or_sync(0xffffffffu, (kc0 >= 0 ? 1u << kc0 : 0u) | (kc1 >= 0 ? 1u << kc1 : 0u) |
                                                               (kp0 >= 0 ? 1u << kp0 : 0u) | (kp1 >= 0 ? 1u << kp1 : 0u));
@@ -784,13 +778,6 @@ __global__ void __launch_bounds__(NW * 32, DIRT_BWD_MIN_BLOCKS * DIRT_BWD_WARPS 
             const int s = __ffs(occupied) - 1;
             occupied &= occupied - 1;
             const bool mc0 = kc0 == s, mc1 = kc1 == s, mp0 = kp0 == s, mp1 = kp1 == s;
-#if DIRT_BWD_SMALL_FACE > 0
-            const unsigned records = __reduce_add_sync(0xffffffffu, (unsigned)mc0 + (unsigned)mc1 + (unsigned)mp0 + (unsigned)mp1);
-            if (records <= DIRT_BWD_SMALL_FACE) {
-                direct |= (mc0 ? 1u : 0u) | (mc1 ? 2u : 0u) | (mp0 ? 4u : 0u) | (mp1 ? 8u : 0u);
-                continue;
-            }
-#endif
             // First butterfly step at operand level: this lane keeps the NS sums of vertex A and hands those of vertex B
             // to lane^16 (the weights were arranged per half-warp when they were stored), and the halves swap one half
             // each of the NS sums of vertex 2.  The remaining steps are the generic transposed butterfly.
@@ -827,41 +814,12 @@ __global__ void __launch_bounds__(NW * 32, DIRT_BWD_MIN_BLOCKS * DIRT_BWD_WARPS 
                 atomicAdd(owner_row + (size_t)vid * owner_stride, total[0]);
             }
         }
-#if DIRT_BWD_SMALL_FACE > 0
-        if (__any_sync(0xffffffffu, direct != 0u)) {
-#pragma unroll
-            for (int rec = 0; rec < 4; ++rec) {
-                if (!(direct & (1u << rec))) continue;
-                const int pix = rec & 1;
-                const PixelTerms& T = term[pix];
-                const bool colour = rec < 2;
-                const int s = colour ? T.key_col : T.key_pos;
-                const int4 q = reinterpret_cast<const int4*>(table + s)[2];
-                const int vid[3] = {q.y, q.z, q.w};
-                const float wA = colour ? T.cA : T.pA, wB = colour ? T.cB : T.pB;
-                const float w[3] = {upper ? wB : wA, upper ? wA : wB, colour ? T.c2 : T.p2};
-#pragma unroll
-                for (int k = 0; k < 3; ++k) {
-                    if (colour) {
-                        if (C == 4) red_add_v4(gcols + (size_t)vid[k] * 4, w[k] * sc[pix][0], w[k] * sc[pix][1 % NS], w[k] * sc[pix][2 % NS], w[k] * sc[pix][3 % NS]);
-                        else if (C == 3 && cs == 3 && gstride == 4) red_add_v4(gcols + (size_t)vid[k] * 4, w[k] * sc[pix][0], w[k] * sc[pix][1 % NS], w[k] * sc[pix][2 % NS], 0.f);
-                        else {
-#pragma unroll
-                            for (int j = 0; j < C; ++j) atomicAdd(gcols + (size_t)vid[k] * gstride + j, w[k] * sc[pix][j]);
-                        }
-                    } else {
-                        red_add_v4(gverts + (size_t)vid[k] * 4, w[k] * sc[pix][C], w[k] * sc[pix][C + 1], 0.f, w[k] * sc[pix][C + 2]);
-                    }
-                }
-            }
-        }
-#endif
     }
 #endif
 }
 
-// grad_vertex_colors of a 3-channel launch is accumulated in 16-byte rows (one vector RED per vertex instead of three
-// scalar ones) and brought to its [.,3] layout afterwards
+// grad_vertex_colors of a 3-channel launch is accumulated in 16-byte rows of the workspace and brought to its [.,3]
+// layout afterwards
 __global__ void __launch_bounds__(256) unpad_rows_kernel(const float* __restrict__ in, float* __restrict__ out, long long rows)
 {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;   // one output element
