@@ -110,6 +110,13 @@ def load(path):
     L.dirt_lighting_forward.argtypes = light_inputs + [vp, i, ll, i, vp]
     L.dirt_lighting_backward.restype = i
     L.dirt_lighting_backward.argtypes = light_inputs + [vp] * 9 + [sz, i, ll, i, vp]
+    sh_inputs = [vp, ll, vp, ll, vp, i]
+    L.dirt_sh_lighting_workspace_bytes.restype = sz
+    L.dirt_sh_lighting_workspace_bytes.argtypes = [i, ll, i]
+    L.dirt_sh_lighting_forward.restype = i
+    L.dirt_sh_lighting_forward.argtypes = sh_inputs + [vp, i, ll, i, vp]
+    L.dirt_sh_lighting_backward.restype = i
+    L.dirt_sh_lighting_backward.argtypes = sh_inputs + [vp] * 5 + [sz, i, ll, i, vp]
     L.dirt_normals_workspace_bytes.restype = sz
     L.dirt_normals_workspace_bytes.argtypes = [i, ll, ll]
     L.dirt_normals_forward.restype = i
@@ -130,7 +137,8 @@ EXPORTED_SYMBOLS = ['dirt_error_string', 'dirt_abi_version', 'dirt_workspace_byt
                     'dirt_texture_sample_backward_deterministic', 'dirt_texture_mip_levels',
                     'dirt_texture_mip_pyramid_bytes', 'dirt_texture_mip_build', 'dirt_texture_sample_trilinear',
                     'dirt_texture_sample_trilinear_backward_bytes', 'dirt_texture_sample_trilinear_backward',
-                    'dirt_rasterise_derivatives']
+                    'dirt_rasterise_derivatives', 'dirt_sh_lighting_workspace_bytes', 'dirt_sh_lighting_forward',
+                    'dirt_sh_lighting_backward']
 
 
 def error_string(code):

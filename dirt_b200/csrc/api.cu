@@ -632,6 +632,92 @@ extern "C" int dirt_lighting_backward(int model, int double_sided, const float* 
     return DIRT_OK;
 }
 
+// element offsets of every per-point buffer stay below 2^62, the chunk count within the grid's x limit, 9*C an int
+static bool sh_shape_ok(int B, long long V, int C, long long sn, long long sa)
+{
+    if (B < 0 || V < 0 || C <= 0 || C > (1 << 26) || sn < 0 || sa < 0) return false;
+    const double limit = 4.0e18, rows = (double)B * V;
+    const double widest = (double)(C > 3 ? C : 3) + sn + sa;
+    if (rows * widest > limit || light_chunks(V) > 0x7fffffffll) return false;
+    if ((double)B * sh_chunks(V) * 9.0 * C * sizeof(float) > limit) return false;
+    return true;
+}
+
+extern "C" size_t dirt_sh_lighting_workspace_bytes(int B, long long V, int C)
+{
+    if (B <= 0 || V <= 0 || C <= 0) return 0;
+    return sizeof(float) * (size_t)B * (size_t)sh_chunks(V) * (size_t)(9 * (size_t)C);
+}
+
+static ShArgs make_sh_args(const float* normals, long long sn, const float* albedo, long long sa, const float* coefficients,
+                           int coefficients_per_item, int B, long long V, int C)
+{
+    ShArgs a = {};
+    a.normals = normals; a.albedo = albedo; a.coefficients = coefficients;
+    a.sn = sn; a.sa = sa;
+    a.item_coef = coefficients_per_item != 0;
+    a.V = V; a.B = B; a.C = C; a.chunks = (int)sh_chunks(V);
+    return a;
+}
+
+static int sh_inputs_check(const ShArgs& a)
+{
+    if (!a.normals || !a.albedo || !a.coefficients) return DIRT_ERR_NULL_POINTER;
+    if ((uintptr_t)a.normals % 4 || (uintptr_t)a.albedo % 4 || (uintptr_t)a.coefficients % 4) return DIRT_ERR_MISALIGNED;
+    return DIRT_OK;
+}
+
+extern "C" int dirt_sh_lighting_forward(const float* normals, long long normals_stride, const float* albedo,
+                                        long long albedo_stride, const float* coefficients, int coefficients_per_item,
+                                        float* out, int B, long long V, int C, void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (!sh_shape_ok(B, V, C, normals_stride, albedo_stride)) return DIRT_ERR_BAD_SHAPE;
+    if ((long long)B * V == 0) return DIRT_OK;
+    ShArgs a = make_sh_args(normals, normals_stride, albedo, albedo_stride, coefficients, coefficients_per_item, B, V, C);
+    a.out = out;
+    const int rc = sh_inputs_check(a);
+    if (rc != DIRT_OK) return rc;
+    if (!out) return DIRT_ERR_NULL_POINTER;
+    if ((uintptr_t)out % 4) return DIRT_ERR_MISALIGNED;
+    CUDA_TRY(launch_sh_lighting_forward(a, (cudaStream_t)cuda_stream, &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
+extern "C" int dirt_sh_lighting_backward(const float* normals, long long normals_stride, const float* albedo,
+                                         long long albedo_stride, const float* coefficients, int coefficients_per_item,
+                                         const float* grad_out, float* grad_normals, float* grad_albedo,
+                                         float* grad_coefficients, void* workspace, size_t workspace_bytes, int B,
+                                         long long V, int C, void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (!sh_shape_ok(B, V, C, normals_stride, albedo_stride)) return DIRT_ERR_BAD_SHAPE;
+    ShArgs a = make_sh_args(normals, normals_stride, albedo, albedo_stride, coefficients, coefficients_per_item, B, V, C);
+    a.grad_out = grad_out;
+    a.g_normals = grad_normals; a.g_albedo = grad_albedo; a.g_coef = grad_coefficients;
+    if ((uintptr_t)grad_normals % 4 || (uintptr_t)grad_albedo % 4 || (uintptr_t)grad_coefficients % 4)
+        return DIRT_ERR_MISALIGNED;
+    if ((long long)B * V > 0 && (grad_normals || grad_albedo || grad_coefficients)) {
+        const int rc = sh_inputs_check(a);
+        if (rc != DIRT_OK) return rc;
+        if (!grad_out) return DIRT_ERR_NULL_POINTER;
+        if ((uintptr_t)grad_out % 4) return DIRT_ERR_MISALIGNED;
+        if (grad_coefficients) {
+            if (!workspace) return DIRT_ERR_NULL_POINTER;
+            if ((uintptr_t)workspace % 4) return DIRT_ERR_MISALIGNED;
+            if (workspace_bytes < dirt_sh_lighting_workspace_bytes(B, V, C)) return DIRT_ERR_WORKSPACE_TOO_SMALL;
+            a.partial = static_cast<float*>(workspace);
+        }
+    }
+    // with no points only the memset of a wanted coefficient gradient is enqueued
+    CUDA_TRY(launch_sh_lighting_backward(a, (cudaStream_t)cuda_stream, &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
 // element offsets of the vertex rows stay below 2^62; vertex ids and incidence ids (k*F + f) are int32
 static bool normals_shape_ok(int mode, int B, long long V, long long F, long long stride)
 {

@@ -9,6 +9,9 @@
 // camera, shininess) are summed without atomics: each CTA writes its sums to its own row of the partials, then one
 // small kernel adds the rows of each item (or of all items, for a shared parameter) in a fixed order.  Two calls on the
 // same inputs therefore give bit-identical parameter gradients.
+//
+// The file also holds the spherical-harmonics environment lighting (dirt_sh_lighting_forward / _backward, DESIGN.md
+// §7.8), which uses the same staging, per-CTA partials and reduction kernel.
 #include "../../include/dirt_b200.h"
 #include "common.cuh"
 
@@ -455,6 +458,229 @@ cudaError_t launch_lighting_backward(const LightArgs& a, cudaStream_t stream, in
         const unsigned blocks = (unsigned)(total < (1ll << 20) ? total : (1ll << 20));
         lighting_reduce_kernel<<<blocks, REDUCE_THREADS, 0, stream>>>(b.partial, jobs, total, a.chunks, a.B,
                                                                       LIGHT_FIXED_PARAMS + a.C);
+        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+        ++*launches;
+    }
+    return cudaSuccess;
+}
+
+// ---- spherical-harmonics environment lighting (dirt_sh_lighting_*, DESIGN.md §7.8) ------------------------------------
+//
+// out_c = albedo_c * E_c, E_c = sum_k (w_l(k) * L_kc) * Y_k(n): the real order-2 SH basis (no Condon-Shortley phase) of
+// the normal as given, band weights 1, 2/3, 1/4 (the clamped cosine's A_l / pi).  The forward pass is laid out as
+// lighting_forward_kernel.  In the backward pass each thread takes SH_POINTS_PER_THREAD points of its item, 256 apart,
+// and (C = 3) keeps its sums of the 27 coefficient gradients in registers until one CTA reduction, so the butterflies
+// are paid once per SH_CHUNK points instead of once per 256.  The partials are reduced by lighting_reduce_kernel.
+
+namespace {
+
+constexpr float SH_K0 = 0.28209479177387814f, SH_K1 = 0.4886025119029199f, SH_K2 = 1.0925484305920792f,
+                SH_K3 = 0.31539156525252005f, SH_K4 = 0.5462742152960396f;
+
+__device__ __forceinline__ float sh_band_weight(int k) { return k == 0 ? 1.f : (k < 4 ? 2.f / 3.f : 0.25f); }
+
+// Y_k(n), k = l^2 + l + m, each product in the restatement's order
+__device__ __forceinline__ void sh_basis(const float n[3], float Y[9])
+{
+    const float x = n[0], y = n[1], z = n[2];
+    Y[0] = SH_K0;
+    Y[1] = __fmul_rn(SH_K1, y);
+    Y[2] = __fmul_rn(SH_K1, z);
+    Y[3] = __fmul_rn(SH_K1, x);
+    Y[4] = __fmul_rn(__fmul_rn(SH_K2, x), y);
+    Y[5] = __fmul_rn(__fmul_rn(SH_K2, y), z);
+    Y[6] = __fmul_rn(SH_K3, __fsub_rn(__fmul_rn(__fmul_rn(3.f, z), z), 1.f));
+    Y[7] = __fmul_rn(__fmul_rn(SH_K2, x), z);
+    Y[8] = __fmul_rn(SH_K4, __fsub_rn(__fmul_rn(x, x), __fmul_rn(y, y)));
+}
+
+// E_c = sum_k (w_k L_kc) Y_k in the fixed order k = 0 .. 8; L: the item's [9, C] coefficients (read-only path)
+__device__ __forceinline__ float sh_irradiance(const float* __restrict__ L, int C, int c, const float Y[9])
+{
+    float e = __fmul_rn(__ldg(L + c), Y[0]);
+#pragma unroll
+    for (int k = 1; k < 9; ++k) e = __fmaf_rn(__fmul_rn(sh_band_weight(k), __ldg(L + k * C + c)), Y[k], e);
+    return e;
+}
+
+// d/dn of sum_k s_k Y_k(n)  (s_0 has no derivative)
+__device__ __forceinline__ void sh_normal_grad(const float n[3], const float s[9], float g[3])
+{
+    const float x = n[0], y = n[1], z = n[2];
+    g[0] = SH_K1 * s[3] + SH_K2 * (y * s[4] + z * s[7]) + (2.f * SH_K4) * (x * s[8]);
+    g[1] = SH_K1 * s[1] + SH_K2 * (x * s[4] + z * s[5]) - (2.f * SH_K4) * (y * s[8]);
+    g[2] = SH_K1 * s[2] + SH_K2 * (y * s[5] + x * s[7]) + (6.f * SH_K3) * (z * s[6]);
+}
+
+__device__ __forceinline__ const float* sh_item(const ShArgs& a, long long b, int C)
+{
+    return a.coefficients + (a.item_coef ? b * 9 * C : 0);
+}
+
+// CT = 3 (albedo and outputs staged like the normals) or 0 (any C, one channel at a time)
+template <int CT>
+__global__ void __launch_bounds__(LIGHT_THREADS) sh_forward_kernel(ShArgs a)
+{
+    __shared__ float stage[LIGHT_THREADS * 3];
+    const int lane = threadIdx.x & 31;
+    float* s = stage + (threadIdx.x & ~31) * 3;
+    const long long v0 = (long long)blockIdx.x * LIGHT_THREADS + (threadIdx.x & ~31);
+    if (v0 >= a.V) return;   // the whole warp
+    const int n = (int)(a.V - v0 < 32 ? a.V - v0 : 32);
+    const int C = CT ? CT : a.C;
+    for (long long b = blockIdx.y; b < a.B; b += gridDim.y) {
+        const long long row0 = b * a.V + v0, row = row0 + lane;
+        const float* L = sh_item(a, b, C);
+        float nrm[3], Y[9];
+        stage_load<3>(a.normals, a.sn, row0, n, s, lane, nrm);
+        sh_basis(nrm, Y);
+        if (CT == 3) {
+            float k[3], o[3];
+            stage_load<3>(a.albedo, a.sa, row0, n, s, lane, k);
+#pragma unroll
+            for (int c = 0; c < 3; ++c) o[c] = __fmul_rn(k[c], sh_irradiance(L, 3, c, Y));
+            stage_store<3>(a.out, row0, n, s, lane, o);
+        } else if (lane < n) {
+            for (int c = 0; c < C; ++c)
+                a.out[row * C + c] = __fmul_rn(__ldg(a.albedo + row * a.sa + c), sh_irradiance(L, C, c, Y));
+        }
+    }
+}
+
+// grad_albedo_c = g_c E_c;  grad_n = sum_c g_c albedo_c dE_c/dn;  grad_L_kc = sum over points of g_c albedo_c w_k Y_k,
+// each CTA's sum to its own row of the partials (lanes without a point add zeros)
+template <int CT>
+__global__ void __launch_bounds__(LIGHT_THREADS) sh_backward_kernel(ShArgs a)
+{
+    __shared__ float stage[LIGHT_THREADS * 3];
+    __shared__ float red[WARPS * RED_SLOTS];
+    constexpr int NACC = CT == 3 ? 27 : 1;
+    const int lane = threadIdx.x & 31;
+    float* s = stage + (threadIdx.x & ~31) * 3;
+    const int C = CT ? CT : a.C;
+    const long long first = (long long)blockIdx.x * SH_CHUNK + (threadIdx.x & ~31);   // the warp's first point
+    for (long long b = blockIdx.y; b < a.B; b += gridDim.y) {
+        const float* L = sh_item(a, b, C);
+        float acc[NACC];
+#pragma unroll
+        for (int j = 0; j < NACC; ++j) acc[j] = 0.f;
+        for (int p = 0; p < SH_POINTS_PER_THREAD; ++p) {
+            const long long v0 = first + (long long)p * LIGHT_THREADS;
+            if (v0 >= a.V) break;   // warp-uniform
+            const int n = (int)(a.V - v0 < 32 ? a.V - v0 : 32);
+            const bool live = lane < n;
+            const long long row0 = b * a.V + v0, row = row0 + lane;
+            float nrm[3], Y[9], sk[9];
+            stage_load<3>(a.normals, a.sn, row0, n, s, lane, nrm);
+            if (!live) nrm[0] = nrm[1] = nrm[2] = 0.f;
+            sh_basis(nrm, Y);
+#pragma unroll
+            for (int k = 0; k < 9; ++k) sk[k] = 0.f;
+            if (CT == 3) {
+                float g[3], k3[3], ga[3];
+                stage_load<3>(a.grad_out, 3, row0, n, s, lane, g);
+                stage_load<3>(a.albedo, a.sa, row0, n, s, lane, k3);
+#pragma unroll
+                for (int c = 0; c < 3; ++c) {
+                    const float h = live ? g[c] * k3[c] : 0.f;
+                    if (a.g_albedo) ga[c] = g[c] * sh_irradiance(L, 3, c, Y);
+#pragma unroll
+                    for (int k = 0; k < 9; ++k) {
+                        const float w = sh_band_weight(k);
+                        sk[k] += h * (w * __ldg(L + k * 3 + c));
+                        acc[k * 3 + c] += h * (w * Y[k]);
+                    }
+                }
+                if (a.g_albedo) stage_store<3>(a.g_albedo, row0, n, s, lane, ga);
+            } else if (live) {
+                for (int c = 0; c < C; ++c) {
+                    const float g = __ldg(a.grad_out + row * C + c), h = g * __ldg(a.albedo + row * a.sa + c);
+                    if (a.g_albedo) a.g_albedo[row * C + c] = g * sh_irradiance(L, C, c, Y);
+#pragma unroll
+                    for (int k = 1; k < 9; ++k) sk[k] += h * (sh_band_weight(k) * __ldg(L + k * C + c));
+                }
+            }
+            if (a.g_normals) {
+                float gn[3];
+                sh_normal_grad(nrm, sk, gn);
+                stage_store<3>(a.g_normals, row0, n, s, lane, gn);
+            }
+        }
+        if (a.partial) {
+            float* dst = a.partial + ((long long)b * a.chunks + blockIdx.x) * (9 * C);
+            if (CT == 3) {
+#pragma unroll
+                for (int r = 0; r < 6; ++r) cta_partial<4>(acc + 4 * r, red, dst + 4 * r);
+                cta_partial<3>(acc + 24, red, dst + 24);
+            } else {
+                // one channel at a time: the thread's points again (their rows are still in cache), then 9 reductions
+                for (int c = 0; c < C; ++c) {
+                    float a9[9];
+#pragma unroll
+                    for (int k = 0; k < 9; ++k) a9[k] = 0.f;
+                    for (int p = 0; p < SH_POINTS_PER_THREAD; ++p) {
+                        const long long v = first + (long long)p * LIGHT_THREADS + lane;
+                        if (v >= a.V) break;
+                        const long long row = b * a.V + v;
+                        const float* np = a.normals + row * a.sn;
+                        const float nrm[3] = {__ldg(np), __ldg(np + 1), __ldg(np + 2)};
+                        float Y[9];
+                        sh_basis(nrm, Y);
+                        const float h = __ldg(a.grad_out + row * C + c) * __ldg(a.albedo + row * a.sa + c);
+#pragma unroll
+                        for (int k = 0; k < 9; ++k) a9[k] += h * (sh_band_weight(k) * Y[k]);
+                    }
+#pragma unroll
+                    for (int k = 0; k < 9; ++k) cta_partial<1>(a9 + k, red, dst + k * C + c);
+                }
+            }
+        }
+    }
+}
+
+inline dim3 sh_grid(long long chunks, int B)
+{
+    return dim3((unsigned)chunks, (unsigned)(B < (int)MAX_ITEMS_PER_GRID ? B : (int)MAX_ITEMS_PER_GRID));
+}
+
+}  // namespace
+
+cudaError_t launch_sh_lighting_forward(const ShArgs& a, cudaStream_t stream, int* launches)
+{
+    if ((long long)a.B * a.V == 0) return cudaSuccess;
+    const dim3 grid = sh_grid(light_chunks(a.V), a.B);
+    if (a.C == 3) sh_forward_kernel<3><<<grid, LIGHT_THREADS, 0, stream>>>(a);
+    else sh_forward_kernel<0><<<grid, LIGHT_THREADS, 0, stream>>>(a);
+    const cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) ++*launches;
+    return e;
+}
+
+cudaError_t launch_sh_lighting_backward(const ShArgs& a, cudaStream_t stream, int* launches)
+{
+    const long long width = 9ll * a.C, total = (a.item_coef ? (long long)a.B : 1ll) * width;
+    cudaError_t e;
+    if ((long long)a.B * a.V == 0) {
+        if (a.g_coef && total && (e = cudaMemsetAsync(a.g_coef, 0, sizeof(float) * (size_t)total, stream)) != cudaSuccess)
+            return e;
+        return cudaSuccess;
+    }
+    if (!a.g_normals && !a.g_albedo && !a.g_coef) return cudaSuccess;
+    ShArgs b = a;
+    if (!a.g_coef) b.partial = nullptr;
+    const dim3 grid = sh_grid(a.chunks, a.B);
+    if (a.C == 3) sh_backward_kernel<3><<<grid, LIGHT_THREADS, 0, stream>>>(b);
+    else sh_backward_kernel<0><<<grid, LIGHT_THREADS, 0, stream>>>(b);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    ++*launches;
+    if (a.g_coef) {
+        // one job: the [9, C] columns of the partials, per item or over every item
+        ReduceJobs jobs = {};
+        jobs.count = 1;
+        jobs.out[0] = a.g_coef; jobs.offset[0] = 0; jobs.width[0] = (int)width; jobs.per_item[0] = a.item_coef;
+        jobs.first[0] = 0; jobs.first[1] = total;
+        const unsigned blocks = (unsigned)(total < (1ll << 20) ? total : (1ll << 20));
+        lighting_reduce_kernel<<<blocks, REDUCE_THREADS, 0, stream>>>(b.partial, jobs, total, a.chunks, a.B, (int)width);
         if ((e = cudaGetLastError()) != cudaSuccess) return e;
         ++*launches;
     }

@@ -5,7 +5,9 @@ include/dirt_b200.h) when their vertices are float32 on a CUDA device in the sha
 torch restatements (`_vertex_normals`, `_vertex_normals_pre_split`) otherwise; see DESIGN.md §7.3.  The three
 reflectance models run CUDA kernels (dirt_lighting_forward / _backward) when their inputs are on one CUDA device in the
 shapes `cuda_route` accepts, and their torch restatements (`_diffuse_directional`, `_specular_directional`,
-`_diffuse_point`) otherwise; see DESIGN.md §7.2.  `split_vertices_by_face` is torch code.
+`_diffuse_point`) otherwise; see DESIGN.md §7.2.  `diffuse_spherical_harmonics` (order-2 SH environment lighting) is
+routed the same way, between dirt_sh_lighting_forward / _backward and `_diffuse_spherical_harmonics`; see DESIGN.md
+§7.8.  `split_vertices_by_face` is torch code.
 """
 import math
 from collections import namedtuple
@@ -114,6 +116,28 @@ def _diffuse_point(vertex_positions, vertex_normals, vertex_colors, light_positi
     return light_color[..., None, :] * vertex_colors * _cosine_term(cosines, double_sided)[..., None]
 
 
+def _sh_basis(n):
+    """The real order-2 spherical harmonics without the Condon-Shortley phase at n [..., 3], used as given (not
+    normalised): [..., 9], index k = l^2 + l + m."""
+    x, y, z = n.unbind(-1)
+    return torch.stack([torch.full_like(x, 0.28209479177387814),
+                        0.4886025119029199 * y, 0.4886025119029199 * z, 0.4886025119029199 * x,
+                        1.0925484305920792 * x * y, 1.0925484305920792 * y * z, 0.31539156525252005 * (3 * z * z - 1),
+                        1.0925484305920792 * x * z, 0.5462742152960396 * (x * x - y * y)], dim=-1)
+
+
+def _diffuse_spherical_harmonics(vertex_normals, vertex_colors, coefficients):
+    """The torch restatement of `diffuse_spherical_harmonics`: its CPU implementation and its specification.
+    Takes tensors of one dtype and device, and keeps that dtype (the tests evaluate it in float64).
+
+    coefficients are the SH coefficients L_lm of the incident radiance; the result is Lambertian reflected radiance,
+    albedo * sum_k w_l(k) L_k Y_k(n), with the clamped cosine's band weights A_l / pi = 1, 2/3, 1/4."""
+    w = torch.tensor([1., 2 / 3, 2 / 3, 2 / 3, 0.25, 0.25, 0.25, 0.25, 0.25], dtype=coefficients.dtype,
+                     device=coefficients.device)
+    irradiance = torch.matmul(_sh_basis(vertex_normals), w[:, None] * coefficients)   # [*, V, C]
+    return vertex_colors * irradiance
+
+
 # ---- the CUDA path --------------------------------------------------------------------------------------------------
 
 Route = namedtuple('Route', 'lead B V C per_item')
@@ -123,9 +147,9 @@ def cuda_route(point_shapes, item_shapes, devices):
     """Whether a reflectance call runs the CUDA kernels, decided from shapes and devices alone.
 
     point_shapes: the shapes of the per-point tensors, colours (or reflectivities) last: [*, V, 3], ..., [*, V, C].
-    item_shapes: (shape, width) of each per-item tensor, width 3 (a direction or position), 'C' (the light colour) or 0
-        (the shininess, a scalar per item); each must have leading shape exactly `*` (one value per item) or none
-        (shared by all points).
+    item_shapes: (shape, width) of each per-item tensor, width 3 (a direction or position), 'C' (the light colour), 0
+        (the shininess, a scalar per item) or a tuple of those (the tail (9, 'C') of SH coefficients); each must have
+        leading shape exactly `*` (one value per item) or none (shared by all points).
     devices: the devices of all the tensors; they must be one CUDA device.
 
     Returns a Route (lead = `*`, B = its product, V, C, per_item flags in the order of item_shapes) or None."""
@@ -144,8 +168,11 @@ def cuda_route(point_shapes, item_shapes, devices):
             return None
     per_item = []
     for shape, width in item_shapes:
-        width = C if width == 'C' else width
-        tail = (width,) if width else ()
+        if isinstance(width, tuple):
+            tail = tuple(C if w == 'C' else w for w in width)
+        else:
+            width = C if width == 'C' else width
+            tail = (width,) if width else ()
         shape = tuple(shape)
         if shape == tail:
             per_item.append(False)
@@ -329,6 +356,80 @@ def diffuse_point(vertex_positions, vertex_normals, vertex_colors, light_positio
         return _diffuse_point(vertex_positions, vertex_normals, vertex_colors, light_position, light_color, double_sided)
     return _reflectance(_lib.LIGHT_DIFFUSE_POINT, double_sided, route, vertex_normals, vertex_colors, light_position,
                         light_color, vertex_positions)
+
+
+# ---- the CUDA path of the spherical-harmonics lighting --------------------------------------------------------------
+
+def _sh_inputs(route, normals, albedo, coefficients):
+    """The input arguments of dirt_sh_lighting_forward / _backward, in their order."""
+    stride = lambda t: t.stride(0) if t.shape[0] > 1 else 0
+    return [_ptr(normals), stride(normals), _ptr(albedo), stride(albedo), _ptr(coefficients), int(route.per_item[0])]
+
+
+class _SphericalHarmonics(torch.autograd.Function):
+    """dirt_sh_lighting_forward with its gradient.  normals [rows, 3] and albedo [rows, C] with unit stride along the row;
+    coefficients contiguous [B, 9, C] or shared [9, C].  The node keeps only its inputs: the backward kernel recomputes
+    the forward from them."""
+
+    @staticmethod
+    def forward(ctx, route, normals, albedo, coefficients):
+        out = torch.empty(route.lead + (route.V, route.C), dtype=torch.float32, device=normals.device)
+        with torch.cuda.device(normals.device):
+            rc = _lib.lib().dirt_sh_lighting_forward(*_sh_inputs(route, normals, albedo, coefficients), _ptr(out),
+                                                     route.B, route.V, route.C, _stream(normals.device))
+        _lib.check(rc, 'DiffuseSphericalHarmonics')
+        ctx.save_for_backward(normals, albedo, coefficients)
+        ctx.route = route
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        want = ctx.needs_input_grad[1:]
+        if not any(want):
+            return (None,) * 4
+        inputs = ctx.saved_tensors
+        route = ctx.route
+        if torch.is_grad_enabled():
+            # create_graph=True: differentiable gradients through the restatement
+            normals, albedo, coefficients = inputs
+            lead, V, C = route.lead, route.V, route.C
+            coef = coefficients.reshape(lead + (9, C)) if route.per_item[0] else coefficients
+            out = _diffuse_spherical_harmonics(normals.reshape(lead + (V, 3)), albedo.reshape(lead + (V, C)), coef)
+            wanted = [t for t, w in zip(inputs, want) if w]
+            grads = iter(torch.autograd.grad(out, wanted, grad_out, create_graph=True))
+            return (None,) + tuple(next(grads) if w else None for w in want)
+        dev = inputs[0].device
+        grads = [torch.empty(t.shape, dtype=torch.float32, device=dev) if w else None for t, w in zip(inputs, want)]
+        lib = _lib.lib()
+        ws_bytes = int(lib.dirt_sh_lighting_workspace_bytes(route.B, route.V, route.C)) if want[2] else 0
+        workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=dev) if ws_bytes else None
+        grad_out = grad_out.to(torch.float32).contiguous()
+        with torch.cuda.device(dev):
+            rc = lib.dirt_sh_lighting_backward(*_sh_inputs(route, *inputs), _ptr(grad_out), *[_ptr(g) for g in grads],
+                                               _ptr(workspace), ws_bytes, route.B, route.V, route.C, _stream(dev))
+        _lib.check(rc, 'DiffuseSphericalHarmonicsGrad')
+        return (None,) + tuple(grads)
+
+
+def diffuse_spherical_harmonics(vertex_normals, vertex_colors, coefficients, name=None):
+    """Lambertian reflectance under an environment given as order-2 spherical harmonics (Ramamoorthi & Hanrahan 2001).
+
+    vertex_normals [*, V, 3] (used as given, not normalised), vertex_colors [*, V, C] (the albedo), coefficients
+    [*, 9, C] (one set per item) or [9, C] (shared): the SH coefficients L_lm of the incident radiance, k = l^2 + l + m,
+    real basis without the Condon-Shortley phase -> [*, V, C] reflected radiance,
+    albedo * sum_k w_l(k) L_k Y_k(n) with w = (1, 2/3, 1/4).  A uniform environment of radiance 1 is
+    L = (2 sqrt(pi), 0, ..., 0) and returns the albedo.  On CUDA in these shapes a fused kernel computes it, with a
+    bit-reproducible coefficient gradient; any other call runs the torch restatement."""
+    vertex_normals = torch.as_tensor(vertex_normals, dtype=torch.float32)
+    dev = vertex_normals.device
+    vertex_colors = torch.as_tensor(vertex_colors, dtype=torch.float32, device=dev)
+    coefficients = torch.as_tensor(coefficients, dtype=torch.float32, device=dev)
+    route = _route([vertex_normals, vertex_colors], [(coefficients, (9, 'C'))])
+    if route is None:
+        return _diffuse_spherical_harmonics(vertex_normals, vertex_colors, coefficients)
+    C = route.C
+    coefficients = (coefficients.reshape((route.B, 9, C)) if route.per_item[0] else coefficients).contiguous()
+    return _SphericalHarmonics.apply(route, _rows(vertex_normals, 3), _rows(vertex_colors, C), coefficients)
 
 
 # ---- the CUDA path of the normals -----------------------------------------------------------------------------------

@@ -337,6 +337,40 @@ int dirt_lighting_backward(int model, int double_sided,
                            float* grad_light, float* grad_light_color, float* grad_camera, float* grad_shininess,
                            void* workspace, size_t workspace_bytes, int B, long long V, int C, void* cuda_stream);
 
+/* Spherical-harmonics environment lighting: Lambertian reflected radiance under order-2 SH incident radiance
+ * (Ramamoorthi & Hanrahan 2001), one value per point and channel.  B items of V points each, C channels:
+ *   normals              float32 [B*V, 3], row stride normals_stride floats, unit stride along the row; used as given
+ *                        (not normalised)
+ *   albedo               float32 [B*V, C], row stride albedo_stride
+ *   coefficients         float32 [B, 9, C] (coefficients_per_item != 0) or [9, C] (shared): L_kc, k = l^2 + l + m
+ *   out, grad_out        float32 [B*V, C], contiguous
+ * With n = (x, y, z), the real basis without the Condon-Shortley phase
+ *   Y0 = 0.28209479177387814, (Y1, Y2, Y3) = 0.4886025119029199 (y, z, x),
+ *   (Y4, Y5, Y7) = 1.0925484305920792 (x y, y z, x z), Y6 = 0.31539156525252005 (3 z^2 - 1),
+ *   Y8 = 0.5462742152960396 (x^2 - y^2),
+ * and the band weights w = 1, 2/3, 1/4 for l = 0, 1, 2:
+ *   out_c = albedo_c * E_c,  E_c = sum_{k = 0..8} (w_l(k) L_kc) Y_k, summed in that order with fused multiply-adds;
+ *   every other operation is one IEEE-rounded fp32 operation.
+ * Backward: the gradients torch autograd gives for the same expressions.  Each gradient output may be NULL, and its work
+ * is skipped; grad_normals [B*V, 3] and grad_albedo [B*V, C] are contiguous, grad_coefficients has the shape of
+ * coefficients.  The coefficient gradient is summed in a fixed order (per-CTA partials in the workspace, then one
+ * reduction kernel, no float atomics): repeated calls give bit-identical results.  The workspace, of at least
+ * dirt_sh_lighting_workspace_bytes(B, V, C) bytes (a function of the shapes alone), is needed only when
+ * grad_coefficients is wanted.
+ * B = 0 or V = 0: nothing is launched (the backward call still zeroes a wanted grad_coefficients).
+ * All pointers 4-byte aligned; row strides >= 0; C <= 2^26. */
+size_t dirt_sh_lighting_workspace_bytes(int B, long long V, int C);
+int dirt_sh_lighting_forward(const float* normals, long long normals_stride,
+                             const float* albedo, long long albedo_stride,
+                             const float* coefficients, int coefficients_per_item,
+                             float* out, int B, long long V, int C, void* cuda_stream);
+int dirt_sh_lighting_backward(const float* normals, long long normals_stride,
+                              const float* albedo, long long albedo_stride,
+                              const float* coefficients, int coefficients_per_item,
+                              const float* grad_out,
+                              float* grad_normals, float* grad_albedo, float* grad_coefficients,
+                              void* workspace, size_t workspace_bytes, int B, long long V, int C, void* cuda_stream);
+
 /* Vertex normals of the reference's lighting module (dirt/lighting.py:34-133) for B items of V vertices sharing the
  * faces:
  *   vertices             float32 [B*V, 3], row stride vertex_stride >= 3 floats, unit stride along the row (the first
