@@ -1,17 +1,22 @@
 // texture.cu -- differentiable texture lookup (dirt_texture_sample / dirt_texture_sample_backward): the bilinear and
 // nearest lookups of the reference's textured sample, restated in torch by examples/textured.py:sample_texture, whose
-// values the forward kernel reproduces bit for bit (DESIGN.md §7.1).
+// values the forward kernel reproduces bit for bit (DESIGN.md §7.1), and the mipmapped (trilinear) lookup of §7.6.
 //
-// Forward: one thread per lookup (C = 1..4) or per output element (any other C).  The index pair arrives as one 8-byte
-// load, the four texels through the read-only path, and the output leaves in vector stores: float2 / float4 for C = 2 / 4,
-// and for C = 3 the warp's 32 x 3 values are staged in shared memory and written as 24 float4.
-// Backward: one thread per lookup.  grad_indices comes from the same four texels.  grad_texture is aggregated inside the
-// warp before it touches global memory: lanes that hit the same texel (MATCH.ANY on its linear index) sum their
-// contributions and the lowest of them issues one reduction (a vector RED for C = 2 / 4).
+// Forward: one thread per lookup (texture_forward_kernel; bilinear and nearest with any C other than 1..4: one per output
+// element).  The index pair arrives as one 8-byte load, the texels through the read-only path, and the output leaves in
+// vector stores: float2 / float4 for C = 2 / 4, and for C = 3 the warp's 32 x 3 values are staged in shared memory and
+// written as 24 float4.
+// Backward: one thread per lookup (texture_backward_kernel).  grad_indices comes from the same texels.  grad_texture is
+// aggregated inside the warp before it touches global memory: lanes that hit the same texel (MATCH.ANY on its linear
+// index) sum their contributions and the lowest of them issues one reduction (a vector RED for C = 2 / 4).
+// Both kernels take MIP as a template parameter: false reads level 0 alone (bilinear or nearest), true the two mip levels
+// around the lookup's level of detail.
 // Deterministic backward (dirt_texture_sample_backward_deterministic): a radix sort of the lookups by base texel, then
 // fixed-order float64 sums per texel; see the section below and DESIGN.md §7.5.
 #include "../../include/dirt_b200.h"
 #include "common.cuh"
+
+#include <type_traits>
 
 namespace dirt {
 
@@ -101,58 +106,197 @@ __device__ __forceinline__ float bilinear(float t00, float t01, float t10, float
     return __fadd_rn(__fadd_rn(__fadd_rn(a, b), c), e);
 }
 
+// ---- levels of a lookup ---------------------------------------------------------------------------------------------
+//
+// A bilinear or nearest lookup reads level 0, the texture.  A mipmapped (trilinear) lookup (DESIGN.md §7.6) reads a
+// pyramid: level k of L is [TB, TH >> k, TW >> k, C]; levels 1 .. L-1 live in the caller's pyramid buffer (mip_offset).
+// Per lookup: lambda from the screen-space derivatives, l = floor(lambda), f = lambda - l, and
+// out = (1-f) * bilinear_l + f * bilinear_{l+1}, with level l+1 not read when f == 0.  Level k >= 1 is read at
+// (index + 0.5) * 2^-k - 0.5, level 0 at the index itself, so that f == 0 at l == 0 is mode bilinear bit for bit.
+
+// level k's dims: the level-0 dims with TH, TW and texels scaled down
+__device__ __forceinline__ TexDims level_dims(const TexDims& d, int k)
+{
+    TexDims e = d;
+    e.TH = d.TH >> k;
+    e.TW = d.TW >> k;
+    e.texels = d.texels >> (2 * k);
+    return e;
+}
+
+// level k of the texture (k = 0) or of the pyramid
+template <typename T>
+__host__ __device__ __forceinline__ T* level_base(T* level0, T* pyramid, const TexDims& d, int k)
+{
+    return k == 0 ? level0 : pyramid + mip_offset(d, k) * d.C;
+}
+
+// (index + 0.5) * 2^-k - 0.5, each operation rounded in that order; the index itself at level 0
+__device__ __forceinline__ float level_index(float i, int k)
+{
+    if (k == 0) return i;
+    return __fsub_rn(__fmul_rn(__fadd_rn(i, 0.5f), __int_as_float((127 - k) << 23)), 0.5f);
+}
+
+struct Lod {
+    int l;      // the finer level read
+    float f;    // the weight of level l + 1; 0: level l alone
+};
+
+// rho^2 = max(d0^2 + d1^2, d2^2 + d3^2) (NaN if either is), lambda = 0.5 log2(rho^2), NaN -> 0, clamped to [0, L-1]
+__device__ __forceinline__ Lod lod_of(float4 v, int L)
+{
+    const float s0 = __fadd_rn(__fmul_rn(v.x, v.x), __fmul_rn(v.y, v.y));
+    const float s1 = __fadd_rn(__fmul_rn(v.z, v.z), __fmul_rn(v.w, v.w));
+    const float rho2 = isnan(s0) || isnan(s1) ? __int_as_float(0x7fc00000) : fmaxf(s0, s1);
+    float lam = __fmul_rn(0.5f, log2f(rho2));
+    lam = isnan(lam) ? 0.f : fminf(fmaxf(lam, 0.f), (float)(L - 1));
+    Lod o;
+    o.l = (int)floorf(lam);
+    o.f = __fsub_rn(lam, (float)o.l);
+    return o;
+}
+
+template <bool VEC>
+__device__ __forceinline__ float4 load_derivatives(const float* derivatives, long long g)
+{
+    if (VEC) return __ldg(reinterpret_cast<const float4*>(derivatives) + g);
+    const float* p = derivatives + 4 * g;
+    return make_float4(__ldg(p), __ldg(p + 1), __ldg(p + 2), __ldg(p + 3));
+}
+
+// One lookup's levels: taps and pointers of level l (0) and, for a mipmapped lookup, l + 1 (1; unused when f == 0).
+// A bilinear or nearest lookup has level 0 alone, l = 0 and f = 0.
+struct Lookup {
+    Taps t0, t1;
+    const float *p0, *p1;   // the lookup's texture at level l / l + 1
+    int w0, w1;             // their widths
+    Lod lod;
+};
+
+__device__ __forceinline__ Lookup trilinear_of(float2 ix, float4 dv, const float* texture, const float* pyramid,
+                                               const TexDims& d, int L, long long g)
+{
+    Lookup q;
+    q.lod = lod_of(dv, L);
+    const int l = q.lod.l, l1 = l + 1 < L ? l + 1 : l;
+    const TexDims d0 = level_dims(d, l), d1 = level_dims(d, l1);
+    q.t0 = taps_of(level_index(ix.x, l), level_index(ix.y, l), d0, g);
+    q.t1 = taps_of(level_index(ix.x, l1), level_index(ix.y, l1), d1, g);
+    // a finite index can map to a non-finite one only past 3.4e38; such a lookup reads nothing, as a non-finite one
+    q.t0.valid = q.t0.valid && q.t1.valid;
+    q.p0 = level_base(texture, pyramid, d, l) + q.t0.base * d.C;
+    q.p1 = level_base(texture, pyramid, d, l1) + q.t1.base * d.C;
+    q.w0 = d0.TW;
+    q.w1 = d1.TW;
+    return q;
+}
+
+// lookup g of a texture with C channels (MIP: its pyramid, derivatives and L levels)
+template <bool MIP, bool VEC>
+__device__ __forceinline__ Lookup lookup_of(const float* texture, const float* pyramid, const float* indices,
+                                            const float* derivatives, const TexDims& d, int C, int L, long long g)
+{
+    const float2 ix = load_index<VEC>(indices, g);
+    if (MIP) return trilinear_of(ix, load_derivatives<VEC>(derivatives, g), texture, pyramid, d, L, g);
+    Lookup q;
+    q.t0 = taps_of(ix.x, ix.y, d, g);
+    q.p0 = texture + q.t0.base * C;
+    q.w0 = d.TW;
+    q.lod.l = 0;
+    q.lod.f = 0.f;
+    return q;
+}
+
 // ---- forward --------------------------------------------------------------------------------------------------------
 
-// One thread per lookup, CT = C in 1..4.  VEC: the pointers are aligned for the vector loads and stores (see
-// launch_texture_forward).  The loop runs per warp, so that the C = 3 staging sees all 32 lanes.
+// channels c0 .. c0 + NV - 1 of the lookup at taps t of a texture of width TW and C channels: the bilinear blend of the
+// four texels, or for nearest the texel (r0, c0) alone
+template <int NV, bool VEC>
+__device__ __forceinline__ void level_rows(const float* tex, const Taps& t, int TW, int C, int c0, bool nearest, float v[NV])
+{
+    float t00[NV], t01[NV], t10[NV], t11[NV];
+    load_row<NV, VEC>(tex + ((long long)t.r0 * TW + t.c0) * C + c0, t00);
+    if (nearest) {
+#pragma unroll
+        for (int j = 0; j < NV; ++j) v[j] = t00[j];
+        return;
+    }
+    load_row<NV, VEC>(tex + ((long long)t.r0 * TW + t.c1) * C + c0, t01);
+    load_row<NV, VEC>(tex + ((long long)t.r1 * TW + t.c0) * C + c0, t10);
+    load_row<NV, VEC>(tex + ((long long)t.r1 * TW + t.c1) * C + c0, t11);
+#pragma unroll
+    for (int j = 0; j < NV; ++j) v[j] = bilinear(t00[j], t01[j], t10[j], t11[j], t.fr, t.fc);
+}
+
+// Channels c0 .. c0 + NV - 1 of lookup g = base + lane go to out.  Every lane of the warp calls it: for C = 3 the warp's
+// values are staged in stage.
 template <int CT, bool VEC>
+__device__ __forceinline__ void store_out(float* out, float* stage, long long base, int c0, int C, long long total,
+                                          const float v[])
+{
+    constexpr int NV = CT ? CT : 1;
+    const int lane = threadIdx.x & 31;
+    const long long g = base + lane;
+    float* o = out + g * C + c0;
+    if (VEC && CT == 4) {
+        if (g < total) *reinterpret_cast<float4*>(o) = make_float4(v[0], v[1 % NV], v[2 % NV], v[3 % NV]);
+    } else if (VEC && CT == 2) {
+        if (g < total) *reinterpret_cast<float2*>(o) = make_float2(v[0], v[1 % NV]);
+    } else if (VEC && CT == 3 && base + 32 <= total) {
+        // the warp's 96 consecutive floats start on a 384-byte boundary: 24 float4 stores
+        float* s = stage + (threadIdx.x & ~31) * 3;
+#pragma unroll
+        for (int j = 0; j < NV; ++j) s[lane * 3 + j] = v[j];
+        __syncwarp();
+        if (lane < 24) *reinterpret_cast<float4*>(out + base * 3 + lane * 4) = reinterpret_cast<const float4*>(s)[lane];
+        __syncwarp();
+    } else if (g < total) {
+#pragma unroll
+        for (int j = 0; j < NV; ++j) o[j] = v[j];
+    }
+}
+
+// One thread per lookup, CT = C in 1..4, or 0 for any C (MIP only: channels in a loop, scalar accesses).  VEC: the
+// pointers are aligned for the vector loads and stores (see forward_ct).  The loop runs per warp, so that the C = 3
+// staging sees all 32 lanes.  MIP: pyramid, derivatives and L as in trilinear_of; unused otherwise.
+template <int CT, bool VEC, bool MIP>
 __global__ void __launch_bounds__(TEX_THREADS) texture_forward_kernel(const float* __restrict__ texture,
                                                                       const float* __restrict__ indices,
-                                                                      float* __restrict__ out, TexDims d)
+                                                                      float* __restrict__ out, TexDims d,
+                                                                      const float* __restrict__ pyramid,
+                                                                      const float* __restrict__ derivatives, int L)
 {
+    constexpr int NV = CT ? CT : 1;
+    const int C = CT ? CT : d.C;
     __shared__ __align__(16) float stage[CT == 3 ? TEX_THREADS * 3 : 1];
     const int lane = threadIdx.x & 31;
     const long long stride = (long long)gridDim.x * TEX_THREADS;
     for (long long base = (long long)blockIdx.x * TEX_THREADS + (threadIdx.x & ~31); base < d.total; base += stride) {
         const long long g = base + lane;
-        float v[CT];
+        // The trilinear lookup is formed once, before the channel loop.  The bilinear one (a single pass) is formed
+        // inside the branch on g: that order takes fewer registers.
+        Lookup q;
+        q.t0.valid = false;
+        if (MIP && g < d.total) q = lookup_of<MIP, VEC>(texture, pyramid, indices, derivatives, d, C, L, g);
+        for (int c0 = 0; c0 < C; c0 += NV) {
+            float v[NV];
 #pragma unroll
-        for (int j = 0; j < CT; ++j) v[j] = 0.f;
-        if (g < d.total) {
-            const float2 ix = load_index<VEC>(indices, g);
-            const Taps t = taps_of(ix.x, ix.y, d, g);
-            if (t.valid) {
-                const float* tex = texture + t.base * CT;
-                float t00[CT], t01[CT], t10[CT], t11[CT];
-                load_row<CT, VEC>(tex + ((long long)t.r0 * d.TW + t.c0) * CT, t00);
-                if (d.mode == DIRT_TEXTURE_NEAREST) {
+            for (int j = 0; j < NV; ++j) v[j] = 0.f;
+            if (MIP || g < d.total) {
+                if (!MIP) q = lookup_of<MIP, VEC>(texture, pyramid, indices, derivatives, d, C, L, g);
+                if (q.t0.valid) {
+                    level_rows<NV, VEC>(q.p0, q.t0, q.w0, C, c0, !MIP && d.mode == DIRT_TEXTURE_NEAREST, v);
+                    if (MIP && q.lod.f != 0.f) {
+                        float u[NV];
+                        level_rows<NV, VEC>(q.p1, q.t1, q.w1, C, c0, false, u);
+                        const float omf = __fsub_rn(1.0f, q.lod.f);
 #pragma unroll
-                    for (int j = 0; j < CT; ++j) v[j] = t00[j];
-                } else {
-                    load_row<CT, VEC>(tex + ((long long)t.r0 * d.TW + t.c1) * CT, t01);
-                    load_row<CT, VEC>(tex + ((long long)t.r1 * d.TW + t.c0) * CT, t10);
-                    load_row<CT, VEC>(tex + ((long long)t.r1 * d.TW + t.c1) * CT, t11);
-#pragma unroll
-                    for (int j = 0; j < CT; ++j) v[j] = bilinear(t00[j], t01[j], t10[j], t11[j], t.fr, t.fc);
+                        for (int j = 0; j < NV; ++j) v[j] = __fadd_rn(__fmul_rn(omf, v[j]), __fmul_rn(q.lod.f, u[j]));
+                    }
                 }
             }
-        }
-        float* o = out + g * CT;
-        if (VEC && CT == 4) {
-            if (g < d.total) *reinterpret_cast<float4*>(o) = make_float4(v[0], v[1 % CT], v[2 % CT], v[3 % CT]);
-        } else if (VEC && CT == 2) {
-            if (g < d.total) *reinterpret_cast<float2*>(o) = make_float2(v[0], v[1 % CT]);
-        } else if (VEC && CT == 3 && base + 32 <= d.total) {
-            // the warp's 96 consecutive floats start on a 384-byte boundary: 24 float4 stores
-            float* s = stage + (threadIdx.x & ~31) * 3;
-#pragma unroll
-            for (int j = 0; j < CT; ++j) s[lane * 3 + j] = v[j];
-            __syncwarp();
-            if (lane < 24) *reinterpret_cast<float4*>(out + base * 3 + lane * 4) = reinterpret_cast<const float4*>(s)[lane];
-            __syncwarp();
-        } else if (g < d.total) {
-#pragma unroll
-            for (int j = 0; j < CT; ++j) o[j] = v[j];
+            store_out<CT, VEC>(out, stage, base, c0, C, d.total, v);
         }
     }
 }
@@ -275,57 +419,123 @@ __device__ __forceinline__ void red_row(float* dst, const float v[NV])
     }
 }
 
-// One thread per lookup.  CT = C in 1..4, or 0 for any C (channels in a loop).  VEC: as in the forward kernel, for
-// indices, grad_indices, grad_out, texture and grad_texture rows.
+// d out / d (row, col) index at one level, through the fractions only, added to (dr, dc): the level's taps t
+// (omr = 1 - t.fr, omc = 1 - t.fc) in its texture tex of width TW.  go: grad_out's row (CT = 0: its channels are read
+// one at a time into go[0]).
 template <int CT, bool VEC>
-__global__ void __launch_bounds__(TEX_THREADS) texture_backward_kernel(const float* __restrict__ texture,
-                                                                       const float* __restrict__ indices,
-                                                                       const float* __restrict__ grad_out,
-                                                                       float* __restrict__ grad_texture,
-                                                                       float* __restrict__ grad_indices, TexDims d)
+__device__ __forceinline__ void index_grad_level(const float* tex, const Taps& t, float omr, float omc, int TW, int C,
+                                                 const float* gout, float go[], float& dr, float& dc)
+{
+    constexpr int NV = CT ? CT : 1;
+    const float* p00 = tex + ((long long)t.r0 * TW + t.c0) * C;
+    const float* p01 = tex + ((long long)t.r0 * TW + t.c1) * C;
+    const float* p10 = tex + ((long long)t.r1 * TW + t.c0) * C;
+    const float* p11 = tex + ((long long)t.r1 * TW + t.c1) * C;
+    for (int c0 = 0; c0 < C; c0 += NV) {
+        float t00[NV], t01[NV], t10[NV], t11[NV];
+        load_row<NV, VEC>(p00 + c0, t00);
+        load_row<NV, VEC>(p01 + c0, t01);
+        load_row<NV, VEC>(p10 + c0, t10);
+        load_row<NV, VEC>(p11 + c0, t11);
+        if (!CT) go[0] = __ldg(gout + c0);
+#pragma unroll
+        for (int j = 0; j < NV; ++j) {
+            dc += go[j] * ((t01[j] - t00[j]) * omr + (t11[j] - t10[j]) * t.fr);
+            dr += go[j] * ((t10[j] - t00[j]) * omc + (t11[j] - t01[j]) * t.fc);
+        }
+    }
+}
+
+// d out / d texture at one level: the first `corners` bilinear weights of taps t (omr, omc as above; times the level
+// weight a when MIP) scattered to the texels of dst (width TW, C channels), summed per texel in the warp with
+// key_offset + the texel index as the key.  A level with t.valid false scatters nothing.  Warp-uniform: every lane
+// takes part in agg_plan.
+template <int CT, bool VEC, bool MIP>
+__device__ __forceinline__ void texel_grad_level(const Taps& t, float omr, float omc, float a, long long key_offset,
+                                                 float* dst_level, int TW, int C, int corners, const float go[],
+                                                 const float* gout, int lane)
+{
+    constexpr int NV = CT ? CT : 1;
+    for (int k = 0; k < corners; ++k) {   // (r0,c0), (r0,c1), (r1,c0), (r1,c1)
+        const int r = (k & 2) ? t.r1 : t.r0, c = (k & 1) ? t.c1 : t.c0;
+        float w = __fmul_rn((k & 1) ? t.fc : omc, (k & 2) ? t.fr : omr);
+        if (MIP) w = __fmul_rn(w, a);
+        const bool on = t.valid && w != 0.f;
+        const long long texel = t.base + (long long)r * TW + c;
+        // texel indices stay below 2^62 (checked in api.cu): bit 63 marks a lane's private key
+        const Agg ag = agg_plan(on ? (unsigned long long)(key_offset + texel) : (1ull << 63) | (unsigned)lane, lane);
+        const bool leader = on && __ffs(ag.peers) - 1 == lane;
+        float* dst = dst_level + texel * C;
+        if (CT) {
+            float v[NV];
+#pragma unroll
+            for (int j = 0; j < NV; ++j) v[j] = on ? go[j] * w : 0.f;
+            agg_sum<NV>(ag, v, lane);
+            if (leader) red_row<NV, VEC>(dst, v);
+        } else {
+            for (int ch = 0; ch < C; ++ch) {
+                float v[1] = {on ? __ldg(gout + ch) * w : 0.f};
+                agg_sum<1>(ag, v, lane);
+                if (leader) atomicAdd(dst + ch, v[0]);
+            }
+        }
+    }
+}
+
+// One thread per lookup.  CT = C in 1..4, or 0 for any C (channels in a loop).  VEC: as in the forward kernel, for
+// indices, derivatives, grad_indices, grad_out, and the rows of texture, pyramid, grad_texture and level_grad.
+// MIP: grad_indices through both levels' fractions, each scaled by 2^-k.  The texel gradients of level 0 go to
+// grad_texture, those of level k >= 1 to level_grad (the pyramid's layout), keyed on the packed texel index (level 0:
+// its texel index; level k: TB * texels + the pyramid's texel index).
+template <int CT, bool VEC, bool MIP>
+__global__ void __launch_bounds__(TEX_THREADS) texture_backward_kernel(
+    const float* __restrict__ texture, const float* __restrict__ indices, const float* __restrict__ grad_out,
+    float* __restrict__ grad_texture, float* __restrict__ grad_indices, TexDims d, const float* __restrict__ pyramid,
+    const float* __restrict__ derivatives, float* __restrict__ level_grad, int L)
 {
     constexpr int NV = CT ? CT : 1;   // channels held in registers at a time
     const int C = CT ? CT : d.C;
     const int lane = threadIdx.x & 31;
-    const bool bilinear_mode = d.mode == DIRT_TEXTURE_BILINEAR;
+    const bool bilinear_mode = MIP || d.mode == DIRT_TEXTURE_BILINEAR;
     const long long stride = (long long)gridDim.x * TEX_THREADS;
     for (long long base = (long long)blockIdx.x * TEX_THREADS + (threadIdx.x & ~31); base < d.total; base += stride) {
         const long long g = base + lane;
         const bool live = g < d.total;
-        Taps t;
-        t.valid = false; t.base = 0; t.r0 = t.r1 = t.c0 = t.c1 = 0; t.fr = t.fc = 0.f;
-        if (live) {
-            const float2 ix = load_index<VEC>(indices, g);
-            t = taps_of(ix.x, ix.y, d, g);
+        Lookup q;
+        q.t0.valid = false;
+        if (!MIP) { q.t0.base = 0; q.t0.r0 = q.t0.r1 = q.t0.c0 = q.t0.c1 = 0; q.t0.fr = q.t0.fc = 0.f; }
+        q.lod.l = 0; q.lod.f = 0.f;
+        if (live) q = lookup_of<MIP, VEC>(texture, pyramid, indices, derivatives, d, C, L, g);
+        if (MIP && !q.t0.valid) {   // an invalid lookup's taps are zero and scatter nothing
+            q.t0.r0 = q.t0.r1 = q.t0.c0 = q.t0.c1 = 0; q.t0.fr = q.t0.fc = 0.f; q.t0.base = 0;
+            q.t1 = q.t0;
+            q.lod.l = 0; q.lod.f = 0.f;
         }
-        const float omr = __fsub_rn(1.0f, t.fr), omc = __fsub_rn(1.0f, t.fc);
+        const float omr = __fsub_rn(1.0f, q.t0.fr), omc = __fsub_rn(1.0f, q.t0.fc);   // level l
+        const bool both = MIP && q.t0.valid && q.lod.f != 0.f;
+        const float omf = __fsub_rn(1.0f, q.lod.f);
         const float* gout = grad_out + g * C;
         float go[NV];
 #pragma unroll
         for (int j = 0; j < NV; ++j) go[j] = 0.f;
-        if (CT && t.valid) load_row<NV, VEC>(gout, go);
+        if (CT && q.t0.valid) load_row<NV, VEC>(gout, go);
 
-        // d out / d (row, col) index, through the fractions only
         if (grad_indices && live) {
             float dr = 0.f, dc = 0.f;
-            if (t.valid && bilinear_mode) {
-                const float* tex = texture + t.base * C;
-                const float* p00 = tex + ((long long)t.r0 * d.TW + t.c0) * C;
-                const float* p01 = tex + ((long long)t.r0 * d.TW + t.c1) * C;
-                const float* p10 = tex + ((long long)t.r1 * d.TW + t.c0) * C;
-                const float* p11 = tex + ((long long)t.r1 * d.TW + t.c1) * C;
-                for (int c0 = 0; c0 < C; c0 += NV) {
-                    float t00[NV], t01[NV], t10[NV], t11[NV];
-                    load_row<NV, VEC>(p00 + c0, t00);
-                    load_row<NV, VEC>(p01 + c0, t01);
-                    load_row<NV, VEC>(p10 + c0, t10);
-                    load_row<NV, VEC>(p11 + c0, t11);
-                    if (!CT) go[0] = __ldg(gout + c0);
-#pragma unroll
-                    for (int j = 0; j < NV; ++j) {
-                        dc += go[j] * ((t01[j] - t00[j]) * omr + (t11[j] - t10[j]) * t.fr);
-                        dr += go[j] * ((t10[j] - t00[j]) * omc + (t11[j] - t01[j]) * t.fc);
-                    }
+            if (q.t0.valid && bilinear_mode)
+                index_grad_level<CT, VEC>(MIP ? q.p0 : texture + q.t0.base * C, q.t0, omr, omc, q.w0, C, gout, go, dr, dc);
+            if (MIP) {
+                float dr1 = 0.f, dc1 = 0.f;
+                if (both)
+                    index_grad_level<CT, VEC>(q.p1, q.t1, __fsub_rn(1.0f, q.t1.fr), __fsub_rn(1.0f, q.t1.fc), q.w1, C, gout,
+                                              go, dr1, dc1);
+                // d index_k / d index = 2^-k
+                const float s0 = __int_as_float((127 - q.lod.l) << 23), s1 = 0.5f * s0;
+                dr = dr * s0;
+                dc = dc * s0;
+                if (both) {
+                    dr = omf * dr + q.lod.f * (dr1 * s1);
+                    dc = omf * dc + q.lod.f * (dc1 * s1);
                 }
             }
             if (VEC) reinterpret_cast<float2*>(grad_indices)[g] = make_float2(dr, dc);
@@ -334,29 +544,21 @@ __global__ void __launch_bounds__(TEX_THREADS) texture_backward_kernel(const flo
 
         // d out / d texture: the bilinear weights (1 for nearest) scattered to the texels, summed per texel in the warp
         if (grad_texture) {
-            const int corners = bilinear_mode ? 4 : 1;
-            for (int k = 0; k < corners; ++k) {   // (r0,c0), (r0,c1), (r1,c0), (r1,c1)
-                const int r = (k & 2) ? t.r1 : t.r0, c = (k & 1) ? t.c1 : t.c0;
-                const float w = __fmul_rn((k & 1) ? t.fc : omc, (k & 2) ? t.fr : omr);
-                const bool on = t.valid && w != 0.f;
-                const long long texel = t.base + (long long)r * d.TW + c;
-                // texel indices stay below 2^62 (checked in api.cu): bit 63 marks a lane's private key
-                const Agg a = agg_plan(on ? (unsigned long long)texel : (1ull << 63) | (unsigned)lane, lane);
-                const bool leader = on && __ffs(a.peers) - 1 == lane;
-                float* dst = grad_texture + texel * C;
-                if (CT) {
-                    float v[NV];
-#pragma unroll
-                    for (int j = 0; j < NV; ++j) v[j] = on ? go[j] * w : 0.f;
-                    agg_sum<NV>(a, v, lane);
-                    if (leader) red_row<NV, VEC>(dst, v);
-                } else {
-                    for (int ch = 0; ch < C; ++ch) {
-                        float v[1] = {on ? __ldg(gout + ch) * w : 0.f};
-                        agg_sum<1>(a, v, lane);
-                        if (leader) atomicAdd(dst + ch, v[0]);
-                    }
+            if (MIP) {
+#pragma unroll 1
+                for (int s = 0; s < 2; ++s) {
+                    const int k = q.lod.l + s;
+                    Taps t = s ? q.t1 : q.t0;
+                    t.valid = s ? both : q.t0.valid;
+                    const long long key_offset = k == 0 ? 0ll : (long long)d.TB * d.texels + mip_offset(d, k);
+                    float* dst_level = k == 0 ? grad_texture : level_grad + mip_offset(d, k) * C;
+                    texel_grad_level<CT, VEC, true>(t, __fsub_rn(1.0f, t.fr), __fsub_rn(1.0f, t.fc),
+                                                    s ? q.lod.f : (both ? omf : 1.0f), key_offset, dst_level,
+                                                    s ? q.w1 : q.w0, C, 4, go, gout, lane);
                 }
+            } else {
+                texel_grad_level<CT, VEC, false>(q.t0, omr, omc, 1.0f, 0, grad_texture, d.TW, C, bilinear_mode ? 4 : 1, go,
+                                                 gout, lane);
             }
         }
     }
@@ -370,31 +572,60 @@ inline unsigned blocks_for(long long work)
     return (unsigned)(b < TEX_MAX_BLOCKS ? b : TEX_MAX_BLOCKS);
 }
 
-template <int CT>
-cudaError_t forward_ct(const float* texture, const float* indices, float* out, const TexDims& d, cudaStream_t stream)
+// f(std::integral_constant<int, CT>()) with the kernels' channel parameter: CT = C for C in 1..4, else 0 (any C)
+template <typename F>
+cudaError_t with_ct(int C, F f)
 {
-    const int vec_bytes = CT == 3 ? 16 : 4 * CT;
-    const bool vec = aligned(indices, 8) && aligned(out, vec_bytes) && (CT == 3 || aligned(texture, 4 * CT));
-    const unsigned blocks = blocks_for(d.total);
-    if (vec) texture_forward_kernel<CT, true><<<blocks, TEX_THREADS, 0, stream>>>(texture, indices, out, d);
-    else texture_forward_kernel<CT, false><<<blocks, TEX_THREADS, 0, stream>>>(texture, indices, out, d);
+    switch (C) {
+        case 1: return f(std::integral_constant<int, 1>());
+        case 2: return f(std::integral_constant<int, 2>());
+        case 3: return f(std::integral_constant<int, 3>());
+        case 4: return f(std::integral_constant<int, 4>());
+        default: return f(std::integral_constant<int, 0>());
+    }
+}
+
+// The vector path needs 8-byte index pairs, 16-byte derivatives, out rows aligned for the float2 / float4 stores (16
+// bytes for the staged C = 3 store), and texture and pyramid rows for the float2 / float4 loads.  Bilinear and nearest
+// with any C run the generic kernel.
+template <int CT, bool MIP>
+cudaError_t forward_ct(const float* texture, const float* pyramid, const float* indices, const float* derivatives,
+                       float* out, const TexDims& d, int L, cudaStream_t stream)
+{
+    if constexpr (CT == 0 && !MIP) {
+        const unsigned blocks = blocks_for(d.total * d.C);
+        const long long step = (long long)blocks * TEX_THREADS;
+        texture_forward_generic_kernel<<<blocks, TEX_THREADS, 0, stream>>>(texture, indices, out, d, step / d.C,
+                                                                            (int)(step % d.C));
+    } else {
+        const int row = CT == 2 || CT == 4 ? 4 * CT : 4;
+        auto kernel = texture_forward_kernel<CT, false, MIP>;
+        if constexpr (CT != 0)   // any C has no vector path
+            if (aligned(indices, 8) && aligned(out, CT == 3 ? 16 : row) && aligned(texture, row) &&
+                (!MIP || (aligned(derivatives, 16) && aligned(pyramid, row))))
+                kernel = texture_forward_kernel<CT, true, MIP>;
+        kernel<<<blocks_for(d.total), TEX_THREADS, 0, stream>>>(texture, indices, out, d, pyramid, derivatives, L);
+    }
     return cudaGetLastError();
 }
 
-template <int CT>
-cudaError_t backward_ct(const float* texture, const float* indices, const float* grad_out, float* grad_texture,
-                        float* grad_indices, const TexDims& d, cudaStream_t stream)
+// The vector path needs 8-byte index pairs and grad_indices pairs, 16-byte derivatives, and the rows of grad_out,
+// texture, pyramid, grad_texture and level_grad aligned for float2 / float4.  For any C it serves the index pairs of
+// the bilinear lookup alone.
+template <int CT, bool MIP>
+cudaError_t backward_ct(const float* texture, const float* pyramid, const float* indices, const float* derivatives,
+                        const float* grad_out, float* grad_texture, float* level_grad, float* grad_indices,
+                        const TexDims& d, int L, cudaStream_t stream)
 {
     const int row = CT == 2 || CT == 4 ? 4 * CT : 4;
-    const bool vec = aligned(indices, 8) && aligned(grad_indices, 8) && aligned(grad_out, row) && aligned(texture, row) &&
-                     aligned(grad_texture, row);
-    const unsigned blocks = blocks_for(d.total);
-    if (vec)
-        texture_backward_kernel<CT, true><<<blocks, TEX_THREADS, 0, stream>>>(texture, indices, grad_out, grad_texture,
-                                                                             grad_indices, d);
-    else
-        texture_backward_kernel<CT, false><<<blocks, TEX_THREADS, 0, stream>>>(texture, indices, grad_out, grad_texture,
-                                                                              grad_indices, d);
+    auto kernel = texture_backward_kernel<CT, false, MIP>;
+    if constexpr (CT != 0 || !MIP)
+        if (aligned(indices, 8) && aligned(grad_indices, 8) && aligned(grad_out, row) && aligned(texture, row) &&
+            aligned(grad_texture, row) &&
+            (!MIP || (aligned(derivatives, 16) && aligned(pyramid, row) && aligned(level_grad, row))))
+            kernel = texture_backward_kernel<CT, true, MIP>;
+    kernel<<<blocks_for(d.total), TEX_THREADS, 0, stream>>>(texture, indices, grad_out, grad_texture, grad_indices, d,
+                                                            pyramid, derivatives, level_grad, L);
     return cudaGetLastError();
 }
 
@@ -818,20 +1049,9 @@ cudaError_t launch_texture_backward_deterministic(const float* texture, const fl
 cudaError_t launch_texture_forward(const float* texture, const float* indices, float* out, const TexDims& d,
                                    cudaStream_t stream, int* launches)
 {
-    cudaError_t e;
-    switch (d.C) {
-        case 1: e = forward_ct<1>(texture, indices, out, d, stream); break;
-        case 2: e = forward_ct<2>(texture, indices, out, d, stream); break;
-        case 3: e = forward_ct<3>(texture, indices, out, d, stream); break;
-        case 4: e = forward_ct<4>(texture, indices, out, d, stream); break;
-        default: {
-            const unsigned blocks = blocks_for(d.total * d.C);
-            const long long step = (long long)blocks * TEX_THREADS;
-            texture_forward_generic_kernel<<<blocks, TEX_THREADS, 0, stream>>>(texture, indices, out, d, step / d.C,
-                                                                                (int)(step % d.C));
-            e = cudaGetLastError();
-        }
-    }
+    const cudaError_t e = with_ct(d.C, [&](auto ct) {
+        return forward_ct<decltype(ct)::value, false>(texture, nullptr, indices, nullptr, out, d, 1, stream);
+    });
     if (e == cudaSuccess) ++*launches;
     return e;
 }
@@ -844,115 +1064,17 @@ cudaError_t launch_texture_backward(const float* texture, const float* indices, 
         (e = cudaMemsetAsync(grad_texture, 0, sizeof(float) * (size_t)d.TB * d.texels * d.C, stream)) != cudaSuccess)
         return e;
     if (d.total == 0 || (!grad_texture && !grad_indices)) return cudaSuccess;
-    switch (d.C) {
-        case 1: e = backward_ct<1>(texture, indices, grad_out, grad_texture, grad_indices, d, stream); break;
-        case 2: e = backward_ct<2>(texture, indices, grad_out, grad_texture, grad_indices, d, stream); break;
-        case 3: e = backward_ct<3>(texture, indices, grad_out, grad_texture, grad_indices, d, stream); break;
-        case 4: e = backward_ct<4>(texture, indices, grad_out, grad_texture, grad_indices, d, stream); break;
-        default: e = backward_ct<0>(texture, indices, grad_out, grad_texture, grad_indices, d, stream);
-    }
+    e = with_ct(d.C, [&](auto ct) {
+        return backward_ct<decltype(ct)::value, false>(texture, nullptr, indices, nullptr, grad_out, grad_texture, nullptr,
+                                                        grad_indices, d, 1, stream);
+    });
     if (e == cudaSuccess) ++*launches;
     return e;
 }
 
-// ---- mipmapped (trilinear) lookup (DESIGN.md §7.6) ------------------------------------------------------------------
-//
-// Level k of L is [TB, TH >> k, TW >> k, C]; levels 1 .. L-1 live in the caller's pyramid buffer (mip_offset).  Per
-// lookup: lambda from the screen-space derivatives, l = floor(lambda), f = lambda - l, and
-// out = (1-f) * bilinear_l + f * bilinear_{l+1}, with level l+1 not read when f == 0.  Level k >= 1 is read at
-// (index + 0.5) * 2^-k - 0.5, level 0 at the index itself, so that f == 0 at l == 0 is mode bilinear bit for bit.
+// ---- mipmapped (trilinear) lookup (DESIGN.md §7.6): the pyramid, its adjoint and the deterministic level terms ------
 
 namespace {
-
-// level k's dims: the level-0 dims with TH, TW and texels scaled down
-__device__ __forceinline__ TexDims level_dims(const TexDims& d, int k)
-{
-    TexDims e = d;
-    e.TH = d.TH >> k;
-    e.TW = d.TW >> k;
-    e.texels = d.texels >> (2 * k);
-    return e;
-}
-
-// level k of the texture (k = 0) or of the pyramid
-template <typename T>
-__host__ __device__ __forceinline__ T* level_base(T* level0, T* pyramid, const TexDims& d, int k)
-{
-    return k == 0 ? level0 : pyramid + mip_offset(d, k) * d.C;
-}
-
-// (index + 0.5) * 2^-k - 0.5, each operation rounded in that order; the index itself at level 0
-__device__ __forceinline__ float level_index(float i, int k)
-{
-    if (k == 0) return i;
-    return __fsub_rn(__fmul_rn(__fadd_rn(i, 0.5f), __int_as_float((127 - k) << 23)), 0.5f);
-}
-
-struct Lod {
-    int l;      // the finer level read
-    float f;    // the weight of level l + 1; 0: level l alone
-};
-
-// rho^2 = max(d0^2 + d1^2, d2^2 + d3^2) (NaN if either is), lambda = 0.5 log2(rho^2), NaN -> 0, clamped to [0, L-1]
-__device__ __forceinline__ Lod lod_of(float4 v, int L)
-{
-    const float s0 = __fadd_rn(__fmul_rn(v.x, v.x), __fmul_rn(v.y, v.y));
-    const float s1 = __fadd_rn(__fmul_rn(v.z, v.z), __fmul_rn(v.w, v.w));
-    const float rho2 = isnan(s0) || isnan(s1) ? __int_as_float(0x7fc00000) : fmaxf(s0, s1);
-    float lam = __fmul_rn(0.5f, log2f(rho2));
-    lam = isnan(lam) ? 0.f : fminf(fmaxf(lam, 0.f), (float)(L - 1));
-    Lod o;
-    o.l = (int)floorf(lam);
-    o.f = __fsub_rn(lam, (float)o.l);
-    return o;
-}
-
-template <bool VEC>
-__device__ __forceinline__ float4 load_derivatives(const float* derivatives, long long g)
-{
-    if (VEC) return __ldg(reinterpret_cast<const float4*>(derivatives) + g);
-    const float* p = derivatives + 4 * g;
-    return make_float4(__ldg(p), __ldg(p + 1), __ldg(p + 2), __ldg(p + 3));
-}
-
-// the bilinear lookup of channels c0 .. c0 + NV - 1 at taps t of a texture of width TW and C channels
-template <int NV, bool VEC>
-__device__ __forceinline__ void bilinear_rows(const float* tex, const Taps& t, int TW, int C, int c0, float v[NV])
-{
-    float t00[NV], t01[NV], t10[NV], t11[NV];
-    load_row<NV, VEC>(tex + ((long long)t.r0 * TW + t.c0) * C + c0, t00);
-    load_row<NV, VEC>(tex + ((long long)t.r0 * TW + t.c1) * C + c0, t01);
-    load_row<NV, VEC>(tex + ((long long)t.r1 * TW + t.c0) * C + c0, t10);
-    load_row<NV, VEC>(tex + ((long long)t.r1 * TW + t.c1) * C + c0, t11);
-#pragma unroll
-    for (int j = 0; j < NV; ++j) v[j] = bilinear(t00[j], t01[j], t10[j], t11[j], t.fr, t.fc);
-}
-
-// One lookup's two levels: taps and pointers of level l (0) and l + 1 (1; unused when f == 0)
-struct Trilinear {
-    Taps t0, t1;
-    const float *p0, *p1;   // the lookup's texture at level l / l + 1
-    int w0, w1;             // their widths
-    Lod lod;
-};
-
-__device__ __forceinline__ Trilinear trilinear_of(float2 ix, float4 dv, const float* texture, const float* pyramid,
-                                                  const TexDims& d, int L, long long g)
-{
-    Trilinear q;
-    q.lod = lod_of(dv, L);
-    const int l = q.lod.l, l1 = l + 1 < L ? l + 1 : l;
-    const TexDims d0 = level_dims(d, l), d1 = level_dims(d, l1);
-    q.t0 = taps_of(level_index(ix.x, l), level_index(ix.y, l), d0, g);
-    q.t1 = taps_of(level_index(ix.x, l1), level_index(ix.y, l1), d1, g);
-    // a finite index can map to a non-finite one only past 3.4e38; such a lookup reads nothing, as a non-finite one
-    q.t0.valid = q.t0.valid && q.t1.valid;
-    q.p0 = level_base(texture, pyramid, d, l) + q.t0.base * d.C;
-    q.p1 = level_base(texture, pyramid, d, l1) + q.t1.base * d.C;
-    q.w0 = d0.TW;
-    q.w1 = d1.TW;
-    return q;
-}
 
 // one thread per element of the next level: ((a + b) + (c + e)) * 0.25 of the 2x2 block, in that order
 __global__ void __launch_bounds__(TEX_THREADS) mip_build_kernel(const float* __restrict__ src, float* __restrict__ dst,
@@ -966,172 +1088,6 @@ __global__ void __launch_bounds__(TEX_THREADS) mip_build_kernel(const float* __r
         const long long down = 2ll * W * C;
         const float a = __ldg(s), b = __ldg(s + C), cc = __ldg(s + down), ee = __ldg(s + down + C);
         dst[e] = __fmul_rn(__fadd_rn(__fadd_rn(a, b), __fadd_rn(cc, ee)), 0.25f);
-    }
-}
-
-// One thread per lookup, CT = C in 1..4 or 0 (any C, one channel at a time).  VEC: indices 8-, derivatives 16-byte
-// aligned, out, texture and pyramid rows aligned for the vector loads and stores (the C = 3 store is staged as in
-// texture_forward_kernel).
-template <int CT, bool VEC>
-__global__ void __launch_bounds__(TEX_THREADS) texture_trilinear_forward_kernel(const float* __restrict__ texture,
-                                                                                const float* __restrict__ pyramid,
-                                                                                const float* __restrict__ indices,
-                                                                                const float* __restrict__ derivatives,
-                                                                                float* __restrict__ out, TexDims d, int L)
-{
-    constexpr int NV = CT ? CT : 1;
-    const int C = CT ? CT : d.C;
-    __shared__ __align__(16) float stage[CT == 3 ? TEX_THREADS * 3 : 1];
-    const int lane = threadIdx.x & 31;
-    const long long stride = (long long)gridDim.x * TEX_THREADS;
-    for (long long base = (long long)blockIdx.x * TEX_THREADS + (threadIdx.x & ~31); base < d.total; base += stride) {
-        const long long g = base + lane;
-        Trilinear q;
-        q.t0.valid = false;
-        if (g < d.total) q = trilinear_of(load_index<VEC>(indices, g), load_derivatives<VEC>(derivatives, g), texture, pyramid, d,
-                                          L, g);
-        for (int c0 = 0; c0 < C; c0 += NV) {
-            float v[NV];
-#pragma unroll
-            for (int j = 0; j < NV; ++j) v[j] = 0.f;
-            if (q.t0.valid) {
-                bilinear_rows<NV, VEC>(q.p0, q.t0, q.w0, C, c0, v);
-                if (q.lod.f != 0.f) {
-                    float u[NV];
-                    bilinear_rows<NV, VEC>(q.p1, q.t1, q.w1, C, c0, u);
-                    const float omf = __fsub_rn(1.0f, q.lod.f);
-#pragma unroll
-                    for (int j = 0; j < NV; ++j) v[j] = __fadd_rn(__fmul_rn(omf, v[j]), __fmul_rn(q.lod.f, u[j]));
-                }
-            }
-            float* o = out + g * C + c0;
-            if (VEC && CT == 4) {
-                if (g < d.total) *reinterpret_cast<float4*>(o) = make_float4(v[0], v[1 % NV], v[2 % NV], v[3 % NV]);
-            } else if (VEC && CT == 2) {
-                if (g < d.total) *reinterpret_cast<float2*>(o) = make_float2(v[0], v[1 % NV]);
-            } else if (VEC && CT == 3 && base + 32 <= d.total) {
-                float* s = stage + (threadIdx.x & ~31) * 3;
-#pragma unroll
-                for (int j = 0; j < NV; ++j) s[lane * 3 + j] = v[j];
-                __syncwarp();
-                if (lane < 24) *reinterpret_cast<float4*>(out + base * 3 + lane * 4) = reinterpret_cast<const float4*>(s)[lane];
-                __syncwarp();
-            } else if (g < d.total) {
-#pragma unroll
-                for (int j = 0; j < NV; ++j) o[j] = v[j];
-            }
-        }
-    }
-}
-
-// One thread per lookup, CT as in the forward kernel.  grad_indices per lookup, through both levels' fractions, each
-// scaled by 2^-k.  The texel gradients of level 0 go to grad_texture, those of level k >= 1 to level_grad (the pyramid's
-// layout), through the warp aggregation of texture_backward_kernel keyed on the packed texel index (level 0: its texel
-// index; level k: TB * texels + the pyramid's texel index).
-template <int CT, bool VEC>
-__global__ void __launch_bounds__(TEX_THREADS) texture_trilinear_backward_kernel(
-    const float* __restrict__ texture, const float* __restrict__ pyramid, const float* __restrict__ indices,
-    const float* __restrict__ derivatives, const float* __restrict__ grad_out, float* __restrict__ grad_texture,
-    float* __restrict__ level_grad, float* __restrict__ grad_indices, TexDims d, int L)
-{
-    constexpr int NV = CT ? CT : 1;
-    const int C = CT ? CT : d.C;
-    const int lane = threadIdx.x & 31;
-    const long long stride = (long long)gridDim.x * TEX_THREADS;
-    for (long long base = (long long)blockIdx.x * TEX_THREADS + (threadIdx.x & ~31); base < d.total; base += stride) {
-        const long long g = base + lane;
-        const bool live = g < d.total;
-        Trilinear q;
-        q.t0.valid = false;
-        q.lod.l = 0; q.lod.f = 0.f;
-        if (live) q = trilinear_of(load_index<VEC>(indices, g), load_derivatives<VEC>(derivatives, g), texture, pyramid, d, L, g);
-        if (!q.t0.valid) {
-            q.t0.r0 = q.t0.r1 = q.t0.c0 = q.t0.c1 = 0; q.t0.fr = q.t0.fc = 0.f; q.t0.base = 0;
-            q.t1 = q.t0;
-            q.lod.l = 0; q.lod.f = 0.f;
-        }
-        const bool both = q.t0.valid && q.lod.f != 0.f;
-        const float omf = __fsub_rn(1.0f, q.lod.f);
-        const float* gout = grad_out + g * C;
-        float go[NV];
-#pragma unroll
-        for (int j = 0; j < NV; ++j) go[j] = 0.f;
-        if (CT && q.t0.valid) load_row<NV, VEC>(gout, go);
-
-        if (grad_indices && live) {
-            float dr0 = 0.f, dc0 = 0.f, dr1 = 0.f, dc1 = 0.f;
-            if (q.t0.valid) {
-#pragma unroll
-                for (int s = 0; s < 2; ++s) {
-                    if (s == 1 && !both) break;
-                    const Taps t = s ? q.t1 : q.t0;
-                    const float* tex = s ? q.p1 : q.p0;
-                    const int TW = s ? q.w1 : q.w0;
-                    const float omr = __fsub_rn(1.0f, t.fr), omc = __fsub_rn(1.0f, t.fc);
-                    float dr = 0.f, dc = 0.f;
-                    for (int c0 = 0; c0 < C; c0 += NV) {
-                        float t00[NV], t01[NV], t10[NV], t11[NV];
-                        load_row<NV, VEC>(tex + ((long long)t.r0 * TW + t.c0) * C + c0, t00);
-                        load_row<NV, VEC>(tex + ((long long)t.r0 * TW + t.c1) * C + c0, t01);
-                        load_row<NV, VEC>(tex + ((long long)t.r1 * TW + t.c0) * C + c0, t10);
-                        load_row<NV, VEC>(tex + ((long long)t.r1 * TW + t.c1) * C + c0, t11);
-                        if (!CT) go[0] = __ldg(gout + c0);
-#pragma unroll
-                        for (int j = 0; j < NV; ++j) {
-                            dc += go[j] * ((t01[j] - t00[j]) * omr + (t11[j] - t10[j]) * t.fr);
-                            dr += go[j] * ((t10[j] - t00[j]) * omc + (t11[j] - t01[j]) * t.fc);
-                        }
-                    }
-                    if (s) { dr1 = dr; dc1 = dc; }
-                    else { dr0 = dr; dc0 = dc; }
-                }
-            }
-            // d index_k / d index = 2^-k
-            const float s0 = __int_as_float((127 - q.lod.l) << 23), s1 = 0.5f * s0;
-            float dr = dr0 * s0, dc = dc0 * s0;
-            if (both) {
-                dr = omf * dr + q.lod.f * (dr1 * s1);
-                dc = omf * dc + q.lod.f * (dc1 * s1);
-            }
-            if (VEC) reinterpret_cast<float2*>(grad_indices)[g] = make_float2(dr, dc);
-            else { grad_indices[2 * g] = dr; grad_indices[2 * g + 1] = dc; }
-        }
-
-        if (grad_texture) {
-#pragma unroll 1
-            for (int s = 0; s < 2; ++s) {   // warp-uniform: every lane takes part in agg_plan
-                const int k = q.lod.l + s;
-                const Taps t = s ? q.t1 : q.t0;
-                const float a = s ? q.lod.f : (both ? omf : 1.0f);
-                const bool level_on = s ? both : q.t0.valid;
-                const float omr = __fsub_rn(1.0f, t.fr), omc = __fsub_rn(1.0f, t.fc);
-                const int TW = s ? q.w1 : q.w0;
-                const long long first = k == 0 ? 0ll : (long long)d.TB * d.texels + mip_offset(d, k);
-                float* dst_level = k == 0 ? grad_texture : level_grad + mip_offset(d, k) * C;
-                for (int corner = 0; corner < 4; ++corner) {   // (r0,c0), (r0,c1), (r1,c0), (r1,c1)
-                    const int r = (corner & 2) ? t.r1 : t.r0, c = (corner & 1) ? t.c1 : t.c0;
-                    const float w = __fmul_rn(__fmul_rn((corner & 1) ? t.fc : omc, (corner & 2) ? t.fr : omr), a);
-                    const bool on = level_on && w != 0.f;
-                    const long long texel = t.base + (long long)r * TW + c;
-                    const Agg ag = agg_plan(on ? (unsigned long long)(first + texel) : (1ull << 63) | (unsigned)lane, lane);
-                    const bool leader = on && __ffs(ag.peers) - 1 == lane;
-                    float* dst = dst_level + texel * C;
-                    if (CT) {
-                        float v[NV];
-#pragma unroll
-                        for (int j = 0; j < NV; ++j) v[j] = on ? go[j] * w : 0.f;
-                        agg_sum<NV>(ag, v, lane);
-                        if (leader) red_row<NV, VEC>(dst, v);
-                    } else {
-                        for (int ch = 0; ch < C; ++ch) {
-                            float v[1] = {on ? __ldg(gout + ch) * w : 0.f};
-                            agg_sum<1>(ag, v, lane);
-                            if (leader) atomicAdd(dst + ch, v[0]);
-                        }
-                    }
-                }
-            }
-        }
     }
 }
 
@@ -1175,49 +1131,6 @@ __global__ void __launch_bounds__(TEX_THREADS) mip_level_terms_kernel(const floa
         level_indices[2 * g + 1] = reads ? level_index(ic, k) : nan;
         for (int ch = 0; ch < d.C; ++ch) level_grad_out[g * d.C + ch] = reads ? __fmul_rn(__ldg(grad_out + g * d.C + ch), a) : 0.f;
     }
-}
-
-template <int CT>
-cudaError_t trilinear_forward_ct(const float* texture, const float* pyramid, const float* indices, const float* derivatives,
-                                 float* out, const TexDims& d, int L, cudaStream_t stream)
-{
-    const int row = CT == 2 || CT == 4 ? 4 * CT : 4;
-    const int out_bytes = CT == 3 ? 16 : row;
-    const bool vec = CT && aligned(indices, 8) && aligned(derivatives, 16) && aligned(out, out_bytes) &&
-                     aligned(texture, row) && aligned(pyramid, row);
-    const unsigned blocks = blocks_for(d.total);
-    if constexpr (CT != 0) {   // any C has no vector path
-        if (vec) {
-            texture_trilinear_forward_kernel<CT, true><<<blocks, TEX_THREADS, 0, stream>>>(texture, pyramid, indices,
-                                                                                          derivatives, out, d, L);
-            return cudaGetLastError();
-        }
-    }
-    texture_trilinear_forward_kernel<CT, false><<<blocks, TEX_THREADS, 0, stream>>>(texture, pyramid, indices, derivatives,
-                                                                                       out, d, L);
-    return cudaGetLastError();
-}
-
-template <int CT>
-cudaError_t trilinear_backward_ct(const float* texture, const float* pyramid, const float* indices, const float* derivatives,
-                                  const float* grad_out, float* grad_texture, float* level_grad, float* grad_indices,
-                                  const TexDims& d, int L, cudaStream_t stream)
-{
-    const int row = CT == 2 || CT == 4 ? 4 * CT : 4;
-    const bool vec = CT && aligned(indices, 8) && aligned(derivatives, 16) && aligned(grad_indices, 8) &&
-                     aligned(grad_out, row) && aligned(texture, row) && aligned(pyramid, row) && aligned(grad_texture, row) &&
-                     aligned(level_grad, row);
-    const unsigned blocks = blocks_for(d.total);
-    if constexpr (CT != 0) {
-        if (vec) {
-            texture_trilinear_backward_kernel<CT, true><<<blocks, TEX_THREADS, 0, stream>>>(
-                texture, pyramid, indices, derivatives, grad_out, grad_texture, level_grad, grad_indices, d, L);
-            return cudaGetLastError();
-        }
-    }
-    texture_trilinear_backward_kernel<CT, false><<<blocks, TEX_THREADS, 0, stream>>>(
-            texture, pyramid, indices, derivatives, grad_out, grad_texture, level_grad, grad_indices, d, L);
-    return cudaGetLastError();
 }
 
 }  // namespace
@@ -1264,14 +1177,9 @@ cudaError_t launch_texture_trilinear_forward(const float* texture, const float* 
                                              int* launches)
 {
     const int L = mip_levels(d.TH, d.TW);
-    cudaError_t e;
-    switch (d.C) {
-        case 1: e = trilinear_forward_ct<1>(texture, pyramid, indices, derivatives, out, d, L, stream); break;
-        case 2: e = trilinear_forward_ct<2>(texture, pyramid, indices, derivatives, out, d, L, stream); break;
-        case 3: e = trilinear_forward_ct<3>(texture, pyramid, indices, derivatives, out, d, L, stream); break;
-        case 4: e = trilinear_forward_ct<4>(texture, pyramid, indices, derivatives, out, d, L, stream); break;
-        default: e = trilinear_forward_ct<0>(texture, pyramid, indices, derivatives, out, d, L, stream);
-    }
+    const cudaError_t e = with_ct(d.C, [&](auto ct) {
+        return forward_ct<decltype(ct)::value, true>(texture, pyramid, indices, derivatives, out, d, L, stream);
+    });
     if (e == cudaSuccess) ++*launches;
     return e;
 }
@@ -1296,13 +1204,10 @@ cudaError_t launch_texture_trilinear_backward(const float* texture, const float*
     // the default kernel: both gradients, or under the deterministic flag grad_indices alone (it has no atomics)
     float* gt = deterministic ? nullptr : grad_texture;
     if (gt || grad_indices) {
-        switch (d.C) {
-            case 1: e = trilinear_backward_ct<1>(texture, pyramid, indices, derivatives, grad_out, gt, s.level_grad, grad_indices, d, L, stream); break;
-            case 2: e = trilinear_backward_ct<2>(texture, pyramid, indices, derivatives, grad_out, gt, s.level_grad, grad_indices, d, L, stream); break;
-            case 3: e = trilinear_backward_ct<3>(texture, pyramid, indices, derivatives, grad_out, gt, s.level_grad, grad_indices, d, L, stream); break;
-            case 4: e = trilinear_backward_ct<4>(texture, pyramid, indices, derivatives, grad_out, gt, s.level_grad, grad_indices, d, L, stream); break;
-            default: e = trilinear_backward_ct<0>(texture, pyramid, indices, derivatives, grad_out, gt, s.level_grad, grad_indices, d, L, stream);
-        }
+        e = with_ct(d.C, [&](auto ct) {
+            return backward_ct<decltype(ct)::value, true>(texture, pyramid, indices, derivatives, grad_out, gt, s.level_grad,
+                                                           grad_indices, d, L, stream);
+        });
         if (e != cudaSuccess) return e;
         ++*launches;
     }

@@ -32,18 +32,31 @@ def uvs_to_pixel_indices(uvs, texture_shape, mode='repeat'):
 
 
 class _SampleTexture(torch.autograd.Function):
-    """dirt_texture_sample with its gradient.  texture [TB, TH, TW, C], indices [B, N, 2], contiguous fp32 CUDA."""
+    """dirt_texture_sample, or for mode 'trilinear' dirt_texture_mip_build then dirt_texture_sample_trilinear, with the
+    gradient.  texture [TB, TH, TW, C], indices [B, N, 2], derivatives [B, N, 4] ('trilinear' only), contiguous fp32
+    CUDA.  The trilinear pyramid is built per call and kept for the backward pass."""
 
     @staticmethod
-    def forward(ctx, texture, indices, mode, out_shape):
+    def forward(ctx, texture, indices, mode, out_shape, derivatives=None):
         TB, TH, TW, C = texture.shape
         B, N = indices.shape[0], indices.shape[1]
+        L = _lib.lib()
         out = torch.empty(out_shape, dtype=torch.float32, device=indices.device)
+        pyramid = None
         with torch.cuda.device(indices.device):
-            rc = _lib.lib().dirt_texture_sample(_ptr(texture), _ptr(indices), _ptr(out), TB, TH, TW, C, B, N, mode,
-                                                _stream_ptr(indices.device))
+            stream = _stream_ptr(indices.device)
+            if mode == 'trilinear':
+                pyramid_floats = int(L.dirt_texture_mip_pyramid_bytes(TB, TH, TW, C)) // 4
+                if pyramid_floats:
+                    pyramid = torch.empty(pyramid_floats, dtype=torch.float32, device=indices.device)
+                rc = L.dirt_texture_mip_build(_ptr(texture), _ptr(pyramid), TB, TH, TW, C, stream)
+                _lib.check(rc, 'SampleTextureMipBuild')
+                rc = L.dirt_texture_sample_trilinear(_ptr(texture), _ptr(pyramid), _ptr(indices), _ptr(derivatives),
+                                                     _ptr(out), TB, TH, TW, C, B, N, stream)
+            else:
+                rc = L.dirt_texture_sample(_ptr(texture), _ptr(indices), _ptr(out), TB, TH, TW, C, B, N, mode, stream)
         _lib.check(rc, 'SampleTexture')
-        ctx.save_for_backward(texture, indices)
+        ctx.save_for_backward(texture, indices, pyramid, derivatives)
         ctx.mode = mode
         return out
 
@@ -52,35 +65,41 @@ class _SampleTexture(torch.autograd.Function):
     def backward(ctx, grad_out):
         want_texture, want_indices = ctx.needs_input_grad[:2]
         if not (want_texture or want_indices):
-            return None, None, None, None
-        texture, indices = ctx.saved_tensors
+            return None, None, None, None, None
+        texture, indices, pyramid, derivatives = ctx.saved_tensors
         TB, TH, TW, C = texture.shape
         B, N = indices.shape[0], indices.shape[1]
+        L = _lib.lib()
         grad_out = grad_out.contiguous().to(torch.float32)
         grad_texture = torch.empty_like(texture) if want_texture else None
         grad_indices = torch.empty_like(indices) if want_indices else None
         # grad_indices alone is per lookup and already reproducible; grad_texture needs the sorted path
-        deterministic = want_texture and torch.are_deterministic_algorithms_enabled()
+        deterministic = bool(want_texture and torch.are_deterministic_algorithms_enabled())
         with torch.cuda.device(indices.device):
-            if deterministic:
-                L = _lib.lib()
+            stream = _stream_ptr(indices.device)
+            if ctx.mode == 'trilinear':
+                scratch_bytes = int(L.dirt_texture_sample_trilinear_backward_bytes(TB, TH, TW, C, B, N, int(deterministic)))
+                scratch = torch.empty(scratch_bytes, dtype=torch.uint8, device=indices.device) if scratch_bytes else None
+                rc = L.dirt_texture_sample_trilinear_backward(
+                    _ptr(texture), _ptr(pyramid), _ptr(indices), _ptr(derivatives), _ptr(grad_out), _ptr(grad_texture),
+                    _ptr(grad_indices), TB, TH, TW, C, B, N, int(deterministic), _ptr(scratch), scratch_bytes, stream)
+            elif deterministic:
                 scratch_bytes = max(int(L.dirt_texture_sample_backward_deterministic_bytes(TB, TH, TW, C, B, N, ctx.mode)), 256)
                 scratch = torch.empty(scratch_bytes, dtype=torch.uint8, device=indices.device)
                 rc = L.dirt_texture_sample_backward_deterministic(
                     _ptr(texture), _ptr(indices), _ptr(grad_out), _ptr(grad_texture), _ptr(grad_indices), TB, TH, TW, C, B, N,
-                    ctx.mode, _ptr(scratch), scratch_bytes, _stream_ptr(indices.device))
-                if rc == _lib.ERR_BAD_SHAPE:
-                    # the shapes passed the forward call: what fails are the sorted path's 32-bit limits
-                    raise RuntimeError(
-                        'sample_texture backward: the texture gradient has no deterministic implementation for %d lookups '
-                        'into %d x %d x %d texels (it needs fewer than 2^31 of each), but '
-                        'torch.use_deterministic_algorithms(True) is set' % (B * N, TB, TH, TW))
+                    ctx.mode, _ptr(scratch), scratch_bytes, stream)
             else:
-                rc = _lib.lib().dirt_texture_sample_backward(_ptr(texture), _ptr(indices), _ptr(grad_out),
-                                                             _ptr(grad_texture), _ptr(grad_indices), TB, TH, TW, C, B, N,
-                                                             ctx.mode, _stream_ptr(indices.device))
+                rc = L.dirt_texture_sample_backward(_ptr(texture), _ptr(indices), _ptr(grad_out), _ptr(grad_texture),
+                                                    _ptr(grad_indices), TB, TH, TW, C, B, N, ctx.mode, stream)
+        if deterministic and rc == _lib.ERR_BAD_SHAPE:
+            # the shapes passed the forward call: what fails are the sorted path's 32-bit limits
+            raise RuntimeError(
+                'sample_texture backward: the texture gradient has no deterministic implementation for %d lookups '
+                'into %d x %d x %d texels (it needs fewer than 2^31 of each), but '
+                'torch.use_deterministic_algorithms(True) is set' % (B * N, TB, TH, TW))
         _lib.check(rc, 'SampleTextureGrad')
-        return grad_texture, grad_indices, None, None
+        return grad_texture, grad_indices, None, None, None
 
 
 def _wrapped_difference(d, sizes):
@@ -122,59 +141,6 @@ def index_derivatives(indices, texture_shape):
             return torch.where(mf <= mb, fwd, bwd)
 
         return torch.cat([along(indices.dim() - 2), along(indices.dim() - 3)], -1)
-
-
-class _SampleTextureTrilinear(torch.autograd.Function):
-    """dirt_texture_sample_trilinear with its gradient.  texture [TB, TH, TW, C], indices [B, N, 2], derivatives
-    [B, N, 4], contiguous fp32 CUDA.  The pyramid is built per call and kept for the backward pass."""
-
-    @staticmethod
-    def forward(ctx, texture, indices, derivatives, out_shape):
-        TB, TH, TW, C = texture.shape
-        B, N = indices.shape[0], indices.shape[1]
-        L = _lib.lib()
-        out = torch.empty(out_shape, dtype=torch.float32, device=indices.device)
-        pyramid_floats = int(L.dirt_texture_mip_pyramid_bytes(TB, TH, TW, C)) // 4
-        pyramid = torch.empty(pyramid_floats, dtype=torch.float32, device=indices.device) if pyramid_floats else None
-        with torch.cuda.device(indices.device):
-            stream = _stream_ptr(indices.device)
-            rc = L.dirt_texture_mip_build(_ptr(texture), _ptr(pyramid), TB, TH, TW, C, stream)
-            _lib.check(rc, 'SampleTextureMipBuild')
-            rc = L.dirt_texture_sample_trilinear(_ptr(texture), _ptr(pyramid), _ptr(indices), _ptr(derivatives), _ptr(out),
-                                                 TB, TH, TW, C, B, N, stream)
-        _lib.check(rc, 'SampleTextureTrilinear')
-        ctx.save_for_backward(texture, pyramid, indices, derivatives)
-        return out
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, grad_out):
-        want_texture, want_indices = ctx.needs_input_grad[:2]
-        if not (want_texture or want_indices):
-            return None, None, None, None
-        texture, pyramid, indices, derivatives = ctx.saved_tensors
-        TB, TH, TW, C = texture.shape
-        B, N = indices.shape[0], indices.shape[1]
-        L = _lib.lib()
-        grad_out = grad_out.contiguous().to(torch.float32)
-        grad_texture = torch.empty_like(texture) if want_texture else None
-        grad_indices = torch.empty_like(indices) if want_indices else None
-        deterministic = int(bool(want_texture and torch.are_deterministic_algorithms_enabled()))
-        scratch_bytes = int(L.dirt_texture_sample_trilinear_backward_bytes(TB, TH, TW, C, B, N, deterministic))
-        scratch = torch.empty(scratch_bytes, dtype=torch.uint8, device=indices.device) if scratch_bytes else None
-        with torch.cuda.device(indices.device):
-            rc = L.dirt_texture_sample_trilinear_backward(
-                _ptr(texture), _ptr(pyramid), _ptr(indices), _ptr(derivatives), _ptr(grad_out), _ptr(grad_texture),
-                _ptr(grad_indices), TB, TH, TW, C, B, N, deterministic, _ptr(scratch), scratch_bytes,
-                _stream_ptr(indices.device))
-        if deterministic and rc == _lib.ERR_BAD_SHAPE:
-            # the shapes passed the forward call: what fails are the sorted path's 32-bit limits
-            raise RuntimeError(
-                'sample_texture backward: the texture gradient has no deterministic implementation for %d lookups '
-                'into %d x %d x %d texels (it needs fewer than 2^31 of each), but '
-                'torch.use_deterministic_algorithms(True) is set' % (B * N, TB, TH, TW))
-        _lib.check(rc, 'SampleTextureTrilinearGrad')
-        return grad_texture, grad_indices, None, None
 
 
 def sample_texture(texture, indices, mode='bilinear', derivatives=None):
@@ -235,5 +201,5 @@ def sample_texture(texture, indices, mode='bilinear', derivatives=None):
     flat = indices.reshape(B, N, 2).contiguous()
     tex = (texture if per_item else texture[None]).contiguous()
     if mode == 'trilinear':
-        return _SampleTextureTrilinear.apply(tex, flat, derivatives.detach().reshape(B, N, 4).contiguous(), out_shape)
+        return _SampleTexture.apply(tex, flat, mode, out_shape, derivatives.detach().reshape(B, N, 4).contiguous())
     return _SampleTexture.apply(tex, flat, _MODES[mode], out_shape)
