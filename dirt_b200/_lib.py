@@ -110,6 +110,11 @@ def load(path):
     L.dirt_lighting_forward.argtypes = light_inputs + [vp, i, ll, i, vp]
     L.dirt_lighting_backward.restype = i
     L.dirt_lighting_backward.argtypes = light_inputs + [vp] * 9 + [sz, i, ll, i, vp]
+    ggx_inputs = [i, i, vp, ll, vp, ll, vp, ll, vp, ll] + [vp, i] * 3
+    L.dirt_ggx_lighting_forward.restype = i
+    L.dirt_ggx_lighting_forward.argtypes = ggx_inputs + [vp, i, ll, i, vp]
+    L.dirt_ggx_lighting_backward.restype = i
+    L.dirt_ggx_lighting_backward.argtypes = ggx_inputs + [vp] * 9 + [sz, i, ll, i, vp]
     sh_inputs = [vp, ll, vp, ll, vp, i]
     L.dirt_sh_lighting_workspace_bytes.restype = sz
     L.dirt_sh_lighting_workspace_bytes.argtypes = [i, ll, i]
@@ -138,7 +143,7 @@ EXPORTED_SYMBOLS = ['dirt_error_string', 'dirt_abi_version', 'dirt_workspace_byt
                     'dirt_texture_mip_pyramid_bytes', 'dirt_texture_mip_build', 'dirt_texture_sample_trilinear',
                     'dirt_texture_sample_trilinear_backward_bytes', 'dirt_texture_sample_trilinear_backward',
                     'dirt_rasterise_derivatives', 'dirt_sh_lighting_workspace_bytes', 'dirt_sh_lighting_forward',
-                    'dirt_sh_lighting_backward']
+                    'dirt_sh_lighting_backward', 'dirt_ggx_lighting_forward', 'dirt_ggx_lighting_backward']
 
 
 def error_string(code):

@@ -632,6 +632,112 @@ extern "C" int dirt_lighting_backward(int model, int double_sided, const float* 
     return DIRT_OK;
 }
 
+// element offsets of every per-point buffer stay below 2^62, the chunk count within the grid's x limit
+static bool ggx_shape_ok(int B, long long V, int C, long long sn, long long sp, long long sr, long long ss)
+{
+    if (B < 0 || V < 0 || C <= 0 || sn < 0 || sp < 0 || sr < 0 || ss < 0) return false;
+    const double limit = 4.0e18, rows = (double)B * V;
+    const double widest = (double)(C > 3 ? C : 3) + sn + sp + sr + ss;
+    if (rows * widest > limit || light_chunks(V) > 0x7fffffffll) return false;
+    if ((double)B * light_chunks(V) * (LIGHT_FIXED_PARAMS + (double)C) * sizeof(float) > limit) return false;
+    return true;
+}
+
+// LightArgs of a GGX call: the specular colour in place of the colours, model = point_light
+static LightArgs make_ggx_args(int point_light, int double_sided, const float* normals, long long sn,
+                               const float* positions, long long sp, const float* roughness, long long sr,
+                               const float* specular, long long ss, const float* light, int light_per_item,
+                               const float* light_color, int light_color_per_item, const float* camera,
+                               int camera_per_item, int B, long long V, int C)
+{
+    LightArgs a = make_light_args(point_light != 0, double_sided, normals, sn, positions, sp, specular, ss, light,
+                                  light_per_item, light_color, light_color_per_item, camera, camera_per_item, nullptr,
+                                  0, B, V, C);
+    a.roughness = roughness;
+    a.sr = sr;
+    return a;
+}
+
+// every input is read
+static int ggx_inputs_check(const LightArgs& a)
+{
+    if (!a.normals || !a.positions || !a.roughness || !a.colors || !a.light || !a.light_color || !a.camera)
+        return DIRT_ERR_NULL_POINTER;
+    if ((uintptr_t)a.normals % 4 || (uintptr_t)a.positions % 4 || (uintptr_t)a.roughness % 4 || (uintptr_t)a.colors % 4 ||
+        (uintptr_t)a.light % 4 || (uintptr_t)a.light_color % 4 || (uintptr_t)a.camera % 4)
+        return DIRT_ERR_MISALIGNED;
+    return DIRT_OK;
+}
+
+extern "C" int dirt_ggx_lighting_forward(int point_light, int double_sided, const float* normals,
+                                         long long normals_stride, const float* positions, long long positions_stride,
+                                         const float* roughness, long long roughness_stride, const float* specular,
+                                         long long specular_stride, const float* light, int light_per_item,
+                                         const float* light_color, int light_color_per_item, const float* camera,
+                                         int camera_per_item, float* out, int B, long long V, int C, void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (!ggx_shape_ok(B, V, C, normals_stride, positions_stride, roughness_stride, specular_stride))
+        return DIRT_ERR_BAD_SHAPE;
+    if ((long long)B * V == 0) return DIRT_OK;
+    LightArgs a = make_ggx_args(point_light, double_sided, normals, normals_stride, positions, positions_stride,
+                                roughness, roughness_stride, specular, specular_stride, light, light_per_item,
+                                light_color, light_color_per_item, camera, camera_per_item, B, V, C);
+    a.out = out;
+    const int rc = ggx_inputs_check(a);
+    if (rc != DIRT_OK) return rc;
+    if (!out) return DIRT_ERR_NULL_POINTER;
+    if ((uintptr_t)out % 4) return DIRT_ERR_MISALIGNED;
+    CUDA_TRY(launch_ggx_forward(a, (cudaStream_t)cuda_stream, &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
+extern "C" int dirt_ggx_lighting_backward(int point_light, int double_sided, const float* normals,
+                                          long long normals_stride, const float* positions, long long positions_stride,
+                                          const float* roughness, long long roughness_stride, const float* specular,
+                                          long long specular_stride, const float* light, int light_per_item,
+                                          const float* light_color, int light_color_per_item, const float* camera,
+                                          int camera_per_item, const float* grad_out, float* grad_normals,
+                                          float* grad_positions, float* grad_roughness, float* grad_specular,
+                                          float* grad_light, float* grad_light_color, float* grad_camera,
+                                          void* workspace, size_t workspace_bytes, int B, long long V, int C,
+                                          void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (!ggx_shape_ok(B, V, C, normals_stride, positions_stride, roughness_stride, specular_stride))
+        return DIRT_ERR_BAD_SHAPE;
+    LightArgs a = make_ggx_args(point_light, double_sided, normals, normals_stride, positions, positions_stride,
+                                roughness, roughness_stride, specular, specular_stride, light, light_per_item,
+                                light_color, light_color_per_item, camera, camera_per_item, B, V, C);
+    a.grad_out = grad_out;
+    a.g_normals = grad_normals; a.g_positions = grad_positions; a.g_roughness = grad_roughness;
+    a.g_colors = grad_specular; a.g_light = grad_light; a.g_light_color = grad_light_color; a.g_camera = grad_camera;
+    float* outs[] = {grad_normals, grad_positions, grad_roughness, grad_specular, grad_light, grad_light_color,
+                     grad_camera};
+    for (float* p : outs)
+        if ((uintptr_t)p % 4) return DIRT_ERR_MISALIGNED;
+    const bool params = grad_light || grad_light_color || grad_camera;
+    if ((long long)B * V > 0 && (params || grad_normals || grad_positions || grad_roughness || grad_specular)) {
+        int rc = ggx_inputs_check(a);
+        if (rc != DIRT_OK) return rc;
+        if (!grad_out) return DIRT_ERR_NULL_POINTER;
+        if ((uintptr_t)grad_out % 4) return DIRT_ERR_MISALIGNED;
+        if (params) {
+            if (!workspace) return DIRT_ERR_NULL_POINTER;
+            if ((uintptr_t)workspace % 4) return DIRT_ERR_MISALIGNED;
+            if (workspace_bytes < dirt_lighting_workspace_bytes(B, V, C)) return DIRT_ERR_WORKSPACE_TOO_SMALL;
+            a.partial = static_cast<float*>(workspace);
+        }
+    }
+    // with no points only the memsets of the wanted parameter gradients are enqueued
+    CUDA_TRY(launch_ggx_backward(a, (cudaStream_t)cuda_stream, &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
 // element offsets of every per-point buffer stay below 2^62, the chunk count within the grid's x limit, 9*C an int
 static bool sh_shape_ok(int B, long long V, int C, long long sn, long long sa)
 {

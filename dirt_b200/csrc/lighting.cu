@@ -10,8 +10,9 @@
 // small kernel adds the rows of each item (or of all items, for a shared parameter) in a fixed order.  Two calls on the
 // same inputs therefore give bit-identical parameter gradients.
 //
-// The file also holds the spherical-harmonics environment lighting (dirt_sh_lighting_forward / _backward, DESIGN.md
-// §7.8), which uses the same staging, per-CTA partials and reduction kernel.
+// The file also holds the GGX specular reflectance (dirt_ggx_lighting_forward / _backward, DESIGN.md §7.9) and the
+// spherical-harmonics environment lighting (dirt_sh_lighting_forward / _backward, DESIGN.md §7.8), which use the same
+// staging, per-CTA partials and reduction kernel.
 #include "../../include/dirt_b200.h"
 #include "common.cuh"
 
@@ -403,6 +404,50 @@ void backward_m(const LightArgs& a, cudaStream_t stream)
     else backward_md<MODEL, false>(a, stream);
 }
 
+// The reduction jobs of the wanted parameter gradients of a partial row [light (3), light colour (C), camera (3),
+// shininess (1)]; camera and shininess only where the model has them.
+ReduceJobs param_jobs(const LightArgs& a, bool camera, bool shininess)
+{
+    ReduceJobs jobs;
+    jobs.count = 0;
+    jobs.first[0] = 0;
+    auto add = [&](float* out, int offset, int width, bool per_item) {
+        if (!out) return;
+        const int k = jobs.count++;
+        jobs.out[k] = out; jobs.offset[k] = offset; jobs.width[k] = width; jobs.per_item[k] = per_item;
+        jobs.first[k + 1] = jobs.first[k] + (per_item ? (long long)a.B : 1ll) * width;
+    };
+    add(a.g_light, 0, 3, a.item_light);
+    add(a.g_light_color, 3, a.C, a.item_color);
+    if (camera) add(a.g_camera, 3 + a.C, 3, a.item_camera);
+    if (shininess) add(a.g_shininess, 6 + a.C, 1, a.item_shininess);
+    return jobs;
+}
+
+// with no points: zeroes the jobs' outputs
+cudaError_t zero_params(const ReduceJobs& jobs, cudaStream_t stream)
+{
+    cudaError_t e;
+    for (int k = 0; k < jobs.count; ++k) {
+        const size_t bytes = sizeof(float) * (size_t)(jobs.first[k + 1] - jobs.first[k]);
+        if (bytes && (e = cudaMemsetAsync(jobs.out[k], 0, bytes, stream)) != cudaSuccess) return e;
+    }
+    return cudaSuccess;
+}
+
+// after the point kernel: adds the partial rows of every job in a fixed order
+cudaError_t reduce_params(const LightArgs& a, const ReduceJobs& jobs, cudaStream_t stream, int* launches)
+{
+    if (!jobs.count) return cudaSuccess;
+    const long long total = jobs.first[jobs.count];
+    const unsigned blocks = (unsigned)(total < (1ll << 20) ? total : (1ll << 20));
+    lighting_reduce_kernel<<<blocks, REDUCE_THREADS, 0, stream>>>(a.partial, jobs, total, a.chunks, a.B,
+                                                                  LIGHT_FIXED_PARAMS + a.C);
+    const cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) ++*launches;
+    return e;
+}
+
 }  // namespace
 
 cudaError_t launch_lighting_forward(const LightArgs& a, cudaStream_t stream, int* launches)
@@ -421,27 +466,9 @@ cudaError_t launch_lighting_forward(const LightArgs& a, cudaStream_t stream, int
 cudaError_t launch_lighting_backward(const LightArgs& a, cudaStream_t stream, int* launches)
 {
     const bool sp = a.model == SP;
-    ReduceJobs jobs;
-    jobs.count = 0;
-    jobs.first[0] = 0;
-    auto add = [&](float* out, int offset, int width, bool per_item) {
-        if (!out) return;
-        const int k = jobs.count++;
-        jobs.out[k] = out; jobs.offset[k] = offset; jobs.width[k] = width; jobs.per_item[k] = per_item;
-        jobs.first[k + 1] = jobs.first[k] + (per_item ? (long long)a.B : 1ll) * width;
-    };
-    add(a.g_light, 0, 3, a.item_light);
-    add(a.g_light_color, 3, a.C, a.item_color);
-    if (sp) add(a.g_camera, 3 + a.C, 3, a.item_camera);
-    if (sp) add(a.g_shininess, 6 + a.C, 1, a.item_shininess);
+    const ReduceJobs jobs = param_jobs(a, sp, sp);
     cudaError_t e;
-    if ((long long)a.B * a.V == 0) {
-        for (int k = 0; k < jobs.count; ++k) {
-            const size_t bytes = sizeof(float) * (size_t)(jobs.first[k + 1] - jobs.first[k]);
-            if (bytes && (e = cudaMemsetAsync(jobs.out[k], 0, bytes, stream)) != cudaSuccess) return e;
-        }
-        return cudaSuccess;
-    }
+    if ((long long)a.B * a.V == 0) return zero_params(jobs, stream);
     const bool per_point = a.g_normals || a.g_colors || (a.model != DD && a.g_positions);
     if (!per_point && !jobs.count) return cudaSuccess;
     LightArgs b = a;
@@ -453,15 +480,331 @@ cudaError_t launch_lighting_backward(const LightArgs& a, cudaStream_t stream, in
     }
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     ++*launches;
-    if (jobs.count) {
-        const long long total = jobs.first[jobs.count];
-        const unsigned blocks = (unsigned)(total < (1ll << 20) ? total : (1ll << 20));
-        lighting_reduce_kernel<<<blocks, REDUCE_THREADS, 0, stream>>>(b.partial, jobs, total, a.chunks, a.B,
-                                                                      LIGHT_FIXED_PARAMS + a.C);
-        if ((e = cudaGetLastError()) != cudaSuccess) return e;
-        ++*launches;
+    return reduce_params(b, jobs, stream, launches);
+}
+
+// ---- GGX microfacet specular reflectance (dirt_ggx_lighting_*, DESIGN.md §7.9) ---------------------------------------
+//
+// out_c = pi * light_color_c * F_c * D * Vis * NdotL on lit points (NdotL > 0 and NdotV > 0), else 0: Trowbridge-Reitz D,
+// height-correlated Smith Vis, Schlick F.  Laid out as lighting_forward_kernel / lighting_backward_kernel, with the
+// roughness read directly (one float per point) and the specular colour F0 in place of the colours.  The geometry of a
+// point and the scalar chain down to f = pi D Vis NdotL are evaluated in double precision: near the centre of a sharp
+// highlight D changes by a relative 2 / a^2 per radian between n and h (about 1000 at the roughness clamp), so fp32
+// rounding of the unit vectors alone (a few 1e-8 rad) would cost about 1e-4 in D and more in its gradient.  The channel
+// loop is fp32.  The backward pass recomputes the forward; the parameter gradients go through cta_partial and
+// lighting_reduce_kernel as the other models'.
+
+namespace {
+
+constexpr float GGX_MIN_ROUGHNESS = 0.045f;
+constexpr double GGX_PI = 3.14159265358979323846;
+
+struct UnitVec {
+    double u[3], norm;   // u = x / (|x| + 1e-12), norm = |x|
+};
+
+__device__ __forceinline__ double ddot3(const double a[3], const double b[3])
+{
+    return a[0] * b[0] + a[1] * b[1] + a[2] * b[2];
+}
+
+__device__ __forceinline__ UnitVec unit_vec(const double x[3])
+{
+    UnitVec y;
+    y.norm = sqrt(ddot3(x, x));
+    const double inv = 1.0 / (y.norm + 1e-12);
+#pragma unroll
+    for (int i = 0; i < 3; ++i) y.u[i] = x[i] * inv;
+    return y;
+}
+
+// gx from gu through u = x / (|x| + 1e-12): gu / (|x| + 1e-12) - u (u . gu) / |x|, as torch: no gradient through the
+// norm of a zero vector
+__device__ __forceinline__ void unit_grad(const UnitVec& y, const double gu[3], double gx[3])
+{
+    const double inv = 1.0 / (y.norm + 1e-12), t = y.norm == 0.0 ? 0.0 : ddot3(y.u, gu) / y.norm;
+#pragma unroll
+    for (int i = 0; i < 3; ++i) gx[i] = gu[i] * inv - y.u[i] * t;
+}
+
+__device__ __forceinline__ void cross3(const double a[3], const double b[3], double c[3])
+{
+    c[0] = a[1] * b[2] - a[2] * b[1];
+    c[1] = a[2] * b[0] - a[0] * b[2];
+    c[2] = a[0] * b[1] - a[1] * b[0];
+}
+
+// The forward's intermediates of one point.  The channel factors: out_c = light_color_c (F0_c + (1 - F0_c) m5) f.
+struct Ggx {
+    UnitVec n, v, l, h;           // n.u: the normal after the double-sided flip s
+    double s;
+    double NL, NV, NH, VH, cr[3]; // cr = n x h
+    double a, a2, A, k, D, GV, GL, den, Vis, m;
+    float f, m5;                  // f = pi D Vis NdotL (0 where not lit), m5 = (1 - VdotH)^5
+    bool lit;
+};
+
+template <bool POINT, bool DS>
+__device__ __forceinline__ Ggx ggx_shade(const LightArgs& a, long long b, const float n[3], const float p[3], float r)
+{
+    Ggx g;
+    const float* L = item_row(a.light, a.item_light, b, 3);
+    const float* cam = item_row(a.camera, a.item_camera, b, 3);
+    double x[3];
+#pragma unroll
+    for (int i = 0; i < 3; ++i) x[i] = n[i];
+    g.n = unit_vec(x);
+#pragma unroll
+    for (int i = 0; i < 3; ++i) x[i] = (double)__ldg(cam + i) - (double)p[i];
+    g.v = unit_vec(x);
+#pragma unroll
+    for (int i = 0; i < 3; ++i) x[i] = POINT ? (double)__ldg(L + i) - (double)p[i] : -(double)__ldg(L + i);
+    g.l = unit_vec(x);
+    // turned to face the camera (no flip at exactly 0)
+    g.s = DS && ddot3(g.n.u, g.v.u) < 0.0 ? -1.0 : 1.0;
+#pragma unroll
+    for (int i = 0; i < 3; ++i) g.n.u[i] *= g.s;
+    g.NV = ddot3(g.n.u, g.v.u);
+    g.NL = ddot3(g.n.u, g.l.u);
+    g.lit = g.NL > 0.0 && g.NV > 0.0;
+#pragma unroll
+    for (int i = 0; i < 3; ++i) x[i] = g.l.u[i] + g.v.u[i];
+    g.h = unit_vec(x);
+    g.NH = ddot3(g.n.u, g.h.u);
+    g.VH = ddot3(g.v.u, g.h.u);
+    cross3(g.n.u, g.h.u, g.cr);
+    g.a = r < GGX_MIN_ROUGHNESS ? (double)GGX_MIN_ROUGHNESS : (double)r;   // NaN passes through, as torch's clamp
+    g.a2 = g.a * g.a;
+    g.A = g.a2 * g.a2;
+    // k = A NdotH^2 + |n x h|^2 rather than NdotH^2 (A - 1) + 1, which cancels for small A
+    g.k = g.A * g.NH * g.NH + ddot3(g.cr, g.cr);
+    g.D = g.A / (GGX_PI * g.k * g.k);
+    g.GV = sqrt(g.NV * g.NV * (1.0 - g.A) + g.A);
+    g.GL = sqrt(g.NL * g.NL * (1.0 - g.A) + g.A);
+    g.den = g.NL * g.GV + g.NV * g.GL;
+    g.Vis = 0.5 / g.den;
+    g.m = 1.0 - g.VH;
+    const double m2 = g.m * g.m;
+    g.m5 = (float)(m2 * m2 * g.m);
+    g.f = g.lit ? (float)(GGX_PI * g.D * g.Vis * g.NL) : 0.f;
+    return g;
+}
+
+__device__ __forceinline__ float ggx_fresnel(float F0, float m5)
+{
+    return F0 + (1.f - F0) * m5;
+}
+
+// CT = 3 (specular colours and outputs staged like the other rows) or 0 (any C, one channel at a time)
+template <bool POINT, bool DS, int CT>
+__global__ void __launch_bounds__(LIGHT_THREADS) ggx_forward_kernel(LightArgs a)
+{
+    __shared__ float stage[LIGHT_THREADS * 3];
+    const int lane = threadIdx.x & 31;
+    float* s = stage + (threadIdx.x & ~31) * 3;
+    const long long v0 = (long long)blockIdx.x * LIGHT_THREADS + (threadIdx.x & ~31);
+    if (v0 >= a.V) return;   // the whole warp
+    const int n = (int)(a.V - v0 < 32 ? a.V - v0 : 32);
+    const int C = CT ? CT : a.C;
+    for (long long b = blockIdx.y; b < a.B; b += gridDim.y) {
+        const long long row0 = b * a.V + v0, row = row0 + lane;
+        float nrm[3], pos[3];
+        stage_load<3>(a.normals, a.sn, row0, n, s, lane, nrm);
+        stage_load<3>(a.positions, a.sp, row0, n, s, lane, pos);
+        const float r = lane < n ? __ldg(a.roughness + row * a.sr) : 0.f;
+        const Ggx g = ggx_shade<POINT, DS>(a, b, nrm, pos, r);
+        const float* lc = item_row(a.light_color, a.item_color, b, C);
+        if (CT == 3) {
+            float F0[3], o[3];
+            stage_load<3>(a.colors, a.sc, row0, n, s, lane, F0);
+#pragma unroll
+            for (int c = 0; c < 3; ++c) o[c] = g.lit ? __ldg(lc + c) * ggx_fresnel(F0[c], g.m5) * g.f : 0.f;
+            stage_store<3>(a.out, row0, n, s, lane, o);
+        } else if (lane < n) {
+            for (int c = 0; c < C; ++c)
+                a.out[row * C + c] =
+                    g.lit ? __ldg(lc + c) * ggx_fresnel(__ldg(a.colors + row * a.sc + c), g.m5) * g.f : 0.f;
+        }
     }
-    return cudaSuccess;
+}
+
+template <bool POINT, bool DS, int CT>
+__global__ void __launch_bounds__(LIGHT_THREADS) ggx_backward_kernel(LightArgs a)
+{
+    __shared__ float stage[LIGHT_THREADS * 3];
+    __shared__ float red[WARPS * RED_SLOTS];
+    const int lane = threadIdx.x & 31;
+    float* s = stage + (threadIdx.x & ~31) * 3;
+    const long long v0 = (long long)blockIdx.x * LIGHT_THREADS + (threadIdx.x & ~31);
+    const int n = v0 >= a.V ? 0 : (int)(a.V - v0 < 32 ? a.V - v0 : 32);   // warp-uniform; 0: the warp only helps reduce
+    const bool live = lane < n;
+    const int C = CT ? CT : a.C;
+    const int P = LIGHT_FIXED_PARAMS + a.C;
+    for (long long b = blockIdx.y; b < a.B; b += gridDim.y) {
+        const long long row0 = b * a.V + v0, row = row0 + lane;
+        float nrm[3] = {0.f, 0.f, 0.f}, pos[3] = {0.f, 0.f, 0.f};
+        if (n) {
+            stage_load<3>(a.normals, a.sn, row0, n, s, lane, nrm);
+            stage_load<3>(a.positions, a.sp, row0, n, s, lane, pos);
+        }
+        const float r = live ? __ldg(a.roughness + row * a.sr) : 0.f;
+        const Ggx g = ggx_shade<POINT, DS>(a, b, nrm, pos, r);
+        const bool lit = live && g.lit;
+        const float* lc = item_row(a.light_color, a.item_color, b, C);
+
+        // out_c = q_c f with q_c = light_color_c F_c, F_c = F0_c + (1 - F0_c) m5:
+        // d/df = sum_c g_c q_c, d/dm5 = f sum_c g_c light_color_c (1 - F0_c), d/dF0_c = g_c light_color_c (1 - m5) f
+        float gf = 0.f, gm5 = 0.f, glc3[3] = {0.f, 0.f, 0.f};
+        if (CT == 3) {
+            float go[3] = {0.f, 0.f, 0.f}, F0[3] = {0.f, 0.f, 0.f}, gF0[3];
+            if (n) {
+                stage_load<3>(a.grad_out, 3, row0, n, s, lane, go);
+                stage_load<3>(a.colors, a.sc, row0, n, s, lane, F0);
+            }
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                const float gl = lit ? go[c] * __ldg(lc + c) : 0.f, F = ggx_fresnel(F0[c], g.m5);
+                gf += gl * F;
+                gm5 += gl * (1.f - F0[c]);
+                gF0[c] = lit ? gl * (1.f - g.m5) * g.f : 0.f;
+                glc3[c] = lit ? go[c] * F * g.f : 0.f;
+            }
+            if (a.g_colors && n) stage_store<3>(a.g_colors, row0, n, s, lane, gF0);
+        } else if (live) {
+            for (int c = 0; c < C; ++c) {
+                const float F0 = __ldg(a.colors + row * a.sc + c);
+                const float gl = lit ? __ldg(a.grad_out + row * C + c) * __ldg(lc + c) : 0.f;
+                gf += gl * ggx_fresnel(F0, g.m5);
+                gm5 += gl * (1.f - F0);
+                if (a.g_colors) a.g_colors[row * C + c] = lit ? gl * (1.f - g.m5) * g.f : 0.f;
+            }
+        }
+
+        // the scalar chain down to the unit vectors, then to the per-point inputs and the parameters
+        float gn[3] = {0.f, 0.f, 0.f}, gp[3] = {0.f, 0.f, 0.f}, gL[3] = {0.f, 0.f, 0.f}, gcam[3] = {0.f, 0.f, 0.f};
+        float gr = 0.f;
+        if (lit) {
+            const double gfd = gf, gVH = -(double)gm5 * (double)g.f * 5.0 * (g.m * g.m) * (g.m * g.m);
+            const double gD = gfd * GGX_PI * g.Vis * g.NL, gVis = gfd * GGX_PI * g.D * g.NL;
+            double gNL = gfd * GGX_PI * g.D * g.Vis;
+            // Vis = 0.5 / den, den = NL GV + NV GL, G* = sqrt(N*^2 (1 - A) + A)
+            const double gden = -gVis * g.Vis / g.den;
+            gNL += gden * g.GV;
+            double gNV = gden * g.GL;
+            const double gQV = gden * g.NL / (2.0 * g.GV), gQL = gden * g.NV / (2.0 * g.GL);
+            gNV += gQV * 2.0 * g.NV * (1.0 - g.A);
+            gNL += gQL * 2.0 * g.NL * (1.0 - g.A);
+            double gA = gQV * (1.0 - g.NV * g.NV) + gQL * (1.0 - g.NL * g.NL);
+            // D = A / (pi k^2), k = A NH^2 + |cr|^2
+            gA += gD / (GGX_PI * g.k * g.k);
+            const double gk = -2.0 * gD * g.D / g.k;
+            gA += gk * g.NH * g.NH;
+            const double gNH = gk * 2.0 * g.A * g.NH;
+            double gcr[3], t[3], gN[3], gh[3], gv[3], gl[3];
+#pragma unroll
+            for (int i = 0; i < 3; ++i) gcr[i] = 2.0 * gk * g.cr[i];
+            cross3(g.h.u, gcr, gN);   // d(n x h)/dn
+            cross3(gcr, g.n.u, gh);   // d(n x h)/dh
+#pragma unroll
+            for (int i = 0; i < 3; ++i) {
+                gN[i] += gNH * g.h.u[i] + gNV * g.v.u[i] + gNL * g.l.u[i];
+                gh[i] += gNH * g.n.u[i] + gVH * g.v.u[i];
+                gv[i] = gVH * g.h.u[i] + gNV * g.n.u[i];
+                gl[i] = gNL * g.n.u[i];
+            }
+            unit_grad(g.h, gh, t);   // h = unit(l + v)
+#pragma unroll
+            for (int i = 0; i < 3; ++i) {
+                gv[i] += t[i];
+                gl[i] += t[i];
+            }
+            unit_grad(g.n, gN, t);   // n = s unit(n_in): the flip's sign twice inside unit_grad, once outside
+#pragma unroll
+            for (int i = 0; i < 3; ++i) gn[i] = (float)(g.s * t[i]);
+            double gtc[3];
+            unit_grad(g.v, gv, gtc);   // v = unit(camera - p)
+            unit_grad(g.l, gl, t);     // l = unit(light - p) or unit(-light)
+#pragma unroll
+            for (int i = 0; i < 3; ++i) {
+                gcam[i] = (float)gtc[i];
+                gp[i] = (float)(POINT ? -gtc[i] - t[i] : -gtc[i]);
+                gL[i] = (float)(POINT ? t[i] : -t[i]);
+            }
+            // A = (a a)^2; torch's clamp passes the gradient at exactly the minimum
+            gr = r >= GGX_MIN_ROUGHNESS ? (float)(gA * 4.0 * g.a2 * g.a) : 0.f;
+        }
+        if (n) {
+            if (a.g_normals) stage_store<3>(a.g_normals, row0, n, s, lane, gn);
+            if (a.g_positions) stage_store<3>(a.g_positions, row0, n, s, lane, gp);
+        }
+        if (a.g_roughness && live) a.g_roughness[row] = gr;
+
+        // this CTA's sums of the parameter gradients (lanes without a lit point add zeros)
+        if (a.partial) {
+            float* dst = a.partial + ((long long)b * a.chunks + blockIdx.x) * P;
+            if (a.g_light) cta_partial<3>(gL, red, dst);
+            if (a.g_light_color) {
+                if (CT == 3) {
+                    cta_partial<3>(glc3, red, dst + 3);
+                } else {
+                    for (int c = 0; c < C; ++c) {
+                        const float v[1] = {lit ? __ldg(a.grad_out + row * C + c) *
+                                                      ggx_fresnel(__ldg(a.colors + row * a.sc + c), g.m5) * g.f : 0.f};
+                        cta_partial<1>(v, red, dst + 3 + c);
+                    }
+                }
+            }
+            if (a.g_camera) cta_partial<3>(gcam, red, dst + 3 + C);
+        }
+    }
+}
+
+template <bool POINT, bool DS>
+void ggx_launch(const LightArgs& a, bool forward, cudaStream_t stream)
+{
+    if (forward) {
+        if (a.C == 3) ggx_forward_kernel<POINT, DS, 3><<<point_grid(a), LIGHT_THREADS, 0, stream>>>(a);
+        else ggx_forward_kernel<POINT, DS, 0><<<point_grid(a), LIGHT_THREADS, 0, stream>>>(a);
+    } else {
+        if (a.C == 3) ggx_backward_kernel<POINT, DS, 3><<<point_grid(a), LIGHT_THREADS, 0, stream>>>(a);
+        else ggx_backward_kernel<POINT, DS, 0><<<point_grid(a), LIGHT_THREADS, 0, stream>>>(a);
+    }
+}
+
+void ggx_dispatch(const LightArgs& a, bool forward, cudaStream_t stream)
+{
+    if (a.model) {
+        if (a.double_sided) ggx_launch<true, true>(a, forward, stream);
+        else ggx_launch<true, false>(a, forward, stream);
+    } else {
+        if (a.double_sided) ggx_launch<false, true>(a, forward, stream);
+        else ggx_launch<false, false>(a, forward, stream);
+    }
+}
+
+}  // namespace
+
+cudaError_t launch_ggx_forward(const LightArgs& a, cudaStream_t stream, int* launches)
+{
+    if ((long long)a.B * a.V == 0) return cudaSuccess;
+    ggx_dispatch(a, true, stream);
+    const cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) ++*launches;
+    return e;
+}
+
+cudaError_t launch_ggx_backward(const LightArgs& a, cudaStream_t stream, int* launches)
+{
+    const ReduceJobs jobs = param_jobs(a, true, false);
+    if ((long long)a.B * a.V == 0) return zero_params(jobs, stream);
+    if (!a.g_normals && !a.g_positions && !a.g_colors && !a.g_roughness && !jobs.count) return cudaSuccess;
+    LightArgs b = a;
+    if (!jobs.count) b.partial = nullptr;
+    ggx_dispatch(b, false, stream);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+    ++*launches;
+    return reduce_params(b, jobs, stream, launches);
 }
 
 // ---- spherical-harmonics environment lighting (dirt_sh_lighting_*, DESIGN.md §7.8) ------------------------------------

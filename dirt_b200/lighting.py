@@ -7,7 +7,9 @@ reflectance models run CUDA kernels (dirt_lighting_forward / _backward) when the
 shapes `cuda_route` accepts, and their torch restatements (`_diffuse_directional`, `_specular_directional`,
 `_diffuse_point`) otherwise; see DESIGN.md §7.2.  `diffuse_spherical_harmonics` (order-2 SH environment lighting) is
 routed the same way, between dirt_sh_lighting_forward / _backward and `_diffuse_spherical_harmonics`; see DESIGN.md
-§7.8.  `split_vertices_by_face` is torch code.
+§7.8.  So are `specular_ggx_directional` and `specular_ggx_point` (GGX microfacet specular), between
+dirt_ggx_lighting_forward / _backward and `_specular_ggx`; see DESIGN.md §7.9.  `split_vertices_by_face` is torch
+code.
 """
 import math
 from collections import namedtuple
@@ -116,6 +118,47 @@ def _diffuse_point(vertex_positions, vertex_normals, vertex_colors, light_positi
     return light_color[..., None, :] * vertex_colors * _cosine_term(cosines, double_sided)[..., None]
 
 
+def _unit(x):
+    return x / (torch.linalg.norm(x, dim=-1, keepdim=True) + 1.e-12)
+
+
+GGX_MIN_ROUGHNESS = 0.045
+
+
+def _specular_ggx(vertex_positions, vertex_normals, vertex_roughness, vertex_specular, light, light_color,
+                  camera_position, point_light, double_sided):
+    """The torch restatement of `specular_ggx_directional` (point_light False, `light` a direction) and
+    `specular_ggx_point` (`light` a position): their CPU implementation and their specification.  Takes tensors of one
+    dtype and device, and keeps that dtype (the tests evaluate it in float64).
+
+    The output is pi * light_color * F * D * Vis * NdotL where NdotL > 0 and NdotV > 0, else 0.  The factor pi makes
+    `diffuse_directional(albedo) + specular_ggx_directional(...)` the usual diffuse-plus-GGX model under one light
+    intensity: `diffuse_directional` returns albedo * I * cos, which is Lambert's radiance albedo / pi * I * cos times pi.
+    Inside the `where`, the points it masks take safe values, so that their gradients are exactly 0 and not NaN."""
+    n = _unit(vertex_normals)
+    v = _unit(camera_position[..., None, :] - vertex_positions)
+    l = _unit(light[..., None, :] - vertex_positions) if point_light else _unit(-light[..., None, :])
+    if double_sided:   # turned to face the camera; no flip at exactly 0
+        n = torch.where((n * v).sum(-1, keepdim=True) < 0, -n, n)
+    n_dot_l = (n * l).sum(-1, keepdim=True)
+    n_dot_v = (n * v).sum(-1, keepdim=True)
+    h = _unit(l + v)
+    n_dot_h = (n * h).sum(-1, keepdim=True)
+    v_dot_h = (v * h).sum(-1, keepdim=True)
+    lit = (n_dot_l > 0) & (n_dot_v > 0)
+    n_dot_l, n_dot_v = torch.where(lit, n_dot_l, 1.), torch.where(lit, n_dot_v, 1.)
+    a = vertex_roughness.clamp(min=GGX_MIN_ROUGHNESS)
+    alpha2 = (a * a).square()
+    # k = NdotH^2 (alpha2 - 1) + 1 for unit n and h, in a form that does not cancel for small alpha2
+    k = torch.where(lit, alpha2 * n_dot_h.square() + torch.linalg.cross(n, h, dim=-1).square().sum(-1, keepdim=True), 1.)
+    D = alpha2 / (math.pi * k * k)
+    vis = 0.5 / (n_dot_l * torch.sqrt(n_dot_v.square() * (1 - alpha2) + alpha2) +
+                 n_dot_v * torch.sqrt(n_dot_l.square() * (1 - alpha2) + alpha2))
+    m = 1 - v_dot_h
+    fresnel = vertex_specular + (1 - vertex_specular) * (m * m).square() * m
+    return torch.where(lit, math.pi * light_color[..., None, :] * fresnel * D * vis * n_dot_l, 0.)
+
+
 def _sh_basis(n):
     """The real order-2 spherical harmonics without the Condon-Shortley phase at n [..., 3], used as given (not
     normalised): [..., 9], index k = l^2 + l + m."""
@@ -143,7 +186,7 @@ def _diffuse_spherical_harmonics(vertex_normals, vertex_colors, coefficients):
 Route = namedtuple('Route', 'lead B V C per_item')
 
 
-def cuda_route(point_shapes, item_shapes, devices):
+def cuda_route(point_shapes, item_shapes, devices, point_widths=None):
     """Whether a reflectance call runs the CUDA kernels, decided from shapes and devices alone.
 
     point_shapes: the shapes of the per-point tensors, colours (or reflectivities) last: [*, V, 3], ..., [*, V, C].
@@ -151,6 +194,8 @@ def cuda_route(point_shapes, item_shapes, devices):
         (the shininess, a scalar per item) or a tuple of those (the tail (9, 'C') of SH coefficients); each must have
         leading shape exactly `*` (one value per item) or none (shared by all points).
     devices: the devices of all the tensors; they must be one CUDA device.
+    point_widths: the last dimension each per-point tensor must have, an int or 'C'; by default 3 for every one but the
+        last, which is C (the GGX model's roughness is 1 wide).
 
     Returns a Route (lead = `*`, B = its product, V, C, per_item flags in the order of item_shapes) or None."""
     devices = list(devices)
@@ -162,9 +207,11 @@ def cuda_route(point_shapes, item_shapes, devices):
     lead, V, C = first[:-2], first[-2], tuple(point_shapes[-1])[-1] if len(point_shapes[-1]) else 0
     if C < 1:
         return None
-    for k, shape in enumerate(point_shapes):
+    if point_widths is None:
+        point_widths = [3] * (len(point_shapes) - 1) + ['C']
+    for shape, width in zip(point_shapes, point_widths):
         shape = tuple(shape)
-        if len(shape) != len(first) or shape[:-1] != first[:-1] or shape[-1] != (C if k == len(point_shapes) - 1 else 3):
+        if len(shape) != len(first) or shape[:-1] != first[:-1] or shape[-1] != (C if width == 'C' else width):
             return None
     per_item = []
     for shape, width in item_shapes:
@@ -186,9 +233,10 @@ def cuda_route(point_shapes, item_shapes, devices):
     return Route(lead, B, V, C, tuple(per_item))
 
 
-def _route(points, items):
+def _route(points, items, point_widths=None):
     tensors = list(points) + [t for t, _ in items]
-    return cuda_route([t.shape for t in points], [(t.shape, w) for t, w in items], [t.device for t in tensors])
+    return cuda_route([t.shape for t in points], [(t.shape, w) for t, w in items], [t.device for t in tensors],
+                      point_widths)
 
 
 def _rows(t, k):
@@ -356,6 +404,115 @@ def diffuse_point(vertex_positions, vertex_normals, vertex_colors, light_positio
         return _diffuse_point(vertex_positions, vertex_normals, vertex_colors, light_position, light_color, double_sided)
     return _reflectance(_lib.LIGHT_DIFFUSE_POINT, double_sided, route, vertex_normals, vertex_colors, light_position,
                         light_color, vertex_positions)
+
+
+# ---- the CUDA path of the GGX specular model -------------------------------------------------------------------------
+
+def _ggx_inputs(point_light, double_sided, route, normals, positions, roughness, specular, light, light_color, camera):
+    """The input arguments of dirt_ggx_lighting_forward / _backward, in their order."""
+    stride = lambda t: t.stride(0) if t.shape[0] > 1 else 0
+    return [int(bool(point_light)), int(bool(double_sided)), _ptr(normals), stride(normals), _ptr(positions),
+            stride(positions), _ptr(roughness), stride(roughness), _ptr(specular), stride(specular), _ptr(light),
+            int(route.per_item[0]), _ptr(light_color), int(route.per_item[1]), _ptr(camera), int(route.per_item[2])]
+
+
+def _restate_ggx(point_light, double_sided, route, normals, positions, roughness, specular, light, light_color, camera):
+    """The restatement on the op's own inputs (flattened per-point rows, per-item rows)."""
+    lead, V, C = route.lead, route.V, route.C
+    point = lambda t, w: t.reshape(lead + (V, w))
+    item = lambda t, per_item, w: t.reshape(lead + (w,)) if per_item else t
+    return _specular_ggx(point(positions, 3), point(normals, 3), point(roughness, 1), point(specular, C),
+                         item(light, route.per_item[0], 3), item(light_color, route.per_item[1], C),
+                         item(camera, route.per_item[2], 3), point_light, double_sided)
+
+
+class _SpecularGGX(torch.autograd.Function):
+    """dirt_ggx_lighting_forward with its gradient.  Per-point inputs are [rows, k] with unit stride along k; per-item
+    inputs contiguous [B, k] or shared [k].  The node keeps only its inputs: the backward kernel recomputes the forward
+    from them."""
+
+    @staticmethod
+    def forward(ctx, point_light, double_sided, route, normals, positions, roughness, specular, light, light_color,
+                camera):
+        out = torch.empty(route.lead + (route.V, route.C), dtype=torch.float32, device=normals.device)
+        inputs = (normals, positions, roughness, specular, light, light_color, camera)
+        with torch.cuda.device(normals.device):
+            rc = _lib.lib().dirt_ggx_lighting_forward(*_ggx_inputs(point_light, double_sided, route, *inputs), _ptr(out),
+                                                      route.B, route.V, route.C, _stream(normals.device))
+        _lib.check(rc, 'SpecularGGX')
+        ctx.save_for_backward(*inputs)
+        ctx.point_light, ctx.double_sided, ctx.route = point_light, double_sided, route
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        want = ctx.needs_input_grad[3:]
+        if not any(want):
+            return (None,) * 10
+        inputs = ctx.saved_tensors
+        if torch.is_grad_enabled():
+            # create_graph=True: differentiable gradients through the restatement
+            out = _restate_ggx(ctx.point_light, ctx.double_sided, ctx.route, *inputs)
+            wanted = [t for t, w in zip(inputs, want) if w]
+            grads = iter(torch.autograd.grad(out, wanted, grad_out, create_graph=True))
+            return (None,) * 3 + tuple(next(grads) if w else None for w in want)
+        route = ctx.route
+        dev = inputs[0].device
+        grads = [torch.empty(t.shape, dtype=torch.float32, device=dev) if w else None for t, w in zip(inputs, want)]
+        lib = _lib.lib()
+        ws_bytes = int(lib.dirt_lighting_workspace_bytes(route.B, route.V, route.C)) if any(want[4:]) else 0
+        workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=dev) if ws_bytes else None
+        grad_out = grad_out.to(torch.float32).contiguous()
+        with torch.cuda.device(dev):
+            rc = lib.dirt_ggx_lighting_backward(*_ggx_inputs(ctx.point_light, ctx.double_sided, route, *inputs),
+                                                _ptr(grad_out), *[_ptr(g) for g in grads], _ptr(workspace), ws_bytes,
+                                                route.B, route.V, route.C, _stream(dev))
+        _lib.check(rc, 'SpecularGGXGrad')
+        return (None,) * 3 + tuple(grads)
+
+
+def _specular_ggx_call(point_light, vertex_positions, vertex_normals, vertex_roughness, vertex_specular, light,
+                       light_color, camera_position, double_sided):
+    vertex_positions = torch.as_tensor(vertex_positions, dtype=torch.float32)
+    dev = vertex_positions.device
+    f = lambda t: torch.as_tensor(t, dtype=torch.float32, device=dev)
+    vertex_normals, vertex_roughness, vertex_specular = f(vertex_normals), f(vertex_roughness), f(vertex_specular)
+    light, light_color, camera_position = f(light), f(light_color), f(camera_position)
+    route = _route([vertex_positions, vertex_normals, vertex_roughness, vertex_specular],
+                   [(light, 3), (light_color, 'C'), (camera_position, 3)], [3, 3, 1, 'C'])
+    if route is None:
+        return _specular_ggx(vertex_positions, vertex_normals, vertex_roughness, vertex_specular, light, light_color,
+                             camera_position, point_light, double_sided)
+    C = route.C
+    item = lambda t, per_item: (t.reshape((route.B,) + t.shape[len(route.lead):]) if per_item else t).contiguous()
+    return _SpecularGGX.apply(point_light, double_sided, route, _rows(vertex_normals, 3), _rows(vertex_positions, 3),
+                              _rows(vertex_roughness, 1), _rows(vertex_specular, C), item(light, route.per_item[0]),
+                              item(light_color, route.per_item[1]), item(camera_position, route.per_item[2]))
+
+
+def specular_ggx_directional(vertex_positions, vertex_normals, vertex_roughness, vertex_specular, light_direction,
+                             light_color, camera_position, double_sided=False, name=None):
+    """GGX microfacet specular reflectance (Cook-Torrance: Trowbridge-Reitz distribution, height-correlated Smith
+    visibility, Schlick Fresnel) under one directional light travelling along `light_direction`.
+
+    vertex_positions, vertex_normals [*, V, 3], vertex_roughness [*, V, 1] (perceptual roughness a, clamped below at
+    0.045; the distribution uses a^4), vertex_specular [*, V, C] (F0), light_direction and camera_position [*, 3] or
+    [3], light_color [*, C] or [C] -> [*, V, C]: pi * light_color * F * D * Vis * (n . l) where n . l > 0 and n . v > 0,
+    else 0.  With the factor pi, `diffuse_directional(albedo) + specular_ggx_directional(...)` is the usual
+    diffuse-plus-GGX model under one light intensity.  double_sided turns normals facing away from the camera towards
+    it.  On CUDA in these shapes fused kernels compute it, with reproducible parameter gradients; any other call runs
+    the torch restatement `_specular_ggx`."""
+    return _specular_ggx_call(False, vertex_positions, vertex_normals, vertex_roughness, vertex_specular,
+                              light_direction, light_color, camera_position, double_sided)
+
+
+def specular_ggx_point(vertex_positions, vertex_normals, vertex_roughness, vertex_specular, light_position, light_color,
+                       camera_position, double_sided=False, name=None):
+    """As `specular_ggx_directional`, under one point light at `light_position`: l = normalize(light_position - p)
+    points from the surface towards the light (unlike `diffuse_point`'s incident direction), and, like
+    `diffuse_point`, there is no distance falloff."""
+    return _specular_ggx_call(True, vertex_positions, vertex_normals, vertex_roughness, vertex_specular,
+                              light_position, light_color, camera_position, double_sided)
 
 
 # ---- the CUDA path of the spherical-harmonics lighting --------------------------------------------------------------

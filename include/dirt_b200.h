@@ -337,6 +337,52 @@ int dirt_lighting_backward(int model, int double_sided,
                            float* grad_light, float* grad_light_color, float* grad_camera, float* grad_shininess,
                            void* workspace, size_t workspace_bytes, int B, long long V, int C, void* cuda_stream);
 
+/* GGX microfacet specular reflectance (Cook-Torrance with the Trowbridge-Reitz distribution, height-correlated Smith
+ * visibility and Schlick's Fresnel term) under one directional (point_light == 0) or point light, one value per point
+ * and channel.  B items of V points each, C channels:
+ *   normals, positions   float32 [B*V, 3], row stride normals_stride / positions_stride floats, unit stride along the row
+ *   roughness            float32 [B*V, 1] (perceptual roughness), row stride roughness_stride
+ *   specular             float32 [B*V, C] (the specular colour F0), row stride specular_stride
+ *   light                float32 [B, 3] (light_per_item != 0) or [3] (shared): direction, or position (point light)
+ *   light_color          float32 [B, C] or [C];  camera float32 [B, 3] or [3]
+ *   out, grad_out        float32 [B*V, C], contiguous
+ * Per point, with unit(x) = x / (|x| + 1e-12):
+ *   n = unit(normal), v = unit(camera - p), l = unit(-light) (directional) or unit(light - p) (point; no falloff)
+ *   double_sided and n . v < 0: n = -n
+ *   h = unit(l + v), a = max(roughness, 0.045), A = a^4, k = A (n . h)^2 + |n x h|^2, D = A / (pi k^2)
+ *   Vis = 0.5 / ((n . l) sqrt((n . v)^2 (1 - A) + A) + (n . v) sqrt((n . l)^2 (1 - A) + A))
+ *   F_c = F0_c + (1 - F0_c) (1 - v . h)^5
+ *   out_c = pi light_color_c F_c D Vis (n . l) where n . l > 0 and n . v > 0, else 0
+ * The geometry and the scalar chain are evaluated in double precision, the channels in fp32; the result is not
+ * bit-identical to any torch evaluation.
+ * Backward: the gradients torch autograd gives for the same expressions: none where the output is masked to 0, none to
+ * a roughness below 0.045 (the full one at exactly 0.045), none through a zero vector's norm.  Each gradient output
+ * may be NULL, and its work is skipped; the per-point ones are contiguous [B*V, k], the parameter ones have the shape
+ * of their input.  Parameter gradients are summed in a fixed order (per-CTA partials in the workspace, then one
+ * reduction kernel): repeated calls give bit-identical results.  The workspace, of at least
+ * dirt_lighting_workspace_bytes(B, V, C) bytes, is needed only when a parameter gradient is wanted.
+ * B = 0 or V = 0: nothing is launched (the backward call still zeroes the wanted parameter gradients).
+ * All pointers 4-byte aligned; row strides >= 0. */
+int dirt_ggx_lighting_forward(int point_light, int double_sided,
+                              const float* normals, long long normals_stride,
+                              const float* positions, long long positions_stride,
+                              const float* roughness, long long roughness_stride,
+                              const float* specular, long long specular_stride,
+                              const float* light, int light_per_item, const float* light_color, int light_color_per_item,
+                              const float* camera, int camera_per_item,
+                              float* out, int B, long long V, int C, void* cuda_stream);
+int dirt_ggx_lighting_backward(int point_light, int double_sided,
+                               const float* normals, long long normals_stride,
+                               const float* positions, long long positions_stride,
+                               const float* roughness, long long roughness_stride,
+                               const float* specular, long long specular_stride,
+                               const float* light, int light_per_item, const float* light_color, int light_color_per_item,
+                               const float* camera, int camera_per_item,
+                               const float* grad_out,
+                               float* grad_normals, float* grad_positions, float* grad_roughness, float* grad_specular,
+                               float* grad_light, float* grad_light_color, float* grad_camera,
+                               void* workspace, size_t workspace_bytes, int B, long long V, int C, void* cuda_stream);
+
 /* Spherical-harmonics environment lighting: Lambertian reflected radiance under order-2 SH incident radiance
  * (Ramamoorthi & Hanrahan 2001), one value per point and channel.  B items of V points each, C channels:
  *   normals              float32 [B*V, 3], row stride normals_stride floats, unit stride along the row; used as given
