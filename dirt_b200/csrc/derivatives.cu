@@ -8,6 +8,10 @@
 namespace dirt {
 
 constexpr int DERIV_THREADS = 256;
+#ifndef DIRT_DERIV_MAX_BLOCKS
+#define DIRT_DERIV_MAX_BLOCKS 0x7fffffffll
+#endif
+constexpr long long DERIV_MAX_BLOCKS = DIRT_DERIV_MAX_BLOCKS;   // gridDim.x; the pixel loop strides past it
 
 struct DerivArgs {
     const int32_t* face_ids;     // [B*H*W]
@@ -123,7 +127,7 @@ cudaError_t launch_gbuffer_derivatives(const int32_t* face_ids, const float* att
     a.W = d.W; a.V = d.V; a.F = d.F; a.C = d.C; a.c0 = first_channel; a.K = count;
     if (a.total == 0) return cudaSuccess;
     const long long want = (a.total + DERIV_THREADS - 1) / DERIV_THREADS;
-    const unsigned blocks = (unsigned)(want < 0x7fffffffll ? want : 0x7fffffffll);
+    const unsigned blocks = (unsigned)(want < DERIV_MAX_BLOCKS ? want : DERIV_MAX_BLOCKS);
     // vector attribute loads: every row's channel c0 is as aligned as the vector
     const uintptr_t first = (uintptr_t)(attributes + first_channel);
     const bool vec2 = first % 8 == 0 && d.C % 2 == 0, vec4 = first % 16 == 0 && d.C % 4 == 0;

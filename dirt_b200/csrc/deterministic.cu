@@ -29,7 +29,10 @@ constexpr int DET_THREADS = 256;
 constexpr int DET_WARPS = DET_THREADS / 32;
 constexpr long long DET_WARP_BOX = 2048;   // boxes of more pixels are swept by a whole CTA
 constexpr unsigned DET_LARGE_CTAS = 1024;  // CTAs of the large-box pass (each takes whole faces)
-constexpr long long DET_MAX_BLOCKS = 1ll << 20;
+#ifndef DIRT_DET_MAX_BLOCKS
+#define DIRT_DET_MAX_BLOCKS (1ll << 20)
+#endif
+constexpr long long DET_MAX_BLOCKS = DIRT_DET_MAX_BLOCKS;
 
 struct DetArgs {
     const float* vertices;

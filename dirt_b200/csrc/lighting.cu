@@ -25,7 +25,14 @@ constexpr int RED_SLOTS = 4;                 // values per reduction round (ligh
 constexpr unsigned FULL = 0xffffffffu;
 constexpr int DD = DIRT_LIGHT_DIFFUSE_DIRECTIONAL, SP = DIRT_LIGHT_SPECULAR_DIRECTIONAL, DP = DIRT_LIGHT_DIFFUSE_POINT;
 constexpr int REDUCE_THREADS = 256;
-constexpr unsigned MAX_ITEMS_PER_GRID = 65535;   // gridDim.y
+#ifndef DIRT_LIGHT_MAX_ITEMS_PER_GRID
+#define DIRT_LIGHT_MAX_ITEMS_PER_GRID 65535
+#endif
+constexpr unsigned MAX_ITEMS_PER_GRID = DIRT_LIGHT_MAX_ITEMS_PER_GRID;   // gridDim.y
+#ifndef DIRT_LIGHT_REDUCE_MAX_BLOCKS
+#define DIRT_LIGHT_REDUCE_MAX_BLOCKS (1ll << 20)
+#endif
+constexpr long long REDUCE_MAX_BLOCKS = DIRT_LIGHT_REDUCE_MAX_BLOCKS;   // lighting_reduce_kernel loops beyond this
 
 // The warp's rows row0 .. row0+n-1 of a [rows, K] tensor with row stride rs: loaded as 32*K consecutive-in-the-row
 // floats per warp (coalesced for rs == K), passed through the warp's slice s of shared memory, K values per lane.
@@ -440,7 +447,7 @@ cudaError_t reduce_params(const LightArgs& a, const ReduceJobs& jobs, cudaStream
 {
     if (!jobs.count) return cudaSuccess;
     const long long total = jobs.first[jobs.count];
-    const unsigned blocks = (unsigned)(total < (1ll << 20) ? total : (1ll << 20));
+    const unsigned blocks = (unsigned)(total < REDUCE_MAX_BLOCKS ? total : REDUCE_MAX_BLOCKS);
     lighting_reduce_kernel<<<blocks, REDUCE_THREADS, 0, stream>>>(a.partial, jobs, total, a.chunks, a.B,
                                                                   LIGHT_FIXED_PARAMS + a.C);
     const cudaError_t e = cudaGetLastError();
@@ -1022,7 +1029,7 @@ cudaError_t launch_sh_lighting_backward(const ShArgs& a, cudaStream_t stream, in
         jobs.count = 1;
         jobs.out[0] = a.g_coef; jobs.offset[0] = 0; jobs.width[0] = (int)width; jobs.per_item[0] = a.item_coef;
         jobs.first[0] = 0; jobs.first[1] = total;
-        const unsigned blocks = (unsigned)(total < (1ll << 20) ? total : (1ll << 20));
+        const unsigned blocks = (unsigned)(total < REDUCE_MAX_BLOCKS ? total : REDUCE_MAX_BLOCKS);
         lighting_reduce_kernel<<<blocks, REDUCE_THREADS, 0, stream>>>(b.partial, jobs, total, a.chunks, a.B, (int)width);
         if ((e = cudaGetLastError()) != cudaSuccess) return e;
         ++*launches;

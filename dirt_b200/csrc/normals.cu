@@ -25,7 +25,10 @@ namespace {
 
 constexpr unsigned FULL = 0xffffffffu;
 constexpr int SCAN_THREADS = 1024;
-constexpr long long MAX_BLOCKS = 1ll << 20;
+#ifndef DIRT_NORMALS_MAX_BLOCKS
+#define DIRT_NORMALS_MAX_BLOCKS (1ll << 20)
+#endif
+constexpr long long MAX_BLOCKS = DIRT_NORMALS_MAX_BLOCKS;
 
 __device__ __forceinline__ float3 ld3(const float* p) { return make_float3(__ldg(p), __ldg(p + 1), __ldg(p + 2)); }
 __device__ __forceinline__ void st3(float* p, float3 a) { p[0] = a.x; p[1] = a.y; p[2] = a.z; }

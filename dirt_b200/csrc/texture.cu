@@ -23,7 +23,10 @@ namespace dirt {
 namespace {
 
 constexpr int TEX_THREADS = 256;
-constexpr long long TEX_MAX_BLOCKS = 1 << 16;   // grid-stride loops beyond this
+#ifndef DIRT_TEX_MAX_BLOCKS
+#define DIRT_TEX_MAX_BLOCKS (1 << 16)
+#endif
+constexpr long long TEX_MAX_BLOCKS = DIRT_TEX_MAX_BLOCKS;   // grid-stride loops beyond this
 constexpr unsigned FULL = 0xffffffffu;
 
 // x mod m with the sign of m (Python / torch.remainder) of an integer-valued x; exact for every int64
@@ -653,7 +656,10 @@ constexpr int RS_RADIX = 256;
 constexpr int RS_WARPS = RS_THREADS / 32;
 constexpr int RS_TILE = 4096;               // lookups per sort tile, 16 per thread
 constexpr long long DET_CHUNK = 4096;       // terms per chunk of a texel's sum
-constexpr unsigned DET_GRID = 8192;         // CTAs of the grid-stride passes
+#ifndef DIRT_TEX_DET_GRID
+#define DIRT_TEX_DET_GRID 8192
+#endif
+constexpr unsigned DET_GRID = DIRT_TEX_DET_GRID;   // CTAs of the grid-stride passes
 
 __device__ __forceinline__ unsigned lookup_key(const float* indices, const TexDims& d, long long g, unsigned sentinel)
 {
