@@ -515,6 +515,82 @@ extern "C" int dirt_texture_sample_trilinear_backward(const float* texture, cons
     return DIRT_OK;
 }
 
+// ---- cube-map lookup ----
+
+// S <= 2^14 keeps a padded face's texel index in int32; the atlas is six face blocks of the texture limits
+static bool cubemap_shape_ok(int TB, int S, int C, int B, long long N, int mode)
+{
+    if (S <= 0 || S > (1 << 14)) return false;
+    return texture_shape_ok(TB, S + 2, S + 2, C, B, N, mode) && (double)TB * 6 * (S + 2) * (S + 2) * C <= 4.0e18 &&
+           (double)B * N * (C > 3 ? C : 3) <= 4.0e18;
+}
+
+static TexDims cubemap_dims(int TB, int S, int C, int B, long long N, int mode)
+{
+    return make_tex_dims(TB, S + 2, S + 2, C, B, N, mode);
+}
+
+extern "C" size_t dirt_cubemap_atlas_bytes(int TB, int S, int C)
+{
+    if (TB < 0 || !cubemap_shape_ok(TB, S, C, TB, 0, DIRT_TEXTURE_BILINEAR)) return 0;
+    return sizeof(float) * 6 * (size_t)TB * (S + 2) * (S + 2) * C;
+}
+
+extern "C" int dirt_cubemap_sample(const float* cubemap, const float* directions, float* atlas, float* out, int TB, int S,
+                                   int C, int B, long long N, int mode, void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (!cubemap_shape_ok(TB, S, C, B, N, mode)) return DIRT_ERR_BAD_SHAPE;
+    if (B == 0 || N == 0) return DIRT_OK;
+    if (!cubemap || !directions || !atlas || !out) return DIRT_ERR_NULL_POINTER;
+    if ((uintptr_t)cubemap % 4 || (uintptr_t)directions % 4 || (uintptr_t)atlas % 4 || (uintptr_t)out % 4)
+        return DIRT_ERR_MISALIGNED;
+    CUDA_TRY(launch_cubemap_forward(cubemap, directions, atlas, out, cubemap_dims(TB, S, C, B, N, mode),
+                                    (cudaStream_t)cuda_stream, &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
+extern "C" size_t dirt_cubemap_sample_backward_bytes(int TB, int S, int C, int B, long long N, int mode, int deterministic)
+{
+    if (!cubemap_shape_ok(TB, S, C, B, N, mode) || (long long)B * N == 0) return 0;
+    if (deterministic && !texture_det_shape_ok(TB, S + 2, S + 2, C, B, N, mode)) return 0;
+    return carve_cubemap_scratch(nullptr, cubemap_dims(TB, S, C, B, N, mode), deterministic != 0).bytes;
+}
+
+extern "C" int dirt_cubemap_sample_backward(const float* atlas, const float* directions, const float* grad_out,
+                                            float* grad_cubemap, float* grad_directions, int TB, int S, int C, int B,
+                                            long long N, int mode, int deterministic, void* scratch, size_t scratch_bytes,
+                                            void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (!cubemap_shape_ok(TB, S, C, B, N, mode)) return DIRT_ERR_BAD_SHAPE;
+    if (deterministic && grad_cubemap && !texture_det_shape_ok(TB, S + 2, S + 2, C, B, N, mode)) return DIRT_ERR_BAD_SHAPE;
+    const TexDims d = cubemap_dims(TB, S, C, B, N, mode);
+    if (d.total > 0) {
+        if (!directions || !grad_out) return DIRT_ERR_NULL_POINTER;
+        if (grad_directions && mode == DIRT_TEXTURE_BILINEAR && !atlas) return DIRT_ERR_NULL_POINTER;
+    }
+    if ((uintptr_t)atlas % 4 || (uintptr_t)directions % 4 || (uintptr_t)grad_out % 4 || (uintptr_t)grad_cubemap % 4 ||
+        (uintptr_t)grad_directions % 4)
+        return DIRT_ERR_MISALIGNED;
+    // the scratch holds the atlas's gradient (and the deterministic path's per-face passes)
+    const bool det = deterministic && grad_cubemap && d.total > 0;
+    const bool uses_scratch = grad_cubemap && d.total > 0;
+    if (uses_scratch) {
+        if (!scratch) return DIRT_ERR_NULL_POINTER;
+        if ((uintptr_t)scratch % 256) return DIRT_ERR_MISALIGNED;
+        if (scratch_bytes < dirt_cubemap_sample_backward_bytes(TB, S, C, B, N, mode, det)) return DIRT_ERR_WORKSPACE_TOO_SMALL;
+    }
+    CUDA_TRY(launch_cubemap_backward(atlas, directions, grad_out, grad_cubemap, grad_directions, d, det,
+                                     carve_cubemap_scratch(uses_scratch ? scratch : nullptr, d, det),
+                                     (cudaStream_t)cuda_stream, &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
 // element offsets of every per-point buffer stay below 2^62, the chunk count within the grid's x limit
 static bool lighting_shape_ok(int model, int B, long long V, int C, long long sn, long long sp, long long sc)
 {

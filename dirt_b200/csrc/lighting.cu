@@ -34,40 +34,6 @@ constexpr unsigned MAX_ITEMS_PER_GRID = DIRT_LIGHT_MAX_ITEMS_PER_GRID;   // grid
 #endif
 constexpr long long REDUCE_MAX_BLOCKS = DIRT_LIGHT_REDUCE_MAX_BLOCKS;   // lighting_reduce_kernel loops beyond this
 
-// The warp's rows row0 .. row0+n-1 of a [rows, K] tensor with row stride rs: loaded as 32*K consecutive-in-the-row
-// floats per warp (coalesced for rs == K), passed through the warp's slice s of shared memory, K values per lane.
-// Lanes >= n get unspecified values.  Warp-collective.
-template <int K>
-__device__ __forceinline__ void stage_load(const float* __restrict__ src, long long rs, long long row0, int n, float* s,
-                                           int lane, float v[K])
-{
-#pragma unroll
-    for (int j = 0; j < K; ++j) {
-        const int idx = j * 32 + lane, r = idx / K, c = idx - r * K;
-        if (r < n) s[idx] = __ldg(src + (row0 + r) * rs + c);
-    }
-    __syncwarp();
-#pragma unroll
-    for (int c = 0; c < K; ++c) v[c] = s[lane * K + c];
-    __syncwarp();
-}
-
-// The reverse: lanes < n write their K values to rows row0 .. row0+n-1 of a contiguous [rows, K] tensor.
-template <int K>
-__device__ __forceinline__ void stage_store(float* __restrict__ dst, long long row0, int n, float* s, int lane,
-                                            const float v[K])
-{
-#pragma unroll
-    for (int c = 0; c < K; ++c) s[lane * K + c] = v[c];
-    __syncwarp();
-#pragma unroll
-    for (int j = 0; j < K; ++j) {
-        const int idx = j * 32 + lane;
-        if (idx < n * K) dst[row0 * K + idx] = s[idx];
-    }
-    __syncwarp();
-}
-
 // dot product in a fixed order: fma(a2, b2, fma(a1, b1, a0 * b0))
 __device__ __forceinline__ float dot3(const float a[3], const float b[3])
 {

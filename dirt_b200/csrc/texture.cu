@@ -1243,4 +1243,405 @@ cudaError_t launch_texture_trilinear_backward(const float* texture, const float*
     return cudaSuccess;
 }
 
+// ---- seamless cube-map lookup (DESIGN.md §7.10) ---------------------------------------------------------------------
+//
+// A lookup selects a face by the direction's major axis and reads the face's padded copy (S + 2 square, a one-texel
+// border from the adjacent faces) with the bilinear rule of texture_forward_kernel, so that a footprint across an edge
+// blends the right texels.  The atlas of padded faces is built per call (cube_atlas_kernel); the backward pass scatters
+// to an atlas-shaped gradient and folds it into the cube map in a fixed order (cube_adjoint_kernel).
+
+namespace {
+
+// Faces +X, -X, +Y, -Y, +Z, -Z are 0 .. 5: the major axis, ties to x over y over z by exact comparisons
+template <typename T>
+__host__ __device__ __forceinline__ int cube_face(T x, T y, T z)
+{
+    const T ax = x < 0 ? -x : x, ay = y < 0 ? -y : y, az = z < 0 ? -z : z;
+    if (ax >= ay && ax >= az) return x > 0 ? 0 : 1;
+    if (ay >= az) return y > 0 ? 2 : 3;
+    return z > 0 ? 4 : 5;
+}
+
+// the OpenGL cube-map table: face f's sc, tc and |ma| (negations and |.| are exact)
+template <typename T>
+__host__ __device__ __forceinline__ void cube_axes(int f, T x, T y, T z, T& sc, T& tc, T& ma)
+{
+    switch (f) {
+        case 0: sc = -z; tc = -y; ma = x; break;
+        case 1: sc = z; tc = -y; ma = -x; break;
+        case 2: sc = x; tc = z; ma = y; break;
+        case 3: sc = x; tc = -z; ma = -y; break;
+        case 4: sc = x; tc = -y; ma = z; break;
+        default: sc = -x; tc = -y; ma = -z; break;
+    }
+}
+
+struct CubeTexel {
+    int f, r, c;
+};
+
+// The cube texel that border texel (i, j) of face f's padded face copies (exactly one of i, j outside 1 .. S): the
+// texel holding the projection of the direction through the border texel's centre, in float64.  The projection never
+// lies within 1 / (S + 1) of a texel edge, so float64 rounding cannot move it.
+__device__ __forceinline__ CubeTexel border_source(int f, int i, int j, int S)
+{
+    const double sc = 2.0 * (j - 0.5) / S - 1.0, tc = 2.0 * (i - 0.5) / S - 1.0;
+    double x, y, z;
+    switch (f) {
+        case 0: x = 1.0; y = -tc; z = -sc; break;
+        case 1: x = -1.0; y = -tc; z = sc; break;
+        case 2: x = sc; y = 1.0; z = tc; break;
+        case 3: x = sc; y = -1.0; z = -tc; break;
+        case 4: x = sc; y = -tc; z = 1.0; break;
+        default: x = -sc; y = -tc; z = -1.0; break;
+    }
+    CubeTexel o;
+    o.f = cube_face(x, y, z);
+    double s2, t2, ma;
+    cube_axes(o.f, x, y, z, s2, t2, ma);
+    const double s = (s2 / ma + 1.0) * 0.5, t = (t2 / ma + 1.0) * 0.5;
+    o.r = min(max((int)floor(t * S), 0), S - 1);
+    o.c = min(max((int)floor(s * S), 0), S - 1);
+    return o;
+}
+
+// padded texel (i, j) of face f, item tb, in the atlas (d: one face's block)
+__device__ __forceinline__ long long atlas_texel(const TexDims& d, int f, long long tb, int i, int j)
+{
+    return (((long long)f * d.TB + tb) * d.TH + i) * d.TW + j;
+}
+
+// One thread per atlas element (face, item, i, j, channel): the face texel inside, the adjacent face's texel on an edge
+// of the border, ((own corner + row neighbour) + column neighbour) / 3 at a corner, each operation rounded in that order.
+__global__ void __launch_bounds__(TEX_THREADS) cube_atlas_kernel(const float* __restrict__ cubemap, float* __restrict__ atlas,
+                                                                 TexDims d)
+{
+    const int S = d.TW - 2, P = d.TW, C = d.C;
+    const long long n = 6ll * d.TB * d.texels * C, stride = (long long)gridDim.x * TEX_THREADS;
+    for (long long e = (long long)blockIdx.x * TEX_THREADS + threadIdx.x; e < n; e += stride) {
+        const long long x = e / C, fb = x / d.texels;   // fb = f * TB + tb
+        const int ch = (int)(e - x * C), f = (int)(fb / d.TB), ij = (int)(x - fb * d.texels), i = ij / P, j = ij - i * P;
+        const long long tb = fb - (long long)f * d.TB;
+        const float* cube = cubemap + tb * 6 * S * (long long)S * C + ch;
+        auto at = [&](CubeTexel t) { return __ldg(cube + (((long long)t.f * S + t.r) * S + t.c) * C); };
+        const bool out_i = i == 0 || i == P - 1, out_j = j == 0 || j == P - 1;
+        float v;
+        if (!out_i && !out_j) {
+            v = at(CubeTexel{f, i - 1, j - 1});
+        } else if (out_i != out_j) {
+            v = at(border_source(f, i, j, S));
+        } else {
+            const int ii = i == 0 ? 1 : S, jj = j == 0 ? 1 : S;
+            const float own = at(CubeTexel{f, ii - 1, jj - 1}), row = at(border_source(f, i, jj, S)),
+                        col = at(border_source(f, ii, j, S));
+            v = __fdiv_rn(__fadd_rn(__fadd_rn(own, row), col), 3.0f);
+        }
+        atlas[e] = v;
+    }
+}
+
+// The border's adjoint: one thread per cube-map element (item, face, r, c, channel) sums, in this order and rounded
+// in fp32, the gradient of its own padded texel, then for each edge of its face it lies on (row 0, row S-1, column 0,
+// column S-1) the gradient of the border texel of the adjacent face that copies it, followed by a third of the
+// gradient of each corner of that face that reads this border texel, and last a third of the gradient of each corner
+// of its own face whose own texel it is.  A gather: no atomics.
+__global__ void __launch_bounds__(TEX_THREADS) cube_adjoint_kernel(const float* __restrict__ grad_atlas,
+                                                                   float* __restrict__ grad_cubemap, TexDims d)
+{
+    const int S = d.TW - 2, P = d.TW, C = d.C;
+    const long long n = 6ll * d.TB * S * S * C, stride = (long long)gridDim.x * TEX_THREADS;
+    for (long long e = (long long)blockIdx.x * TEX_THREADS + threadIdx.x; e < n; e += stride) {
+        const long long x = e / C, tf = x / ((long long)S * S);   // tf = tb * 6 + f
+        const int ch = (int)(e - x * C), rc = (int)(x - tf * S * S), r = rc / S, c = rc - r * S, f = (int)(tf % 6);
+        const long long tb = tf / 6;
+        auto at = [&](int g, int i, int j) { return __ldg(grad_atlas + atlas_texel(d, g, tb, i, j) * C + ch); };
+        float acc = at(f, r + 1, c + 1);
+        if (r == 0 || r == S - 1 || c == 0 || c == S - 1) {
+#pragma unroll 1
+            for (int k = 0; k < 4; ++k) {
+                if (!(k == 0 ? r == 0 : k == 1 ? r == S - 1 : k == 2 ? c == 0 : c == S - 1)) continue;
+                // the neighbour across this edge, and among its own neighbours across its edges the border texel
+                // (qi, qj) of its face that copies (f, r, c)
+                const CubeTexel y = k < 2 ? border_source(f, k == 0 ? 0 : P - 1, c + 1, S)
+                                          : border_source(f, r + 1, k == 2 ? 0 : P - 1, S);
+#pragma unroll 1
+                for (int m = 0; m < 4; ++m) {
+                    if (!(m == 0 ? y.r == 0 : m == 1 ? y.r == S - 1 : m == 2 ? y.c == 0 : y.c == S - 1)) continue;
+                    const int qi = m < 2 ? (m == 0 ? 0 : P - 1) : y.r + 1, qj = m < 2 ? y.c + 1 : (m == 2 ? 0 : P - 1);
+                    const CubeTexel z = border_source(y.f, qi, qj, S);
+                    if (z.f != f || z.r != r || z.c != c) continue;
+                    acc = __fadd_rn(acc, at(y.f, qi, qj));
+                    // the corners of face y.f beside (qi, qj) read it as their row or column neighbour
+                    if (m < 2) {
+                        if (qj == 1) acc = __fadd_rn(acc, __fdiv_rn(at(y.f, qi, 0), 3.0f));
+                        if (qj == S) acc = __fadd_rn(acc, __fdiv_rn(at(y.f, qi, P - 1), 3.0f));
+                    } else {
+                        if (qi == 1) acc = __fadd_rn(acc, __fdiv_rn(at(y.f, 0, qj), 3.0f));
+                        if (qi == S) acc = __fadd_rn(acc, __fdiv_rn(at(y.f, P - 1, qj), 3.0f));
+                    }
+                    break;
+                }
+            }
+            // the corners of its own face whose own texel it is
+            for (int k = 0; k < 4; ++k) {
+                const int ci = k < 2 ? 0 : P - 1, cj = (k & 1) ? P - 1 : 0;
+                if ((ci == 0 ? r == 0 : r == S - 1) && (cj == 0 ? c == 0 : c == S - 1))
+                    acc = __fadd_rn(acc, __fdiv_rn(at(f, ci, cj), 3.0f));
+            }
+        }
+        grad_cubemap[e] = acc;
+    }
+}
+
+// A lookup on the atlas: taps of the padded face (base: the face's block of the lookup's item), and the face
+// coordinates its direction gradient needs.
+struct CubeLookup {
+    Taps t;
+    int face;
+    float sc, tc, ma;   // the face's table entries, ma = |major component|
+};
+
+// (t * S - 0.5) + 1 and the like, each operation rounded in the order of tests/cubemap_restatement.py
+__device__ __forceinline__ CubeLookup cube_lookup(const float v[3], const TexDims& d, long long g)
+{
+    CubeLookup q;
+    Taps& t = q.t;
+    t.r0 = t.r1 = t.c0 = t.c1 = 0;
+    t.fr = t.fc = 0.f;
+    t.base = 0;
+    q.face = 0;
+    q.sc = q.tc = 0.f;
+    q.ma = 1.f;
+    t.valid = isfinite(v[0]) && isfinite(v[1]) && isfinite(v[2]) && (v[0] != 0.f || v[1] != 0.f || v[2] != 0.f);
+    if (!t.valid) return q;
+    q.face = cube_face(v[0], v[1], v[2]);
+    cube_axes(q.face, v[0], v[1], v[2], q.sc, q.tc, q.ma);
+    const int S = d.TW - 2;
+    const float Sf = (float)S;
+    const float s = __fmul_rn(__fadd_rn(__fdiv_rn(q.sc, q.ma), 1.0f), 0.5f);
+    const float tt = __fmul_rn(__fadd_rn(__fdiv_rn(q.tc, q.ma), 1.0f), 0.5f);
+    const long long tb = d.TB == 1 ? 0ll : g / d.N;
+    t.base = atlas_texel(d, q.face, tb, 0, 0);
+    if (d.mode == DIRT_TEXTURE_NEAREST) {
+        t.r0 = t.r1 = min(max((int)floorf(__fmul_rn(tt, Sf)), 0), S - 1) + 1;
+        t.c0 = t.c1 = min(max((int)floorf(__fmul_rn(s, Sf)), 0), S - 1) + 1;
+        return q;
+    }
+    const float pr = __fadd_rn(__fsub_rn(__fmul_rn(tt, Sf), 0.5f), 1.0f);
+    const float pc = __fadd_rn(__fsub_rn(__fmul_rn(s, Sf), 0.5f), 1.0f);
+    const float flr = floorf(pr), flc = floorf(pc);
+    t.fr = __fsub_rn(pr, flr);
+    t.fc = __fsub_rn(pc, flc);
+    t.r0 = (int)flr;
+    t.c0 = (int)flc;
+    t.r1 = t.r0 + 1;
+    t.c1 = t.c0 + 1;
+    return q;
+}
+
+// One thread per lookup, CT = C in 1..4 or 0 (any C, one channel at a time).  The 12-byte direction rows go through
+// the warp's slice of shared memory; VEC: atlas and out rows aligned for the vector loads and stores (as forward_ct).
+template <int CT, bool VEC>
+__global__ void __launch_bounds__(TEX_THREADS) cube_forward_kernel(const float* __restrict__ atlas,
+                                                                   const float* __restrict__ directions,
+                                                                   float* __restrict__ out, TexDims d)
+{
+    constexpr int NV = CT ? CT : 1;
+    const int C = CT ? CT : d.C;
+    __shared__ __align__(16) float stage[TEX_THREADS * 3];
+    float* s = stage + (threadIdx.x & ~31) * 3;
+    const int lane = threadIdx.x & 31;
+    const long long stride = (long long)gridDim.x * TEX_THREADS;
+    for (long long base = (long long)blockIdx.x * TEX_THREADS + (threadIdx.x & ~31); base < d.total; base += stride) {
+        const long long g = base + lane;
+        const int n = d.total - base < 32 ? (int)(d.total - base) : 32;
+        float dir[3];
+        stage_load<3>(directions, 3, base, n, s, lane, dir);
+        CubeLookup q = cube_lookup(dir, d, g);
+        if (g >= d.total) q.t.valid = false;
+        for (int c0 = 0; c0 < C; c0 += NV) {
+            float v[NV];
+#pragma unroll
+            for (int j = 0; j < NV; ++j) v[j] = 0.f;
+            if (q.t.valid) level_rows<NV, VEC>(atlas + q.t.base * C, q.t, d.TW, C, c0, d.mode == DIRT_TEXTURE_NEAREST, v);
+            store_out<CT, VEC>(out, stage, base, c0, C, d.total, v);
+        }
+    }
+}
+
+// One thread per lookup: grad_directions through the fractions (index_grad_level, then the chain to the direction in
+// registers), and the texel terms scattered to grad_atlas (texel_grad_level).  VEC: also grad_out and grad_atlas rows.
+template <int CT, bool VEC>
+__global__ void __launch_bounds__(TEX_THREADS) cube_backward_kernel(const float* __restrict__ atlas,
+                                                                    const float* __restrict__ directions,
+                                                                    const float* __restrict__ grad_out,
+                                                                    float* __restrict__ grad_atlas,
+                                                                    float* __restrict__ grad_directions, TexDims d)
+{
+    constexpr int NV = CT ? CT : 1;
+    const int C = CT ? CT : d.C;
+    __shared__ float stage[TEX_THREADS * 3];
+    float* s = stage + (threadIdx.x & ~31) * 3;
+    const int lane = threadIdx.x & 31;
+    const bool bilinear_mode = d.mode == DIRT_TEXTURE_BILINEAR;
+    const long long stride = (long long)gridDim.x * TEX_THREADS;
+    for (long long base = (long long)blockIdx.x * TEX_THREADS + (threadIdx.x & ~31); base < d.total; base += stride) {
+        const long long g = base + lane;
+        const bool live = g < d.total;
+        const int n = d.total - base < 32 ? (int)(d.total - base) : 32;
+        float dir[3];
+        stage_load<3>(directions, 3, base, n, s, lane, dir);
+        CubeLookup q = cube_lookup(dir, d, g);
+        if (!live) q.t.valid = false;   // its taps are never used to address memory
+        const float omr = __fsub_rn(1.0f, q.t.fr), omc = __fsub_rn(1.0f, q.t.fc);
+        const float* gout = grad_out + g * C;
+        float go[NV];
+#pragma unroll
+        for (int j = 0; j < NV; ++j) go[j] = 0.f;
+        if (CT && q.t.valid) load_row<NV, VEC>(gout, go);
+
+        if (grad_directions) {
+            float gd[3] = {0.f, 0.f, 0.f};
+            if (q.t.valid && bilinear_mode) {
+                float dr = 0.f, dc = 0.f;
+                index_grad_level<CT, VEC>(atlas + q.t.base * C, q.t, omr, omc, d.TW, C, gout, go, dr, dc);
+                // s = (sc / ma + 1) / 2, t likewise, pc = s * S + 1/2, pr = t * S + 1/2
+                const float h = 0.5f * (float)(d.TW - 2) / q.ma;
+                const float gsc = dc * h, gtc = dr * h, gma = -(gsc * q.sc + gtc * q.tc) / q.ma;
+                switch (q.face) {
+                    case 0: gd[0] = gma; gd[1] = -gtc; gd[2] = -gsc; break;
+                    case 1: gd[0] = -gma; gd[1] = -gtc; gd[2] = gsc; break;
+                    case 2: gd[0] = gsc; gd[1] = gma; gd[2] = gtc; break;
+                    case 3: gd[0] = gsc; gd[1] = -gma; gd[2] = -gtc; break;
+                    case 4: gd[0] = gsc; gd[1] = -gtc; gd[2] = gma; break;
+                    default: gd[0] = -gsc; gd[1] = -gtc; gd[2] = -gma; break;
+                }
+            }
+            stage_store<3>(grad_directions, base, n, s, lane, gd);
+        }
+        if (grad_atlas)
+            texel_grad_level<CT, VEC, false>(q.t, omr, omc, 1.0f, 0, grad_atlas, d.TW, C, bilinear_mode ? 4 : 1, go, gout,
+                                             lane);
+    }
+}
+
+// Deterministic path, per face f: the padded (row, col) of the lookups on face f (whole numbers for nearest), NaN for
+// the others and for invalid lookups, which the §7.5 path skips
+__global__ void __launch_bounds__(TEX_THREADS) cube_face_indices_kernel(const float* __restrict__ directions, TexDims d,
+                                                                        int f, float* __restrict__ face_indices)
+{
+    const long long stride = (long long)gridDim.x * TEX_THREADS;
+    for (long long g = (long long)blockIdx.x * TEX_THREADS + threadIdx.x; g < d.total; g += stride) {
+        const float v[3] = {__ldg(directions + 3 * g), __ldg(directions + 3 * g + 1), __ldg(directions + 3 * g + 2)};
+        const CubeLookup q = cube_lookup(v, d, g);
+        const bool on = q.t.valid && q.face == f;
+        const float nan = __int_as_float(0x7fc00000);
+        // r0 + fr is the padded row pr exactly (pr - floor(pr) is exact), so the sorted path forms the same taps
+        face_indices[2 * g] = on ? (float)q.t.r0 + q.t.fr : nan;
+        face_indices[2 * g + 1] = on ? (float)q.t.c0 + q.t.fc : nan;
+    }
+}
+
+template <int CT>
+cudaError_t cube_forward_ct(const float* atlas, const float* directions, float* out, const TexDims& d, cudaStream_t stream)
+{
+    const int row = CT == 2 || CT == 4 ? 4 * CT : 4;
+    auto kernel = cube_forward_kernel<CT, false>;
+    if constexpr (CT != 0)
+        if (aligned(out, CT == 3 ? 16 : row) && aligned(atlas, row)) kernel = cube_forward_kernel<CT, true>;
+    kernel<<<blocks_for(d.total), TEX_THREADS, 0, stream>>>(atlas, directions, out, d);
+    return cudaGetLastError();
+}
+
+template <int CT>
+cudaError_t cube_backward_ct(const float* atlas, const float* directions, const float* grad_out, float* grad_atlas,
+                             float* grad_directions, const TexDims& d, cudaStream_t stream)
+{
+    const int row = CT == 2 || CT == 4 ? 4 * CT : 4;
+    auto kernel = cube_backward_kernel<CT, false>;
+    if constexpr (CT != 0)
+        if (aligned(grad_out, row) && aligned(atlas, row) && aligned(grad_atlas, row)) kernel = cube_backward_kernel<CT, true>;
+    kernel<<<blocks_for(d.total), TEX_THREADS, 0, stream>>>(atlas, directions, grad_out, grad_atlas, grad_directions, d);
+    return cudaGetLastError();
+}
+
+}  // namespace
+
+CubeScratch carve_cubemap_scratch(void* base, const TexDims& d, bool deterministic)
+{
+    CubeScratch s = {};
+    char* p = static_cast<char*>(base);
+    size_t off = 0;
+    auto take = [&](size_t bytes) {
+        char* r = p && bytes ? p + off : nullptr;
+        off = align_up(off + bytes, 256);
+        return r;
+    };
+    s.grad_atlas = reinterpret_cast<float*>(take(6 * (size_t)d.TB * d.texels * d.C * sizeof(float)));
+    if (deterministic) {
+        s.indices = reinterpret_cast<float*>(take((size_t)d.total * 2 * sizeof(float)));
+        s.det = take(carve_texture_det_scratch(nullptr, d).bytes);
+    }
+    s.bytes = off;
+    return s;
+}
+
+cudaError_t launch_cubemap_forward(const float* cubemap, const float* directions, float* atlas, float* out,
+                                   const TexDims& d, cudaStream_t stream, int* launches)
+{
+    cube_atlas_kernel<<<blocks_for(6ll * d.TB * d.texels * d.C), TEX_THREADS, 0, stream>>>(cubemap, atlas, d);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+    ++*launches;
+    if (d.total == 0) return cudaSuccess;
+    e = with_ct(d.C, [&](auto ct) { return cube_forward_ct<decltype(ct)::value>(atlas, directions, out, d, stream); });
+    if (e == cudaSuccess) ++*launches;
+    return e;
+}
+
+cudaError_t launch_cubemap_backward(const float* atlas, const float* directions, const float* grad_out, float* grad_cubemap,
+                                    float* grad_directions, const TexDims& d, bool deterministic, const CubeScratch& s,
+                                    cudaStream_t stream, int* launches)
+{
+    const int S = d.TW - 2;
+    cudaError_t e;
+    if (d.total == 0) {
+        if (grad_cubemap &&
+            (e = cudaMemsetAsync(grad_cubemap, 0, sizeof(float) * 6 * (size_t)d.TB * S * S * d.C, stream)) != cudaSuccess)
+            return e;
+        return cudaSuccess;
+    }
+    if (!grad_cubemap) deterministic = false;
+    if (grad_cubemap && !deterministic &&
+        (e = cudaMemsetAsync(s.grad_atlas, 0, sizeof(float) * 6 * (size_t)d.TB * d.texels * d.C, stream)) != cudaSuccess)
+        return e;
+    // the default kernel: both gradients, or under the deterministic flag grad_directions alone (it has no atomics)
+    float* ga = grad_cubemap && !deterministic ? s.grad_atlas : nullptr;
+    if (ga || grad_directions) {
+        e = with_ct(d.C, [&](auto ct) {
+            return cube_backward_ct<decltype(ct)::value>(atlas, directions, grad_out, ga, grad_directions, d, stream);
+        });
+        if (e != cudaSuccess) return e;
+        ++*launches;
+    }
+    if (!grad_cubemap) return cudaSuccess;
+    if (deterministic) {
+        // face f's block of grad_atlas, every texel written, by the §7.5 path over the lookups on face f
+        for (int f = 0; f < 6; ++f) {
+            cube_face_indices_kernel<<<blocks_for(d.total), TEX_THREADS, 0, stream>>>(directions, d, f, s.indices);
+            if ((e = cudaGetLastError()) != cudaSuccess) return e;
+            ++*launches;
+            if ((e = launch_texture_backward_deterministic(nullptr, s.indices, grad_out,
+                                                           s.grad_atlas + (size_t)f * d.TB * d.texels * d.C, nullptr, d,
+                                                           carve_texture_det_scratch(s.det, d), stream, launches)) !=
+                cudaSuccess)
+                return e;
+        }
+    }
+    cube_adjoint_kernel<<<blocks_for(6ll * d.TB * S * S * d.C), TEX_THREADS, 0, stream>>>(s.grad_atlas, grad_cubemap, d);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    ++*launches;
+    return cudaSuccess;
+}
+
 }  // namespace dirt

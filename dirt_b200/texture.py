@@ -203,3 +203,100 @@ def sample_texture(texture, indices, mode='bilinear', derivatives=None):
     if mode == 'trilinear':
         return _SampleTexture.apply(tex, flat, mode, out_shape, derivatives.detach().reshape(B, N, 4).contiguous())
     return _SampleTexture.apply(tex, flat, _MODES[mode], out_shape)
+
+
+class _SampleCubemap(torch.autograd.Function):
+    """dirt_cubemap_sample / dirt_cubemap_sample_backward.  cubemap [TB, 6, S, S, C], directions [B, N, 3], contiguous
+    fp32 CUDA.  The atlas of padded faces is built per call and kept for the backward pass in place of the cube map."""
+
+    @staticmethod
+    def forward(ctx, cubemap, directions, mode, out_shape):
+        TB, _, S, _, C = cubemap.shape
+        B, N = directions.shape[0], directions.shape[1]
+        L = _lib.lib()
+        out = torch.empty(out_shape, dtype=torch.float32, device=directions.device)
+        atlas = torch.empty(int(L.dirt_cubemap_atlas_bytes(TB, S, C)) // 4, dtype=torch.float32, device=directions.device)
+        with torch.cuda.device(directions.device):
+            rc = L.dirt_cubemap_sample(_ptr(cubemap), _ptr(directions), _ptr(atlas), _ptr(out), TB, S, C, B, N, mode,
+                                       _stream_ptr(directions.device))
+        _lib.check(rc, 'SampleCubemap')
+        ctx.save_for_backward(atlas, directions)
+        ctx.mode, ctx.shape = mode, (TB, S, C)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_out):
+        want_cubemap, want_directions = ctx.needs_input_grad[:2]
+        if not (want_cubemap or want_directions):
+            return None, None, None, None
+        atlas, directions = ctx.saved_tensors
+        TB, S, C = ctx.shape
+        B, N = directions.shape[0], directions.shape[1]
+        L = _lib.lib()
+        grad_out = grad_out.contiguous().to(torch.float32)
+        grad_cubemap = torch.empty((TB, 6, S, S, C), dtype=torch.float32, device=directions.device) if want_cubemap else None
+        grad_directions = torch.empty_like(directions) if want_directions else None
+        # grad_directions alone is per lookup and already reproducible; grad_cubemap needs the sorted path
+        deterministic = bool(want_cubemap and torch.are_deterministic_algorithms_enabled())
+        scratch_bytes = int(L.dirt_cubemap_sample_backward_bytes(TB, S, C, B, N, ctx.mode, int(deterministic)))
+        scratch = torch.empty(scratch_bytes, dtype=torch.uint8, device=directions.device) if scratch_bytes else None
+        with torch.cuda.device(directions.device):
+            rc = L.dirt_cubemap_sample_backward(
+                _ptr(atlas), _ptr(directions), _ptr(grad_out), _ptr(grad_cubemap), _ptr(grad_directions), TB, S, C, B, N,
+                ctx.mode, int(deterministic), _ptr(scratch), scratch_bytes, _stream_ptr(directions.device))
+        if deterministic and rc == _lib.ERR_BAD_SHAPE:
+            # the shapes passed the forward call: what fails are the sorted path's 32-bit limits
+            raise RuntimeError(
+                'sample_cubemap backward: the cube-map gradient has no deterministic implementation for %d lookups '
+                'into %d x 6 x %d x %d texels (it needs fewer than 2^31 lookups and padded texels per face), but '
+                'torch.use_deterministic_algorithms(True) is set' % (B * N, TB, S, S))
+        _lib.check(rc, 'SampleCubemapGrad')
+        return grad_cubemap, grad_directions, None, None
+
+
+def sample_cubemap(cubemap, directions, mode='bilinear'):
+    """Reads a cube map in the given directions, seamlessly across its edges and corners, with gradients to the texels
+    and to the directions.
+
+    Args:
+        cubemap: float32 tensor [6, S, S, C], shared by every lookup, or [B, 6, S, S, C], one cube map per batch item.
+            Faces +X, -X, +Y, -Y, +Z, -Z, each oriented as in OpenGL: face texel (0, 0) is at the face's (s, t) =
+            (0, 0) corner, rows running along t
+        directions: float32 tensor [..., 3] for a shared cube map, [B, ..., 3] for per-item cube maps; any length
+        mode: 'bilinear' (the four texels around the lookup; near an edge or a corner they come from the adjacent faces,
+            so there is no seam) or 'nearest' (the texel the lookup falls in; no gradient to the directions)
+
+    Returns:
+        float32 tensor directions.shape[:-1] + (C,), equal bit for bit to the torch restatement in
+        tests/cubemap_restatement.py (DESIGN.md §7.10).  A zero or non-finite direction returns 0 in every channel and
+        passes no gradient back.  Under torch.use_deterministic_algorithms(True) the cube-map gradient is
+        bit-reproducible.
+
+    Needs CUDA tensors (there is no CPU kernel); anything else array-like is moved to the current CUDA device.
+    """
+    if mode not in _MODES:
+        raise ValueError("sample_cubemap: mode must be 'bilinear' or 'nearest', not %r" % (mode,))
+    device = _pick_device(cubemap, directions)
+    cubemap = _as_f32(cubemap, device)
+    directions = _as_f32(directions, device)
+    if cubemap.dim() not in (4, 5) or cubemap.shape[-4] != 6 or cubemap.shape[-3] != cubemap.shape[-2]:
+        raise ValueError('SampleCubemap expects cubemap.shape == [6, size, size, channels] or '
+                         '[None, 6, size, size, channels]')
+    if cubemap.shape[-2] <= 0 or cubemap.shape[-1] <= 0:
+        raise ValueError('SampleCubemap expects a cube map with positive size and channels')
+    if directions.dim() < 1 or directions.shape[-1] != 3:
+        raise ValueError('SampleCubemap expects directions.shape[-1] == 3')
+    per_item = cubemap.dim() == 5
+    if per_item and (directions.dim() < 2 or directions.shape[0] != cubemap.shape[0]):
+        raise ValueError('SampleCubemap expects directions of per-item cube maps to be at least 2D, and '
+                         'directions.shape[0] == cubemap.shape[0]')
+    _require_cuda(cubemap, directions)
+    out_shape = tuple(directions.shape[:-1]) + (int(cubemap.shape[-1]),)
+    B = int(directions.shape[0]) if per_item else 1
+    N = 1
+    for n in directions.shape[(1 if per_item else 0):-1]:
+        N *= int(n)
+    flat = directions.reshape(B, N, 3).contiguous()
+    cube = (cubemap if per_item else cubemap[None]).contiguous()
+    return _SampleCubemap.apply(cube, flat, _MODES[mode], out_shape)

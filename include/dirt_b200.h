@@ -291,6 +291,40 @@ int dirt_texture_sample_trilinear_backward(const float* texture, const float* py
                                            int TB, int TH, int TW, int C, int B, long long N, int deterministic,
                                            void* scratch, size_t scratch_bytes, void* cuda_stream);
 
+/* Seamless cube-map lookup (DESIGN.md §7.10), with gradients to the texels and to the directions.
+ *   cubemap          float32 [TB, 6, S, S, C], faces +X, -X, +Y, -Y, +Z, -Z; TB = 1 (shared) or TB = B (one per item)
+ *   directions       float32 [B, N, 3], any length; out, grad_out float32 [B, N, C]
+ *   grad_cubemap     float32 [TB, 6, S, S, C]; grad_directions float32 [B, N, 3]
+ *   atlas            the padded faces [6, TB, S+2, S+2, C], dirt_cubemap_atlas_bytes(TB, S, C) bytes, written by
+ *                    dirt_cubemap_sample and read by dirt_cubemap_sample_backward (grad_directions of a bilinear lookup)
+ * Face: the component of largest magnitude (ties to x over y over z), with the OpenGL table of (sc, tc, ma):
+ * +X (-z, -y), -X (z, -y), +Y (x, z), -Y (x, -z), +Z (x, -y), -Z (-x, -y), ma = |major component|;
+ * s = (sc / ma + 1) * 0.5, t = (tc / ma + 1) * 0.5, each operation rounded in fp32 in that order.
+ *   mode DIRT_TEXTURE_BILINEAR: the bilinear rule of dirt_texture_sample on face f's padded face at
+ *        ((t * S - 0.5) + 1, (s * S - 0.5) + 1).  A border texel beside an edge is the adjacent face's texel that
+ *        holds the projection of the direction through its centre; a border corner is ((own corner texel + row
+ *        neighbour) + column neighbour) / 3.  So a lookup within half a texel of an edge blends the adjacent face.
+ *   mode DIRT_TEXTURE_NEAREST: face texel (clamp(floor(t * S), 0, S-1), clamp(floor(s * S), 0, S-1)); no direction
+ *        gradient.
+ * A zero or non-finite direction returns 0 in every channel, reads no texel and contributes no gradient.
+ * Backward: grad_cubemap is written in full (zeroed for no lookups); grad_directions is written once per lookup.
+ * Either may be NULL, and that half of the work is skipped.  deterministic != 0: grad_cubemap is bit-reproducible
+ * (per face, the path of dirt_texture_sample_backward_deterministic over that face's padded block, then the border's
+ * fixed-order adjoint), with that path's limits (B*N < 2^31, TB*(S+2)^2 < 2^31 - 1, else DIRT_ERR_BAD_SHAPE); an item's
+ * gradient then does not depend on the other items.  scratch: at least dirt_cubemap_sample_backward_bytes(...) bytes,
+ * 256-byte aligned, owned by the caller, needing no initialisation, a function of the shapes alone; read only when
+ * grad_cubemap is wanted and there are lookups (it may be NULL otherwise).
+ * S in 1 .. 2^14.  B = 0 or N = 0: nothing is launched (the backward call still zeroes grad_cubemap).  All pointers
+ * 4-byte aligned; row-aligned atlas, out, grad_out enable the vector paths. */
+size_t dirt_cubemap_atlas_bytes(int TB, int S, int C);
+int dirt_cubemap_sample(const float* cubemap, const float* directions, float* atlas, float* out,
+                        int TB, int S, int C, int B, long long N, int mode, void* cuda_stream);
+size_t dirt_cubemap_sample_backward_bytes(int TB, int S, int C, int B, long long N, int mode, int deterministic);
+int dirt_cubemap_sample_backward(const float* atlas, const float* directions, const float* grad_out,
+                                 float* grad_cubemap, float* grad_directions,
+                                 int TB, int S, int C, int B, long long N, int mode, int deterministic,
+                                 void* scratch, size_t scratch_bytes, void* cuda_stream);
+
 /* Reflectance models of the reference's lighting module (dirt/lighting.py:182-343), one value per point and channel.
  * B items of V points each, C channels:
  *   normals, positions   float32 [B*V, 3], row stride normals_stride / positions_stride floats, unit stride along the row
