@@ -490,7 +490,8 @@ int dirt_last_launch_count(void);
 /* Profiling hooks (replace the reference's compile-time TIME_SECTIONS stamps,
  * csrc/rasterise_egl.cpp:284-286,398-405): bracket ONE kernel of subsequent calls on this thread with
  * CUDA events recorded on the call's own stream.  which: 0 = off, 1 = forward raster kernel,
- * 2 = backward (assemble-grads) kernel.  dirt_kernel_timer_elapsed_ms() waits for the last bracketed
+ * 2 = backward (assemble-grads) kernel, 3 = triangle-setup kernel (of every call that runs it; a
+ * backward call handed the forward's workspace does not).  dirt_kernel_timer_elapsed_ms() waits for the last bracketed
  * launch and returns its duration in milliseconds (negative if nothing was timed). */
 int dirt_kernel_timer_enable(int which);
 float dirt_kernel_timer_elapsed_ms(void);
