@@ -110,6 +110,14 @@ def load(path):
     L.dirt_cubemap_sample_backward_bytes.argtypes = [i] * 4 + [ctypes.c_longlong, i, i]
     L.dirt_cubemap_sample_backward.restype = i
     L.dirt_cubemap_sample_backward.argtypes = [vp] * 5 + [i] * 4 + [ctypes.c_longlong, i, i, vp, sz, vp]
+    L.dirt_cubemap_mip_atlas_bytes.restype = sz
+    L.dirt_cubemap_mip_atlas_bytes.argtypes = [i] * 3
+    L.dirt_cubemap_sample_trilinear.restype = i
+    L.dirt_cubemap_sample_trilinear.argtypes = [vp] * 5 + [i] * 4 + [ctypes.c_longlong, vp]
+    L.dirt_cubemap_sample_trilinear_backward_bytes.restype = sz
+    L.dirt_cubemap_sample_trilinear_backward_bytes.argtypes = [i] * 4 + [ctypes.c_longlong, i]
+    L.dirt_cubemap_sample_trilinear_backward.restype = i
+    L.dirt_cubemap_sample_trilinear_backward.argtypes = [vp] * 7 + [i] * 4 + [ctypes.c_longlong, i, vp, sz, vp]
     ll = ctypes.c_longlong
     light_inputs = [i, i, vp, ll, vp, ll, vp, ll] + [vp, i] * 4
     L.dirt_lighting_workspace_bytes.restype = sz
@@ -153,7 +161,8 @@ EXPORTED_SYMBOLS = ['dirt_error_string', 'dirt_abi_version', 'dirt_workspace_byt
                     'dirt_rasterise_derivatives', 'dirt_sh_lighting_workspace_bytes', 'dirt_sh_lighting_forward',
                     'dirt_sh_lighting_backward', 'dirt_ggx_lighting_forward', 'dirt_ggx_lighting_backward',
                     'dirt_cubemap_atlas_bytes', 'dirt_cubemap_sample', 'dirt_cubemap_sample_backward_bytes',
-                    'dirt_cubemap_sample_backward']
+                    'dirt_cubemap_sample_backward', 'dirt_cubemap_mip_atlas_bytes', 'dirt_cubemap_sample_trilinear',
+                    'dirt_cubemap_sample_trilinear_backward_bytes', 'dirt_cubemap_sample_trilinear_backward']
 
 
 def error_string(code):

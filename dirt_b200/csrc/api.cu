@@ -593,6 +593,80 @@ extern "C" int dirt_cubemap_sample_backward(const float* atlas, const float* dir
     return DIRT_OK;
 }
 
+// ---- mipmapped cube-map lookup ----
+
+// the bilinear cube-map lookup's limits; the mip atlas is at most 4/3 of level 0's plus its borders
+static bool cubemap_mip_shape_ok(int TB, int S, int C, int B, long long N)
+{
+    return cubemap_shape_ok(TB, S, C, B, N, DIRT_TEXTURE_BILINEAR) && (double)TB * 8 * (S + 2) * (S + 2) * C <= 4.0e18;
+}
+
+extern "C" size_t dirt_cubemap_mip_atlas_bytes(int TB, int S, int C)
+{
+    if (TB < 0 || !cubemap_mip_shape_ok(TB, S, C, TB, 0)) return 0;
+    return sizeof(float) * cubemap_mip_atlas_texels(cubemap_dims(TB, S, C, TB, 0, DIRT_TEXTURE_BILINEAR)) * C;
+}
+
+extern "C" int dirt_cubemap_sample_trilinear(const float* cubemap, const float* directions, const float* lod, float* atlas,
+                                             float* out, int TB, int S, int C, int B, long long N, void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (!cubemap_mip_shape_ok(TB, S, C, B, N)) return DIRT_ERR_BAD_SHAPE;
+    if (B == 0 || N == 0) return DIRT_OK;
+    if (!cubemap || !directions || !lod || !atlas || !out) return DIRT_ERR_NULL_POINTER;
+    if ((uintptr_t)cubemap % 4 || (uintptr_t)directions % 4 || (uintptr_t)lod % 4 || (uintptr_t)atlas % 4 ||
+        (uintptr_t)out % 4)
+        return DIRT_ERR_MISALIGNED;
+    CUDA_TRY(launch_cubemap_mip_forward(cubemap, directions, lod, atlas, out,
+                                        cubemap_dims(TB, S, C, B, N, DIRT_TEXTURE_BILINEAR), (cudaStream_t)cuda_stream,
+                                        &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
+extern "C" size_t dirt_cubemap_sample_trilinear_backward_bytes(int TB, int S, int C, int B, long long N, int deterministic)
+{
+    if (!cubemap_mip_shape_ok(TB, S, C, B, N) || (long long)B * N == 0) return 0;
+    if (deterministic && !texture_det_shape_ok(TB, S + 2, S + 2, C, B, N, DIRT_TEXTURE_BILINEAR)) return 0;
+    return carve_cubemap_mip_scratch(nullptr, cubemap_dims(TB, S, C, B, N, DIRT_TEXTURE_BILINEAR), deterministic != 0).bytes;
+}
+
+extern "C" int dirt_cubemap_sample_trilinear_backward(const float* atlas, const float* directions, const float* lod,
+                                                      const float* grad_out, float* grad_cubemap, float* grad_directions,
+                                                      float* grad_lod, int TB, int S, int C, int B, long long N,
+                                                      int deterministic, void* scratch, size_t scratch_bytes,
+                                                      void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (!cubemap_mip_shape_ok(TB, S, C, B, N)) return DIRT_ERR_BAD_SHAPE;
+    if (deterministic && grad_cubemap && !texture_det_shape_ok(TB, S + 2, S + 2, C, B, N, DIRT_TEXTURE_BILINEAR))
+        return DIRT_ERR_BAD_SHAPE;
+    const TexDims d = cubemap_dims(TB, S, C, B, N, DIRT_TEXTURE_BILINEAR);
+    if (d.total > 0) {
+        if (!directions || !lod || !grad_out) return DIRT_ERR_NULL_POINTER;
+        if ((grad_directions || grad_lod) && !atlas) return DIRT_ERR_NULL_POINTER;
+    }
+    if ((uintptr_t)atlas % 4 || (uintptr_t)directions % 4 || (uintptr_t)lod % 4 || (uintptr_t)grad_out % 4 ||
+        (uintptr_t)grad_cubemap % 4 || (uintptr_t)grad_directions % 4 || (uintptr_t)grad_lod % 4)
+        return DIRT_ERR_MISALIGNED;
+    // the scratch holds the atlas's and the pyramid's gradients (and the deterministic path's per-level passes)
+    const bool det = deterministic && grad_cubemap && d.total > 0;
+    const bool uses_scratch = grad_cubemap && d.total > 0;
+    if (uses_scratch) {
+        if (!scratch) return DIRT_ERR_NULL_POINTER;
+        if ((uintptr_t)scratch % 256) return DIRT_ERR_MISALIGNED;
+        if (scratch_bytes < dirt_cubemap_sample_trilinear_backward_bytes(TB, S, C, B, N, det))
+            return DIRT_ERR_WORKSPACE_TOO_SMALL;
+    }
+    CUDA_TRY(launch_cubemap_mip_backward(atlas, directions, lod, grad_out, grad_cubemap, grad_directions, grad_lod, d, det,
+                                         carve_cubemap_mip_scratch(uses_scratch ? scratch : nullptr, d, det),
+                                         (cudaStream_t)cuda_stream, &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
 // element offsets of every per-point buffer stay below 2^62, the chunk count within the grid's x limit
 static bool lighting_shape_ok(int model, int B, long long V, int C, long long sn, long long sp, long long sc)
 {

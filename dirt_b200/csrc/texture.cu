@@ -1439,12 +1439,82 @@ __device__ __forceinline__ CubeLookup cube_lookup(const float v[3], const TexDim
     return q;
 }
 
+// ---- mipmapped (trilinear) cube-map lookup (DESIGN.md §7.11) ------------------------------------------------------
+//
+// Level k of a cube map of S texels per edge is the §7.6 box pyramid of each face, S >> k per edge, read with the
+// bilinear rule above on its own padded faces.  The mip atlas packs the levels' atlases [6, TB, (S>>k)+2, (S>>k)+2, C]
+// in level order; CubeMip::offset[k] is level k's first texel.  lod is given per lookup, in levels.
+
+struct CubeMip {
+    const float* lod;                     // [B*N] levels of detail
+    int L;                                // levels
+    long long offset[MIP_MAX_LEVELS];     // first texel of level k's atlas in the mip atlas
+};
+
+// the dims of level k's atlas, d those of level 0's
+__host__ __device__ __forceinline__ TexDims cube_level_dims(const TexDims& d, int k)
+{
+    TexDims e = d;
+    e.TW = e.TH = ((d.TW - 2) >> k) + 2;
+    e.texels = (long long)e.TW * e.TW;
+    return e;
+}
+
+// lambda = lod, NaN -> 0, clamped to [0, L-1]; l = floor(lambda), f = lambda - l
+__device__ __forceinline__ Lod cube_lod_of(float x, int L)
+{
+    const float lam = isnan(x) ? 0.f : fminf(fmaxf(x, 0.f), (float)(L - 1));
+    Lod o;
+    o.l = (int)floorf(lam);
+    o.f = __fsub_rn(lam, (float)o.l);
+    return o;
+}
+
+// The two levels the backward pass reads, k0 = min(l, L-2) and k0 + 1 (both 0 when L = 1), and the forward's weights
+// of each: (1-f, f) when f != 0, (1, 0) at level l < L-1, (0, 1) at l = L-1.  The difference of the two levels is
+// d out / d lod.
+struct CubeMipPair {
+    int k0, k1;
+    float a0, a1;
+};
+
+__device__ __forceinline__ CubeMipPair cube_mip_pair(const Lod& lod, int L)
+{
+    CubeMipPair p;
+    if (L == 1) {
+        p.k0 = p.k1 = 0;
+        p.a0 = 1.f;
+        p.a1 = 0.f;
+    } else if (lod.l == L - 1) {
+        p.k0 = L - 2;
+        p.k1 = L - 1;
+        p.a0 = 0.f;
+        p.a1 = 1.f;
+    } else {
+        p.k0 = lod.l;
+        p.k1 = lod.l + 1;
+        p.a0 = lod.f != 0.f ? __fsub_rn(1.0f, lod.f) : 1.0f;
+        p.a1 = lod.f;
+    }
+    return p;
+}
+
+// Per-CTA accumulation of the coarse levels in shared memory: the levels whose atlases (all six faces of one item)
+// fit CUBE_SMEM_FLOATS floats together, from level L-1 downwards.  -DDIRT_CUBE_MIP_SMEM_FLOATS=0 turns it off (a
+// budget, not one of the grid caps above).
+#ifdef DIRT_CUBE_MIP_SMEM_FLOATS
+constexpr int CUBE_SMEM_FLOATS = DIRT_CUBE_MIP_SMEM_FLOATS;
+#else
+constexpr int CUBE_SMEM_FLOATS = 6144;
+#endif
+
 // One thread per lookup, CT = C in 1..4 or 0 (any C, one channel at a time).  The 12-byte direction rows go through
 // the warp's slice of shared memory; VEC: atlas and out rows aligned for the vector loads and stores (as forward_ct).
-template <int CT, bool VEC>
+// MIP: the atlas is the mip atlas of m, and a lookup reads level l and, when f != 0, level l + 1.
+template <int CT, bool VEC, bool MIP>
 __global__ void __launch_bounds__(TEX_THREADS) cube_forward_kernel(const float* __restrict__ atlas,
                                                                    const float* __restrict__ directions,
-                                                                   float* __restrict__ out, TexDims d)
+                                                                   float* __restrict__ out, TexDims d, CubeMip m)
 {
     constexpr int NV = CT ? CT : 1;
     const int C = CT ? CT : d.C;
@@ -1457,26 +1527,90 @@ __global__ void __launch_bounds__(TEX_THREADS) cube_forward_kernel(const float* 
         const int n = d.total - base < 32 ? (int)(d.total - base) : 32;
         float dir[3];
         stage_load<3>(directions, 3, base, n, s, lane, dir);
-        CubeLookup q = cube_lookup(dir, d, g);
+        Lod lod;
+        lod.l = 0;
+        lod.f = 0.f;
+        if (MIP) lod = cube_lod_of(g < d.total ? __ldg(m.lod + g) : 0.f, m.L);
+        const int l1 = lod.l + 1 < m.L ? lod.l + 1 : lod.l;
+        const TexDims d0 = MIP ? cube_level_dims(d, lod.l) : d, d1 = cube_level_dims(d, l1);
+        CubeLookup q = cube_lookup(dir, d0, g);
+        CubeLookup q1;
+        if (MIP) q1 = cube_lookup(dir, d1, g);
         if (g >= d.total) q.t.valid = false;
         for (int c0 = 0; c0 < C; c0 += NV) {
             float v[NV];
 #pragma unroll
             for (int j = 0; j < NV; ++j) v[j] = 0.f;
-            if (q.t.valid) level_rows<NV, VEC>(atlas + q.t.base * C, q.t, d.TW, C, c0, d.mode == DIRT_TEXTURE_NEAREST, v);
+            if (q.t.valid) {
+                level_rows<NV, VEC>((MIP ? atlas + m.offset[lod.l] * C : atlas) + q.t.base * C, q.t, d0.TW, C, c0,
+                                    !MIP && d.mode == DIRT_TEXTURE_NEAREST, v);
+                if (MIP && lod.f != 0.f) {
+                    float u[NV];
+                    level_rows<NV, VEC>(atlas + (m.offset[l1] + q1.t.base) * C, q1.t, d1.TW, C, c0, false, u);
+                    const float omf = __fsub_rn(1.0f, lod.f);
+#pragma unroll
+                    for (int j = 0; j < NV; ++j) v[j] = __fadd_rn(__fmul_rn(omf, v[j]), __fmul_rn(lod.f, u[j]));
+                }
+            }
             store_out<CT, VEC>(out, stage, base, c0, C, d.total, v);
         }
     }
 }
 
+// The shared-memory half of the coarse-level accumulation: the lookups' texel terms of levels >= first go to acc
+// (level k's atlas at acc + (m.offset[k] - m.offset[first]) * C, one item's six faces) by shared-memory atomics; then
+// flush adds every non-zero element to grad_atlas with one reduction per CTA and element.
+struct CubeSmem {
+    float* acc;     // NULL: no level is accumulated in shared memory
+    int first;      // the first level accumulated there (L when none)
+};
+
+// d out / d texel of one lookup's taps t (weights times a) added to the level's accumulator acc (width TW, C
+// channels) with shared-memory atomics; the products are texel_grad_level's
+template <int CT>
+__device__ __forceinline__ void texel_grad_smem(const Taps& t, float a, float* acc, int TW, int C, const float go[],
+                                                const float* gout)
+{
+    constexpr int NV = CT ? CT : 1;
+    const float omr = __fsub_rn(1.0f, t.fr), omc = __fsub_rn(1.0f, t.fc);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const int r = (k & 2) ? t.r1 : t.r0, c = (k & 1) ? t.c1 : t.c0;
+        const float w = __fmul_rn(__fmul_rn((k & 1) ? t.fc : omc, (k & 2) ? t.fr : omr), a);
+        if (w == 0.f) continue;
+        float* dst = acc + (t.base + (long long)r * TW + c) * C;
+        if (CT) {
+#pragma unroll
+            for (int j = 0; j < NV; ++j) atomicAdd(dst + j, go[j] * w);
+        } else {
+            for (int ch = 0; ch < C; ++ch) atomicAdd(dst + ch, __ldg(gout + ch) * w);
+        }
+    }
+}
+
+__device__ __forceinline__ void cube_smem_flush(const CubeSmem& sm, const CubeMip& m, float* grad_atlas, int C)
+{
+    __syncthreads();
+    const long long n = (m.offset[m.L] - m.offset[sm.first]) * C;
+    float* dst = grad_atlas + m.offset[sm.first] * C;
+    for (long long e = threadIdx.x; e < n; e += TEX_THREADS) {
+        const float v = sm.acc[e];
+        if (v != 0.f) atomicAdd(dst + e, v);
+    }
+}
+
 // One thread per lookup: grad_directions through the fractions (index_grad_level, then the chain to the direction in
 // registers), and the texel terms scattered to grad_atlas (texel_grad_level).  VEC: also grad_out and grad_atlas rows.
-template <int CT, bool VEC>
+// MIP: the two levels of cube_mip_pair, grad_directions through both levels' fractions (d p / d t = S >> k at level
+// k), grad_lod the difference of the two levels' values; the texel terms go to the levels' atlases in grad_atlas, or
+// for the coarse levels of a CTA whose lookups share one cube map to shared memory first (CubeSmem).
+template <int CT, bool VEC, bool MIP>
 __global__ void __launch_bounds__(TEX_THREADS) cube_backward_kernel(const float* __restrict__ atlas,
                                                                     const float* __restrict__ directions,
                                                                     const float* __restrict__ grad_out,
                                                                     float* __restrict__ grad_atlas,
-                                                                    float* __restrict__ grad_directions, TexDims d)
+                                                                    float* __restrict__ grad_directions, TexDims d,
+                                                                    CubeMip m, float* __restrict__ grad_lod, int smem_first)
 {
     constexpr int NV = CT ? CT : 1;
     const int C = CT ? CT : d.C;
@@ -1484,6 +1618,17 @@ __global__ void __launch_bounds__(TEX_THREADS) cube_backward_kernel(const float*
     float* s = stage + (threadIdx.x & ~31) * 3;
     const int lane = threadIdx.x & 31;
     const bool bilinear_mode = d.mode == DIRT_TEXTURE_BILINEAR;
+    CubeSmem sm;
+    sm.acc = nullptr;
+    sm.first = m.L;
+    if (MIP && CUBE_SMEM_FLOATS > 0 && grad_atlas && smem_first < m.L) {
+        extern __shared__ float cube_smem[];
+        sm.acc = cube_smem;
+        sm.first = smem_first;
+        const long long n = (m.offset[m.L] - m.offset[sm.first]) * C;
+        for (long long e = threadIdx.x; e < n; e += TEX_THREADS) sm.acc[e] = 0.f;
+        __syncthreads();
+    }
     const long long stride = (long long)gridDim.x * TEX_THREADS;
     for (long long base = (long long)blockIdx.x * TEX_THREADS + (threadIdx.x & ~31); base < d.total; base += stride) {
         const long long g = base + lane;
@@ -1491,22 +1636,61 @@ __global__ void __launch_bounds__(TEX_THREADS) cube_backward_kernel(const float*
         const int n = d.total - base < 32 ? (int)(d.total - base) : 32;
         float dir[3];
         stage_load<3>(directions, 3, base, n, s, lane, dir);
-        CubeLookup q = cube_lookup(dir, d, g);
+        float x = 0.f;
+        CubeMipPair p;
+        p.k0 = p.k1 = 0;
+        p.a0 = 1.f;
+        p.a1 = 0.f;
+        if (MIP) {
+            x = live ? __ldg(m.lod + g) : 0.f;
+            p = cube_mip_pair(cube_lod_of(x, m.L), m.L);
+        }
+        const TexDims d0 = MIP ? cube_level_dims(d, p.k0) : d, d1 = cube_level_dims(d, p.k1);
+        CubeLookup q = cube_lookup(dir, d0, g);
+        CubeLookup q1;
+        if (MIP) q1 = cube_lookup(dir, d1, g);
         if (!live) q.t.valid = false;   // its taps are never used to address memory
         const float omr = __fsub_rn(1.0f, q.t.fr), omc = __fsub_rn(1.0f, q.t.fc);
         const float* gout = grad_out + g * C;
+        const float* lev0 = MIP ? atlas + m.offset[p.k0] * C : atlas;
+        const float* lev1 = atlas + m.offset[p.k1] * C;
         float go[NV];
 #pragma unroll
         for (int j = 0; j < NV; ++j) go[j] = 0.f;
         if (CT && q.t.valid) load_row<NV, VEC>(gout, go);
 
+        if (MIP && grad_lod) {
+            // d out / d lod = sum_c grad_out_c (b_{k1,c} - b_{k0,c}); 0 where the clamp is active, for NaN and L = 1
+            float gl = 0.f;
+            if (q.t.valid && m.L > 1 && x >= 0.f && x <= (float)(m.L - 1)) {
+                for (int c0 = 0; c0 < C; c0 += NV) {
+                    float v[NV], u[NV];
+                    level_rows<NV, VEC>(lev0 + q.t.base * C, q.t, d0.TW, C, c0, false, v);
+                    level_rows<NV, VEC>(lev1 + q1.t.base * C, q1.t, d1.TW, C, c0, false, u);
+#pragma unroll
+                    for (int j = 0; j < NV; ++j) gl += (CT ? go[j] : __ldg(gout + c0)) * (u[j] - v[j]);
+                }
+            }
+            if (live) grad_lod[g] = gl;
+        }
+
         if (grad_directions) {
             float gd[3] = {0.f, 0.f, 0.f};
             if (q.t.valid && bilinear_mode) {
                 float dr = 0.f, dc = 0.f;
-                index_grad_level<CT, VEC>(atlas + q.t.base * C, q.t, omr, omc, d.TW, C, gout, go, dr, dc);
+                if (!MIP || p.a0 != 0.f) index_grad_level<CT, VEC>(lev0 + q.t.base * C, q.t, omr, omc, d0.TW, C, gout, go, dr, dc);
+                if (MIP) {
+                    // d p_k / d t = S >> k at level k, the levels blended by their weights
+                    float dr1 = 0.f, dc1 = 0.f;
+                    if (p.a1 != 0.f)
+                        index_grad_level<CT, VEC>(lev1 + q1.t.base * C, q1.t, __fsub_rn(1.0f, q1.t.fr),
+                                                  __fsub_rn(1.0f, q1.t.fc), d1.TW, C, gout, go, dr1, dc1);
+                    const float s0 = (float)(d0.TW - 2), s1 = (float)(d1.TW - 2);
+                    dr = p.a0 * (dr * s0) + p.a1 * (dr1 * s1);
+                    dc = p.a0 * (dc * s0) + p.a1 * (dc1 * s1);
+                }
                 // s = (sc / ma + 1) / 2, t likewise, pc = s * S + 1/2, pr = t * S + 1/2
-                const float h = 0.5f * (float)(d.TW - 2) / q.ma;
+                const float h = 0.5f * (MIP ? 1.0f : (float)(d.TW - 2)) / q.ma;
                 const float gsc = dc * h, gtc = dr * h, gma = -(gsc * q.sc + gtc * q.tc) / q.ma;
                 switch (q.face) {
                     case 0: gd[0] = gma; gd[1] = -gtc; gd[2] = -gsc; break;
@@ -1519,10 +1703,30 @@ __global__ void __launch_bounds__(TEX_THREADS) cube_backward_kernel(const float*
             }
             stage_store<3>(grad_directions, base, n, s, lane, gd);
         }
-        if (grad_atlas)
-            texel_grad_level<CT, VEC, false>(q.t, omr, omc, 1.0f, 0, grad_atlas, d.TW, C, bilinear_mode ? 4 : 1, go, gout,
-                                             lane);
+        if (grad_atlas) {
+            if (MIP) {
+#pragma unroll 1
+                for (int i = 0; i < 2; ++i) {
+                    const int k = i ? p.k1 : p.k0;
+                    Taps t = i ? q1.t : q.t;
+                    const float a = i ? p.a1 : p.a0;
+                    const bool on = q.t.valid && a != 0.f, shared = k >= sm.first;
+                    if (on && shared)
+                        texel_grad_smem<CT>(t, a, sm.acc + (m.offset[k] - m.offset[sm.first]) * C, i ? d1.TW : d0.TW, C,
+                                            go, gout);
+                    t.valid = on && !shared;
+                    if (__any_sync(FULL, t.valid))   // warp-uniform: texel_grad_level is collective
+                        texel_grad_level<CT, VEC, true>(t, __fsub_rn(1.0f, t.fr), __fsub_rn(1.0f, t.fc), a, m.offset[k],
+                                                        grad_atlas + m.offset[k] * C, i ? d1.TW : d0.TW, C, 4, go, gout,
+                                                        lane);
+                }
+            } else {
+                texel_grad_level<CT, VEC, false>(q.t, omr, omc, 1.0f, 0, grad_atlas, d.TW, C, bilinear_mode ? 4 : 1, go,
+                                                 gout, lane);
+            }
+        }
     }
+    if (MIP && sm.acc) cube_smem_flush(sm, m, grad_atlas, C);
 }
 
 // Deterministic path, per face f: the padded (row, col) of the lookups on face f (whole numbers for nearest), NaN for
@@ -1542,27 +1746,92 @@ __global__ void __launch_bounds__(TEX_THREADS) cube_face_indices_kernel(const fl
     }
 }
 
-template <int CT>
-cudaError_t cube_forward_ct(const float* atlas, const float* directions, float* out, const TexDims& d, cudaStream_t stream)
+// Deterministic mipmapped path, per level k and face f: the padded (row, col) at level k of the lookups on face f
+// that read level k with a non-zero weight, NaN for the others (and invalid lookups), which the §7.5 path skips; with
+// write_grad_out also grad_out times each lookup's weight of level k (0 where it does not read it), fp32
+__global__ void __launch_bounds__(TEX_THREADS) cube_mip_terms_kernel(const float* __restrict__ directions, TexDims d,
+                                                                     CubeMip m, const float* __restrict__ grad_out, int k,
+                                                                     int f, bool write_grad_out,
+                                                                     float* __restrict__ level_indices,
+                                                                     float* __restrict__ level_grad_out)
+{
+    const TexDims dk = cube_level_dims(d, k);
+    const long long stride = (long long)gridDim.x * TEX_THREADS;
+    for (long long g = (long long)blockIdx.x * TEX_THREADS + threadIdx.x; g < d.total; g += stride) {
+        const float v[3] = {__ldg(directions + 3 * g), __ldg(directions + 3 * g + 1), __ldg(directions + 3 * g + 2)};
+        const CubeMipPair p = cube_mip_pair(cube_lod_of(__ldg(m.lod + g), m.L), m.L);
+        const float a = k == p.k0 ? p.a0 : k == p.k1 ? p.a1 : 0.f;
+        const CubeLookup q = cube_lookup(v, dk, g);
+        const bool on = q.t.valid && q.face == f && a != 0.f;
+        const float nan = __int_as_float(0x7fc00000);
+        level_indices[2 * g] = on ? (float)q.t.r0 + q.t.fr : nan;
+        level_indices[2 * g + 1] = on ? (float)q.t.c0 + q.t.fc : nan;
+        if (write_grad_out)
+            for (int ch = 0; ch < d.C; ++ch) level_grad_out[g * d.C + ch] = __fmul_rn(__ldg(grad_out + g * d.C + ch), a);
+    }
+}
+
+template <int CT, bool MIP>
+cudaError_t cube_forward_ct(const float* atlas, const float* directions, float* out, const TexDims& d, const CubeMip& m,
+                            cudaStream_t stream)
 {
     const int row = CT == 2 || CT == 4 ? 4 * CT : 4;
-    auto kernel = cube_forward_kernel<CT, false>;
+    auto kernel = cube_forward_kernel<CT, false, MIP>;
     if constexpr (CT != 0)
-        if (aligned(out, CT == 3 ? 16 : row) && aligned(atlas, row)) kernel = cube_forward_kernel<CT, true>;
-    kernel<<<blocks_for(d.total), TEX_THREADS, 0, stream>>>(atlas, directions, out, d);
+        if (aligned(out, CT == 3 ? 16 : row) && aligned(atlas, row)) kernel = cube_forward_kernel<CT, true, MIP>;
+    kernel<<<blocks_for(d.total), TEX_THREADS, 0, stream>>>(atlas, directions, out, d, m);
     return cudaGetLastError();
 }
 
-template <int CT>
+// MIP: the shared-memory levels (smem_first < m.L) take (offset[L] - offset[smem_first]) * C floats of dynamic shared
+// memory, and the grid is capped at 8 CTAs per SM, so that each CTA flushes them once for many lookups
+template <int CT, bool MIP>
 cudaError_t cube_backward_ct(const float* atlas, const float* directions, const float* grad_out, float* grad_atlas,
-                             float* grad_directions, const TexDims& d, cudaStream_t stream)
+                             float* grad_directions, const TexDims& d, const CubeMip& m, float* grad_lod, int smem_first,
+                             cudaStream_t stream)
 {
     const int row = CT == 2 || CT == 4 ? 4 * CT : 4;
-    auto kernel = cube_backward_kernel<CT, false>;
+    auto kernel = cube_backward_kernel<CT, false, MIP>;
     if constexpr (CT != 0)
-        if (aligned(grad_out, row) && aligned(atlas, row) && aligned(grad_atlas, row)) kernel = cube_backward_kernel<CT, true>;
-    kernel<<<blocks_for(d.total), TEX_THREADS, 0, stream>>>(atlas, directions, grad_out, grad_atlas, grad_directions, d);
+        if (aligned(grad_out, row) && aligned(atlas, row) && aligned(grad_atlas, row))
+            kernel = cube_backward_kernel<CT, true, MIP>;
+    unsigned blocks = blocks_for(d.total);
+    size_t smem = 0;
+    if (MIP && grad_atlas && smem_first < m.L) {
+        smem = sizeof(float) * (size_t)(m.offset[m.L] - m.offset[smem_first]) * d.C;
+        int dev = 0, sms = 0;
+        cudaError_t e;
+        if ((e = cudaGetDevice(&dev)) != cudaSuccess ||
+            (e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev)) != cudaSuccess)
+            return e;
+        blocks = blocks < 8u * sms ? blocks : 8u * sms;
+    }
+    kernel<<<blocks, TEX_THREADS, smem, stream>>>(atlas, directions, grad_out, grad_atlas, grad_directions, d, m, grad_lod,
+                                                  smem_first);
     return cudaGetLastError();
+}
+
+// the mip atlas's levels: offset[k], k = 0 .. L, of level k's first texel
+CubeMip cube_mip_of(const TexDims& d, const float* lod)
+{
+    CubeMip m = {};
+    m.lod = lod;
+    m.L = mip_levels(d.TW - 2, d.TW - 2);
+    for (int k = 0; k < m.L; ++k) {
+        const long long P = ((d.TW - 2) >> k) + 2;
+        m.offset[k + 1] = m.offset[k] + 6ll * d.TB * P * P;
+    }
+    return m;
+}
+
+// the first level accumulated in shared memory: the coarsest levels whose atlases fit CUBE_SMEM_FLOATS together, for
+// a shared cube map (every CTA's lookups read one item); L for none
+int cube_smem_first(const TexDims& d, const CubeMip& m)
+{
+    int first = m.L;
+    if (d.TB == 1)
+        while (first > 0 && (m.offset[m.L] - m.offset[first - 1]) * d.C <= CUBE_SMEM_FLOATS) --first;
+    return first;
 }
 
 }  // namespace
@@ -1594,7 +1863,9 @@ cudaError_t launch_cubemap_forward(const float* cubemap, const float* directions
     if (e != cudaSuccess) return e;
     ++*launches;
     if (d.total == 0) return cudaSuccess;
-    e = with_ct(d.C, [&](auto ct) { return cube_forward_ct<decltype(ct)::value>(atlas, directions, out, d, stream); });
+    e = with_ct(d.C, [&](auto ct) {
+        return cube_forward_ct<decltype(ct)::value, false>(atlas, directions, out, d, CubeMip{}, stream);
+    });
     if (e == cudaSuccess) ++*launches;
     return e;
 }
@@ -1619,7 +1890,8 @@ cudaError_t launch_cubemap_backward(const float* atlas, const float* directions,
     float* ga = grad_cubemap && !deterministic ? s.grad_atlas : nullptr;
     if (ga || grad_directions) {
         e = with_ct(d.C, [&](auto ct) {
-            return cube_backward_ct<decltype(ct)::value>(atlas, directions, grad_out, ga, grad_directions, d, stream);
+            return cube_backward_ct<decltype(ct)::value, false>(atlas, directions, grad_out, ga, grad_directions, d,
+                                                                 CubeMip{}, nullptr, 0, stream);
         });
         if (e != cudaSuccess) return e;
         ++*launches;
@@ -1641,6 +1913,130 @@ cudaError_t launch_cubemap_backward(const float* atlas, const float* directions,
     cube_adjoint_kernel<<<blocks_for(6ll * d.TB * S * S * d.C), TEX_THREADS, 0, stream>>>(s.grad_atlas, grad_cubemap, d);
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     ++*launches;
+    return cudaSuccess;
+}
+
+// ---- mipmapped cube-map lookup (DESIGN.md §7.11) ----
+
+// the cube maps [TB, 6, S, S, C] as one texture of 6 * TB faces, the §7.6 pyramid's level 0
+static TexDims cube_faces_dims(const TexDims& d)
+{
+    TexDims p = d;
+    p.TB = 6 * d.TB;
+    p.TH = p.TW = d.TW - 2;
+    p.texels = (long long)p.TW * p.TW;
+    p.total = 0;
+    p.mode = DIRT_TEXTURE_BILINEAR;
+    return p;
+}
+
+size_t cubemap_mip_atlas_texels(const TexDims& d) { return (size_t)cube_mip_of(d, nullptr).offset[mip_levels(d.TW - 2, d.TW - 2)]; }
+
+CubeMipScratch carve_cubemap_mip_scratch(void* base, const TexDims& d, bool deterministic)
+{
+    CubeMipScratch s = {};
+    char* p = static_cast<char*>(base);
+    size_t off = 0;
+    auto take = [&](size_t bytes) {
+        char* r = p && bytes ? p + off : nullptr;
+        off = align_up(off + bytes, 256);
+        return r;
+    };
+    const TexDims pd = cube_faces_dims(d);
+    const int L = mip_levels(pd.TW, pd.TW);
+    s.grad_atlas = reinterpret_cast<float*>(take(cubemap_mip_atlas_texels(d) * d.C * sizeof(float)));
+    s.level_grad = reinterpret_cast<float*>(take((size_t)mip_pyramid_texels(pd, L) * d.C * sizeof(float)));
+    if (deterministic) {
+        s.indices = reinterpret_cast<float*>(take((size_t)d.total * 2 * sizeof(float)));
+        s.grad_out = reinterpret_cast<float*>(take((size_t)d.total * d.C * sizeof(float)));
+        s.det = take(carve_texture_det_scratch(nullptr, d).bytes);
+    }
+    s.bytes = off;
+    return s;
+}
+
+// The pyramid is built in level 0's slot of the atlas (it holds 6 TB (S + 2)^2 texels, the pyramid fewer than
+// 6 TB S^2 / 3), the atlases of levels 1 .. L-1 from it, and level 0's atlas last, over it.
+cudaError_t launch_cubemap_mip_forward(const float* cubemap, const float* directions, const float* lod, float* atlas,
+                                       float* out, const TexDims& d, cudaStream_t stream, int* launches)
+{
+    const TexDims pd = cube_faces_dims(d);
+    const CubeMip m = cube_mip_of(d, lod);
+    cudaError_t e = launch_texture_mip_build(cubemap, atlas, pd, stream, launches);
+    if (e != cudaSuccess) return e;
+    for (int k = m.L - 1; k >= 0; --k) {
+        const TexDims dk = cube_level_dims(d, k);
+        cube_atlas_kernel<<<blocks_for(6ll * d.TB * dk.texels * d.C), TEX_THREADS, 0, stream>>>(
+            k == 0 ? cubemap : atlas + mip_offset(pd, k) * d.C, atlas + m.offset[k] * d.C, dk);
+        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+        ++*launches;
+    }
+    e = with_ct(d.C, [&](auto ct) { return cube_forward_ct<decltype(ct)::value, true>(atlas, directions, out, d, m, stream); });
+    if (e == cudaSuccess) ++*launches;
+    return e;
+}
+
+cudaError_t launch_cubemap_mip_backward(const float* atlas, const float* directions, const float* lod, const float* grad_out,
+                                        float* grad_cubemap, float* grad_directions, float* grad_lod, const TexDims& d,
+                                        bool deterministic, const CubeMipScratch& s, cudaStream_t stream, int* launches)
+{
+    const TexDims pd = cube_faces_dims(d);
+    const CubeMip m = cube_mip_of(d, lod);
+    cudaError_t e;
+    if (d.total == 0) {
+        if (grad_cubemap &&
+            (e = cudaMemsetAsync(grad_cubemap, 0, sizeof(float) * (size_t)pd.TB * pd.texels * d.C, stream)) != cudaSuccess)
+            return e;
+        return cudaSuccess;
+    }
+    if (!grad_cubemap) deterministic = false;
+    if (grad_cubemap && !deterministic &&
+        (e = cudaMemsetAsync(s.grad_atlas, 0, sizeof(float) * m.offset[m.L] * d.C, stream)) != cudaSuccess)
+        return e;
+    // the default kernel: every gradient, or under the deterministic flag grad_directions and grad_lod (no atomics)
+    float* ga = grad_cubemap && !deterministic ? s.grad_atlas : nullptr;
+    if (ga || grad_directions || grad_lod) {
+        const int smem_first = cube_smem_first(d, m);
+        e = with_ct(d.C, [&](auto ct) {
+            return cube_backward_ct<decltype(ct)::value, true>(atlas, directions, grad_out, ga, grad_directions, d, m,
+                                                                grad_lod, smem_first, stream);
+        });
+        if (e != cudaSuccess) return e;
+        ++*launches;
+    }
+    if (!grad_cubemap) return cudaSuccess;
+    if (deterministic) {
+        // block (k, f) of grad_atlas, every texel written, by the §7.5 path over the lookups that read level k on face f
+        for (int k = 0; k < m.L; ++k) {
+            const TexDims dk = cube_level_dims(d, k);
+            for (int f = 0; f < 6; ++f) {
+                cube_mip_terms_kernel<<<blocks_for(d.total), TEX_THREADS, 0, stream>>>(directions, d, m, grad_out, k, f, f == 0,
+                                                                                        s.indices, s.grad_out);
+                if ((e = cudaGetLastError()) != cudaSuccess) return e;
+                ++*launches;
+                float* gk = s.grad_atlas + (m.offset[k] + (size_t)f * d.TB * dk.texels) * d.C;
+                if ((e = launch_texture_backward_deterministic(nullptr, s.indices, s.grad_out, gk, nullptr, dk,
+                                                               carve_texture_det_scratch(s.det, dk), stream, launches)) !=
+                    cudaSuccess)
+                    return e;
+            }
+        }
+    }
+    // each level's border adjoint into the pyramid's layout (level 0: grad_cubemap), then the pyramid's adjoint
+    for (int k = 0; k < m.L; ++k) {
+        const TexDims dk = cube_level_dims(d, k);
+        const long long S = dk.TW - 2;
+        cube_adjoint_kernel<<<blocks_for(6ll * d.TB * S * S * d.C), TEX_THREADS, 0, stream>>>(
+            s.grad_atlas + m.offset[k] * d.C, k == 0 ? grad_cubemap : s.level_grad + mip_offset(pd, k) * d.C, dk);
+        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+        ++*launches;
+    }
+    if (m.L > 1) {
+        mip_collapse_kernel<<<blocks_for((long long)pd.TB * pd.texels * d.C), TEX_THREADS, 0, stream>>>(grad_cubemap,
+                                                                                                       s.level_grad, pd, m.L);
+        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+        ++*launches;
+    }
     return cudaSuccess;
 }
 

@@ -255,7 +255,61 @@ class _SampleCubemap(torch.autograd.Function):
         return grad_cubemap, grad_directions, None, None
 
 
-def sample_cubemap(cubemap, directions, mode='bilinear'):
+class _SampleCubemapMip(torch.autograd.Function):
+    """dirt_cubemap_sample_trilinear / dirt_cubemap_sample_trilinear_backward.  cubemap [TB, 6, S, S, C], directions
+    [B, N, 3], lod [B, N], contiguous fp32 CUDA.  The mip atlas (every level's padded faces) is built per call and kept
+    for the backward pass in place of the cube map."""
+
+    @staticmethod
+    def forward(ctx, cubemap, directions, lod, out_shape):
+        TB, _, S, _, C = cubemap.shape
+        B, N = directions.shape[0], directions.shape[1]
+        L = _lib.lib()
+        out = torch.empty(out_shape, dtype=torch.float32, device=directions.device)
+        atlas = torch.empty(int(L.dirt_cubemap_mip_atlas_bytes(TB, S, C)) // 4, dtype=torch.float32,
+                            device=directions.device)
+        with torch.cuda.device(directions.device):
+            rc = L.dirt_cubemap_sample_trilinear(_ptr(cubemap), _ptr(directions), _ptr(lod), _ptr(atlas), _ptr(out), TB, S,
+                                                 C, B, N, _stream_ptr(directions.device))
+        _lib.check(rc, 'SampleCubemapTrilinear')
+        ctx.save_for_backward(atlas, directions, lod)
+        ctx.shape = (TB, S, C)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_out):
+        want_cubemap, want_directions, want_lod = ctx.needs_input_grad[:3]
+        if not (want_cubemap or want_directions or want_lod):
+            return None, None, None, None
+        atlas, directions, lod = ctx.saved_tensors
+        TB, S, C = ctx.shape
+        B, N = directions.shape[0], directions.shape[1]
+        L = _lib.lib()
+        grad_out = grad_out.contiguous().to(torch.float32)
+        dev = directions.device
+        grad_cubemap = torch.empty((TB, 6, S, S, C), dtype=torch.float32, device=dev) if want_cubemap else None
+        grad_directions = torch.empty_like(directions) if want_directions else None
+        grad_lod = torch.empty_like(lod) if want_lod else None
+        # grad_directions and grad_lod are per lookup and already reproducible; grad_cubemap needs the sorted path
+        deterministic = bool(want_cubemap and torch.are_deterministic_algorithms_enabled())
+        scratch_bytes = int(L.dirt_cubemap_sample_trilinear_backward_bytes(TB, S, C, B, N, int(deterministic)))
+        scratch = torch.empty(scratch_bytes, dtype=torch.uint8, device=dev) if scratch_bytes else None
+        with torch.cuda.device(dev):
+            rc = L.dirt_cubemap_sample_trilinear_backward(
+                _ptr(atlas), _ptr(directions), _ptr(lod), _ptr(grad_out), _ptr(grad_cubemap), _ptr(grad_directions),
+                _ptr(grad_lod), TB, S, C, B, N, int(deterministic), _ptr(scratch), scratch_bytes, _stream_ptr(dev))
+        if deterministic and rc == _lib.ERR_BAD_SHAPE:
+            # the shapes passed the forward call: what fails are the sorted path's 32-bit limits
+            raise RuntimeError(
+                'sample_cubemap backward: the cube-map gradient has no deterministic implementation for %d lookups '
+                'into %d x 6 x %d x %d texels (it needs fewer than 2^31 lookups and padded texels per face), but '
+                'torch.use_deterministic_algorithms(True) is set' % (B * N, TB, S, S))
+        _lib.check(rc, 'SampleCubemapTrilinearGrad')
+        return grad_cubemap, grad_directions, grad_lod, None
+
+
+def sample_cubemap(cubemap, directions, mode='bilinear', lod=None):
     """Reads a cube map in the given directions, seamlessly across its edges and corners, with gradients to the texels
     and to the directions.
 
@@ -265,18 +319,30 @@ def sample_cubemap(cubemap, directions, mode='bilinear'):
             (0, 0) corner, rows running along t
         directions: float32 tensor [..., 3] for a shared cube map, [B, ..., 3] for per-item cube maps; any length
         mode: 'bilinear' (the four texels around the lookup; near an edge or a corner they come from the adjacent faces,
-            so there is no seam) or 'nearest' (the texel the lookup falls in; no gradient to the directions)
+            so there is no seam), 'nearest' (the texel the lookup falls in; no gradient to the directions) or
+            'trilinear' (bilinear lookups of the two levels of the cube map's box pyramid around `lod`, blended;
+            DESIGN.md §7.11)
+        lod: 'trilinear' only, and required there: the level of detail in levels, 0 the finest and
+            log2(S) the 1 x 1 level of an S = 2^n map (an odd S has level 0 alone).  A float, or a float32 tensor
+            broadcastable to directions.shape[:-1]; it gets a gradient (the difference of the two levels' values,
+            0 where it is clamped to the pyramid or NaN).  lod <= 0 returns exactly what 'bilinear' returns, and an
+            integer lod = k the bilinear lookup of level k.  A typical use maps a roughness to a level.
 
     Returns:
         float32 tensor directions.shape[:-1] + (C,), equal bit for bit to the torch restatement in
-        tests/cubemap_restatement.py (DESIGN.md §7.10).  A zero or non-finite direction returns 0 in every channel and
+        tests/cubemap_restatement.py (DESIGN.md §7.10; 'trilinear': tests/cubemap_mip_restatement.py).  A zero or non-finite direction returns 0 in every channel and
         passes no gradient back.  Under torch.use_deterministic_algorithms(True) the cube-map gradient is
         bit-reproducible.
 
     Needs CUDA tensors (there is no CPU kernel); anything else array-like is moved to the current CUDA device.
     """
-    if mode not in _MODES:
-        raise ValueError("sample_cubemap: mode must be 'bilinear' or 'nearest', not %r" % (mode,))
+    if mode not in _MODES and mode != 'trilinear':
+        raise ValueError("sample_cubemap: mode must be 'bilinear', 'nearest' or 'trilinear', not %r" % (mode,))
+    if mode == 'trilinear' and lod is None:
+        raise ValueError("sample_cubemap: mode 'trilinear' needs lod, a float or a tensor broadcastable to "
+                         "directions.shape[:-1]")
+    if mode != 'trilinear' and lod is not None:
+        raise ValueError("sample_cubemap: lod is only used by mode 'trilinear', not by %r" % (mode,))
     device = _pick_device(cubemap, directions)
     cubemap = _as_f32(cubemap, device)
     directions = _as_f32(directions, device)
@@ -291,7 +357,17 @@ def sample_cubemap(cubemap, directions, mode='bilinear'):
     if per_item and (directions.dim() < 2 or directions.shape[0] != cubemap.shape[0]):
         raise ValueError('SampleCubemap expects directions of per-item cube maps to be at least 2D, and '
                          'directions.shape[0] == cubemap.shape[0]')
-    _require_cuda(cubemap, directions)
+    if mode == 'trilinear':
+        lod = _as_f32(lod, device)
+        try:
+            # broadcast before the autograd Function, so that autograd sums the gradient of a broadcast lod
+            lod = lod.expand(directions.shape[:-1])
+        except RuntimeError:
+            raise ValueError('SampleCubemap expects lod broadcastable to directions.shape[:-1] = %s, got %s'
+                             % (tuple(directions.shape[:-1]), tuple(lod.shape)))
+        _require_cuda(cubemap, directions, lod)
+    else:
+        _require_cuda(cubemap, directions)
     out_shape = tuple(directions.shape[:-1]) + (int(cubemap.shape[-1]),)
     B = int(directions.shape[0]) if per_item else 1
     N = 1
@@ -299,4 +375,6 @@ def sample_cubemap(cubemap, directions, mode='bilinear'):
         N *= int(n)
     flat = directions.reshape(B, N, 3).contiguous()
     cube = (cubemap if per_item else cubemap[None]).contiguous()
+    if mode == 'trilinear':
+        return _SampleCubemapMip.apply(cube, flat, lod.reshape(B, N).contiguous(), out_shape)
     return _SampleCubemap.apply(cube, flat, _MODES[mode], out_shape)

@@ -325,6 +325,34 @@ int dirt_cubemap_sample_backward(const float* atlas, const float* directions, co
                                  int TB, int S, int C, int B, long long N, int mode, int deterministic,
                                  void* scratch, size_t scratch_bytes, void* cuda_stream);
 
+/* Mipmapped (trilinear) cube-map lookup (DESIGN.md §7.11), with gradients to the texels, the directions and the level
+ * of detail.  Shapes, faces and the per-level lookup as for dirt_cubemap_sample's bilinear mode, and:
+ *   lod              float32 [B, N], the level of detail in levels, 0 the finest; grad_lod float32 [B, N]
+ *   atlas            the padded faces of every level, dirt_cubemap_mip_atlas_bytes(TB, S, C) bytes, written by
+ *                    dirt_cubemap_sample_trilinear; the only state dirt_cubemap_sample_trilinear_backward reads
+ * Levels: L = dirt_texture_mip_levels(S, S); level k >= 1 is each face's 2x2 box mean of level k-1 (S >> k per edge),
+ * bit for bit dirt_texture_mip_build of the [6*TB, S, S, C] faces.  Level k is read at ((t * S_k - 0.5) + 1,
+ * (s * S_k - 0.5) + 1) on its own padded faces (S_k = S >> k), whose border comes from the adjacent faces at level k.
+ * lambda = lod, NaN -> 0, clamped to [0, L-1]; l = floor(lambda), f = lambda - l;
+ * out = (1-f) * b_l + f * b_{l+1}, each operation rounded in that order, and b_l alone (level l+1 not read) when
+ * f == 0: lod <= 0 is dirt_cubemap_sample's bilinear lookup bit for bit.
+ * Backward: grad_cubemap through both levels' weights, each level's border adjoint and the pyramid's adjoint;
+ * grad_directions through both levels' fractions; grad_lod = sum_c grad_out_c * (b_{m+1,c} - b_{m,c}),
+ * m = min(floor(lambda), L-2), and 0 where lod < 0, lod > L-1, lod is NaN, L = 1 or the direction is invalid.
+ * Any of the three may be NULL, and its work is skipped.  deterministic != 0: grad_cubemap is bit-reproducible (per
+ * level and face, the path of dirt_texture_sample_backward_deterministic, then the fixed-order adjoints), with the
+ * limits of dirt_cubemap_sample_backward's deterministic path.  scratch as for dirt_cubemap_sample_backward, at least
+ * dirt_cubemap_sample_trilinear_backward_bytes(...) bytes.  B = 0 or N = 0: nothing is launched (the backward call
+ * still zeroes grad_cubemap). */
+size_t dirt_cubemap_mip_atlas_bytes(int TB, int S, int C);
+int dirt_cubemap_sample_trilinear(const float* cubemap, const float* directions, const float* lod, float* atlas,
+                                  float* out, int TB, int S, int C, int B, long long N, void* cuda_stream);
+size_t dirt_cubemap_sample_trilinear_backward_bytes(int TB, int S, int C, int B, long long N, int deterministic);
+int dirt_cubemap_sample_trilinear_backward(const float* atlas, const float* directions, const float* lod,
+                                           const float* grad_out, float* grad_cubemap, float* grad_directions,
+                                           float* grad_lod, int TB, int S, int C, int B, long long N, int deterministic,
+                                           void* scratch, size_t scratch_bytes, void* cuda_stream);
+
 /* Reflectance models of the reference's lighting module (dirt/lighting.py:182-343), one value per point and channel.
  * B items of V points each, C channels:
  *   normals, positions   float32 [B*V, 3], row stride normals_stride / positions_stride floats, unit stride along the row
