@@ -118,6 +118,24 @@ def load(path):
     L.dirt_cubemap_sample_trilinear_backward_bytes.argtypes = [i] * 4 + [ctypes.c_longlong, i]
     L.dirt_cubemap_sample_trilinear_backward.restype = i
     L.dirt_cubemap_sample_trilinear_backward.argtypes = [vp] * 7 + [i] * 4 + [ctypes.c_longlong, i, vp, sz, vp]
+    L.dirt_cubemap_ggx_atlas_bytes.restype = sz
+    L.dirt_cubemap_ggx_atlas_bytes.argtypes = [i] * 3
+    L.dirt_cubemap_ggx_prefilter.restype = i
+    L.dirt_cubemap_ggx_prefilter.argtypes = [vp] * 2 + [i] * 3 + [vp]
+    L.dirt_cubemap_sample_ggx.restype = i
+    L.dirt_cubemap_sample_ggx.argtypes = [vp] * 5 + [i] * 4 + [ctypes.c_longlong, vp]
+    L.dirt_cubemap_sample_ggx_backward_bytes.restype = sz
+    L.dirt_cubemap_sample_ggx_backward_bytes.argtypes = [i] * 4 + [ctypes.c_longlong, i]
+    L.dirt_cubemap_sample_ggx_backward.restype = i
+    L.dirt_cubemap_sample_ggx_backward.argtypes = [vp] * 7 + [i] * 4 + [ctypes.c_longlong, i, vp, sz, vp]
+    L.dirt_ggx_brdf_table.restype = i
+    L.dirt_ggx_brdf_table.argtypes = [vp, i, vp]
+    L.dirt_cubemap_sh_project_bytes.restype = sz
+    L.dirt_cubemap_sh_project_bytes.argtypes = [i] * 3
+    L.dirt_cubemap_sh_project.restype = i
+    L.dirt_cubemap_sh_project.argtypes = [vp, vp, vp, sz] + [i] * 3 + [vp]
+    L.dirt_cubemap_sh_project_backward.restype = i
+    L.dirt_cubemap_sh_project_backward.argtypes = [vp, vp, vp, sz] + [i] * 3 + [vp]
     ll = ctypes.c_longlong
     light_inputs = [i, i, vp, ll, vp, ll, vp, ll] + [vp, i] * 4
     L.dirt_lighting_workspace_bytes.restype = sz
@@ -162,7 +180,10 @@ EXPORTED_SYMBOLS = ['dirt_error_string', 'dirt_abi_version', 'dirt_workspace_byt
                     'dirt_sh_lighting_backward', 'dirt_ggx_lighting_forward', 'dirt_ggx_lighting_backward',
                     'dirt_cubemap_atlas_bytes', 'dirt_cubemap_sample', 'dirt_cubemap_sample_backward_bytes',
                     'dirt_cubemap_sample_backward', 'dirt_cubemap_mip_atlas_bytes', 'dirt_cubemap_sample_trilinear',
-                    'dirt_cubemap_sample_trilinear_backward_bytes', 'dirt_cubemap_sample_trilinear_backward']
+                    'dirt_cubemap_sample_trilinear_backward_bytes', 'dirt_cubemap_sample_trilinear_backward',
+                    'dirt_cubemap_ggx_atlas_bytes', 'dirt_cubemap_ggx_prefilter', 'dirt_cubemap_sample_ggx',
+                    'dirt_cubemap_sample_ggx_backward_bytes', 'dirt_cubemap_sample_ggx_backward', 'dirt_ggx_brdf_table',
+                    'dirt_cubemap_sh_project_bytes', 'dirt_cubemap_sh_project', 'dirt_cubemap_sh_project_backward']
 
 
 def error_string(code):

@@ -667,6 +667,148 @@ extern "C" int dirt_cubemap_sample_trilinear_backward(const float* atlas, const 
     return DIRT_OK;
 }
 
+// ---- split-sum GGX image-based lighting ----
+
+// the mipmapped lookup's limits; the prefiltered levels, their normalisers and the texel table add less than the mip
+// atlas again
+static bool cubemap_ggx_shape_ok(int TB, int S, int C, int B, long long N)
+{
+    return cubemap_mip_shape_ok(TB, S, C, B, N) && (double)TB * 16 * (S + 2) * (S + 2) * (C + 4) <= 4.0e18;
+}
+
+extern "C" size_t dirt_cubemap_ggx_atlas_bytes(int TB, int S, int C)
+{
+    if (TB < 0 || !cubemap_ggx_shape_ok(TB, S, C, TB, 0)) return 0;
+    return sizeof(float) * (size_t)ggx_layout(cubemap_dims(TB, S, C, TB, 0, DIRT_TEXTURE_BILINEAR)).floats;
+}
+
+extern "C" int dirt_cubemap_ggx_prefilter(const float* cubemap, float* atlas, int TB, int S, int C, void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (TB < 0 || !cubemap_ggx_shape_ok(TB, S, C, TB, 0)) return DIRT_ERR_BAD_SHAPE;
+    if (TB == 0) return DIRT_OK;
+    if (!cubemap || !atlas) return DIRT_ERR_NULL_POINTER;
+    if ((uintptr_t)cubemap % 4 || (uintptr_t)atlas % 16) return DIRT_ERR_MISALIGNED;
+    CUDA_TRY(launch_ggx_prefilter(cubemap, atlas, cubemap_dims(TB, S, C, TB, 0, DIRT_TEXTURE_BILINEAR),
+                                  (cudaStream_t)cuda_stream, &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
+extern "C" int dirt_cubemap_sample_ggx(const float* cubemap, const float* directions, const float* lod, float* atlas,
+                                       float* out, int TB, int S, int C, int B, long long N, void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (!cubemap_ggx_shape_ok(TB, S, C, B, N)) return DIRT_ERR_BAD_SHAPE;
+    if (B == 0 || N == 0) return DIRT_OK;
+    if (!cubemap || !directions || !lod || !atlas || !out) return DIRT_ERR_NULL_POINTER;
+    if ((uintptr_t)cubemap % 4 || (uintptr_t)directions % 4 || (uintptr_t)lod % 4 || (uintptr_t)atlas % 16 ||
+        (uintptr_t)out % 4)
+        return DIRT_ERR_MISALIGNED;
+    CUDA_TRY(launch_cubemap_ggx_forward(cubemap, directions, lod, atlas, out,
+                                        cubemap_dims(TB, S, C, B, N, DIRT_TEXTURE_BILINEAR), (cudaStream_t)cuda_stream,
+                                        &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
+extern "C" size_t dirt_cubemap_sample_ggx_backward_bytes(int TB, int S, int C, int B, long long N, int deterministic)
+{
+    if (!cubemap_ggx_shape_ok(TB, S, C, B, N) || (long long)B * N == 0) return 0;
+    if (deterministic && !texture_det_shape_ok(TB, S + 2, S + 2, C, B, N, DIRT_TEXTURE_BILINEAR)) return 0;
+    return carve_cubemap_ggx_scratch(nullptr, cubemap_dims(TB, S, C, B, N, DIRT_TEXTURE_BILINEAR), deterministic != 0).bytes;
+}
+
+extern "C" int dirt_cubemap_sample_ggx_backward(const float* atlas, const float* directions, const float* lod,
+                                                const float* grad_out, float* grad_cubemap, float* grad_directions,
+                                                float* grad_lod, int TB, int S, int C, int B, long long N, int deterministic,
+                                                void* scratch, size_t scratch_bytes, void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (!cubemap_ggx_shape_ok(TB, S, C, B, N)) return DIRT_ERR_BAD_SHAPE;
+    if (deterministic && grad_cubemap && !texture_det_shape_ok(TB, S + 2, S + 2, C, B, N, DIRT_TEXTURE_BILINEAR))
+        return DIRT_ERR_BAD_SHAPE;
+    const TexDims d = cubemap_dims(TB, S, C, B, N, DIRT_TEXTURE_BILINEAR);
+    if (d.total > 0) {
+        if (!directions || !lod || !grad_out) return DIRT_ERR_NULL_POINTER;
+        // the lookups read the atlas; the prefilter's adjoint reads its normalisers and texel table
+        if ((grad_directions || grad_lod || grad_cubemap) && !atlas) return DIRT_ERR_NULL_POINTER;
+    }
+    if ((uintptr_t)atlas % 16 || (uintptr_t)directions % 4 || (uintptr_t)lod % 4 || (uintptr_t)grad_out % 4 ||
+        (uintptr_t)grad_cubemap % 4 || (uintptr_t)grad_directions % 4 || (uintptr_t)grad_lod % 4)
+        return DIRT_ERR_MISALIGNED;
+    const bool det = deterministic && grad_cubemap && d.total > 0;
+    const bool uses_scratch = grad_cubemap && d.total > 0;
+    if (uses_scratch) {
+        if (!scratch) return DIRT_ERR_NULL_POINTER;
+        if ((uintptr_t)scratch % 256) return DIRT_ERR_MISALIGNED;
+        if (scratch_bytes < dirt_cubemap_sample_ggx_backward_bytes(TB, S, C, B, N, det)) return DIRT_ERR_WORKSPACE_TOO_SMALL;
+    }
+    CUDA_TRY(launch_cubemap_ggx_backward(atlas, directions, lod, grad_out, grad_cubemap, grad_directions, grad_lod, d, det,
+                                         carve_cubemap_ggx_scratch(uses_scratch ? scratch : nullptr, d, det),
+                                         (cudaStream_t)cuda_stream, &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
+// S <= 2^14 and the [TB, 6, S, S, C] elements within int64, as the cube-map lookup
+static bool cubemap_sh_shape_ok(int TB, int S, int C)
+{
+    return TB >= 0 && S > 0 && S <= (1 << 14) && C > 0 && (double)TB * 6 * S * S * C <= 4.0e18;
+}
+
+extern "C" size_t dirt_cubemap_sh_project_bytes(int TB, int S, int C)
+{
+    return cubemap_sh_shape_ok(TB, S, C) && TB > 0 ? sh_project_scratch_bytes(TB, S, C) : 0;
+}
+
+extern "C" int dirt_cubemap_sh_project(const float* cubemap, float* coeffs, void* scratch, size_t scratch_bytes, int TB,
+                                       int S, int C, void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (!cubemap_sh_shape_ok(TB, S, C)) return DIRT_ERR_BAD_SHAPE;
+    if (TB == 0) return DIRT_OK;
+    if (!cubemap || !coeffs || !scratch) return DIRT_ERR_NULL_POINTER;
+    if ((uintptr_t)cubemap % 4 || (uintptr_t)coeffs % 4 || (uintptr_t)scratch % 256) return DIRT_ERR_MISALIGNED;
+    if (scratch_bytes < sh_project_scratch_bytes(TB, S, C)) return DIRT_ERR_WORKSPACE_TOO_SMALL;
+    CUDA_TRY(launch_sh_project(cubemap, coeffs, scratch, TB, S, C, (cudaStream_t)cuda_stream, &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
+extern "C" int dirt_cubemap_sh_project_backward(const float* grad_coeffs, float* grad_cubemap, void* scratch,
+                                                size_t scratch_bytes, int TB, int S, int C, void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (!cubemap_sh_shape_ok(TB, S, C)) return DIRT_ERR_BAD_SHAPE;
+    if (TB == 0) return DIRT_OK;
+    if (!grad_coeffs || !grad_cubemap || !scratch) return DIRT_ERR_NULL_POINTER;
+    if ((uintptr_t)grad_coeffs % 4 || (uintptr_t)grad_cubemap % 4 || (uintptr_t)scratch % 256) return DIRT_ERR_MISALIGNED;
+    if (scratch_bytes < sh_project_scratch_bytes(TB, S, C)) return DIRT_ERR_WORKSPACE_TOO_SMALL;
+    CUDA_TRY(launch_sh_project_backward(grad_coeffs, grad_cubemap, scratch, TB, S, C, (cudaStream_t)cuda_stream,
+                                        &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
+extern "C" int dirt_ggx_brdf_table(float* table, int N, void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (N < 0 || N > 4096) return DIRT_ERR_BAD_SHAPE;
+    if (N == 0) return DIRT_OK;
+    if (!table) return DIRT_ERR_NULL_POINTER;
+    if ((uintptr_t)table % 4) return DIRT_ERR_MISALIGNED;
+    CUDA_TRY(launch_ggx_brdf_table(table, N, (cudaStream_t)cuda_stream, &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
 // element offsets of every per-point buffer stay below 2^62, the chunk count within the grid's x limit
 static bool lighting_shape_ok(int model, int B, long long V, int C, long long sn, long long sp, long long sc)
 {

@@ -1957,17 +1957,19 @@ CubeMipScratch carve_cubemap_mip_scratch(void* base, const TexDims& d, bool dete
 
 // The pyramid is built in level 0's slot of the atlas (it holds 6 TB (S + 2)^2 texels, the pyramid fewer than
 // 6 TB S^2 / 3), the atlases of levels 1 .. L-1 from it, and level 0's atlas last, over it.
-cudaError_t launch_cubemap_mip_forward(const float* cubemap, const float* directions, const float* lod, float* atlas,
-                                       float* out, const TexDims& d, cudaStream_t stream, int* launches)
+// every level's atlas from level 0 (cubemap) and levels 1 .. L-1 (the pyramid layout at levels), coarsest first, then
+// the lookups
+static cudaError_t cube_mip_atlas_lookup(const float* cubemap, const float* levels, const float* directions,
+                                         const float* lod, float* atlas, float* out, const TexDims& d, cudaStream_t stream,
+                                         int* launches)
 {
     const TexDims pd = cube_faces_dims(d);
     const CubeMip m = cube_mip_of(d, lod);
-    cudaError_t e = launch_texture_mip_build(cubemap, atlas, pd, stream, launches);
-    if (e != cudaSuccess) return e;
+    cudaError_t e;
     for (int k = m.L - 1; k >= 0; --k) {
         const TexDims dk = cube_level_dims(d, k);
         cube_atlas_kernel<<<blocks_for(6ll * d.TB * dk.texels * d.C), TEX_THREADS, 0, stream>>>(
-            k == 0 ? cubemap : atlas + mip_offset(pd, k) * d.C, atlas + m.offset[k] * d.C, dk);
+            k == 0 ? cubemap : levels + mip_offset(pd, k) * d.C, atlas + m.offset[k] * d.C, dk);
         if ((e = cudaGetLastError()) != cudaSuccess) return e;
         ++*launches;
     }
@@ -1976,10 +1978,22 @@ cudaError_t launch_cubemap_mip_forward(const float* cubemap, const float* direct
     return e;
 }
 
-cudaError_t launch_cubemap_mip_backward(const float* atlas, const float* directions, const float* lod, const float* grad_out,
-                                        float* grad_cubemap, float* grad_directions, float* grad_lod, const TexDims& d,
-                                        bool deterministic, const CubeMipScratch& s, cudaStream_t stream, int* launches)
+cudaError_t launch_cubemap_mip_forward(const float* cubemap, const float* directions, const float* lod, float* atlas,
+                                       float* out, const TexDims& d, cudaStream_t stream, int* launches)
 {
+    const cudaError_t e = launch_texture_mip_build(cubemap, atlas, cube_faces_dims(d), stream, launches);
+    if (e != cudaSuccess) return e;
+    return cube_mip_atlas_lookup(cubemap, atlas, directions, lod, atlas, out, d, stream, launches);
+}
+
+// the lookups' gradients, and the cube map's by level: level 0 to grad_cubemap, levels 1 .. L-1 to s.level_grad; *done
+// when grad_cubemap is complete (no lookups, or no grad_cubemap)
+static cudaError_t cube_mip_level_grads(const float* atlas, const float* directions, const float* lod,
+                                        const float* grad_out, float* grad_cubemap, float* grad_directions, float* grad_lod,
+                                        const TexDims& d, bool deterministic, const CubeMipScratch& s, cudaStream_t stream,
+                                        int* launches, bool* done)
+{
+    *done = true;
     const TexDims pd = cube_faces_dims(d);
     const CubeMip m = cube_mip_of(d, lod);
     cudaError_t e;
@@ -2031,12 +2045,71 @@ cudaError_t launch_cubemap_mip_backward(const float* atlas, const float* directi
         if ((e = cudaGetLastError()) != cudaSuccess) return e;
         ++*launches;
     }
+    *done = false;
+    return cudaSuccess;
+}
+
+cudaError_t launch_cubemap_mip_backward(const float* atlas, const float* directions, const float* lod, const float* grad_out,
+                                        float* grad_cubemap, float* grad_directions, float* grad_lod, const TexDims& d,
+                                        bool deterministic, const CubeMipScratch& s, cudaStream_t stream, int* launches)
+{
+    const TexDims pd = cube_faces_dims(d);
+    const CubeMip m = cube_mip_of(d, lod);
+    bool done;
+    cudaError_t e = cube_mip_level_grads(atlas, directions, lod, grad_out, grad_cubemap, grad_directions, grad_lod, d,
+                                         deterministic, s, stream, launches, &done);
+    if (e != cudaSuccess || done) return e;
     if (m.L > 1) {
         mip_collapse_kernel<<<blocks_for((long long)pd.TB * pd.texels * d.C), TEX_THREADS, 0, stream>>>(grad_cubemap,
                                                                                                        s.level_grad, pd, m.L);
         if ((e = cudaGetLastError()) != cudaSuccess) return e;
         ++*launches;
     }
+    return cudaSuccess;
+}
+
+// ---- split-sum GGX lookup (DESIGN.md §7.12): §7.11's lookup on the GGX-prefiltered levels (ibl.cu) ----
+
+CubeGgxScratch carve_cubemap_ggx_scratch(void* base, const TexDims& d, bool deterministic)
+{
+    CubeGgxScratch s = {};
+    s.mip = carve_cubemap_mip_scratch(base, d, deterministic);
+    const TexDims pd = cube_faces_dims(d);
+    const size_t src = sizeof(float) * (size_t)mip_pyramid_texels(pd, mip_levels(pd.TW, pd.TW)) * d.C;
+    s.src_grad = base && src ? reinterpret_cast<float*>(static_cast<char*>(base) + s.mip.bytes) : nullptr;
+    s.bytes = align_up(s.mip.bytes + src, 256);
+    return s;
+}
+
+cudaError_t launch_cubemap_ggx_forward(const float* cubemap, const float* directions, const float* lod, float* atlas,
+                                       float* out, const TexDims& d, cudaStream_t stream, int* launches)
+{
+    const cudaError_t e = launch_ggx_prefilter(cubemap, atlas, d, stream, launches);
+    if (e != cudaSuccess) return e;
+    return cube_mip_atlas_lookup(cubemap, atlas + ggx_layout(d).levels, directions, lod, atlas, out, d, stream, launches);
+}
+
+// the lookups' backward pass and border adjoints as §7.11's, then the prefilter's adjoint into the box levels (level 0
+// straight into grad_cubemap) and the box pyramid's adjoint
+cudaError_t launch_cubemap_ggx_backward(const float* atlas, const float* directions, const float* lod, const float* grad_out,
+                                        float* grad_cubemap, float* grad_directions, float* grad_lod, const TexDims& d,
+                                        bool deterministic, const CubeGgxScratch& s, cudaStream_t stream, int* launches)
+{
+    const TexDims pd = cube_faces_dims(d);
+    const int L = mip_levels(pd.TW, pd.TW);
+    bool done;
+    cudaError_t e = cube_mip_level_grads(atlas, directions, lod, grad_out, grad_cubemap, grad_directions, grad_lod, d,
+                                         deterministic, s.mip, stream, launches, &done);
+    if (e != cudaSuccess || done || L == 1) return e;
+    if ((e = cudaMemsetAsync(s.src_grad, 0, sizeof(float) * (size_t)mip_pyramid_texels(pd, L) * d.C, stream)) != cudaSuccess)
+        return e;
+    if ((e = launch_ggx_prefilter_adjoint(atlas, s.mip.level_grad, s.src_grad, grad_cubemap, d, stream, launches)) !=
+        cudaSuccess)
+        return e;
+    mip_collapse_kernel<<<blocks_for((long long)pd.TB * pd.texels * d.C), TEX_THREADS, 0, stream>>>(grad_cubemap, s.src_grad,
+                                                                                                   pd, L);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    ++*launches;
     return cudaSuccess;
 }
 

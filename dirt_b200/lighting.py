@@ -8,8 +8,9 @@ shapes `cuda_route` accepts, and their torch restatements (`_diffuse_directional
 `_diffuse_point`) otherwise; see DESIGN.md §7.2.  `diffuse_spherical_harmonics` (order-2 SH environment lighting) is
 routed the same way, between dirt_sh_lighting_forward / _backward and `_diffuse_spherical_harmonics`; see DESIGN.md
 §7.8.  So are `specular_ggx_directional` and `specular_ggx_point` (GGX microfacet specular), between
-dirt_ggx_lighting_forward / _backward and `_specular_ggx`; see DESIGN.md §7.9.  `split_vertices_by_face` is torch
-code.
+dirt_ggx_lighting_forward / _backward and `_specular_ggx`; see DESIGN.md §7.9.  `ggx_environment_brdf` and
+`specular_ggx_environment` (split-sum GGX environment lighting, DESIGN.md §7.12) are torch code around a CUDA table and
+the CUDA cube-map lookup; `cubemap_spherical_harmonics` projects a cube map onto order-2 SH with CUDA kernels.  `split_vertices_by_face` is torch code.
 """
 import math
 from collections import namedtuple
@@ -513,6 +514,128 @@ def specular_ggx_point(vertex_positions, vertex_normals, vertex_roughness, verte
     `diffuse_point`, there is no distance falloff."""
     return _specular_ggx_call(True, vertex_positions, vertex_normals, vertex_roughness, vertex_specular,
                               light_position, light_color, camera_position, double_sided)
+
+
+# ---- split-sum GGX image-based lighting (DESIGN.md §7.12) ----------------------------------------------------------
+
+GGX_BRDF_TABLE_SIZE = 128
+_BRDF_TABLES = {}
+
+
+def _ggx_brdf_table(device):
+    """The split-sum table [N, N, 2] of dirt_ggx_brdf_table on `device`, built once per device."""
+    key = (device.type, device.index if device.index is not None else torch.cuda.current_device())
+    if key not in _BRDF_TABLES:
+        N = GGX_BRDF_TABLE_SIZE
+        table = torch.empty((N, N, 2), dtype=torch.float32, device=device)
+        with torch.cuda.device(device):
+            rc = _lib.lib().dirt_ggx_brdf_table(table.data_ptr(), N, torch.cuda.current_stream(device).cuda_stream)
+        _lib.check(rc, 'GGXBRDFTable')
+        _BRDF_TABLES[key] = table
+    return _BRDF_TABLES[key]
+
+
+def ggx_environment_brdf(n_dot_v, roughness):
+    """The split-sum GGX BRDF (A, B): the integrals over light directions of (1 - F_c) D Vis (n.l) and F_c D Vis (n.l),
+    F_c = (1 - v.h)^5, with `specular_ggx_directional`'s D and Vis (roughness clamped below at 0.045).  Under a uniform
+    environment of radiance E, E * (F0 * A + B) is `specular_ggx_directional / pi` integrated over light directions.
+
+    n_dot_v, roughness: float32 CUDA tensors (or floats), broadcastable together -> [..., 2].  A bilinear read of a
+    128 x 128 table (nodes at (i + 0.5) / 128 on both axes, clamped to the outer nodes), differentiable in both
+    arguments; the table comes from a CUDA kernel and is kept once per device."""
+    device = next((t.device for t in (n_dot_v, roughness) if isinstance(t, torch.Tensor)), None)
+    if device is None or device.type != 'cuda':
+        device = torch.device('cuda')
+    n_dot_v = torch.as_tensor(n_dot_v, dtype=torch.float32, device=device)
+    roughness = torch.as_tensor(roughness, dtype=torch.float32, device=device)
+    n_dot_v, roughness = torch.broadcast_tensors(n_dot_v, roughness)
+    table = _ggx_brdf_table(device)
+    N = table.shape[0]
+
+    def split(u):
+        x = (u * N - 0.5).clamp(0., N - 1.)
+        i0 = x.detach().floor().clamp(max=N - 2).long()
+        return i0, (x - i0)[..., None]
+
+    i0, fx = split(n_dot_v)
+    j0, fy = split(roughness)
+    return ((table[i0, j0] * (1. - fy) + table[i0, j0 + 1] * fy) * (1. - fx) +
+            (table[i0 + 1, j0] * (1. - fy) + table[i0 + 1, j0 + 1] * fy) * fx)
+
+
+class _CubemapSH(torch.autograd.Function):
+    """dirt_cubemap_sh_project / _backward: cubemap [TB, 6, S, S, C] contiguous fp32 CUDA -> [TB, 9, C]."""
+
+    @staticmethod
+    def forward(ctx, cubemap):
+        TB, _, S, _, C = cubemap.shape
+        L = _lib.lib()
+        out = torch.empty((TB, 9, C), dtype=torch.float32, device=cubemap.device)
+        nbytes = int(L.dirt_cubemap_sh_project_bytes(TB, S, C))
+        scratch = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=cubemap.device)
+        with torch.cuda.device(cubemap.device):
+            rc = L.dirt_cubemap_sh_project(cubemap.data_ptr(), out.data_ptr(), scratch.data_ptr(), nbytes, TB, S, C,
+                                           torch.cuda.current_stream(cubemap.device).cuda_stream)
+        _lib.check(rc, 'CubemapSH')
+        ctx.shape = (TB, S, C)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad):
+        TB, S, C = ctx.shape
+        L = _lib.lib()
+        grad = grad.contiguous().to(torch.float32)
+        out = torch.empty((TB, 6, S, S, C), dtype=torch.float32, device=grad.device)
+        nbytes = int(L.dirt_cubemap_sh_project_bytes(TB, S, C))
+        scratch = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=grad.device)
+        with torch.cuda.device(grad.device):
+            rc = L.dirt_cubemap_sh_project_backward(grad.data_ptr(), out.data_ptr(), scratch.data_ptr(), nbytes, TB, S, C,
+                                                    torch.cuda.current_stream(grad.device).cuda_stream)
+        _lib.check(rc, 'CubemapSHGrad')
+        return out
+
+
+def cubemap_spherical_harmonics(cubemap):
+    """The order-2 SH coefficients of the radiance in a cube map: L_k = sum_j L(l_j) Y_k(l_j) Omega_j over its texels,
+    with the texel directions and solid angles of the split-sum prefilter (DESIGN.md §7.12) and the basis of
+    `diffuse_spherical_harmonics`, which takes the result as it stands, so that diffuse and specular lighting come from
+    one map.
+
+    cubemap: float32 CUDA tensor [6, S, S, C] or [B, 6, S, S, C] -> [9, C] or [B, 9, C].  A CUDA reduction in a fixed
+    order (float64 partial sums), so bit-reproducible; the gradient to the cube map is elementwise."""
+    if not isinstance(cubemap, torch.Tensor) or cubemap.device.type != 'cuda':
+        raise RuntimeError('cubemap_spherical_harmonics needs a CUDA tensor (there is no CPU kernel)')
+    if cubemap.dim() not in (4, 5) or cubemap.shape[-4] != 6 or cubemap.shape[-3] != cubemap.shape[-2] or \
+            cubemap.shape[-2] <= 0 or cubemap.shape[-1] <= 0:
+        raise ValueError('cubemap_spherical_harmonics expects cubemap.shape == [6, S, S, C] or [B, 6, S, S, C]')
+    per_item = cubemap.dim() == 5
+    cube = (cubemap if per_item else cubemap[None]).to(torch.float32).contiguous()
+    out = _CubemapSH.apply(cube)
+    return out if per_item else out[0]
+
+
+def specular_ggx_environment(vertex_positions, vertex_normals, vertex_roughness, vertex_specular, cubemap,
+                             camera_position, double_sided=True, name=None):
+    """GGX specular reflection of an environment cube map, by the split-sum approximation: the cube map prefiltered
+    with the GGX lobe (`sample_cubemap(..., mode='ggx')`) read in the mirror direction, times F0 * A + B of
+    `ggx_environment_brdf`.  In radiance units, like `diffuse_spherical_harmonics`.
+
+    vertex_positions, vertex_normals [*, V, 3], vertex_roughness [*, V, 1], vertex_specular [*, V, C] (F0), cubemap
+    [6, S, S, C] (shared) or [B, 6, S, S, C] (one per item, with * = B), camera_position [*, 3] or [3] -> [*, V, C].
+    As in `specular_ggx_directional`, v runs towards the camera, double_sided turns normals facing away from it towards
+    it, and the result is 0 where n . v <= 0.  Composed in torch from the CUDA lookup and table."""
+    from .texture import sample_cubemap
+    n = _unit(vertex_normals)
+    v = _unit(camera_position[..., None, :] - vertex_positions)
+    if double_sided:
+        n = torch.where((n * v).sum(-1, keepdim=True) < 0, -n, n)
+    n_dot_v = (n * v).sum(-1, keepdim=True)
+    lit = n_dot_v > 0
+    reflected = 2. * n_dot_v * n - v
+    roughness = vertex_roughness[..., 0]
+    radiance = sample_cubemap(cubemap, reflected, mode='ggx', roughness=roughness)
+    ab = ggx_environment_brdf(n_dot_v[..., 0].clamp(0., 1.), roughness)
+    return torch.where(lit, radiance * (vertex_specular * ab[..., :1] + ab[..., 1:]), 0.)
 
 
 # ---- the CUDA path of the spherical-harmonics lighting --------------------------------------------------------------

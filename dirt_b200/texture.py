@@ -256,24 +256,26 @@ class _SampleCubemap(torch.autograd.Function):
 
 
 class _SampleCubemapMip(torch.autograd.Function):
-    """dirt_cubemap_sample_trilinear / dirt_cubemap_sample_trilinear_backward.  cubemap [TB, 6, S, S, C], directions
-    [B, N, 3], lod [B, N], contiguous fp32 CUDA.  The mip atlas (every level's padded faces) is built per call and kept
-    for the backward pass in place of the cube map."""
+    """dirt_cubemap_sample_trilinear / dirt_cubemap_sample_trilinear_backward, or with ggx the dirt_cubemap_sample_ggx
+    pair.  cubemap [TB, 6, S, S, C], directions [B, N, 3], lod [B, N], contiguous fp32 CUDA.  The mip atlas (every
+    level's padded faces; with ggx also the prefiltered levels, their normalisers and the texel table) is built per
+    call and kept for the backward pass in place of the cube map."""
 
     @staticmethod
-    def forward(ctx, cubemap, directions, lod, out_shape):
+    def forward(ctx, cubemap, directions, lod, out_shape, ggx=False):
         TB, _, S, _, C = cubemap.shape
         B, N = directions.shape[0], directions.shape[1]
         L = _lib.lib()
         out = torch.empty(out_shape, dtype=torch.float32, device=directions.device)
-        atlas = torch.empty(int(L.dirt_cubemap_mip_atlas_bytes(TB, S, C)) // 4, dtype=torch.float32,
-                            device=directions.device)
+        atlas_bytes = L.dirt_cubemap_ggx_atlas_bytes if ggx else L.dirt_cubemap_mip_atlas_bytes
+        atlas = torch.empty(int(atlas_bytes(TB, S, C)) // 4, dtype=torch.float32, device=directions.device)
+        sample = L.dirt_cubemap_sample_ggx if ggx else L.dirt_cubemap_sample_trilinear
         with torch.cuda.device(directions.device):
-            rc = L.dirt_cubemap_sample_trilinear(_ptr(cubemap), _ptr(directions), _ptr(lod), _ptr(atlas), _ptr(out), TB, S,
-                                                 C, B, N, _stream_ptr(directions.device))
-        _lib.check(rc, 'SampleCubemapTrilinear')
+            rc = sample(_ptr(cubemap), _ptr(directions), _ptr(lod), _ptr(atlas), _ptr(out), TB, S, C, B, N,
+                        _stream_ptr(directions.device))
+        _lib.check(rc, 'SampleCubemapGGX' if ggx else 'SampleCubemapTrilinear')
         ctx.save_for_backward(atlas, directions, lod)
-        ctx.shape = (TB, S, C)
+        ctx.shape, ctx.ggx = (TB, S, C), ggx
         return out
 
     @staticmethod
@@ -281,7 +283,7 @@ class _SampleCubemapMip(torch.autograd.Function):
     def backward(ctx, grad_out):
         want_cubemap, want_directions, want_lod = ctx.needs_input_grad[:3]
         if not (want_cubemap or want_directions or want_lod):
-            return None, None, None, None
+            return None, None, None, None, None
         atlas, directions, lod = ctx.saved_tensors
         TB, S, C = ctx.shape
         B, N = directions.shape[0], directions.shape[1]
@@ -293,10 +295,13 @@ class _SampleCubemapMip(torch.autograd.Function):
         grad_lod = torch.empty_like(lod) if want_lod else None
         # grad_directions and grad_lod are per lookup and already reproducible; grad_cubemap needs the sorted path
         deterministic = bool(want_cubemap and torch.are_deterministic_algorithms_enabled())
-        scratch_bytes = int(L.dirt_cubemap_sample_trilinear_backward_bytes(TB, S, C, B, N, int(deterministic)))
+        backward_bytes, backward = ((L.dirt_cubemap_sample_ggx_backward_bytes, L.dirt_cubemap_sample_ggx_backward) if ctx.ggx
+                                    else (L.dirt_cubemap_sample_trilinear_backward_bytes,
+                                          L.dirt_cubemap_sample_trilinear_backward))
+        scratch_bytes = int(backward_bytes(TB, S, C, B, N, int(deterministic)))
         scratch = torch.empty(scratch_bytes, dtype=torch.uint8, device=dev) if scratch_bytes else None
         with torch.cuda.device(dev):
-            rc = L.dirt_cubemap_sample_trilinear_backward(
+            rc = backward(
                 _ptr(atlas), _ptr(directions), _ptr(lod), _ptr(grad_out), _ptr(grad_cubemap), _ptr(grad_directions),
                 _ptr(grad_lod), TB, S, C, B, N, int(deterministic), _ptr(scratch), scratch_bytes, _stream_ptr(dev))
         if deterministic and rc == _lib.ERR_BAD_SHAPE:
@@ -305,11 +310,11 @@ class _SampleCubemapMip(torch.autograd.Function):
                 'sample_cubemap backward: the cube-map gradient has no deterministic implementation for %d lookups '
                 'into %d x 6 x %d x %d texels (it needs fewer than 2^31 lookups and padded texels per face), but '
                 'torch.use_deterministic_algorithms(True) is set' % (B * N, TB, S, S))
-        _lib.check(rc, 'SampleCubemapTrilinearGrad')
-        return grad_cubemap, grad_directions, grad_lod, None
+        _lib.check(rc, 'SampleCubemapGGXGrad' if ctx.ggx else 'SampleCubemapTrilinearGrad')
+        return grad_cubemap, grad_directions, grad_lod, None, None
 
 
-def sample_cubemap(cubemap, directions, mode='bilinear', lod=None):
+def sample_cubemap(cubemap, directions, mode='bilinear', lod=None, roughness=None):
     """Reads a cube map in the given directions, seamlessly across its edges and corners, with gradients to the texels
     and to the directions.
 
@@ -327,22 +332,33 @@ def sample_cubemap(cubemap, directions, mode='bilinear', lod=None):
             broadcastable to directions.shape[:-1]; it gets a gradient (the difference of the two levels' values,
             0 where it is clamped to the pyramid or NaN).  lod <= 0 returns exactly what 'bilinear' returns, and an
             integer lod = k the bilinear lookup of level k.  A typical use maps a roughness to a level.
+        roughness: 'ggx' only, and required there: the GGX roughness of a split-sum environment lookup (DESIGN.md
+            §7.12).  'ggx' is 'trilinear' with lod = roughness * (L-1) on the levels of the cube map prefiltered with
+            the GGX lobe of roughness k / (L-1) (level 0 the map itself); a float or a float32 tensor broadcastable
+            to directions.shape[:-1], with a gradient (L-1 times lod's).  roughness <= 0 returns exactly what
+            'bilinear' returns.  Needs an even S (L >= 2); the prefiltered levels are rebuilt on every call.
 
     Returns:
         float32 tensor directions.shape[:-1] + (C,), equal bit for bit to the torch restatement in
-        tests/cubemap_restatement.py (DESIGN.md §7.10; 'trilinear': tests/cubemap_mip_restatement.py).  A zero or non-finite direction returns 0 in every channel and
+        tests/cubemap_restatement.py (DESIGN.md §7.10; 'trilinear': tests/cubemap_mip_restatement.py; 'ggx': the
+        same level blend of the prefiltered levels, which tests/cubemap_ggx_restatement.py defines).  A zero or non-finite direction returns 0 in every channel and
         passes no gradient back.  Under torch.use_deterministic_algorithms(True) the cube-map gradient is
         bit-reproducible.
 
     Needs CUDA tensors (there is no CPU kernel); anything else array-like is moved to the current CUDA device.
     """
-    if mode not in _MODES and mode != 'trilinear':
-        raise ValueError("sample_cubemap: mode must be 'bilinear', 'nearest' or 'trilinear', not %r" % (mode,))
+    if mode not in _MODES and mode not in ('trilinear', 'ggx'):
+        raise ValueError("sample_cubemap: mode must be 'bilinear', 'nearest', 'trilinear' or 'ggx', not %r" % (mode,))
     if mode == 'trilinear' and lod is None:
         raise ValueError("sample_cubemap: mode 'trilinear' needs lod, a float or a tensor broadcastable to "
                          "directions.shape[:-1]")
     if mode != 'trilinear' and lod is not None:
         raise ValueError("sample_cubemap: lod is only used by mode 'trilinear', not by %r" % (mode,))
+    if mode == 'ggx' and roughness is None:
+        raise ValueError("sample_cubemap: mode 'ggx' needs roughness, a float or a tensor broadcastable to "
+                         "directions.shape[:-1]")
+    if mode != 'ggx' and roughness is not None:
+        raise ValueError("sample_cubemap: roughness is only used by mode 'ggx', not by %r" % (mode,))
     device = _pick_device(cubemap, directions)
     cubemap = _as_f32(cubemap, device)
     directions = _as_f32(directions, device)
@@ -357,7 +373,14 @@ def sample_cubemap(cubemap, directions, mode='bilinear', lod=None):
     if per_item and (directions.dim() < 2 or directions.shape[0] != cubemap.shape[0]):
         raise ValueError('SampleCubemap expects directions of per-item cube maps to be at least 2D, and '
                          'directions.shape[0] == cubemap.shape[0]')
-    if mode == 'trilinear':
+    if mode == 'ggx':
+        S = int(cubemap.shape[-2])
+        if S % 2:
+            raise ValueError("sample_cubemap: mode 'ggx' needs an even cube-map size (a mip chain of at least two "
+                             "levels), got %d; with one level the roughness would be ignored" % S)
+        # lod = roughness * (L-1) in torch, so that autograd carries lod's gradient to the roughness
+        lod = _as_f32(roughness, device) * float(_mip_level_count(S) - 1)
+    if mode in ('trilinear', 'ggx'):
         lod = _as_f32(lod, device)
         try:
             # broadcast before the autograd Function, so that autograd sums the gradient of a broadcast lod
@@ -375,6 +398,15 @@ def sample_cubemap(cubemap, directions, mode='bilinear', lod=None):
         N *= int(n)
     flat = directions.reshape(B, N, 3).contiguous()
     cube = (cubemap if per_item else cubemap[None]).contiguous()
-    if mode == 'trilinear':
-        return _SampleCubemapMip.apply(cube, flat, lod.reshape(B, N).contiguous(), out_shape)
+    if mode in ('trilinear', 'ggx'):
+        return _SampleCubemapMip.apply(cube, flat, lod.reshape(B, N).contiguous(), out_shape, mode == 'ggx')
     return _SampleCubemap.apply(cube, flat, _MODES[mode], out_shape)
+
+
+def _mip_level_count(S):
+    """Levels of an S x S face's box pyramid: one more per halving while the edge is even."""
+    L = 1
+    while S > 0 and S % 2 == 0:
+        S //= 2
+        L += 1
+    return L

@@ -353,6 +353,51 @@ int dirt_cubemap_sample_trilinear_backward(const float* atlas, const float* dire
                                            float* grad_lod, int TB, int S, int C, int B, long long N, int deterministic,
                                            void* scratch, size_t scratch_bytes, void* cuda_stream);
 
+/* Split-sum GGX image-based lighting (DESIGN.md §7.12).  Shapes as for dirt_cubemap_sample_trilinear, and:
+ *   atlas            dirt_cubemap_ggx_atlas_bytes(TB, S, C) bytes, 16-byte aligned: the mip atlas of the prefiltered
+ *                    levels, then (float offsets) the prefiltered levels 1 .. L-1 in the layout of
+ *                    dirt_texture_mip_build's pyramid of the [6*TB, S, S, C] faces, their normalisers W in the pyramid
+ *                    layout of 6 faces of 1 channel (shared by every item), the texel table (one float4 per texel
+ *                    of levels 0 .. L-1 of the 6 faces: direction, solid angle) and the cone table (one float4 per
+ *                    16 x 16 block of those faces: axis, half-angle).  The offsets are pure functions of
+ *                    (TB, S, C): DESIGN.md §7.12.
+ * Levels: L = dirt_texture_mip_levels(S, S); level 0 is the cube map; level k >= 1 (S >> k per edge, roughness
+ * r = k / (L-1), alpha2 = max(r, 0.045)^4) is P_k(r) = sum_j w_j src_j / W(r), w_j = D(c_j) c_j Omega_j,
+ * D(c) = alpha2 / (pi k^2), k = alpha2 + (1-c)(1-alpha2)/2, c_j the fp32 cosine between the texel directions, over the
+ * texels j of box level min(k, s*) (s* the coarsest level of at least 16 texels per edge, 0 when S < 16) with c_j > 0
+ * and c_j >= c_k = max(0, 1 - 2 (sqrt(1000) - 1) alpha2 / (1 - alpha2)).
+ * dirt_cubemap_ggx_prefilter writes the texel table, levels 1 .. L-1 and W (and uses level 0's slot of the mip atlas
+ * as scratch); dirt_cubemap_sample_ggx calls it, builds the mip atlas of the levels and looks up as
+ * dirt_cubemap_sample_trilinear does on them.  The backward pass reads the atlas alone: the lookup's gradients as
+ * dirt_cubemap_sample_trilinear_backward's, then the prefilter's adjoint (a gather over the same pairs, no atomics)
+ * and the box pyramid's.  scratch: dirt_cubemap_sample_ggx_backward_bytes bytes, 256-byte aligned, when grad_cubemap
+ * is given and B*N > 0. */
+size_t dirt_cubemap_ggx_atlas_bytes(int TB, int S, int C);
+int dirt_cubemap_ggx_prefilter(const float* cubemap, float* atlas, int TB, int S, int C, void* cuda_stream);
+int dirt_cubemap_sample_ggx(const float* cubemap, const float* directions, const float* lod, float* atlas, float* out,
+                            int TB, int S, int C, int B, long long N, void* cuda_stream);
+size_t dirt_cubemap_sample_ggx_backward_bytes(int TB, int S, int C, int B, long long N, int deterministic);
+int dirt_cubemap_sample_ggx_backward(const float* atlas, const float* directions, const float* lod, const float* grad_out,
+                                     float* grad_cubemap, float* grad_directions, float* grad_lod, int TB, int S, int C,
+                                     int B, long long N, int deterministic, void* scratch, size_t scratch_bytes,
+                                     void* cuda_stream);
+/* The split-sum BRDF table, float32 [N, N, 2] = (A, B) at n.v = (i + 0.5) / N (row i) and roughness (j + 0.5) / N
+ * (column j): A = integral of (1 - F_c) D Vis (n.l), B = of F_c D Vis (n.l) over light directions, F_c = (1 - v.h)^5,
+ * D and Vis those of dirt_ggx_lighting_forward; a fixed midpoint rule in float64 over the GGX half-vector
+ * distribution.  N <= 4096. */
+int dirt_ggx_brdf_table(float* table, int N, void* cuda_stream);
+/* Order-2 SH projection of cube maps, cubemap float32 [TB, 6, S, S, C] -> coeffs float32 [TB, 9, C]:
+ * L_k = sum_j L(l_j) Y_k(l_j) Omega_j over the texels j with the texel table's direction and solid angle (level 0 of
+ * dirt_cubemap_ggx_prefilter's table), Y the real order-2 basis of dirt_sh_lighting_forward.  Per item and chunk of
+ * texels the sums are float64 in a fixed order, then added over the chunks in order and rounded once: bit-reproducible.
+ * The backward pass writes grad_cubemap = Omega_j sum_k Y_k(l_j) grad_coeffs_k in full.  scratch:
+ * dirt_cubemap_sh_project_bytes(TB, S, C) bytes, 256-byte aligned (the texel table and the partial sums). */
+size_t dirt_cubemap_sh_project_bytes(int TB, int S, int C);
+int dirt_cubemap_sh_project(const float* cubemap, float* coeffs, void* scratch, size_t scratch_bytes, int TB, int S, int C,
+                            void* cuda_stream);
+int dirt_cubemap_sh_project_backward(const float* grad_coeffs, float* grad_cubemap, void* scratch, size_t scratch_bytes,
+                                     int TB, int S, int C, void* cuda_stream);
+
 /* Reflectance models of the reference's lighting module (dirt/lighting.py:182-343), one value per point and channel.
  * B items of V points each, C channels:
  *   normals, positions   float32 [B*V, 3], row stride normals_stride / positions_stride floats, unit stride along the row
