@@ -136,6 +136,12 @@ def load(path):
     L.dirt_cubemap_sh_project.argtypes = [vp, vp, vp, sz] + [i] * 3 + [vp]
     L.dirt_cubemap_sh_project_backward.restype = i
     L.dirt_cubemap_sh_project_backward.argtypes = [vp, vp, vp, sz] + [i] * 3 + [vp]
+    L.dirt_latlong_samples.restype = i
+    L.dirt_latlong_samples.argtypes = [i] * 3
+    L.dirt_latlong_to_cubemap.restype = i
+    L.dirt_latlong_to_cubemap.argtypes = [vp] * 2 + [i] * 5 + [vp]
+    L.dirt_latlong_to_cubemap_backward.restype = i
+    L.dirt_latlong_to_cubemap_backward.argtypes = [vp] * 2 + [i] * 5 + [vp]
     ll = ctypes.c_longlong
     light_inputs = [i, i, vp, ll, vp, ll, vp, ll] + [vp, i] * 4
     L.dirt_lighting_workspace_bytes.restype = sz
@@ -183,7 +189,8 @@ EXPORTED_SYMBOLS = ['dirt_error_string', 'dirt_abi_version', 'dirt_workspace_byt
                     'dirt_cubemap_sample_trilinear_backward_bytes', 'dirt_cubemap_sample_trilinear_backward',
                     'dirt_cubemap_ggx_atlas_bytes', 'dirt_cubemap_ggx_prefilter', 'dirt_cubemap_sample_ggx',
                     'dirt_cubemap_sample_ggx_backward_bytes', 'dirt_cubemap_sample_ggx_backward', 'dirt_ggx_brdf_table',
-                    'dirt_cubemap_sh_project_bytes', 'dirt_cubemap_sh_project', 'dirt_cubemap_sh_project_backward']
+                    'dirt_cubemap_sh_project_bytes', 'dirt_cubemap_sh_project', 'dirt_cubemap_sh_project_backward',
+                    'dirt_latlong_samples', 'dirt_latlong_to_cubemap', 'dirt_latlong_to_cubemap_backward']
 
 
 def error_string(code):

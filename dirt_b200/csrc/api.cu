@@ -796,6 +796,51 @@ extern "C" int dirt_cubemap_sh_project_backward(const float* grad_coeffs, float*
     return DIRT_OK;
 }
 
+// ---- equirectangular panoramas to cube maps ----
+
+// H, W <= 2^20 keep a sample's rows and columns within half a texel of its fp32 coordinates, and S * n at most
+// 2^21 / pi + S < 2^20, so the sub-sample numerators 2k + 1 are exact in fp32; n <= 4096 keeps n^2 exact in fp32; the
+// elements within int64
+static bool latlong_shape_ok(int TB, int H, int W, int S, int C)
+{
+    if (TB < 0 || H < 1 || W < 1 || H > (1 << 20) || W > (1 << 20) || S < 1 || S > (1 << 14) || C < 1) return false;
+    return latlong_samples(H, W, S) <= 4096 && (double)TB * H * W * C <= 4.0e18 && (double)TB * 6 * S * S * C <= 4.0e18;
+}
+
+extern "C" int dirt_latlong_samples(int H, int W, int S)
+{
+    if (H < 1 || W < 1 || S < 1) return 0;
+    return latlong_samples(H, W, S);
+}
+
+extern "C" int dirt_latlong_to_cubemap(const float* panorama, float* cubemap, int TB, int H, int W, int S, int C,
+                                       void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (!latlong_shape_ok(TB, H, W, S, C)) return DIRT_ERR_BAD_SHAPE;
+    if (TB == 0) return DIRT_OK;
+    if (!panorama || !cubemap) return DIRT_ERR_NULL_POINTER;
+    if ((uintptr_t)panorama % 4 || (uintptr_t)cubemap % 4) return DIRT_ERR_MISALIGNED;
+    CUDA_TRY(launch_latlong_forward(panorama, cubemap, TB, H, W, S, C, (cudaStream_t)cuda_stream, &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
+extern "C" int dirt_latlong_to_cubemap_backward(const float* grad_cubemap, float* grad_panorama, int TB, int H, int W,
+                                                int S, int C, void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (!latlong_shape_ok(TB, H, W, S, C)) return DIRT_ERR_BAD_SHAPE;
+    if (TB == 0) return DIRT_OK;
+    if (!grad_cubemap || !grad_panorama) return DIRT_ERR_NULL_POINTER;
+    if ((uintptr_t)grad_cubemap % 4 || (uintptr_t)grad_panorama % 4) return DIRT_ERR_MISALIGNED;
+    CUDA_TRY(launch_latlong_backward(grad_cubemap, grad_panorama, TB, H, W, S, C, (cudaStream_t)cuda_stream, &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
 extern "C" int dirt_ggx_brdf_table(float* table, int N, void* cuda_stream)
 {
     int launches = 0;

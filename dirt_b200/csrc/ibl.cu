@@ -40,21 +40,6 @@ constexpr unsigned IBL_FULL = 0xffffffffu;
 constexpr float IBL_CONE_SLACK = 4e-3f;           // radians added to the cone test: fp32 acos near 1 is good to ~4e-4
 constexpr double IBL_MIN_ROUGHNESS = 0.045;       // GGX_MIN_ROUGHNESS of lighting.py, in float64
 
-// the point (sc, tc) of face f's plane as a direction: the face table of border_source (texture.cu)
-template <typename T>
-__host__ __device__ __forceinline__ void face_point(int f, T sc, T tc, T& x, T& y, T& z)
-{
-    const T one = T(1);
-    switch (f) {
-        case 0: x = one; y = -tc; z = -sc; break;
-        case 1: x = -one; y = -tc; z = sc; break;
-        case 2: x = sc; y = one; z = tc; break;
-        case 3: x = sc; y = -one; z = -tc; break;
-        case 4: x = sc; y = -tc; z = one; break;
-        default: x = -sc; y = -tc; z = -one; break;
-    }
-}
-
 // One thread per texel of every level: (direction, solid angle).  sc = (2c+1)/S_k - 1 and tc = (2r+1)/S_k - 1 in
 // fp32, the face table, then x / sqrt(fma(z, z, fma(y, y, x*x))) for each component, each operation rounded in that
 // order; the solid angle by the corner formula in float64, rounded once.

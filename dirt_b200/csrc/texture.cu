@@ -81,34 +81,6 @@ __device__ __forceinline__ float2 load_index(const float* indices, long long g)
     return make_float2(__ldg(indices + 2 * g), __ldg(indices + 2 * g + 1));
 }
 
-// the CT channels of one texel (or of one grad_out row) through the read-only path
-template <int CT, bool VEC>
-__device__ __forceinline__ void load_row(const float* p, float v[CT])
-{
-    if (VEC && CT == 4) {
-        const float4 q = __ldg(reinterpret_cast<const float4*>(p));
-        v[0] = q.x; v[1 % CT] = q.y; v[2 % CT] = q.z; v[3 % CT] = q.w;
-    } else if (VEC && CT == 2) {
-        const float2 q = __ldg(reinterpret_cast<const float2*>(p));
-        v[0] = q.x; v[1 % CT] = q.y;
-    } else {
-#pragma unroll
-        for (int j = 0; j < CT; ++j) v[j] = __ldg(p + j);
-    }
-}
-
-// examples/textured.py's expression, one IEEE-rounded operation at a time and in its order:
-// t00*(1-fc)*(1-fr) + t01*fc*(1-fr) + t10*(1-fc)*fr + t11*fc*fr
-__device__ __forceinline__ float bilinear(float t00, float t01, float t10, float t11, float fr, float fc)
-{
-    const float omr = __fsub_rn(1.0f, fr), omc = __fsub_rn(1.0f, fc);
-    const float a = __fmul_rn(__fmul_rn(t00, omc), omr);
-    const float b = __fmul_rn(__fmul_rn(t01, fc), omr);
-    const float c = __fmul_rn(__fmul_rn(t10, omc), fr);
-    const float e = __fmul_rn(__fmul_rn(t11, fc), fr);
-    return __fadd_rn(__fadd_rn(__fadd_rn(a, b), c), e);
-}
-
 // ---- levels of a lookup ---------------------------------------------------------------------------------------------
 //
 // A bilinear or nearest lookup reads level 0, the texture.  A mipmapped (trilinear) lookup (DESIGN.md §7.6) reads a

@@ -5,9 +5,11 @@ uv coordinates to fractional texel indices (plain torch, any device), `sample_te
 (dirt_texture_sample / dirt_texture_sample_backward of include/dirt_b200.h).  The values are those of the torch
 restatement in examples/textured.py, bit for bit; see DESIGN.md §7.1.  `mode='trilinear'` reads a mip pyramid of the
 texture at a level of detail taken from screen-space index derivatives (`index_derivatives` makes them from an index
-image); see DESIGN.md §7.6.
+image); see DESIGN.md §7.6.  `latlong_to_cubemap` converts an equirectangular panorama to the cube map that
+`sample_cubemap` reads (DESIGN.md §7.13).
 """
 import ctypes
+import math
 
 import torch
 from torch.autograd.function import once_differentiable
@@ -410,3 +412,81 @@ def _mip_level_count(S):
         S //= 2
         L += 1
     return L
+
+
+class _LatlongToCubemap(torch.autograd.Function):
+    """dirt_latlong_to_cubemap / dirt_latlong_to_cubemap_backward.  panorama [TB, H, W, C] contiguous fp32 CUDA.  The
+    operator depends on the shapes alone, so the backward pass keeps nothing but them."""
+
+    @staticmethod
+    def forward(ctx, panorama, size):
+        TB, H, W, C = panorama.shape
+        L = _lib.lib()
+        out = torch.empty((TB, 6, size, size, C), dtype=torch.float32, device=panorama.device)
+        with torch.cuda.device(panorama.device):
+            rc = L.dirt_latlong_to_cubemap(_ptr(panorama), _ptr(out), TB, H, W, size, C, _stream_ptr(panorama.device))
+        _lib.check(rc, 'LatlongToCubemap')
+        ctx.shape = (TB, H, W, size, C)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_out):
+        if not ctx.needs_input_grad[0]:
+            return None, None
+        TB, H, W, S, C = ctx.shape
+        grad_out = grad_out.contiguous().to(torch.float32)
+        grad_panorama = torch.empty((TB, H, W, C), dtype=torch.float32, device=grad_out.device)
+        with torch.cuda.device(grad_out.device):
+            rc = _lib.lib().dirt_latlong_to_cubemap_backward(_ptr(grad_out), _ptr(grad_panorama), TB, H, W, S, C,
+                                                             _stream_ptr(grad_out.device))
+        _lib.check(rc, 'LatlongToCubemapGrad')
+        return grad_panorama, None
+
+
+def latlong_to_cubemap(panorama, size):
+    """Converts an equirectangular (latitude-longitude) panorama to a cube map, with the gradient to the panorama.
+
+    Args:
+        panorama: float32 tensor [H, W, C], or [B, H, W, C] for one panorama per batch item; any H, W >= 1.  Row 0 is
+            the zenith (+Y); texel (r, c) is centred at theta = (r + 1/2) pi / H from +Y and longitude
+            phi = (c + 1/2) 2 pi / W - pi, in direction (sin theta sin phi, cos theta, -sin theta cos phi): the centre
+            column faces -Z and, seen from inside, columns run towards +X (`latlong_directions` gives these directions)
+        size: S, the cube map's texels per face edge
+
+    Returns:
+        float32 tensor [6, S, S, C] or [B, 6, S, S, C] for `sample_cubemap` and `lighting.cubemap_spherical_harmonics`.
+        Each cube texel is the mean of n x n bilinear lookups of the panorama at its sub-sample directions,
+        n = max(1, ceil(max(W, 2H) / (pi S))), at least one sample per panorama texel at the centre of a side face.
+        Columns wrap around; rows do not (a lookup near a pole blends the pole row with itself).  Equal bit for bit
+        to the torch restatement in tests/latlong_restatement.py (DESIGN.md §7.13).  The gradient is a gather with no
+        atomics, so it is bit-reproducible with or without torch.use_deterministic_algorithms(True).
+
+    Needs CUDA tensors (there is no CPU kernel); anything else array-like is moved to the current CUDA device.
+    """
+    device = _pick_device(panorama)
+    panorama = _as_f32(panorama, device)
+    if panorama.dim() not in (3, 4):
+        raise ValueError('LatlongToCubemap expects panorama.shape == [height, width, channels] or '
+                         '[None, height, width, channels]')
+    if panorama.shape[-3] <= 0 or panorama.shape[-2] <= 0 or panorama.shape[-1] <= 0:
+        raise ValueError('LatlongToCubemap expects a panorama with positive height, width and channels')
+    if isinstance(size, bool) or int(size) != size or size <= 0:
+        raise ValueError('LatlongToCubemap expects a positive integer size, got %r' % (size,))
+    _require_cuda(panorama)
+    per_item = panorama.dim() == 4
+    out = _LatlongToCubemap.apply((panorama if per_item else panorama[None]).contiguous(), int(size))
+    return out if per_item else out[0]
+
+
+def latlong_directions(height, width, device=None):
+    """The unit directions of an equirectangular panorama's texel centres, float32 [height, width, 3], in the
+    convention of `latlong_to_cubemap` (computed in float64, rounded once).  `sample_cubemap(cubemap,
+    latlong_directions(H, W))` turns a cube map back into a panorama, for example to view or export a fitted one."""
+    if int(height) != height or int(width) != width or height <= 0 or width <= 0:
+        raise ValueError('latlong_directions expects a positive integer height and width, got %r, %r' % (height, width))
+    theta = (torch.arange(int(height), dtype=torch.float64, device=device) + 0.5) * (math.pi / height)
+    phi = (torch.arange(int(width), dtype=torch.float64, device=device) + 0.5) * (2 * math.pi / width) - math.pi
+    st, ct = torch.sin(theta)[:, None], torch.cos(theta)[:, None]
+    sp, cp = torch.sin(phi)[None, :], torch.cos(phi)[None, :]
+    return torch.stack([st * sp, ct.expand(-1, int(width)), -st * cp], -1).to(torch.float32)

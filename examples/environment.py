@@ -34,9 +34,9 @@ def cubemap_directions(size, device=None):
     return d / d.norm(dim=-1, keepdim=True)
 
 
-def procedural_cubemap(size=128, device=None):
-    """An HDR-ish sky over a checkered ground, with a sun: [6, size, size, 3]."""
-    d = cubemap_directions(size, device)
+def sky(d):
+    """An HDR-ish sky over a checkered ground, with a sun, in unit directions d [..., 3] -> [..., 3]."""
+    device = d.device
     up = d[..., 1:2]
     sky = torch.tensor([0.25, 0.45, 0.9], device=device) * (0.6 + 0.4 * up) + 0.3 * (1 - up.abs())
     u, v = d[..., 0] / (d[..., 1].abs() + 0.2), d[..., 2] / (d[..., 1].abs() + 0.2)
@@ -45,6 +45,11 @@ def procedural_cubemap(size=128, device=None):
     sun_dir = torch.tensor([0.4, 0.6, -0.7], device=device)
     sun = 8.0 * torch.exp(-(1 - (d * (sun_dir / sun_dir.norm())).sum(-1, keepdim=True)) * 400.)
     return torch.where(up > 0, sky, ground) + sun
+
+
+def procedural_cubemap(size=128, device=None):
+    """`sky` at the texel centres of a cube map: [6, size, size, 3]."""
+    return sky(cubemap_directions(size, device))
 
 
 def sphere(level=4, device=None):

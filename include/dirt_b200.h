@@ -398,6 +398,27 @@ int dirt_cubemap_sh_project(const float* cubemap, float* coeffs, void* scratch, 
 int dirt_cubemap_sh_project_backward(const float* grad_coeffs, float* grad_cubemap, void* scratch, size_t scratch_bytes,
                                      int TB, int S, int C, void* cuda_stream);
 
+/* Equirectangular (latitude-longitude) panoramas to cube maps (DESIGN.md §7.13), panorama float32 [TB, H, W, C] ->
+ * cubemap float32 [TB, 6, S, S, C] (faces and orientation as for dirt_cubemap_sample), with the adjoint.
+ * Panorama row 0 is the zenith (+Y); texel (r, c) is centred at theta = (r + 1/2) pi / H, phi = (c + 1/2) 2 pi / W - pi,
+ * direction (sin theta sin phi, cos theta, -sin theta cos phi): the centre column faces -Z and columns run towards +X.
+ * Cube texel (f, r, c) is the fp32 mean of n x n samples, n = dirt_latlong_samples(H, W, S)
+ * = max(1, ceil(max(W, 2H) / (pi S))) in float64.  Sample (i, j) lies at sc = (2(c n + j) + 1) / (S n) - 1,
+ * tc = (2(r n + i) + 1) / (S n) - 1 on the face's plane (|major| = 1, not normalised); phi = atan2f(x, -z),
+ * theta = atan2f(sqrtf(x*x + z*z), y), u = phi * fp32(1/(2 pi)) + 0.5, v = theta * fp32(1/pi), and the bilinear rule of
+ * dirt_texture_sample at padded row (v H - 0.5) + 1, column u W - 0.5 of the panorama padded by a copy of row 0 above
+ * and of row H-1 below: columns wrap, rows do not.  The n^2 samples are summed in row-major order and the sum divided
+ * by n^2, each operation rounded in fp32 in that order.
+ * The backward pass writes grad_panorama in full: a gather over the same (sample, texel) pairs in a fixed order, with
+ * no atomics and no scratch, so bit-reproducible.
+ * H, W in 1 .. 2^20, S in 1 .. 2^14, n <= 4096 (n^2 exact in fp32), else DIRT_ERR_BAD_SHAPE (dirt_latlong_samples
+ * returns 0 for H, W or S below 1).  TB = 0: nothing is launched.  All pointers 4-byte aligned; 8- or 16-byte aligned
+ * rows enable the vector paths for C = 2, 4. */
+int dirt_latlong_samples(int H, int W, int S);
+int dirt_latlong_to_cubemap(const float* panorama, float* cubemap, int TB, int H, int W, int S, int C, void* cuda_stream);
+int dirt_latlong_to_cubemap_backward(const float* grad_cubemap, float* grad_panorama, int TB, int H, int W, int S, int C,
+                                     void* cuda_stream);
+
 /* Reflectance models of the reference's lighting module (dirt/lighting.py:182-343), one value per point and channel.
  * B items of V points each, C channels:
  *   normals, positions   float32 [B*V, 3], row stride normals_stride / positions_stride floats, unit stride along the row
