@@ -18,9 +18,9 @@
 //  (1) The tile's 10x12 halo of `face_ids` and of `pixels` arrive by TMA (cp.async.bulk.tensor, one elected lane, one
 //      mbarrier each) -- or, for tiles touching the frame border and for tensors TMA cannot describe, by per-lane
 //      cp.async with at()'s clamping.
-//  (2) FACE TABLE: the distinct faces among the tile's 64 pixels and its 32-pixel ring get a slot each (warp match +
-//      a small open-addressing hash in shared memory); their interpolation planes and vertex positions (TriInterp +
-//      TriXY, 96 B) are copied into the table with cp.async while the Scharr sums are computed.
+//  (2) FACE TABLE: the distinct faces among the tile's 64 pixels and its 32-pixel ring get a slot each, in order of
+//      first sight (warp match + ballot prefix count); their interpolation planes and vertex positions (TriInterp +
+//      TriXY, 96 B) are copied into the table with cp.async as soon as the slot is known.
 //  (3) G-BUFFER TILE: every lane evaluates (barycentrics, clip_w) of its two pixels and of one ring pixel from the table
 //      and parks them in shared memory; the dilation of assemble_grads (:155-194) then only reads neighbouring entries.
 //  (4) Every per-pixel term of assemble_grads is a product  scalar * barycentric  destined for vertex k of one face:
@@ -189,14 +189,17 @@ __device__ __forceinline__ void scharr_smem_c4(const float* __restrict__ tile, i
 }
 
 // the rare tiles that need it (right frame edge) call it out of line: it is ~1000 instructions when inlined four times
-template <int N0>
-__device__ __noinline__ void scharr_global_call(const float* __restrict__ pixels, int b, int row, int col, int B, int H, int W, int cs,
-                                                int c0, float* sxy)
-{
+// (returned by value, in registers: an array argument would give the kernel a stack frame)
+struct ScharrSums {
     float sx[3], sy[3];
-    scharr_global<N0>(pixels, b, row, col, Frame{B, H, W}, cs, c0, sx, sy);
-#pragma unroll
-    for (int k = 0; k < 3; ++k) { sxy[k] = sx[k]; sxy[3 + k] = sy[k]; }
+};
+template <int N0>
+__device__ __noinline__ ScharrSums scharr_global_call(const float* __restrict__ pixels, int b, int row, int col, int B, int H, int W,
+                                                      int cs, int c0)
+{
+    ScharrSums r;
+    scharr_global<N0>(pixels, b, row, col, Frame{B, H, W}, cs, c0, r.sx, r.sy);
+    return r;
 }
 
 // preferred neighbour offset of the dilation (csrc/rasterise_grad_egl.cu:185-190), as a step in the G-buffer tile:
@@ -534,7 +537,6 @@ __global__ void __launch_bounds__(NW * 32, DIRT_BWD_MIN_BLOCKS * DIRT_BWD_WARPS 
         }
         cp_async_commit();
     }
-    if (lane < NSLOT) keys[lane] = -1;
 
     // ---- (2) face ids -> slots of the tile's face table ---------------------------------------------------------------
     if (use_tma) mbar_wait(&bars[0], 0);
@@ -564,47 +566,51 @@ __global__ void __launch_bounds__(NW * 32, DIRT_BWD_MIN_BLOCKS * DIRT_BWD_WARPS 
         if (!in0) near0 = false;
         if (!in1) near1 = false;
     }
-    // slots: one leader per distinct id (warp match) inserts it into the open-addressing hash `keys`
-    bool overflow = false;
-    auto slot_of = [&](int id) -> int {
-        const unsigned peers = __match_any_sync(0xffffffffu, id);
-        const int leader = __ffs(peers) - 1;
-        int slot = -1;
-        if (id >= 0 && lane == leader) {
-            int h = (NSLOT == 32) ? (int)(((unsigned)id * 2654435761u) >> 27) : (int)__umulhi((unsigned)id * 2654435761u, (unsigned)NSLOT);
-#pragma unroll 1
-            for (int probe = 0; probe < NSLOT; ++probe) {
-                const int old = atomicCAS(&keys[h], -1, id);
-                if (old == -1 || old == id) { slot = h; break; }
-                h = (h + 1 == NSLOT) ? 0 : h + 1;
-            }
-            if (slot < 0) overflow = true;
+    // slots in order of first sight, three rounds (pixel 0, pixel 1, ring cell of every lane).  A lane whose face an
+    // earlier round has seen finds its slot in `keys`; the faces new in a round get the next slots from a ballot prefix
+    // count over one leader per distinct id (warp match), and the leader starts that face's 96-byte table copy at once.
+    // Counting every distinct face keeps the overflow rule exact: the tile overflows when there are more than NSLOT.
+    int nslot = 0;   // warp-uniform: distinct faces seen so far
+    auto slot_of = [&](int id, int known) -> int {
+        int slot = known;
+        const int nk = min(nslot, NSLOT);
+        if (__any_sync(0xffffffffu, id >= 0 && slot < 0)) {
+#pragma unroll 4
+            for (int s = 0; s < nk; ++s) slot = (slot < 0 && keys[s] == id) ? s : slot;
         }
-        return __shfl_sync(0xffffffffu, slot, leader);
+        const bool fresh = id >= 0 && slot < 0;
+        if (__any_sync(0xffffffffu, fresh)) {
+            const unsigned peers = __match_any_sync(0xffffffffu, id);
+            const int leader = __ffs(peers) - 1;
+            const unsigned leaders = __ballot_sync(0xffffffffu, fresh && lane == leader);
+            const int mine = nslot + __popc(leaders & ((1u << lane) - 1u));
+            if (fresh && lane == leader && mine < NSLOT) {
+                keys[mine] = id;
+                const uint4* src = reinterpret_cast<const uint4*>(itp_b + id);
+                uint4* dst = reinterpret_cast<uint4*>(table + mine);
+#pragma unroll
+                for (int i = 0; i < 4; ++i) cp_async_16(dst + i, src + i);
+                const uint4* srcx = reinterpret_cast<const uint4*>(xy_b + id);
+                cp_async_16(dst + 4, srcx);
+                cp_async_16(dst + 5, srcx + 1);
+            }
+            const int got = __shfl_sync(0xffffffffu, mine, leader);
+            if (fresh) slot = got;
+            nslot += __popc(leaders);
+            __syncwarp();   // keys[] of this round visible to the next one
+        }
+        return slot;
     };
-    const int slot0 = slot_of(id0);
-    const int s1 = slot_of(id1);
-    const int slotr = slot_of(idr);
-    __syncwarp();
-    if (__any_sync(0xffffffffu, overflow)) {
+    const int slot0 = slot_of(id0, -1);
+    const int s1 = slot_of(id1, id1 == id0 ? slot0 : -1);
+    const int slotr = slot_of(idr, -1);
+    cp_async_commit();
+    if (nslot > NSLOT) {
         // more distinct faces than slots: the reference-shaped path for this tile
+        cp_async_wait_all();
         if (use_tma && want_pos) mbar_wait(&bars[1], 0);
         tile_generic<C>(vertices, pixels, grad_pixels, face_ids, gverts, gcols, itp_b, Frame{d.B, H, W}, d.V, b, col, row0, cs, c0, gstride, want_pos, want_col);
         return;
-    }
-    // fill the table: the lane whose index is an occupied slot copies that face's 96 bytes
-    {
-        const int k = lane < NSLOT ? keys[lane] : -1;
-        if (k >= 0) {
-            const uint4* src = reinterpret_cast<const uint4*>(itp_b + k);
-            uint4* dst = reinterpret_cast<uint4*>(table + lane);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) cp_async_16(dst + i, src + i);
-            const uint4* srcx = reinterpret_cast<const uint4*>(xy_b + k);
-            cp_async_16(dst + 4, srcx);
-            cp_async_16(dst + 5, srcx + 1);
-        }
-        cp_async_commit();
     }
 
     // ---- (3) G-buffer tile: this lane's two pixels and its ring cell ---------------------------------------------------
@@ -664,14 +670,13 @@ __global__ void __launch_bounds__(NW * 32, DIRT_BWD_MIN_BLOCKS * DIRT_BWD_WARPS 
             if (C == 4) scharr_smem_c4(tile, lrow0 + pix + 1, lcol + 1, sx, sy, sx1, sy1);
             else scharr_smem<C, N0>(tile, lrow0 + pix + 1, lcol + 1 + PxTile<C>::COL0, sx, sy);
         } else {
-            float t[6];
-            scharr_global_call<N0>(pixels, b, row, col, d.B, H, W, cs, c0, t);
+            const ScharrSums t = scharr_global_call<N0>(pixels, b, row, col, d.B, H, W, cs, c0);
 #pragma unroll
-            for (int k = 0; k < 3; ++k) { sx[k] = t[k]; sy[k] = t[3 + k]; }
+            for (int k = 0; k < 3; ++k) { sx[k] = t.sx[k]; sy[k] = t.sy[k]; }
             if (TWO_GROUPS) {
-                scharr_global_call<1>(pixels, b, row, col, d.B, H, W, cs, c0 + 3, t);
+                const ScharrSums t1 = scharr_global_call<1>(pixels, b, row, col, d.B, H, W, cs, c0 + 3);
 #pragma unroll
-                for (int k = 0; k < 3; ++k) { sx1[k] = t[k]; sy1[k] = t[3 + k]; }
+                for (int k = 0; k < 3; ++k) { sx1[k] = t1.sx[k]; sy1[k] = t1.sy[k]; }
             }
         }
         float dLdx = 0.f, dLdy = 0.f, gx1 = 0.f, gy1 = 0.f;
@@ -778,11 +783,15 @@ __global__ void __launch_bounds__(NW * 32, DIRT_BWD_MIN_BLOCKS * DIRT_BWD_WARPS 
             const int s = __ffs(occupied) - 1;
             occupied &= occupied - 1;
             const bool mc0 = kc0 == s, mc1 = kc1 == s, mp0 = kp0 == s, mp1 = kp1 == s;
+            // the face's vertex ids are read before the butterfly, so that the read is done when the sum is
+            const int4 q = reinterpret_cast<const int4*>(table + s)[2];   // {sC, v0, v1, v2}
             // First butterfly step at operand level: this lane keeps the NS sums of vertex A and hands those of vertex B
             // to lane^16 (the weights were arranged per half-warp when they were stored), and the halves swap one half
             // each of the NS sums of vertex 2.  The remaining steps are the generic transposed butterfly.
             constexpr int H2 = (NS + 1) / 2;
             float keep[NS], send[NS], third[NS];
+#pragma unroll
+            for (int j = 0; j < NS; ++j) keep[j] = send[j] = third[j] = 0.f;
 #pragma unroll
             for (int pix = 0; pix < 2; ++pix) {
                 const PixelTerms& T = term[pix];
@@ -792,9 +801,9 @@ __global__ void __launch_bounds__(NW * 32, DIRT_BWD_MIN_BLOCKS * DIRT_BWD_WARPS 
 #pragma unroll
                 for (int j = 0; j < NS; ++j) {
                     const float a = (j < C) ? wcA : wpA, bb = (j < C) ? wcB : wpB, cc = (j < C) ? wc2 : wp2;
-                    keep[j] = (pix == 0) ? a * sc[pix][j] : fmaf(a, sc[pix][j], keep[j]);
-                    send[j] = (pix == 0) ? bb * sc[pix][j] : fmaf(bb, sc[pix][j], send[j]);
-                    third[j] = (pix == 0) ? cc * sc[pix][j] : fmaf(cc, sc[pix][j], third[j]);
+                    keep[j] = fmaf(a, sc[pix][j], keep[j]);
+                    send[j] = fmaf(bb, sc[pix][j], send[j]);
+                    third[j] = fmaf(cc, sc[pix][j], third[j]);
                 }
             }
             float v[NS + H2];
@@ -809,7 +818,6 @@ __global__ void __launch_bounds__(NW * 32, DIRT_BWD_MIN_BLOCKS * DIRT_BWD_WARPS 
             float total[1];
             TransposedReduce<NS + H2, 4>::run(v, lane, 8, total);
             if (owner >= 0) {
-                const int4 q = reinterpret_cast<const int4*>(table + s)[2];   // {sC, v0, v1, v2}
                 const int vid = (owner & 1) ? q.z : ((owner & 2) ? q.w : q.y);
                 atomicAdd(owner_row + (size_t)vid * owner_stride, total[0]);
             }
