@@ -392,6 +392,11 @@ __global__ void __launch_bounds__(DIRT_SETUP_THREADS, DIRT_SETUP_MIN_BLOCKS) set
     }
 }
 
+static unsigned setup_blocks(long long total)
+{
+    return (unsigned)max((total + DIRT_SETUP_THREADS - 1) / DIRT_SETUP_THREADS, 1ll);
+}
+
 cudaError_t launch_setup_and_bin(const float* vertices, const int32_t* faces, const float* vertex_colors, const Workspace& ws,
                                  const Dims& d, cudaStream_t stream, int* launches)
 {
@@ -399,11 +404,10 @@ cudaError_t launch_setup_and_bin(const float* vertices, const int32_t* faces, co
     const long long total = (long long)d.B * d.F;
     cudaError_t e;
     if ((e = cudaMemsetAsync(ws.tile_count, 0, ws.zero_bytes, stream)) != cudaSuccess) return e;
-    if (total > 0) {
-        ScopedKernelTimer timer(3, stream);
-        setup_kernel<true><<<(unsigned)((total + DIRT_SETUP_THREADS - 1) / DIRT_SETUP_THREADS), DIRT_SETUP_THREADS, 0, stream>>>(vertices, faces, vertex_colors, ws, d);
-        ++*launches;
-    }
+    // at least one block, even without faces: its first thread leaves the tag, which a later call reusing the workspace checks
+    ScopedKernelTimer timer(3, stream);
+    setup_kernel<true><<<setup_blocks(total), DIRT_SETUP_THREADS, 0, stream>>>(vertices, faces, vertex_colors, ws, d);
+    ++*launches;
     return cudaGetLastError();
 }
 
@@ -413,11 +417,9 @@ cudaError_t launch_setup_only(const float* vertices, const int32_t* faces, const
     const long long total = (long long)d.B * d.F;
     cudaError_t e;
     if ((e = cudaMemsetAsync(ws.header, 0, sizeof(Header), stream)) != cudaSuccess) return e;
-    if (total > 0) {
-        ScopedKernelTimer timer(3, stream);
-        setup_kernel<false><<<(unsigned)((total + DIRT_SETUP_THREADS - 1) / DIRT_SETUP_THREADS), DIRT_SETUP_THREADS, 0, stream>>>(vertices, faces, nullptr, ws, d);
-        ++*launches;
-    }
+    ScopedKernelTimer timer(3, stream);
+    setup_kernel<false><<<setup_blocks(total), DIRT_SETUP_THREADS, 0, stream>>>(vertices, faces, nullptr, ws, d);
+    ++*launches;
     return cudaGetLastError();
 }
 

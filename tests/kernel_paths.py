@@ -137,6 +137,26 @@ def coplanar_tie_scene(channels=3, batch=1, seed=0):
 LARGE_FACE = 87   # index of the large face in coplanar_tie_scene: after 40 + 12 + 35 lower-index faces
 
 
+def bin_overflow_scene(batch=1, n=1200, second=300):
+    """`n` random faces of about 13 x 7 px stacked in the middle of a 96 x 64 frame, C = 3, so that the raster pass's
+    three list levels all fill: the busiest tile takes about 1040 references against bins of BIN_CAP, the busiest row
+    of tiles about 1580 past its bins against row lists of 1024 entries, and the rest goes to the image's large list.
+    With batch=2 the second image keeps its first `second` faces (the rest degenerate): bins and row lists only, with
+    the busiest row 185 entries past its bins."""
+    rng = np.random.default_rng(12)
+    W, H = 96, 64
+    tri = rng.uniform(-0.28, 0.28, size=(n, 3, 2)) + np.array([0.1, -0.05])
+    z = rng.uniform(-0.8, 0.8, size=(n, 3, 1))
+    verts = np.concatenate([tri, z, np.ones((n, 3, 1))], axis=2).reshape(1, n * 3, 4).astype(np.float32)
+    s = dict(background=rng.uniform(size=(1, H, W, 3)).astype(np.float32), vertices=verts,
+             vertex_colors=rng.uniform(size=(1, n * 3, 3)).astype(np.float32),
+             faces=np.arange(n * 3, dtype=np.int32).reshape(1, n, 3))
+    if batch == 2:
+        s = {k: np.concatenate([v, v], axis=0) for k, v in s.items()}
+        s['faces'][1, second:] = 0
+    return s
+
+
 def coverage_masks(vertices, faces, H, W):
     """bool [F,H,W]: the pixels each face of one image covers when drawn alone (the oracle's coverage rule, with no
     depth test involved)."""

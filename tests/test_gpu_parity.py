@@ -460,19 +460,10 @@ def test_pixel_jacobians_of_the_cylinder(cuda_lib, oracle):
 
 def test_bin_overflow_paths(cuda_lib, oracle):
     # one-pass binning: a tile's bin holds 128 references; the rest goes to the overflow list of the tile's row of tiles
-    # (1024 entries per row and image), and when that is full too to the image's large list.  600 stacked faces of ~4x4
-    # tiles each: ~600 references per tile against bins of 128 and ~1900 overflow entries per row -> all three levels.
-    rng = np.random.default_rng(12)
-    n, W, H = 600, 96, 64
-    centre = np.array([0.1, -0.05])
-    tri = rng.uniform(-0.28, 0.28, size=(n, 3, 2)) + centre
-    z = rng.uniform(-0.8, 0.8, size=(n, 3, 1))
-    verts = np.concatenate([tri, z, np.ones((n, 3, 1))], axis=2).reshape(1, n * 3, 4).astype(np.float32)
-    s = dict(background=rng.uniform(size=(1, H, W, 3)).astype(np.float32), vertices=verts,
-             vertex_colors=rng.uniform(size=(1, n * 3, 3)).astype(np.float32),
-             faces=np.arange(n * 3, dtype=np.int32).reshape(1, n, 3))
-    _check_scene(oracle, s, label='bin overflow')
-    # two images with different loads: the lists are per image
-    s2 = {k: np.concatenate([v, v], axis=0) for k, v in s.items()}
-    s2['faces'][1, 150:] = 0   # image 1: 150 real faces (bin + row list only), the rest degenerate
-    _check_scene(oracle, s2, label='bin overflow, two images')
+    # (1024 entries per row and image), and when that is full too to the image's large list.  1200 stacked faces reach
+    # all three levels (tests/test_setup_records_host.py counts them on the CPU, tests/test_gpu_setup_records.py in
+    # the workspace).
+    import kernel_paths as kp
+    _check_scene(oracle, kp.bin_overflow_scene(), label='bin overflow')
+    # two images with different loads: the lists are per image (image 1: bins and row lists only)
+    _check_scene(oracle, kp.bin_overflow_scene(batch=2), label='bin overflow, two images')
