@@ -168,6 +168,18 @@ def load(path):
     L.dirt_normals_forward.argtypes = [i, vp, ll, vp, vp, vp, sz, i, ll, ll, vp]
     L.dirt_normals_backward.restype = i
     L.dirt_normals_backward.argtypes = [i, vp, ll, vp, vp, vp, vp, sz, i, ll, ll, vp]
+    tangent_inputs = [vp, ll, vp, ll, ll, vp, ll, vp]
+    L.dirt_tangents_workspace_bytes.restype = sz
+    L.dirt_tangents_workspace_bytes.argtypes = [i, ll, ll]
+    L.dirt_tangents_forward.restype = i
+    L.dirt_tangents_forward.argtypes = tangent_inputs + [vp, vp, sz, i, ll, ll, vp]
+    L.dirt_tangents_backward.restype = i
+    L.dirt_tangents_backward.argtypes = tangent_inputs + [vp] * 5 + [sz, i, ll, ll, vp]
+    normal_map_inputs = [vp, ll, vp, ll, vp, ll]
+    L.dirt_normal_map_forward.restype = i
+    L.dirt_normal_map_forward.argtypes = normal_map_inputs + [vp, i, ll, vp]
+    L.dirt_normal_map_backward.restype = i
+    L.dirt_normal_map_backward.argtypes = normal_map_inputs + [vp] * 4 + [i, ll, vp]
     return L
 
 
@@ -190,7 +202,9 @@ EXPORTED_SYMBOLS = ['dirt_error_string', 'dirt_abi_version', 'dirt_workspace_byt
                     'dirt_cubemap_ggx_atlas_bytes', 'dirt_cubemap_ggx_prefilter', 'dirt_cubemap_sample_ggx',
                     'dirt_cubemap_sample_ggx_backward_bytes', 'dirt_cubemap_sample_ggx_backward', 'dirt_ggx_brdf_table',
                     'dirt_cubemap_sh_project_bytes', 'dirt_cubemap_sh_project', 'dirt_cubemap_sh_project_backward',
-                    'dirt_latlong_samples', 'dirt_latlong_to_cubemap', 'dirt_latlong_to_cubemap_backward']
+                    'dirt_latlong_samples', 'dirt_latlong_to_cubemap', 'dirt_latlong_to_cubemap_backward',
+                    'dirt_tangents_workspace_bytes', 'dirt_tangents_forward', 'dirt_tangents_backward',
+                    'dirt_normal_map_forward', 'dirt_normal_map_backward']
 
 
 def error_string(code):

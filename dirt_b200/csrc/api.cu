@@ -1237,6 +1237,155 @@ extern "C" int dirt_normals_backward(int mode, const float* vertices, long long 
     return DIRT_OK;
 }
 
+// ---- vertex tangents and normal mapping (DESIGN.md §7.14) ----------------------------------------------------------
+
+// as normals_shape_ok, with the uv and normal rows' strides and the uvs' item stride
+static bool tangents_shape_ok(int B, long long V, long long F, long long vs, long long us, long long uis, long long ns)
+{
+    if (!normals_shape_ok(DIRT_NORMALS_AVERAGE, B, V, F, vs) || us < 2 || uis < 0 || ns < 3) return false;
+    const double rows = (double)B * V;
+    return rows * us + (double)B * uis <= 4.0e18 && rows * ns <= 4.0e18 && rows * 4 <= 4.0e18;
+}
+
+extern "C" size_t dirt_tangents_workspace_bytes(int B, long long V, long long F)
+{
+    return dirt_normals_workspace_bytes(B, V, F);
+}
+
+static int tangents_check(const float* vertices, const float* uvs, const float* normals, const int32_t* faces,
+                          const void* workspace, size_t workspace_bytes, int B, long long V, long long F)
+{
+    const int rc = normals_check(vertices, faces, workspace, workspace_bytes, B, V, F);
+    if (rc != DIRT_OK) return rc;
+    if (!uvs || !normals) return DIRT_ERR_NULL_POINTER;
+    if ((uintptr_t)uvs % 4 || (uintptr_t)normals % 4) return DIRT_ERR_MISALIGNED;
+    return DIRT_OK;
+}
+
+static TangentArgs make_tangent_args(const float* vertices, long long vertex_stride, const float* uvs, long long uv_stride,
+                                     long long uv_item_stride, const float* normals, long long normals_stride,
+                                     const int32_t* faces, int B, long long V, long long F)
+{
+    TangentArgs a = {};
+    a.m = make_normals_args(DIRT_NORMALS_AVERAGE, vertices, vertex_stride, faces, B, V, F);
+    a.uvs = uvs; a.uv_stride = uv_stride; a.uv_item_stride = uv_item_stride;
+    a.normals = normals; a.normal_stride = normals_stride;
+    return a;
+}
+
+extern "C" int dirt_tangents_forward(const float* vertices, long long vertex_stride, const float* uvs, long long uv_stride,
+                                     long long uv_item_stride, const float* normals, long long normals_stride,
+                                     const int32_t* faces, float* tangents, void* workspace, size_t workspace_bytes, int B,
+                                     long long V, long long F, void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (!tangents_shape_ok(B, V, F, vertex_stride, uv_stride, uv_item_stride, normals_stride)) return DIRT_ERR_BAD_SHAPE;
+    if ((long long)B * V == 0) return DIRT_OK;
+    const int rc = tangents_check(vertices, uvs, normals, faces, workspace, workspace_bytes, B, V, F);
+    if (rc != DIRT_OK) return rc;
+    if (!tangents) return DIRT_ERR_NULL_POINTER;
+    if ((uintptr_t)tangents % 4) return DIRT_ERR_MISALIGNED;
+    TangentArgs a = make_tangent_args(vertices, vertex_stride, uvs, uv_stride, uv_item_stride, normals, normals_stride,
+                                      faces, B, V, F);
+    a.out = tangents;
+    CUDA_TRY(launch_tangents_forward(a, carve_normals_workspace(F > 0 ? workspace : nullptr, B, V, F),
+                                     (cudaStream_t)cuda_stream, &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
+extern "C" int dirt_tangents_backward(const float* vertices, long long vertex_stride, const float* uvs, long long uv_stride,
+                                      long long uv_item_stride, const float* normals, long long normals_stride,
+                                      const int32_t* faces, const float* grad_tangents, float* grad_vertices,
+                                      float* grad_uvs, float* grad_normals, void* workspace, size_t workspace_bytes, int B,
+                                      long long V, long long F, void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (!tangents_shape_ok(B, V, F, vertex_stride, uv_stride, uv_item_stride, normals_stride)) return DIRT_ERR_BAD_SHAPE;
+    if ((uintptr_t)grad_vertices % 4 || (uintptr_t)grad_uvs % 4 || (uintptr_t)grad_normals % 4) return DIRT_ERR_MISALIGNED;
+    if ((long long)B * V == 0 || (!grad_vertices && !grad_uvs && !grad_normals)) return DIRT_OK;
+    const int rc = tangents_check(vertices, uvs, normals, faces, workspace, workspace_bytes, B, V, F);
+    if (rc != DIRT_OK) return rc;
+    if (!grad_tangents) return DIRT_ERR_NULL_POINTER;
+    if ((uintptr_t)grad_tangents % 4) return DIRT_ERR_MISALIGNED;
+    TangentArgs a = make_tangent_args(vertices, vertex_stride, uvs, uv_stride, uv_item_stride, normals, normals_stride,
+                                      faces, B, V, F);
+    a.grad = grad_tangents;
+    a.g_vertices = grad_vertices; a.g_uvs = grad_uvs; a.g_normals = grad_normals;
+    CUDA_TRY(launch_tangents_backward(a, carve_normals_workspace(F > 0 ? workspace : nullptr, B, V, F),
+                                      (cudaStream_t)cuda_stream, &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
+// element offsets of every per-point buffer stay below 2^62, the chunk count within the grid's x limit
+static bool normal_map_shape_ok(int B, long long V, long long sn, long long st, long long sm)
+{
+    if (B < 0 || V < 0 || sn < 0 || st < 0 || sm < 0) return false;
+    const double rows = (double)B * V;
+    return rows * (4.0 + sn + st + sm) <= 4.0e18 && light_chunks(V) <= 0x7fffffffll;
+}
+
+static NormalMapArgs make_normal_map_args(const float* normals, long long sn, const float* tangents, long long st,
+                                          const float* samples, long long sm, int B, long long V)
+{
+    NormalMapArgs a = {};
+    a.normals = normals; a.tangents = tangents; a.samples = samples;
+    a.sn = sn; a.st = st; a.sm = sm;
+    a.B = B; a.V = V;
+    return a;
+}
+
+static int normal_map_inputs_check(const NormalMapArgs& a)
+{
+    if (!a.normals || !a.tangents || !a.samples) return DIRT_ERR_NULL_POINTER;
+    if ((uintptr_t)a.normals % 4 || (uintptr_t)a.tangents % 4 || (uintptr_t)a.samples % 4) return DIRT_ERR_MISALIGNED;
+    return DIRT_OK;
+}
+
+extern "C" int dirt_normal_map_forward(const float* normals, long long normals_stride, const float* tangents,
+                                       long long tangents_stride, const float* samples, long long samples_stride,
+                                       float* out, int B, long long V, void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (!normal_map_shape_ok(B, V, normals_stride, tangents_stride, samples_stride)) return DIRT_ERR_BAD_SHAPE;
+    if ((long long)B * V == 0) return DIRT_OK;
+    NormalMapArgs a = make_normal_map_args(normals, normals_stride, tangents, tangents_stride, samples, samples_stride, B, V);
+    const int rc = normal_map_inputs_check(a);
+    if (rc != DIRT_OK) return rc;
+    if (!out) return DIRT_ERR_NULL_POINTER;
+    if ((uintptr_t)out % 4) return DIRT_ERR_MISALIGNED;
+    a.out = out;
+    CUDA_TRY(launch_normal_map_forward(a, (cudaStream_t)cuda_stream, &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
+extern "C" int dirt_normal_map_backward(const float* normals, long long normals_stride, const float* tangents,
+                                        long long tangents_stride, const float* samples, long long samples_stride,
+                                        const float* grad_out, float* grad_normals, float* grad_tangents,
+                                        float* grad_samples, int B, long long V, void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (!normal_map_shape_ok(B, V, normals_stride, tangents_stride, samples_stride)) return DIRT_ERR_BAD_SHAPE;
+    if ((uintptr_t)grad_normals % 4 || (uintptr_t)grad_tangents % 4 || (uintptr_t)grad_samples % 4) return DIRT_ERR_MISALIGNED;
+    if ((long long)B * V == 0 || (!grad_normals && !grad_tangents && !grad_samples)) return DIRT_OK;
+    NormalMapArgs a = make_normal_map_args(normals, normals_stride, tangents, tangents_stride, samples, samples_stride, B, V);
+    const int rc = normal_map_inputs_check(a);
+    if (rc != DIRT_OK) return rc;
+    if (!grad_out) return DIRT_ERR_NULL_POINTER;
+    if ((uintptr_t)grad_out % 4) return DIRT_ERR_MISALIGNED;
+    a.grad_out = grad_out;
+    a.g_normals = grad_normals; a.g_tangents = grad_tangents; a.g_samples = grad_samples;
+    CUDA_TRY(launch_normal_map_backward(a, (cudaStream_t)cuda_stream, &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
 extern "C" int dirt_workspace_status(const void* workspace, size_t workspace_bytes, int B, int H, int W, int C, int V, int F,
                                      void* cuda_stream)
 {

@@ -12,7 +12,8 @@
 //
 // The file also holds the GGX specular reflectance (dirt_ggx_lighting_forward / _backward, DESIGN.md §7.9) and the
 // spherical-harmonics environment lighting (dirt_sh_lighting_forward / _backward, DESIGN.md §7.8), which use the same
-// staging, per-CTA partials and reduction kernel.
+// staging, per-CTA partials and reduction kernel, and the tangent-space normal mapping (dirt_normal_map_forward /
+// _backward, DESIGN.md §7.14), which uses the same staging and grid.
 #include "../../include/dirt_b200.h"
 #include "common.cuh"
 
@@ -1001,6 +1002,162 @@ cudaError_t launch_sh_lighting_backward(const ShArgs& a, cudaStream_t stream, in
         ++*launches;
     }
     return cudaSuccess;
+}
+
+// ---- tangent-space normal mapping (dirt_normal_map_*, DESIGN.md §7.14) -----------------------------------------------
+//
+// n = unit(normal), T = unit(t - (n . t) n) for the tangent's xyz t, s = -1 if its w < 0 else +1,
+// out = unit(m.x T + m.y s (n x T) + m.z n) for the tangent-space sample m; unit(x) = x / (|x| + 1e-12).  One thread per
+// point, laid out as lighting_forward_kernel; the backward kernel recomputes the forward.  No parameter is shared by
+// the points, so there is no reduction.
+
+namespace {
+
+__device__ __forceinline__ void nm_cross(const float a[3], const float b[3], float c[3])
+{
+    c[0] = __fsub_rn(__fmul_rn(a[1], b[2]), __fmul_rn(a[2], b[1]));
+    c[1] = __fsub_rn(__fmul_rn(a[2], b[0]), __fmul_rn(a[0], b[2]));
+    c[2] = __fsub_rn(__fmul_rn(a[0], b[1]), __fmul_rn(a[1], b[0]));
+}
+
+// u = x / (|x| + 1e-12); returns |x|
+__device__ __forceinline__ float nm_unit(const float x[3], float u[3])
+{
+    const float nr = __fsqrt_rn(dot3(x, x)), d = __fadd_rn(nr, 1.e-12f);
+#pragma unroll
+    for (int i = 0; i < 3; ++i) u[i] = __fdiv_rn(x[i], d);
+    return nr;
+}
+
+// torch autograd's gradient of x / (|x| + 1e-12) for the output gradient g (none through the norm of a zero vector)
+__device__ __forceinline__ void nm_unit_grad(const float x[3], const float g[3], float gx[3])
+{
+    const float nr = __fsqrt_rn(dot3(x, x)), d = __fadd_rn(nr, 1.e-12f);
+    const float gd = -__fdiv_rn(dot3(g, x), __fmul_rn(d, d));
+    const float k = nr == 0.f ? 0.f : __fdiv_rn(gd, nr);
+#pragma unroll
+    for (int i = 0; i < 3; ++i) gx[i] = __fmaf_rn(x[i], k, __fdiv_rn(g[i], d));
+}
+
+// The forward's intermediates of one point.
+struct Perturb {
+    float n[3], d, x[3], T[3], s, c[3], y[3];   // n, d = n . t, x = t - d n, T, s, c = n x T, y = the sum out normalises
+};
+
+__device__ __forceinline__ Perturb perturb(const float nrm[3], const float t[4], const float m[3])
+{
+    Perturb p;
+    nm_unit(nrm, p.n);
+    p.d = dot3(p.n, t);
+#pragma unroll
+    for (int i = 0; i < 3; ++i) p.x[i] = __fsub_rn(t[i], __fmul_rn(p.d, p.n[i]));
+    nm_unit(p.x, p.T);
+    p.s = t[3] < 0.f ? -1.f : 1.f;
+    nm_cross(p.n, p.T, p.c);
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+        p.y[i] = __fmaf_rn(m[2], p.n[i], __fmaf_rn(__fmul_rn(m[1], p.s), p.c[i], __fmul_rn(m[0], p.T[i])));
+    return p;
+}
+
+__global__ void __launch_bounds__(LIGHT_THREADS) normal_map_forward_kernel(NormalMapArgs a)
+{
+    __shared__ float stage[LIGHT_THREADS * 4];
+    const int lane = threadIdx.x & 31;
+    float* s = stage + (threadIdx.x & ~31) * 4;
+    const long long v0 = (long long)blockIdx.x * LIGHT_THREADS + (threadIdx.x & ~31);
+    if (v0 >= a.V) return;   // the whole warp
+    const int n = (int)(a.V - v0 < 32 ? a.V - v0 : 32);
+    for (long long b = blockIdx.y; b < a.B; b += gridDim.y) {
+        const long long row0 = b * a.V + v0;
+        float nrm[3], t[4], m[3], o[3];
+        stage_load<3>(a.normals, a.sn, row0, n, s, lane, nrm);
+        stage_load<4>(a.tangents, a.st, row0, n, s, lane, t);
+        stage_load<3>(a.samples, a.sm, row0, n, s, lane, m);
+        const Perturb p = perturb(nrm, t, m);
+        nm_unit(p.y, o);
+        stage_store<3>(a.out, row0, n, s, lane, o);
+    }
+}
+
+__global__ void __launch_bounds__(LIGHT_THREADS) normal_map_backward_kernel(NormalMapArgs a)
+{
+    __shared__ float stage[LIGHT_THREADS * 4];
+    const int lane = threadIdx.x & 31;
+    float* s = stage + (threadIdx.x & ~31) * 4;
+    const long long v0 = (long long)blockIdx.x * LIGHT_THREADS + (threadIdx.x & ~31);
+    if (v0 >= a.V) return;   // the whole warp
+    const int n = (int)(a.V - v0 < 32 ? a.V - v0 : 32);
+    for (long long b = blockIdx.y; b < a.B; b += gridDim.y) {
+        const long long row0 = b * a.V + v0;
+        float nrm[3], t[4], m[3], g[3], gy[3];
+        stage_load<3>(a.normals, a.sn, row0, n, s, lane, nrm);
+        stage_load<4>(a.tangents, a.st, row0, n, s, lane, t);
+        stage_load<3>(a.samples, a.sm, row0, n, s, lane, m);
+        stage_load<3>(a.grad_out, 3, row0, n, s, lane, g);
+        const Perturb p = perturb(nrm, t, m);
+        nm_unit_grad(p.y, g, gy);
+        if (a.g_samples) {
+            float gm[3];
+            gm[0] = dot3(gy, p.T);
+            gm[1] = __fmul_rn(p.s, dot3(gy, p.c));
+            gm[2] = dot3(gy, p.n);
+            stage_store<3>(a.g_samples, row0, n, s, lane, gm);
+        }
+        if (!a.g_normals && !a.g_tangents) continue;
+        // y = m.x T + m.y s (n x T) + m.z n: with q = m.y s gy, a . (n x T) gives T x q to n and q x n to T
+        float q[3], gT[3], gn[3], tq[3], qn[3], gx[3];
+#pragma unroll
+        for (int i = 0; i < 3; ++i) q[i] = __fmul_rn(__fmul_rn(m[1], p.s), gy[i]);
+        nm_cross(p.T, q, tq);
+        nm_cross(q, p.n, qn);
+#pragma unroll
+        for (int i = 0; i < 3; ++i) {
+            gT[i] = __fmaf_rn(m[0], gy[i], qn[i]);
+            gn[i] = __fmaf_rn(m[2], gy[i], tq[i]);
+        }
+        nm_unit_grad(p.x, gT, gx);
+        // x = t - d n, d = n . t:  g_t = gx - (gx . n) n,  g_n += -d gx - (gx . n) t
+        const float gxn = dot3(gx, p.n);
+        float gt[4];
+#pragma unroll
+        for (int i = 0; i < 3; ++i) {
+            gt[i] = __fsub_rn(gx[i], __fmul_rn(gxn, p.n[i]));
+            gn[i] = __fsub_rn(__fsub_rn(gn[i], __fmul_rn(p.d, gx[i])), __fmul_rn(gxn, t[i]));
+        }
+        gt[3] = 0.f;
+        if (a.g_tangents) stage_store<4>(a.g_tangents, row0, n, s, lane, gt);
+        if (a.g_normals) {
+            float gnrm[3];
+            nm_unit_grad(nrm, gn, gnrm);
+            stage_store<3>(a.g_normals, row0, n, s, lane, gnrm);
+        }
+    }
+}
+
+inline dim3 normal_map_grid(const NormalMapArgs& a)
+{
+    return dim3((unsigned)light_chunks(a.V), (unsigned)(a.B < (int)MAX_ITEMS_PER_GRID ? a.B : (int)MAX_ITEMS_PER_GRID));
+}
+
+}  // namespace
+
+cudaError_t launch_normal_map_forward(const NormalMapArgs& a, cudaStream_t stream, int* launches)
+{
+    if ((long long)a.B * a.V == 0) return cudaSuccess;
+    normal_map_forward_kernel<<<normal_map_grid(a), LIGHT_THREADS, 0, stream>>>(a);
+    const cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) ++*launches;
+    return e;
+}
+
+cudaError_t launch_normal_map_backward(const NormalMapArgs& a, cudaStream_t stream, int* launches)
+{
+    if ((long long)a.B * a.V == 0 || (!a.g_normals && !a.g_tangents && !a.g_samples)) return cudaSuccess;
+    normal_map_backward_kernel<<<normal_map_grid(a), LIGHT_THREADS, 0, stream>>>(a);
+    const cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) ++*launches;
+    return e;
 }
 
 }  // namespace dirt

@@ -14,6 +14,9 @@
 // than LONG_ROW is summed by the whole warp instead (lane-strided partial sums, then a butterfly), so that a high-valence
 // vertex does not hold up its warp's other 31 lanes.  Either way each sum has one fixed order for given faces, and two
 // calls give bit-identical results.
+//
+// The file also holds the vertex tangents (dirt_tangents_forward / _backward, DESIGN.md §7.14), which use the same
+// adjacency, workspace and per-vertex passes.
 #include <cub/block/block_scan.cuh>
 
 #include "../../include/dirt_b200.h"
@@ -50,6 +53,30 @@ __device__ __forceinline__ float3 cross3(float3 a, float3 b)
     return make_float3(__fsub_rn(__fmul_rn(a.y, b.z), __fmul_rn(a.z, b.y)),
                        __fsub_rn(__fmul_rn(a.z, b.x), __fmul_rn(a.x, b.z)),
                        __fsub_rn(__fmul_rn(a.x, b.y), __fmul_rn(a.y, b.x)));
+}
+
+// Two float3 summed side by side: the (t_f, b_f) of a face, or a corner's position and uv gradients.
+struct Frame {
+    float3 t, b;
+};
+__device__ __forceinline__ Frame add3(Frame a, Frame b) { return Frame{add3(a.t, b.t), add3(a.b, b.b)}; }
+__device__ __forceinline__ float3 zero_of(float3) { return make_float3(0.f, 0.f, 0.f); }
+__device__ __forceinline__ Frame zero_of(Frame) { return Frame{zero_of(float3()), zero_of(float3())}; }
+// one butterfly step: p += p of the lane o away
+__device__ __forceinline__ void add_xor(float3& p, int o)
+{
+    p.x = __fadd_rn(p.x, __shfl_xor_sync(FULL, p.x, o));
+    p.y = __fadd_rn(p.y, __shfl_xor_sync(FULL, p.y, o));
+    p.z = __fadd_rn(p.z, __shfl_xor_sync(FULL, p.z, o));
+}
+__device__ __forceinline__ void add_xor(Frame& p, int o)
+{
+    add_xor(p.t, o);
+    add_xor(p.b, o);
+}
+__device__ __forceinline__ float3 scale3(float3 a, float k)
+{
+    return make_float3(__fmul_rn(a.x, k), __fmul_rn(a.y, k), __fmul_rn(a.z, k));
 }
 
 // x / (|x| + 1e-12)
@@ -170,11 +197,14 @@ __global__ void __launch_bounds__(NORMALS_THREADS) rank_kernel(const int* __rest
 // The sum over the row [lo, hi) of item b of term(b, i) for its incidence ids i.  Rows of up to LONG_ROW ids are summed by
 // their own lane in row order; longer rows by the whole warp, one after another, each lane summing every 32nd id and the
 // warp adding the lanes' sums as a butterfly.  Warp-collective: every lane calls it, inactive ones with an empty row.
+// The terms are float3 (normals) or Frame (tangent frames and their gradients), summed component by component.
 template <class Term>
-__device__ __forceinline__ float3 row_sum(const int* __restrict__ inc, int lo, int hi, long long b, const Term& term)
+__device__ __forceinline__ auto row_sum(const int* __restrict__ inc, int lo, int hi, long long b, const Term& term)
+    -> decltype(term(b, 0))
 {
+    using T = decltype(term(b, 0));
     const int lane = threadIdx.x & 31;
-    float3 s = make_float3(0.f, 0.f, 0.f);
+    T s = zero_of(T());
     const bool long_row = hi - lo > NORMALS_LONG_ROW;
     if (!long_row)
         for (int j = lo; j < hi; ++j) s = add3(s, term(b, __ldg(inc + j)));
@@ -184,14 +214,10 @@ __device__ __forceinline__ float3 row_sum(const int* __restrict__ inc, int lo, i
         pending &= pending - 1;
         const int l = __shfl_sync(FULL, lo, src), h = __shfl_sync(FULL, hi, src);
         const long long bb = __shfl_sync(FULL, b, src);
-        float3 p = make_float3(0.f, 0.f, 0.f);
+        T p = zero_of(T());
         for (int j = l + lane; j < h; j += 32) p = add3(p, term(bb, __ldg(inc + j)));
 #pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            p.x = __fadd_rn(p.x, __shfl_xor_sync(FULL, p.x, o));
-            p.y = __fadd_rn(p.y, __shfl_xor_sync(FULL, p.y, o));
-            p.z = __fadd_rn(p.z, __shfl_xor_sync(FULL, p.z, o));
-        }
+        for (int o = 16; o > 0; o >>= 1) add_xor(p, o);
         if (lane == src) s = p;
     }
     return s;
@@ -301,6 +327,177 @@ inline unsigned blocks_for(long long n)
     return (unsigned)(b < 1 ? 1 : (b < MAX_BLOCKS ? b : MAX_BLOCKS));
 }
 
+// ---- the vertex tangents (DESIGN.md §7.14) ------------------------------------------------------------------------------
+//
+// Face f with corners p0, p1, p2 and uvs (u_k, v_k): e1 = p1 - p0, e2 = p2 - p0, (du_k, dv_k) = uv_k - uv0,
+// s = sign(du1 dv2 - du2 dv1), t_f = unit(s (e1 dv2 - e2 dv1)), b_f = unit(s (e2 du1 - e1 du2)).  The vertex passes sum
+// t_f (and b_f) over the rows of the normals' adjacency, recomputing each face as the normals' passes do.
+
+// A face's edges, its uv differences and the sign of its uv area.
+struct UvFace {
+    Corners c;
+    float du1, dv1, du2, dv2, s;
+};
+
+__device__ __forceinline__ const float* uv_row(const TangentArgs& a, long long b, int v)
+{
+    return a.uvs + b * a.uv_item_stride + v * a.uv_stride;
+}
+
+__device__ __forceinline__ UvFace uv_face(const TangentArgs& a, long long b, int f)
+{
+    UvFace u;
+    u.c = corners(a.m, b, f);
+    const float* q0 = uv_row(a, b, u.c.v[0]);
+    const float* q1 = uv_row(a, b, u.c.v[1]);
+    const float* q2 = uv_row(a, b, u.c.v[2]);
+    const float u0 = __ldg(q0), v0 = __ldg(q0 + 1);
+    u.du1 = __fsub_rn(__ldg(q1), u0);
+    u.dv1 = __fsub_rn(__ldg(q1 + 1), v0);
+    u.du2 = __fsub_rn(__ldg(q2), u0);
+    u.dv2 = __fsub_rn(__ldg(q2 + 1), v0);
+    const float r = __fsub_rn(__fmul_rn(u.du1, u.dv2), __fmul_rn(u.du2, u.dv1));
+    u.s = r > 0.f ? 1.f : (r < 0.f ? -1.f : 0.f);
+    return u;
+}
+
+// s (e1 dv2 - e2 dv1): the face's unnormalised dp/du direction
+__device__ __forceinline__ float3 face_u(const UvFace& u)
+{
+    const float3 e1 = u.c.e1, e2 = u.c.e2;
+    return make_float3(__fmul_rn(u.s, __fsub_rn(__fmul_rn(e1.x, u.dv2), __fmul_rn(e2.x, u.dv1))),
+                       __fmul_rn(u.s, __fsub_rn(__fmul_rn(e1.y, u.dv2), __fmul_rn(e2.y, u.dv1))),
+                       __fmul_rn(u.s, __fsub_rn(__fmul_rn(e1.z, u.dv2), __fmul_rn(e2.z, u.dv1))));
+}
+
+// (t_f, b_f) of the face of incidence i
+struct FaceFrame {
+    const TangentArgs& a;
+    __device__ __forceinline__ Frame operator()(long long b, int i) const
+    {
+        const UvFace u = uv_face(a, b, i % a.m.F);
+        const float3 e1 = u.c.e1, e2 = u.c.e2;
+        const float3 y = make_float3(__fmul_rn(u.s, __fsub_rn(__fmul_rn(e2.x, u.du1), __fmul_rn(e1.x, u.du2))),
+                                     __fmul_rn(u.s, __fsub_rn(__fmul_rn(e2.y, u.du1), __fmul_rn(e1.y, u.du2))),
+                                     __fmul_rn(u.s, __fsub_rn(__fmul_rn(e2.z, u.du1), __fmul_rn(e1.z, u.du2))));
+        return Frame{normalise(face_u(u)), normalise(y)};
+    }
+};
+
+// t_f alone (the backward's vertex pass)
+struct FaceTangent {
+    const TangentArgs& a;
+    __device__ __forceinline__ float3 operator()(long long b, int i) const
+    {
+        return normalise(face_u(uv_face(a, b, i % a.m.F)));
+    }
+};
+
+// The gradients of corner k of the face of incidence i = k*F + f: to its position (t) and to its v coordinate (b.y;
+// b.x and b.z stay 0, as du reaches t_f only through the sign).  g_t of the face is the sum over its corners of the
+// gradient of the vertex they feed.
+struct TangentCornerGrad {
+    const TangentArgs& a;
+    __device__ __forceinline__ Frame operator()(long long b, int i) const
+    {
+        const int k = i / a.m.F, f = i - k * a.m.F;
+        const UvFace u = uv_face(a, b, f);
+        float3 gt = make_float3(0.f, 0.f, 0.f);
+#pragma unroll
+        for (int j = 0; j < 3; ++j) gt = add3(gt, ld3(a.gt + 3 * (b * a.m.V + u.c.v[j])));
+        const float3 gy = scale3(normalise_grad(face_u(u), gt), u.s);   // to e1 dv2 - e2 dv1
+        const float3 g1 = scale3(gy, u.dv2), g2 = scale3(gy, -u.dv1);   // d/d e1, d/d e2
+        const float gdv2 = dot3(gy, u.c.e1), gdv1 = -dot3(gy, u.c.e2);
+        Frame g = zero_of(Frame());
+        if (k == 1) {
+            g.t = g1;
+            g.b.y = gdv1;
+        } else if (k == 2) {
+            g.t = g2;
+            g.b.y = gdv2;
+        } else {
+            g.t = make_float3(-__fadd_rn(g1.x, g2.x), -__fadd_rn(g1.y, g2.y), -__fadd_rn(g1.z, g2.z));
+            g.b.y = -__fadd_rn(gdv1, gdv2);
+        }
+        return g;
+    }
+};
+
+// A row with no incidences (F = 0: there is no adjacency to read)
+__device__ __forceinline__ Row tangent_row(const TangentArgs& a, long long t0)
+{
+    if (a.m.F) return row_of(a.m, t0);
+    Row r;
+    r.t = t0 + (threadIdx.x & 31);
+    r.active = r.t < a.m.total;
+    r.b = 0;
+    r.lo = r.hi = 0;
+    return r;
+}
+
+// n = unit(normal), x = t - (n . t) n: the vector T normalises
+struct Gram {
+    float3 n, x;
+    float d;
+};
+
+__device__ __forceinline__ Gram gram(const TangentArgs& a, const Row& r, float3 t)
+{
+    Gram g;
+    g.n = r.active ? normalise(ld3(a.normals + r.t * a.normal_stride)) : make_float3(0.f, 0.f, 0.f);
+    g.d = dot3(g.n, t);
+    g.x = sub3(t, scale3(g.n, g.d));
+    return g;
+}
+
+__global__ void __launch_bounds__(NORMALS_THREADS) tangents_forward_kernel(TangentArgs a)
+{
+    FOR_EACH_ROW(a.m) {
+        const Row r = tangent_row(a, t0);
+        const Frame s = row_sum(a.m.inc, r.lo, r.hi, r.b, FaceFrame{a});
+        const Gram g = gram(a, r, s.t);
+        const float3 T = normalise(g.x);
+        const float w = dot3(cross3(g.n, T), s.b) < 0.f ? -1.f : 1.f;
+        if (r.active) {
+            st3(a.out + 4 * r.t, T);
+            a.out[4 * r.t + 3] = w;
+        }
+    }
+}
+
+// gt = the gradient of the vertex's sum of face tangents; grad_normals, which is local to the vertex
+__global__ void __launch_bounds__(NORMALS_THREADS) tangents_vertex_grad_kernel(TangentArgs a)
+{
+    FOR_EACH_ROW(a.m) {
+        const Row r = tangent_row(a, t0);
+        const float3 t = row_sum(a.m.inc, r.lo, r.hi, r.b, FaceTangent{a});
+        if (!r.active) continue;
+        const Gram g = gram(a, r, t);
+        const float3 gx = normalise_grad(g.x, ld3(a.grad + 4 * r.t));
+        const float gxn = dot3(gx, g.n);
+        // x = t - d n, d = n . t:  g_t = gx - (gx . n) n,  g_n = -d gx - (gx . n) t
+        if (a.gt) st3(a.gt + 3 * r.t, sub3(gx, scale3(g.n, gxn)));
+        if (a.g_normals) {
+            const float3 gn = sub3(scale3(gx, -g.d), scale3(t, gxn));
+            st3(a.g_normals + 3 * r.t, normalise_grad(ld3(a.normals + r.t * a.normal_stride), gn));
+        }
+    }
+}
+
+__global__ void __launch_bounds__(NORMALS_THREADS) tangents_corner_grad_kernel(TangentArgs a)
+{
+    FOR_EACH_ROW(a.m) {
+        const Row r = tangent_row(a, t0);
+        const Frame g = row_sum(a.m.inc, r.lo, r.hi, r.b, TangentCornerGrad{a});
+        if (!r.active) continue;
+        if (a.g_vertices) st3(a.g_vertices + 3 * r.t, g.t);
+        if (a.g_uvs) {
+            a.g_uvs[2 * r.t] = 0.f;
+            a.g_uvs[2 * r.t + 1] = g.b.y;
+        }
+    }
+}
+
 }  // namespace
 
 NormalsWorkspace carve_normals_workspace(void* base, int B, long long V, long long F)
@@ -383,6 +580,50 @@ cudaError_t launch_normals_backward(NormalsArgs a, const NormalsWorkspace& w, cu
     }
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     ++*launches;
+    return cudaSuccess;
+}
+
+cudaError_t launch_tangents_forward(TangentArgs a, const NormalsWorkspace& w, cudaStream_t stream, int* launches)
+{
+    cudaError_t e;
+    if (a.m.total == 0) return cudaSuccess;
+    if (a.m.F > 0 &&
+        (e = launch_corner_adjacency(a.m.faces, 0, 1, a.m.V, a.m.F, w.counts, w.offsets, w.unsorted, w.inc, stream,
+                                     launches)) != cudaSuccess)
+        return e;
+    a.m.offsets = w.offsets;
+    a.m.inc = w.inc;
+    tangents_forward_kernel<<<blocks_for(a.m.total), NORMALS_THREADS, 0, stream>>>(a);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    ++*launches;
+    return cudaSuccess;
+}
+
+cudaError_t launch_tangents_backward(TangentArgs a, const NormalsWorkspace& w, cudaStream_t stream, int* launches)
+{
+    cudaError_t e;
+    if (a.m.total == 0) return cudaSuccess;
+    const size_t rows = (size_t)a.m.total;
+    if (a.m.F == 0) {
+        // every row is empty: T = 0 whatever the inputs, so no gradient reaches anything
+        if (a.g_vertices && (e = cudaMemsetAsync(a.g_vertices, 0, sizeof(float) * 3 * rows, stream)) != cudaSuccess) return e;
+        if (a.g_uvs && (e = cudaMemsetAsync(a.g_uvs, 0, sizeof(float) * 2 * rows, stream)) != cudaSuccess) return e;
+        if (a.g_normals && (e = cudaMemsetAsync(a.g_normals, 0, sizeof(float) * 3 * rows, stream)) != cudaSuccess) return e;
+        return cudaSuccess;
+    }
+    const bool corner = a.g_vertices || a.g_uvs;
+    if (!corner && !a.g_normals) return cudaSuccess;
+    a.m.offsets = w.offsets;
+    a.m.inc = w.inc;
+    a.gt = corner ? w.gs : nullptr;
+    tangents_vertex_grad_kernel<<<blocks_for(a.m.total), NORMALS_THREADS, 0, stream>>>(a);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    ++*launches;
+    if (corner) {
+        tangents_corner_grad_kernel<<<blocks_for(a.m.total), NORMALS_THREADS, 0, stream>>>(a);
+        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+        ++*launches;
+    }
     return cudaSuccess;
 }
 

@@ -11,6 +11,9 @@ routed the same way, between dirt_sh_lighting_forward / _backward and `_diffuse_
 dirt_ggx_lighting_forward / _backward and `_specular_ggx`; see DESIGN.md §7.9.  `ggx_environment_brdf` and
 `specular_ggx_environment` (split-sum GGX environment lighting, DESIGN.md §7.12) are torch code around a CUDA table and
 the CUDA cube-map lookup; `cubemap_spherical_harmonics` projects a cube map onto order-2 SH with CUDA kernels.  `split_vertices_by_face` is torch code.
+`vertex_tangents` and `perturb_normals` (tangent-space normal mapping, DESIGN.md §7.14) run CUDA kernels
+(dirt_tangents_* and dirt_normal_map_*) in the shapes `tangents_route` and `cuda_route` accept, and their torch
+restatements (`_vertex_tangents`, `_perturb_normals`) otherwise.
 """
 import math
 from collections import namedtuple
@@ -803,3 +806,233 @@ def _normals(mode, route, vertices, faces):
         rows = rows.contiguous()
     out = _Normals.apply(mode, route, rows, faces)
     return out.reshape(route.lead + (route.V, 3))
+
+
+# ---- tangent-space normal mapping (DESIGN.md §7.14) -------------------------------------------------------------------
+
+def _vertex_tangents(vertices, uvs, faces, vertex_normals):
+    """The torch restatement of `vertex_tangents`: its CPU implementation and its specification.  Keeps the dtype of its
+    inputs (the tests evaluate it in float64)."""
+    vertices, faces = _prepare(vertices, faces)
+    p = vertices[..., :3]
+    uvs = uvs if isinstance(uvs, torch.Tensor) else torch.as_tensor(uvs, dtype=p.dtype, device=p.device)
+    n = vertex_normals if isinstance(vertex_normals, torch.Tensor) else torch.as_tensor(vertex_normals, dtype=p.dtype,
+                                                                                        device=p.device)
+    corners, tex = p[..., faces, :], uvs[..., faces, :]   # [*, F, 3, 3], [*, F, 3, 2]
+    e1, e2 = corners[..., 1, :] - corners[..., 0, :], corners[..., 2, :] - corners[..., 0, :]
+    d1, d2 = tex[..., 1, :] - tex[..., 0, :], tex[..., 2, :] - tex[..., 0, :]
+    du1, dv1, du2, dv2 = d1[..., :1], d1[..., 1:], d2[..., :1], d2[..., 1:]
+    s = torch.sign(du1 * dv2 - du2 * dv1)
+    t_f = _unit(s * (e1 * dv2 - e2 * dv1))   # the unit dp/du direction of each face
+    b_f = _unit(s * (e2 * du1 - e1 * du2))   # the unit dp/dv direction
+    t_v = b_v = torch.zeros(t_f.shape[:-2] + p.shape[-2:], dtype=t_f.dtype, device=t_f.device)
+    for corner in range(3):
+        t_v = t_v.index_add(-2, faces[:, corner], t_f)
+    for corner in range(3):
+        b_v = b_v.index_add(-2, faces[:, corner], b_f)
+    n = _unit(n)
+    T = _unit(t_v - (n * t_v).sum(-1, keepdim=True) * n)
+    w = 1. - 2. * ((torch.linalg.cross(n, T, dim=-1) * b_v).sum(-1, keepdim=True) < 0).to(T.dtype)
+    return torch.cat([T, w], -1)
+
+
+def _perturb_normals(normals, tangents, tangent_space_normals):
+    """The torch restatement of `perturb_normals`: its CPU implementation and its specification.  Keeps the dtype of its
+    inputs (the tests evaluate it in float64)."""
+    n = _unit(normals)
+    t = tangents[..., :3]
+    T = _unit(t - (n * t).sum(-1, keepdim=True) * n)
+    s = 1. - 2. * (tangents[..., 3:] < 0).to(T.dtype)
+    m = tangent_space_normals
+    return _unit(m[..., :1] * T + m[..., 1:2] * (s * torch.linalg.cross(n, T, dim=-1)) + m[..., 2:] * n)
+
+
+TangentsRoute = namedtuple('TangentsRoute', 'lead B V F uv_per_item')
+
+
+def tangents_route(vertex, uv, normal, face_shape, face_dtype):
+    """Whether a `vertex_tangents` call runs the CUDA kernels, decided from shapes, dtypes and devices alone.  vertex,
+    uv and normal are (shape, dtype, device) of the vertices, uvs and vertex normals.  The vertices and faces must be
+    as `normals_route` accepts them; the uvs float32 [V, 2] (shared) or [*, V, 2] and the normals float32 [*, V, 3],
+    both on the vertices' device.  Returns a TangentsRoute (lead = `*`, B, V, F, uv_per_item) or None."""
+    r = normals_route(vertex[0], vertex[1], vertex[2], face_shape, face_dtype)
+    if r is None:
+        return None
+    for shape, dtype, device in (uv, normal):
+        if dtype != torch.float32 or device != vertex[2]:
+            return None
+    if tuple(normal[0]) != r.lead + (r.V, 3):
+        return None
+    if tuple(uv[0]) == (r.V, 2):
+        per_item = False
+    elif tuple(uv[0]) == r.lead + (r.V, 2):
+        per_item = True
+    else:
+        return None
+    return TangentsRoute(r.lead, r.B, r.V, r.F, per_item)
+
+
+def _tangents_route(vertices, uvs, vertex_normals, faces):
+    if not all(isinstance(t, torch.Tensor) for t in (vertices, uvs, vertex_normals)):
+        return None
+    faces = faces if isinstance(faces, torch.Tensor) else torch.as_tensor(faces)
+    meta = lambda t: (t.shape, t.dtype, t.device)
+    return tangents_route(meta(vertices), meta(uvs), meta(vertex_normals), faces.shape, faces.dtype)
+
+
+def _point_rows(t, k):
+    """`_rows`, with a row stride of at least k (the C ABI's requirement for these rows)."""
+    r = _rows(t, k)
+    return r.contiguous() if r.shape[0] > 1 and r.stride(0) < k else r
+
+
+def _stride(rows, k):
+    return rows.stride(0) if rows.shape[0] > 1 else k
+
+
+class _Tangents(torch.autograd.Function):
+    """dirt_tangents_forward with its gradient.  rows, normals: [B*V, 3]; uvs: [B*V, 2] (per item) or [V, 2] (shared), all
+    with unit stride along the row; faces: int32 [F, 3] on their device.  The node keeps its inputs and the forward's
+    workspace, whose adjacency the backward kernels read."""
+
+    @staticmethod
+    def forward(ctx, route, rows, uvs, normals, faces):
+        dev = rows.device
+        lib = _lib.lib()
+        out = torch.empty((route.B * route.V, 4), dtype=torch.float32, device=dev)
+        ws_bytes = int(lib.dirt_tangents_workspace_bytes(route.B, route.V, route.F))
+        workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=dev) if ws_bytes else None
+        with torch.cuda.device(dev):
+            rc = lib.dirt_tangents_forward(*_tangent_inputs(route, rows, uvs, normals, faces), _ptr(out), _ptr(workspace),
+                                           ws_bytes, route.B, route.V, route.F, _stream(dev))
+        _lib.check(rc, 'VertexTangents')
+        ctx.save_for_backward(rows, uvs, normals, faces)
+        ctx.route, ctx.workspace, ctx.ws_bytes = route, workspace, ws_bytes
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        want = ctx.needs_input_grad[1:4]
+        if not any(want):
+            return (None,) * 5
+        rows, uvs, normals, faces = ctx.saved_tensors
+        route = ctx.route
+        inputs = (rows, uvs, normals)
+        if torch.is_grad_enabled():
+            # create_graph=True: differentiable gradients through the restatement, on the faces the kernels used
+            valid = faces[((faces >= 0) & (faces < route.V)).all(1)]
+            lead, V = route.lead, route.V
+            out = _vertex_tangents(rows.reshape(lead + (V, 3)), uvs.reshape(lead + (V, 2)) if route.uv_per_item else uvs,
+                                   valid, normals.reshape(lead + (V, 3)))
+            wanted = [t for t, w in zip(inputs, want) if w]
+            grads = iter(torch.autograd.grad(out, wanted, grad_out.reshape(out.shape), create_graph=True))
+            return (None,) + tuple(next(grads) if w else None for w in want) + (None,)
+        dev = rows.device
+        n = route.B * route.V
+        grads = [torch.empty((n, k), dtype=torch.float32, device=dev) if w else None for k, w in zip((3, 2, 3), want)]
+        grad_out = grad_out.to(torch.float32).contiguous()
+        lib = _lib.lib()
+        with torch.cuda.device(dev):
+            rc = lib.dirt_tangents_backward(*_tangent_inputs(route, rows, uvs, normals, faces), _ptr(grad_out),
+                                            *[_ptr(g) for g in grads], _ptr(ctx.workspace), ctx.ws_bytes, route.B,
+                                            route.V, route.F, _stream(dev))
+        _lib.check(rc, 'VertexTangentsGrad')
+        if grads[1] is not None and not route.uv_per_item:
+            grads[1] = grads[1].reshape(route.B, route.V, 2).sum(0)   # shared uvs: one fixed-order sum over the items
+        return (None,) + tuple(grads) + (None,)
+
+
+def _tangent_inputs(route, rows, uvs, normals, faces):
+    """The input arguments of dirt_tangents_forward / _backward, in their order."""
+    uv_stride = _stride(uvs, 2)
+    return [_ptr(rows), _stride(rows, 3), _ptr(uvs), uv_stride, route.V * uv_stride if route.uv_per_item else 0,
+            _ptr(normals), _stride(normals, 3), _ptr(faces)]
+
+
+def vertex_tangents(vertices, uvs, faces, vertex_normals, name=None):
+    """Per-vertex tangent frames for tangent-space normal mapping.
+
+    vertices [*, V, 3|4] (a w column is ignored), uvs [V, 2] (shared by the batch) or [*, V, 2], faces [F, 3] int32 or
+    int64, vertex_normals [*, V, 3] (for example `vertex_normals(vertices, faces)`) -> [*, V, 4]: a unit tangent T
+    orthogonal to the vertex normal, along the sum over the vertex's face corners of each face's unit dp/du direction,
+    and a handedness w = +-1, so that the bitangent w (n x T) points along +v.  Faces with degenerate uvs add nothing,
+    a vertex no face names gets (0, 0, 0, 1), and mirrored uvs give w = -1.  Gradients reach the positions, the v
+    coordinates of the uvs (u enters only through the sign of the uv area) and the normals; none passes through w.
+    On CUDA in the shapes `tangents_route` accepts, deterministic kernels compute it (a face with an index outside
+    [0, V) is then left out); any other call runs the torch restatement `_vertex_tangents` (DESIGN.md §7.14)."""
+    route = _tangents_route(vertices, uvs, vertex_normals, faces)
+    if route is None:
+        return _vertex_tangents(vertices, uvs, faces, vertex_normals)
+    faces = torch.as_tensor(faces).to(device=vertices.device)
+    if faces.dtype == torch.int64:
+        faces = faces.clamp(-1, (1 << 31) - 1)   # above int32: >= V, so left out like any other invalid index
+    faces = faces.to(torch.int32).contiguous()
+    out = _Tangents.apply(route, _point_rows(vertices[..., :3], 3), _point_rows(uvs, 2),
+                          _point_rows(vertex_normals, 3), faces)
+    return out.reshape(route.lead + (route.V, 4))
+
+
+class _NormalMap(torch.autograd.Function):
+    """dirt_normal_map_forward with its gradient.  normals [rows, 3], tangents [rows, 4] and samples [rows, 3] with unit
+    stride along the row.  The node keeps only its inputs: the backward kernel recomputes the forward from them."""
+
+    @staticmethod
+    def forward(ctx, route, normals, tangents, samples):
+        out = torch.empty(route.lead + (route.V, 3), dtype=torch.float32, device=normals.device)
+        with torch.cuda.device(normals.device):
+            rc = _lib.lib().dirt_normal_map_forward(*_normal_map_inputs(normals, tangents, samples), _ptr(out), route.B,
+                                                    route.V, _stream(normals.device))
+        _lib.check(rc, 'PerturbNormals')
+        ctx.save_for_backward(normals, tangents, samples)
+        ctx.route = route
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        want = ctx.needs_input_grad[1:]
+        if not any(want):
+            return (None,) * 4
+        inputs = ctx.saved_tensors
+        route = ctx.route
+        if torch.is_grad_enabled():
+            # create_graph=True: differentiable gradients through the restatement
+            lead, V = route.lead, route.V
+            out = _perturb_normals(*[t.reshape(lead + (V, t.shape[-1])) for t in inputs])
+            wanted = [t for t, w in zip(inputs, want) if w]
+            grads = iter(torch.autograd.grad(out, wanted, grad_out, create_graph=True))
+            return (None,) + tuple(next(grads) if w else None for w in want)
+        dev = inputs[0].device
+        grads = [torch.empty((t.shape[0], t.shape[1]), dtype=torch.float32, device=dev) if w else None
+                 for t, w in zip(inputs, want)]
+        grad_out = grad_out.to(torch.float32).contiguous()
+        with torch.cuda.device(dev):
+            rc = _lib.lib().dirt_normal_map_backward(*_normal_map_inputs(*inputs), _ptr(grad_out),
+                                                     *[_ptr(g) for g in grads], route.B, route.V, _stream(dev))
+        _lib.check(rc, 'PerturbNormalsGrad')
+        return (None,) + tuple(grads)
+
+
+def _normal_map_inputs(normals, tangents, samples):
+    """The input arguments of dirt_normal_map_forward / _backward, in their order."""
+    stride = lambda t: t.stride(0) if t.shape[0] > 1 else 0
+    return [_ptr(normals), stride(normals), _ptr(tangents), stride(tangents), _ptr(samples), stride(samples)]
+
+
+def perturb_normals(normals, tangents, tangent_space_normals, name=None):
+    """Tangent-space normal mapping: the normals rotated by a normal map's samples in the frame (n, T, s (n x T)).
+
+    normals [*, N, 3] (interpolated, so not unit length), tangents [*, N, 4] (the interpolated output of
+    `vertex_tangents`), tangent_space_normals [*, N, 3] (already decoded to [-1, 1], e.g. 2 * sample_texture(...) - 1;
+    the decoding and the green-channel convention are the caller's) -> [*, N, 3]:
+    unit(m.x T + m.y s (n x T) + m.z n) with n = unit(normals), T = unit(t - (n . t) n), s = -1 if t.w < 0 else +1.
+    A point with a zero normal (a background pixel) gives 0.  Gradients reach the normals, the tangents' xyz and the
+    samples.  On CUDA in these shapes a fused kernel computes it, reading G-buffer channel slices in place; any other
+    call runs the torch restatement `_perturb_normals` (DESIGN.md §7.14)."""
+    normals = torch.as_tensor(normals, dtype=torch.float32)
+    dev = normals.device
+    tangents = torch.as_tensor(tangents, dtype=torch.float32, device=dev)
+    tangent_space_normals = torch.as_tensor(tangent_space_normals, dtype=torch.float32, device=dev)
+    route = _route([normals, tangents, tangent_space_normals], [], [3, 4, 3])
+    if route is None:
+        return _perturb_normals(normals, tangents, tangent_space_normals)
+    return _NormalMap.apply(route, _rows(normals, 3), _rows(tangents, 4), _rows(tangent_space_normals, 3))

@@ -578,6 +578,57 @@ int dirt_normals_backward(int mode, const float* vertices, long long vertex_stri
                           const float* grad_normals, float* grad_vertices, void* workspace, size_t workspace_bytes,
                           int B, long long V, long long F, void* cuda_stream);
 
+/* Vertex tangents for tangent-space normal mapping, for B items of V vertices sharing the faces:
+ *   vertices             float32 [B*V, 3], row stride vertex_stride >= 3 floats, unit stride along the row
+ *   uvs                  float32, the uv of vertex v of item b at uvs + b*uv_item_stride + v*uv_stride, uv_stride >= 2,
+ *                        unit stride along the row (uv_item_stride 0: one set shared by the batch)
+ *   normals              float32 [B*V, 3], row stride normals_stride >= 3, e.g. the output of dirt_normals_forward
+ *   faces                int32 [F, 3], shared by the batch
+ *   tangents, grad_tangents   float32 [B*V, 4], contiguous
+ * With unit(x) = x / (|x| + 1e-12) and, for face f with corners p0, p1, p2 and uvs (u_k, v_k),
+ * e1 = p1 - p0, e2 = p2 - p0, (du_k, dv_k) = uv_k - uv0, s = sign(du1 dv2 - du2 dv1) (0 when it is 0):
+ *   t_f = unit(s (e1 dv2 - e2 dv1)),  b_f = unit(s (e2 du1 - e1 du2)),
+ *   t_v, b_v = the sums of t_f, b_f over every corner of every face that is v,  n = unit(normal_v),
+ *   tangent_v = (T, w),  T = unit(t_v - (n . t_v) n),  w = -1 if (n x T) . b_v < 0 else +1.
+ * A face with degenerate uvs adds nothing; a vertex no face names gets (0, 0, 0, 1).  A face with an index outside
+ * [0, V) is left out.
+ * Backward: the gradients torch autograd gives the same expressions.  None passes through w or the sign, so du gets 0;
+ * the w column of grad_tangents is ignored.  grad_vertices [B*V, 3], grad_uvs [B*V, 2] (one row per item and vertex,
+ * also for shared uvs: the caller sums them over the items) and grad_normals [B*V, 3] are contiguous; each may be NULL,
+ * and its work is skipped.
+ * Workspace: dirt_tangents_workspace_bytes(B, V, F) bytes, the layout of dirt_normals_workspace_bytes.  The forward
+ * call writes the vertex -> face-corner adjacency into it and the backward call reads it there, as for the normals.
+ * Every sum has one fixed order (no float atomics): repeated calls give bit-identical tangents and gradients.
+ * B = 0 or V = 0: nothing is launched; F = 0: every vertex gets (0, 0, 0, 1) and the gradients are zeroed.
+ * V < 2^31, 3F < 2^31; all pointers 4-byte aligned. */
+size_t dirt_tangents_workspace_bytes(int B, long long V, long long F);
+int dirt_tangents_forward(const float* vertices, long long vertex_stride, const float* uvs, long long uv_stride,
+                          long long uv_item_stride, const float* normals, long long normals_stride, const int32_t* faces,
+                          float* tangents, void* workspace, size_t workspace_bytes,
+                          int B, long long V, long long F, void* cuda_stream);
+int dirt_tangents_backward(const float* vertices, long long vertex_stride, const float* uvs, long long uv_stride,
+                           long long uv_item_stride, const float* normals, long long normals_stride, const int32_t* faces,
+                           const float* grad_tangents, float* grad_vertices, float* grad_uvs, float* grad_normals,
+                           void* workspace, size_t workspace_bytes, int B, long long V, long long F, void* cuda_stream);
+
+/* Tangent-space normal mapping, one value per point.  B items of V points each:
+ *   normals              float32 [B*V, 3], row stride normals_stride (interpolated: not unit length)
+ *   tangents             float32 [B*V, 4], row stride tangents_stride (interpolated dirt_tangents_forward output)
+ *   samples              float32 [B*V, 3], row stride samples_stride: the tangent-space normal, decoded to [-1, 1]
+ *   out, grad_out        float32 [B*V, 3], contiguous
+ * With unit(x) = x / (|x| + 1e-12), n = unit(normal), T = unit(t.xyz - (n . t.xyz) n), s = -1 if t.w < 0 else +1:
+ *   out = unit(m.x T + m.y s (n x T) + m.z n);  a point with n = 0 gives 0.
+ * Backward: the gradients torch autograd gives the same expressions.  grad_normals [B*V, 3], grad_tangents [B*V, 4]
+ * (its w column 0) and grad_samples [B*V, 3] are contiguous; each may be NULL, and its work is skipped.
+ * B = 0 or V = 0: nothing is launched.  All pointers 4-byte aligned; row strides >= 0. */
+int dirt_normal_map_forward(const float* normals, long long normals_stride, const float* tangents,
+                            long long tangents_stride, const float* samples, long long samples_stride,
+                            float* out, int B, long long V, void* cuda_stream);
+int dirt_normal_map_backward(const float* normals, long long normals_stride, const float* tangents,
+                             long long tangents_stride, const float* samples, long long samples_stride,
+                             const float* grad_out, float* grad_normals, float* grad_tangents, float* grad_samples,
+                             int B, long long V, void* cuda_stream);
+
 /* Number of kernels the last call on this thread launched (bench.py's gpu_launches). */
 int dirt_last_launch_count(void);
 
