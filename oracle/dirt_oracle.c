@@ -534,10 +534,12 @@ static inline float scharr_comp(float nn, float np, float pn, float pp, float mn
 static void backward_image_group(const float* verts, const Tri* tris, const int32_t* ids_rows, int rb,
                                  const float* pixels, const float* grad_pixels,
                                  double* gverts /*[V,4]*/, int b, int B, int H, int W, int C, int c0, int n, int r0, int r1,
-                                 uint8_t* dilated /*[B,H,W] of this group, or NULL*/)
+                                 uint8_t* codes /*[B,H,W] of this group, or NULL*/)
 {
     /* rows [r0, r1) of the image; ids_rows holds the visibility buffer from row rb on (rb <= r0 - 1 unless r0 == 0).
-     * `dilated` marks the pixels that take a neighbour's face (the reference's debug_thingy[..., 0] = 1e-2, :172) */
+     * `codes` receives the dilation code of every pixel (include/dirt_b200.h, dirt_rasterise_backward_deterministic):
+     * bits 0-1  0: no position term, 1: the own face takes it, 2 / 3: the neighbour of the first / second attempt does
+     * (the reference's debug_thingy[..., 0] = 1e-2, :172); bit 2: the preferred step runs along the row (interior pixels) */
 #define IDS(r_, c_) ids_rows[((r_) - rb) * W + (c_)]
     for (int r = r0; r < r1; ++r)
         for (int c = 0; c < W; ++c) {
@@ -561,10 +563,12 @@ static void backward_image_group(const float* verts, const Tri* tris, const int3
             if (f >= 0) tri_gbuffer(&tris[f], c, r, g);
 
             /* dilation (:155-194), interior pixels only */
+            int code = 1;
             if (c > 0 && r > 0 && c < W - 1 && r < H - 1) {
                 float l1x = (fabsf(sx[0]) + fabsf(sx[1])) + fabsf(sx[2]);
                 float l1y = (fabsf(sy[0]) + fabsf(sy[1])) + fabsf(sy[2]);
                 int dx = (l1x > l1y) ? 1 : 0, dy = (l1x > l1y) ? 0 : 1; /* buffer (GL, y-up) orientation */
+                if (dx) code |= 4;
                 if ((c + r) % 2 == 1) { dx = -dx; dy = -dy; }
                 for (int attempt = 0; attempt < 2; ++attempt) {
                     int nc = c + dx, nr = r - dy; /* buffer_y + dy is image row r - dy */
@@ -578,7 +582,7 @@ static void backward_image_group(const float* verts, const Tri* tris, const int3
                         if (differs && g[3] > gn[3]) {
                             g[0] = gn[0]; g[1] = gn[1]; g[2] = gn[2]; g[3] = gn[3];
                             f = fn;
-                            if (dilated) dilated[((size_t)b * H + r) * W + c] = 1;
+                            code += 1 + attempt;
                             break;
                         }
                     }
@@ -586,6 +590,7 @@ static void backward_image_group(const float* verts, const Tri* tris, const int3
                 }
             }
 
+            if (codes) codes[((size_t)b * H + r) * W + c] = (uint8_t)(f >= 0 ? code : 0);
             if (f >= 0) { /* position gradients (:196-232) */
                 const Tri* t = &tris[f];
                 size_t pix = ((size_t)b * H + r) * W + c;
@@ -614,12 +619,12 @@ static void backward_image_group(const float* verts, const Tri* tris, const int3
 #undef IDS
 }
 
-/* dirt_oracle_backward with the dilation decisions: `dilated` (NULL, or zeroed uint8 [n_groups, B, H, W] with one
- * plane per channel group in call order) gets 1 where a pixel takes a neighbour's face */
+/* dirt_oracle_backward with the dilation decisions: `codes` (NULL, or uint8 [n_groups, B, H, W] with one plane per
+ * channel group in call order) gets every pixel's dilation code (backward_image_group) */
 int dirt_oracle_backward_ex(const float* vertices, const int32_t* faces, const float* pixels,
                             const float* grad_pixels, float* grad_background, float* grad_vertices,
                             float* grad_vertex_colors, int B, int H, int W, int C, int V, int F,
-                            const int* channel_groups, int n_groups, uint8_t* dilated)
+                            const int* channel_groups, int n_groups, uint8_t* codes)
 {
     if (B < 0 || H <= 0 || W <= 0 || C <= 0 || V < 0 || F < 0) return -1;
     int* groups = (int*)malloc(sizeof(int) * (size_t)(C + 1));
@@ -681,7 +686,7 @@ int dirt_oracle_backward_ex(const float* vertices, const int32_t* faces, const f
         int c0 = 0;
         for (int gi = 0; gi < ng; ++gi) {
             backward_image_group(verts, tris, ids, rb, pixels, grad_pixels, gv, b, B, H, W, C, c0, groups[gi], r0, r1,
-                                 dilated ? dilated + (size_t)gi * B * H * W : NULL);
+                                 codes ? codes + (size_t)gi * B * H * W : NULL);
             c0 += groups[gi];
         }
         free(ids); free(keys);

@@ -110,7 +110,9 @@ def backward(vertices, faces, pixels, grad_pixels, channel_groups=None, return_d
     """RasteriseGrad: -> grad_background [B,H,W,C], grad_vertices [B,V,4], grad_vertex_colors [B,V,C].
     With return_dilation, also a list with one bool [B,H,W] mask per channel group (the given groups, or the greedy
     split): the pixels whose position gradient goes to a neighbour's face, as oracle/ref.py backward returns them from
-    the reference kernel."""
+    the reference kernel.  With return_dilation='codes' the list holds uint8 [B,H,W] planes of the full dilation codes
+    instead, as dirt_rasterise_backward_deterministic leaves them in its scratch (include/dirt_b200.h): bits 0-1 none /
+    own face / first / second neighbour, bit 2 the step along the row; the mask is (code & 3) >= 2."""
     vertices, faces = _f32(vertices), _i32(faces)
     pixels, grad_pixels = _f32(pixels), _f32(grad_pixels)
     B, H, W, C = pixels.shape
@@ -125,13 +127,15 @@ def backward(vertices, faces, pixels, grad_pixels, channel_groups=None, return_d
         arr = (ctypes.c_int * len(channel_groups))(*channel_groups)
         groups_ptr, ng = arr, len(channel_groups)
     n_masks = len(channel_groups) if channel_groups is not None else len(default_groups(C))
-    dilated = np.zeros((n_masks, B, H, W), np.uint8) if return_dilation else None
+    dilated = np.zeros((n_masks, B, H, W), np.uint8) if return_dilation else None   # codes (see above)
     rc = lib().dirt_oracle_backward_ex(_ptr(vertices), _ptr(faces), _ptr(pixels), _ptr(grad_pixels),
                                        _ptr(gb), _ptr(gv), _ptr(gc), B, H, W, C, V, F, groups_ptr, ng,
                                        _ptr(dilated) if return_dilation else None)
     if rc != 0:
         raise RuntimeError('dirt_oracle_backward failed: %d' % rc)
-    return (gb, gv, gc, list(dilated.astype(bool))) if return_dilation else (gb, gv, gc)
+    if not return_dilation:
+        return gb, gv, gc
+    return gb, gv, gc, list(dilated) if return_dilation == 'codes' else list((dilated & 3) >= 2)
 
 
 class TriExport(ctypes.Structure):
