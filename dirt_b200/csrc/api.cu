@@ -4,6 +4,8 @@
 #include "../../include/dirt_b200.h"
 #include "common.cuh"
 
+#include <initializer_list>
+
 using namespace dirt;
 
 static_assert(BWD_SHARED_GEOMETRY == DIRT_BWD_SHARED_GEOMETRY && BWD_SKIP_POSITION == DIRT_BWD_SKIP_POSITION &&
@@ -854,18 +856,58 @@ extern "C" int dirt_ggx_brdf_table(float* table, int N, void* cuda_stream)
     return DIRT_OK;
 }
 
-// element offsets of every per-point buffer stay below 2^62, the chunk count within the grid's x limit
+// ---- the fused per-point ops: reflectance, GGX, spherical harmonics and normal mapping ----------------------------
+
+// element offsets of every per-point buffer stay below 2^62 (B * V rows of at most `width` floats plus the inputs' row
+// strides), the chunk count within the grid's x limit
+static bool points_shape_ok(int B, long long V, double width, std::initializer_list<long long> strides)
+{
+    if (B < 0 || V < 0) return false;
+    for (long long s : strides) {
+        if (s < 0) return false;
+        width += s;
+    }
+    return (double)B * V * width <= 4.0e18 && light_chunks(V) <= 0x7fffffffll;
+}
+
+// the partial rows of the reflectance and GGX parameter gradients stay below 2^62 bytes
+static bool light_partials_ok(int B, long long V, int C)
+{
+    return (double)B * light_chunks(V) * (LIGHT_FIXED_PARAMS + (double)C) * sizeof(float) <= 4.0e18;
+}
+
+// gradient outputs may be NULL (not wanted), but not misaligned
+static bool aligned(std::initializer_list<const void*> ptrs)
+{
+    for (const void* p : ptrs)
+        if ((uintptr_t)p % 4) return false;
+    return true;
+}
+
+// buffers a call reads or writes: DIRT_ERR_NULL_POINTER if one is NULL, else DIRT_ERR_MISALIGNED if one is not 4-byte
+// aligned
+static int required_check(std::initializer_list<const void*> ptrs)
+{
+    for (const void* p : ptrs)
+        if (!p) return DIRT_ERR_NULL_POINTER;
+    return aligned(ptrs) ? DIRT_OK : DIRT_ERR_MISALIGNED;
+}
+
+// the partials workspace of the per-item parameter gradients, `need` bytes, set as *partial when it passes
+static int partials_check(void* workspace, size_t workspace_bytes, size_t need, float** partial)
+{
+    const int rc = required_check({workspace});
+    if (rc != DIRT_OK) return rc;
+    if (workspace_bytes < need) return DIRT_ERR_WORKSPACE_TOO_SMALL;
+    *partial = static_cast<float*>(workspace);
+    return DIRT_OK;
+}
+
 static bool lighting_shape_ok(int model, int B, long long V, int C, long long sn, long long sp, long long sc)
 {
-    if (model != DIRT_LIGHT_DIFFUSE_DIRECTIONAL && model != DIRT_LIGHT_SPECULAR_DIRECTIONAL &&
-        model != DIRT_LIGHT_DIFFUSE_POINT)
-        return false;
-    if (B < 0 || V < 0 || C <= 0 || sn < 0 || sp < 0 || sc < 0) return false;
-    const double limit = 4.0e18, rows = (double)B * V;
-    const double widest = (double)(C > 3 ? C : 3) + sn + sp + sc;
-    if (rows * widest > limit || light_chunks(V) > 0x7fffffffll) return false;
-    if ((double)B * light_chunks(V) * (LIGHT_FIXED_PARAMS + (double)C) * sizeof(float) > limit) return false;
-    return true;
+    const bool known = model == DIRT_LIGHT_DIFFUSE_DIRECTIONAL || model == DIRT_LIGHT_SPECULAR_DIRECTIONAL ||
+                       model == DIRT_LIGHT_DIFFUSE_POINT;
+    return known && C > 0 && points_shape_ok(B, V, C > 3 ? C : 3, {sn, sp, sc}) && light_partials_ok(B, V, C);
 }
 
 extern "C" size_t dirt_lighting_workspace_bytes(int B, long long V, int C)
@@ -894,13 +936,10 @@ static LightArgs make_light_args(int model, int double_sided, const float* norma
 // the inputs a model reads are required, the others ignored
 static int lighting_inputs_check(const LightArgs& a)
 {
-    const bool pos = a.model != DIRT_LIGHT_DIFFUSE_DIRECTIONAL, sp = a.model == DIRT_LIGHT_SPECULAR_DIRECTIONAL;
-    if (!a.normals || !a.colors || !a.light || !a.light_color || (pos && !a.positions) || (sp && (!a.camera || !a.shininess)))
-        return DIRT_ERR_NULL_POINTER;
-    if ((uintptr_t)a.normals % 4 || (uintptr_t)a.colors % 4 || (uintptr_t)a.light % 4 || (uintptr_t)a.light_color % 4 ||
-        (pos && (uintptr_t)a.positions % 4) || (sp && ((uintptr_t)a.camera % 4 || (uintptr_t)a.shininess % 4)))
-        return DIRT_ERR_MISALIGNED;
-    return DIRT_OK;
+    if (a.model == DIRT_LIGHT_DIFFUSE_DIRECTIONAL) return required_check({a.normals, a.colors, a.light, a.light_color});
+    if (a.model == DIRT_LIGHT_DIFFUSE_POINT)
+        return required_check({a.normals, a.positions, a.colors, a.light, a.light_color});
+    return required_check({a.normals, a.positions, a.colors, a.light, a.light_color, a.camera, a.shininess});
 }
 
 extern "C" int dirt_lighting_forward(int model, int double_sided, const float* normals, long long normals_stride,
@@ -918,10 +957,9 @@ extern "C" int dirt_lighting_forward(int model, int double_sided, const float* n
                                   colors_stride, light, light_per_item, light_color, light_color_per_item, camera,
                                   camera_per_item, shininess, shininess_per_item, B, V, C);
     a.out = out;
-    const int rc = lighting_inputs_check(a);
+    int rc = lighting_inputs_check(a);
+    if (rc == DIRT_OK) rc = required_check({out});
     if (rc != DIRT_OK) return rc;
-    if (!out) return DIRT_ERR_NULL_POINTER;
-    if ((uintptr_t)out % 4) return DIRT_ERR_MISALIGNED;
     CUDA_TRY(launch_lighting_forward(a, (cudaStream_t)cuda_stream, &launches));
     t_last_launches = launches;
     return DIRT_OK;
@@ -949,21 +987,15 @@ extern "C" int dirt_lighting_backward(int model, int double_sided, const float* 
     a.g_positions = model != DIRT_LIGHT_DIFFUSE_DIRECTIONAL ? grad_positions : nullptr;
     a.g_camera = sp ? grad_camera : nullptr;
     a.g_shininess = sp ? grad_shininess : nullptr;
-    float* outs[] = {a.g_normals, a.g_positions, a.g_colors, a.g_light, a.g_light_color, a.g_camera, a.g_shininess};
-    for (float* p : outs)
-        if ((uintptr_t)p % 4) return DIRT_ERR_MISALIGNED;
+    if (!aligned({a.g_normals, a.g_positions, a.g_colors, a.g_light, a.g_light_color, a.g_camera, a.g_shininess}))
+        return DIRT_ERR_MISALIGNED;
     const bool params = a.g_light || a.g_light_color || a.g_camera || a.g_shininess;
     if ((long long)B * V > 0 && (params || a.g_normals || a.g_positions || a.g_colors)) {
         int rc = lighting_inputs_check(a);
+        if (rc == DIRT_OK) rc = required_check({grad_out});
+        if (rc == DIRT_OK && params)
+            rc = partials_check(workspace, workspace_bytes, dirt_lighting_workspace_bytes(B, V, C), &a.partial);
         if (rc != DIRT_OK) return rc;
-        if (!grad_out) return DIRT_ERR_NULL_POINTER;
-        if ((uintptr_t)grad_out % 4) return DIRT_ERR_MISALIGNED;
-        if (params) {
-            if (!workspace) return DIRT_ERR_NULL_POINTER;
-            if ((uintptr_t)workspace % 4) return DIRT_ERR_MISALIGNED;
-            if (workspace_bytes < dirt_lighting_workspace_bytes(B, V, C)) return DIRT_ERR_WORKSPACE_TOO_SMALL;
-            a.partial = static_cast<float*>(workspace);
-        }
     }
     // with no points only the memsets of the wanted parameter gradients are enqueued
     CUDA_TRY(launch_lighting_backward(a, (cudaStream_t)cuda_stream, &launches));
@@ -971,15 +1003,9 @@ extern "C" int dirt_lighting_backward(int model, int double_sided, const float* 
     return DIRT_OK;
 }
 
-// element offsets of every per-point buffer stay below 2^62, the chunk count within the grid's x limit
 static bool ggx_shape_ok(int B, long long V, int C, long long sn, long long sp, long long sr, long long ss)
 {
-    if (B < 0 || V < 0 || C <= 0 || sn < 0 || sp < 0 || sr < 0 || ss < 0) return false;
-    const double limit = 4.0e18, rows = (double)B * V;
-    const double widest = (double)(C > 3 ? C : 3) + sn + sp + sr + ss;
-    if (rows * widest > limit || light_chunks(V) > 0x7fffffffll) return false;
-    if ((double)B * light_chunks(V) * (LIGHT_FIXED_PARAMS + (double)C) * sizeof(float) > limit) return false;
-    return true;
+    return C > 0 && points_shape_ok(B, V, C > 3 ? C : 3, {sn, sp, sr, ss}) && light_partials_ok(B, V, C);
 }
 
 // LightArgs of a GGX call: the specular colour in place of the colours, model = point_light
@@ -995,17 +1021,6 @@ static LightArgs make_ggx_args(int point_light, int double_sided, const float* n
     a.roughness = roughness;
     a.sr = sr;
     return a;
-}
-
-// every input is read
-static int ggx_inputs_check(const LightArgs& a)
-{
-    if (!a.normals || !a.positions || !a.roughness || !a.colors || !a.light || !a.light_color || !a.camera)
-        return DIRT_ERR_NULL_POINTER;
-    if ((uintptr_t)a.normals % 4 || (uintptr_t)a.positions % 4 || (uintptr_t)a.roughness % 4 || (uintptr_t)a.colors % 4 ||
-        (uintptr_t)a.light % 4 || (uintptr_t)a.light_color % 4 || (uintptr_t)a.camera % 4)
-        return DIRT_ERR_MISALIGNED;
-    return DIRT_OK;
 }
 
 extern "C" int dirt_ggx_lighting_forward(int point_light, int double_sided, const float* normals,
@@ -1024,10 +1039,9 @@ extern "C" int dirt_ggx_lighting_forward(int point_light, int double_sided, cons
                                 roughness, roughness_stride, specular, specular_stride, light, light_per_item,
                                 light_color, light_color_per_item, camera, camera_per_item, B, V, C);
     a.out = out;
-    const int rc = ggx_inputs_check(a);
+    int rc = required_check({normals, positions, roughness, specular, light, light_color, camera});
+    if (rc == DIRT_OK) rc = required_check({out});
     if (rc != DIRT_OK) return rc;
-    if (!out) return DIRT_ERR_NULL_POINTER;
-    if ((uintptr_t)out % 4) return DIRT_ERR_MISALIGNED;
     CUDA_TRY(launch_ggx_forward(a, (cudaStream_t)cuda_stream, &launches));
     t_last_launches = launches;
     return DIRT_OK;
@@ -1054,22 +1068,15 @@ extern "C" int dirt_ggx_lighting_backward(int point_light, int double_sided, con
     a.grad_out = grad_out;
     a.g_normals = grad_normals; a.g_positions = grad_positions; a.g_roughness = grad_roughness;
     a.g_colors = grad_specular; a.g_light = grad_light; a.g_light_color = grad_light_color; a.g_camera = grad_camera;
-    float* outs[] = {grad_normals, grad_positions, grad_roughness, grad_specular, grad_light, grad_light_color,
-                     grad_camera};
-    for (float* p : outs)
-        if ((uintptr_t)p % 4) return DIRT_ERR_MISALIGNED;
+    if (!aligned({grad_normals, grad_positions, grad_roughness, grad_specular, grad_light, grad_light_color, grad_camera}))
+        return DIRT_ERR_MISALIGNED;
     const bool params = grad_light || grad_light_color || grad_camera;
     if ((long long)B * V > 0 && (params || grad_normals || grad_positions || grad_roughness || grad_specular)) {
-        int rc = ggx_inputs_check(a);
+        int rc = required_check({normals, positions, roughness, specular, light, light_color, camera});
+        if (rc == DIRT_OK) rc = required_check({grad_out});
+        if (rc == DIRT_OK && params)
+            rc = partials_check(workspace, workspace_bytes, dirt_lighting_workspace_bytes(B, V, C), &a.partial);
         if (rc != DIRT_OK) return rc;
-        if (!grad_out) return DIRT_ERR_NULL_POINTER;
-        if ((uintptr_t)grad_out % 4) return DIRT_ERR_MISALIGNED;
-        if (params) {
-            if (!workspace) return DIRT_ERR_NULL_POINTER;
-            if ((uintptr_t)workspace % 4) return DIRT_ERR_MISALIGNED;
-            if (workspace_bytes < dirt_lighting_workspace_bytes(B, V, C)) return DIRT_ERR_WORKSPACE_TOO_SMALL;
-            a.partial = static_cast<float*>(workspace);
-        }
     }
     // with no points only the memsets of the wanted parameter gradients are enqueued
     CUDA_TRY(launch_ggx_backward(a, (cudaStream_t)cuda_stream, &launches));
@@ -1077,15 +1084,11 @@ extern "C" int dirt_ggx_lighting_backward(int point_light, int double_sided, con
     return DIRT_OK;
 }
 
-// element offsets of every per-point buffer stay below 2^62, the chunk count within the grid's x limit, 9*C an int
+// 9*C an int, and the partial rows of the coefficient gradient below 2^62 bytes
 static bool sh_shape_ok(int B, long long V, int C, long long sn, long long sa)
 {
-    if (B < 0 || V < 0 || C <= 0 || C > (1 << 26) || sn < 0 || sa < 0) return false;
-    const double limit = 4.0e18, rows = (double)B * V;
-    const double widest = (double)(C > 3 ? C : 3) + sn + sa;
-    if (rows * widest > limit || light_chunks(V) > 0x7fffffffll) return false;
-    if ((double)B * sh_chunks(V) * 9.0 * C * sizeof(float) > limit) return false;
-    return true;
+    return C > 0 && C <= (1 << 26) && points_shape_ok(B, V, C > 3 ? C : 3, {sn, sa}) &&
+           (double)B * sh_chunks(V) * 9.0 * C * sizeof(float) <= 4.0e18;
 }
 
 extern "C" size_t dirt_sh_lighting_workspace_bytes(int B, long long V, int C)
@@ -1105,13 +1108,6 @@ static ShArgs make_sh_args(const float* normals, long long sn, const float* albe
     return a;
 }
 
-static int sh_inputs_check(const ShArgs& a)
-{
-    if (!a.normals || !a.albedo || !a.coefficients) return DIRT_ERR_NULL_POINTER;
-    if ((uintptr_t)a.normals % 4 || (uintptr_t)a.albedo % 4 || (uintptr_t)a.coefficients % 4) return DIRT_ERR_MISALIGNED;
-    return DIRT_OK;
-}
-
 extern "C" int dirt_sh_lighting_forward(const float* normals, long long normals_stride, const float* albedo,
                                         long long albedo_stride, const float* coefficients, int coefficients_per_item,
                                         float* out, int B, long long V, int C, void* cuda_stream)
@@ -1122,10 +1118,9 @@ extern "C" int dirt_sh_lighting_forward(const float* normals, long long normals_
     if ((long long)B * V == 0) return DIRT_OK;
     ShArgs a = make_sh_args(normals, normals_stride, albedo, albedo_stride, coefficients, coefficients_per_item, B, V, C);
     a.out = out;
-    const int rc = sh_inputs_check(a);
+    int rc = required_check({normals, albedo, coefficients});
+    if (rc == DIRT_OK) rc = required_check({out});
     if (rc != DIRT_OK) return rc;
-    if (!out) return DIRT_ERR_NULL_POINTER;
-    if ((uintptr_t)out % 4) return DIRT_ERR_MISALIGNED;
     CUDA_TRY(launch_sh_lighting_forward(a, (cudaStream_t)cuda_stream, &launches));
     t_last_launches = launches;
     return DIRT_OK;
@@ -1143,19 +1138,13 @@ extern "C" int dirt_sh_lighting_backward(const float* normals, long long normals
     ShArgs a = make_sh_args(normals, normals_stride, albedo, albedo_stride, coefficients, coefficients_per_item, B, V, C);
     a.grad_out = grad_out;
     a.g_normals = grad_normals; a.g_albedo = grad_albedo; a.g_coef = grad_coefficients;
-    if ((uintptr_t)grad_normals % 4 || (uintptr_t)grad_albedo % 4 || (uintptr_t)grad_coefficients % 4)
-        return DIRT_ERR_MISALIGNED;
+    if (!aligned({grad_normals, grad_albedo, grad_coefficients})) return DIRT_ERR_MISALIGNED;
     if ((long long)B * V > 0 && (grad_normals || grad_albedo || grad_coefficients)) {
-        const int rc = sh_inputs_check(a);
+        int rc = required_check({normals, albedo, coefficients});
+        if (rc == DIRT_OK) rc = required_check({grad_out});
+        if (rc == DIRT_OK && grad_coefficients)
+            rc = partials_check(workspace, workspace_bytes, dirt_sh_lighting_workspace_bytes(B, V, C), &a.partial);
         if (rc != DIRT_OK) return rc;
-        if (!grad_out) return DIRT_ERR_NULL_POINTER;
-        if ((uintptr_t)grad_out % 4) return DIRT_ERR_MISALIGNED;
-        if (grad_coefficients) {
-            if (!workspace) return DIRT_ERR_NULL_POINTER;
-            if ((uintptr_t)workspace % 4) return DIRT_ERR_MISALIGNED;
-            if (workspace_bytes < dirt_sh_lighting_workspace_bytes(B, V, C)) return DIRT_ERR_WORKSPACE_TOO_SMALL;
-            a.partial = static_cast<float*>(workspace);
-        }
     }
     // with no points only the memset of a wanted coefficient gradient is enqueued
     CUDA_TRY(launch_sh_lighting_backward(a, (cudaStream_t)cuda_stream, &launches));
@@ -1320,14 +1309,6 @@ extern "C" int dirt_tangents_backward(const float* vertices, long long vertex_st
     return DIRT_OK;
 }
 
-// element offsets of every per-point buffer stay below 2^62, the chunk count within the grid's x limit
-static bool normal_map_shape_ok(int B, long long V, long long sn, long long st, long long sm)
-{
-    if (B < 0 || V < 0 || sn < 0 || st < 0 || sm < 0) return false;
-    const double rows = (double)B * V;
-    return rows * (4.0 + sn + st + sm) <= 4.0e18 && light_chunks(V) <= 0x7fffffffll;
-}
-
 static NormalMapArgs make_normal_map_args(const float* normals, long long sn, const float* tangents, long long st,
                                           const float* samples, long long sm, int B, long long V)
 {
@@ -1338,26 +1319,18 @@ static NormalMapArgs make_normal_map_args(const float* normals, long long sn, co
     return a;
 }
 
-static int normal_map_inputs_check(const NormalMapArgs& a)
-{
-    if (!a.normals || !a.tangents || !a.samples) return DIRT_ERR_NULL_POINTER;
-    if ((uintptr_t)a.normals % 4 || (uintptr_t)a.tangents % 4 || (uintptr_t)a.samples % 4) return DIRT_ERR_MISALIGNED;
-    return DIRT_OK;
-}
-
 extern "C" int dirt_normal_map_forward(const float* normals, long long normals_stride, const float* tangents,
                                        long long tangents_stride, const float* samples, long long samples_stride,
                                        float* out, int B, long long V, void* cuda_stream)
 {
     int launches = 0;
     t_last_launches = 0;
-    if (!normal_map_shape_ok(B, V, normals_stride, tangents_stride, samples_stride)) return DIRT_ERR_BAD_SHAPE;
+    if (!points_shape_ok(B, V, 4, {normals_stride, tangents_stride, samples_stride})) return DIRT_ERR_BAD_SHAPE;
     if ((long long)B * V == 0) return DIRT_OK;
     NormalMapArgs a = make_normal_map_args(normals, normals_stride, tangents, tangents_stride, samples, samples_stride, B, V);
-    const int rc = normal_map_inputs_check(a);
+    int rc = required_check({normals, tangents, samples});
+    if (rc == DIRT_OK) rc = required_check({out});
     if (rc != DIRT_OK) return rc;
-    if (!out) return DIRT_ERR_NULL_POINTER;
-    if ((uintptr_t)out % 4) return DIRT_ERR_MISALIGNED;
     a.out = out;
     CUDA_TRY(launch_normal_map_forward(a, (cudaStream_t)cuda_stream, &launches));
     t_last_launches = launches;
@@ -1371,14 +1344,13 @@ extern "C" int dirt_normal_map_backward(const float* normals, long long normals_
 {
     int launches = 0;
     t_last_launches = 0;
-    if (!normal_map_shape_ok(B, V, normals_stride, tangents_stride, samples_stride)) return DIRT_ERR_BAD_SHAPE;
-    if ((uintptr_t)grad_normals % 4 || (uintptr_t)grad_tangents % 4 || (uintptr_t)grad_samples % 4) return DIRT_ERR_MISALIGNED;
+    if (!points_shape_ok(B, V, 4, {normals_stride, tangents_stride, samples_stride})) return DIRT_ERR_BAD_SHAPE;
+    if (!aligned({grad_normals, grad_tangents, grad_samples})) return DIRT_ERR_MISALIGNED;
     if ((long long)B * V == 0 || (!grad_normals && !grad_tangents && !grad_samples)) return DIRT_OK;
     NormalMapArgs a = make_normal_map_args(normals, normals_stride, tangents, tangents_stride, samples, samples_stride, B, V);
-    const int rc = normal_map_inputs_check(a);
+    int rc = required_check({normals, tangents, samples});
+    if (rc == DIRT_OK) rc = required_check({grad_out});
     if (rc != DIRT_OK) return rc;
-    if (!grad_out) return DIRT_ERR_NULL_POINTER;
-    if ((uintptr_t)grad_out % 4) return DIRT_ERR_MISALIGNED;
     a.grad_out = grad_out;
     a.g_normals = grad_normals; a.g_tangents = grad_tangents; a.g_samples = grad_samples;
     CUDA_TRY(launch_normal_map_backward(a, (cudaStream_t)cuda_stream, &launches));

@@ -257,97 +257,131 @@ def _ptr(t):
     return t.data_ptr() if t is not None else None
 
 
-_MODEL_NAMES = {_lib.LIGHT_DIFFUSE_DIRECTIONAL: 'DiffuseDirectional', _lib.LIGHT_SPECULAR_DIRECTIONAL: 'SpecularDirectional',
-                _lib.LIGHT_DIFFUSE_POINT: 'DiffusePoint'}
+def _point_stride(t):
+    """The row stride of per-point rows in the fused per-point ops' arguments: 0 for one row or an input not read."""
+    return t.stride(0) if t is not None and t.shape[0] > 1 else 0
 
 
-def _restate(model, double_sided, route, normals, positions, colors, light, light_color, camera, shininess):
-    """The restatement on the op's own inputs (flattened per-point rows, per-item rows): its value has the op's output
-    shape, and autograd through it gives differentiable gradients (double backward)."""
-    lead, V, C = route.lead, route.V, route.C
-    point = lambda t, w: t.reshape(lead + (V, w))
-    item = lambda t, per_item, tail: t.reshape(lead + tail) if per_item else t
-    p_light, p_color, *p_rest = route.per_item
-    n, k = point(normals, 3), point(colors, C)
-    L, lc = item(light, p_light, (3,)), item(light_color, p_color, (C,))
-    if model == _lib.LIGHT_DIFFUSE_DIRECTIONAL:
-        return _diffuse_directional(n, k, L, lc, double_sided)
-    if model == _lib.LIGHT_DIFFUSE_POINT:
-        return _diffuse_point(point(positions, 3), n, k, L, lc, double_sided)
-    return _specular_directional(point(positions, 3), n, k, L, lc, item(camera, p_rest[0], (3,)),
-                                 item(shininess, p_rest[1], ()), double_sided)
+def _flat_item(t, route, per_item):
+    """A per-item input [*, ...] as contiguous [B, ...]; a shared one contiguous as it is."""
+    return (t.reshape((route.B,) + t.shape[len(route.lead):]) if per_item else t).contiguous()
 
 
-class _Reflectance(torch.autograd.Function):
-    """dirt_lighting_forward with its gradient.  Per-point inputs are [rows, k] with unit stride along k; per-item inputs
-    contiguous [B, k] or shared [k] (shininess [B] or []).  The node keeps only its inputs: the backward kernel
-    recomputes the forward from them."""
+def _unflat_points(t, route):
+    """Per-point rows [rows, k] as [*, V, k]."""
+    return t.reshape(route.lead + (route.V, t.shape[-1]))
 
-    @staticmethod
-    def forward(ctx, model, double_sided, route, normals, positions, colors, light, light_color, camera, shininess):
-        out = torch.empty(route.lead + (route.V, route.C), dtype=torch.float32, device=normals.device)
-        with torch.cuda.device(normals.device):
-            rc = _lib.lib().dirt_lighting_forward(*_inputs(model, double_sided, route, normals, positions, colors, light,
-                                                           light_color, camera, shininess), _ptr(out), route.B, route.V,
-                                                  route.C, _stream(normals.device))
-        _lib.check(rc, _MODEL_NAMES[model])
-        ctx.save_for_backward(normals, positions, colors, light, light_color, camera, shininess)
-        ctx.model, ctx.double_sided, ctx.route = model, double_sided, route
-        return out
 
-    @staticmethod
-    def backward(ctx, grad_out):
-        want = ctx.needs_input_grad[3:]
-        if not any(want):
-            return (None,) * 10
-        inputs = ctx.saved_tensors
-        if torch.is_grad_enabled():
-            # create_graph=True: differentiable gradients through the restatement
-            out = _restate(ctx.model, ctx.double_sided, ctx.route, *inputs)
-            wanted = [t for t, w in zip(inputs, want) if w]
-            grads = iter(torch.autograd.grad(out, wanted, grad_out, create_graph=True))
-            return (None,) * 3 + tuple(next(grads) if w else None for w in want)
-        route = ctx.route
-        dev = inputs[0].device
-        grads = [torch.empty(t.shape, dtype=torch.float32, device=dev) if w and t is not None else None
-                 for t, w in zip(inputs, want)]
-        lib = _lib.lib()
-        ws_bytes = int(lib.dirt_lighting_workspace_bytes(route.B, route.V, route.C)) if any(
-            g is not None for g in grads[3:]) else 0
-        workspace = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev) if ws_bytes else None
-        grad_out = grad_out.to(torch.float32).contiguous()
-        with torch.cuda.device(dev):
-            rc = lib.dirt_lighting_backward(*_inputs(ctx.model, ctx.double_sided, route, *inputs), _ptr(grad_out),
-                                            *[_ptr(g) for g in grads], _ptr(workspace), ws_bytes, route.B, route.V,
-                                            route.C, _stream(dev))
-        _lib.check(rc, _MODEL_NAMES[ctx.model] + 'Grad')
-        return (None,) * 3 + tuple(grads)
+def _unflat_item(t, route, per_item):
+    """A per-item input [B, ...] as [*, ...]; a shared one as it is."""
+    return t.reshape(route.lead + t.shape[1:]) if per_item else t
 
 
 def _stream(device):
     return torch.cuda.current_stream(device).cuda_stream
 
 
+def _bvc(route):
+    return route.B, route.V, route.C
+
+
+# A fused per-point op: reflectance, GGX, spherical harmonics or normal mapping.
+#   name: the op's name in errors (its backward's is name + 'Grad');
+#   forward, backward: its entry points in the library;
+#   inputs(*flags, route, *inputs): their input arguments, in their order;
+#   sizes(route): their size arguments;
+#   restate(*flags, route, *inputs): the torch restatement on the op's own inputs, in the output's shape;
+#   first_param: the index of the first per-item parameter.  The gradients of these parameters need a partials
+#     workspace of workspace_bytes(B, V, C) bytes, where workspace_bytes is an entry point; both are None for an op
+#     without such parameters, whose backward then takes no workspace.
+_PointOp = namedtuple('_PointOp', 'name forward backward inputs sizes restate first_param workspace_bytes',
+                      defaults=(None, None))
+
+
+class _PointFunction(torch.autograd.Function):
+    """The forward entry point of a _PointOp with its gradient.  flags are the op's non-tensor arguments (the model or
+    point_light, then double_sided; none for the SH lighting and the normal map).  Per-point inputs are [rows, k] with
+    unit stride along k; per-item inputs contiguous [B, ...] or shared.  The node keeps only its inputs: the backward
+    kernel recomputes the forward from them."""
+
+    @staticmethod
+    def forward(ctx, op, flags, route, *inputs):
+        dev = inputs[0].device
+        out = torch.empty(route.lead + (route.V, route.C), dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            rc = getattr(_lib.lib(), op.forward)(*op.inputs(*flags, route, *inputs), _ptr(out), *op.sizes(route),
+                                                 _stream(dev))
+        _lib.check(rc, op.name)
+        ctx.save_for_backward(*inputs)
+        ctx.op, ctx.flags, ctx.route = op, flags, route
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        op, flags, route = ctx.op, ctx.flags, ctx.route
+        want = ctx.needs_input_grad[3:]
+        if not any(want):
+            return (None,) * (3 + len(want))
+        inputs = ctx.saved_tensors
+        if torch.is_grad_enabled():
+            # create_graph=True: differentiable gradients through the restatement
+            out = op.restate(*flags, route, *inputs)
+            wanted = [t for t, w in zip(inputs, want) if w]
+            grads = iter(torch.autograd.grad(out, wanted, grad_out, create_graph=True))
+            return (None,) * 3 + tuple(next(grads) if w else None for w in want)
+        dev = inputs[0].device
+        grads = [torch.empty(t.shape, dtype=torch.float32, device=dev) if w else None for t, w in zip(inputs, want)]
+        lib = _lib.lib()
+        workspace_args = ()
+        if op.workspace_bytes is not None:
+            ws_bytes = int(getattr(lib, op.workspace_bytes)(*_bvc(route))) if any(want[op.first_param:]) else 0
+            workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=dev) if ws_bytes else None
+            workspace_args = (_ptr(workspace), ws_bytes)
+        grad_out = grad_out.to(torch.float32).contiguous()
+        with torch.cuda.device(dev):
+            rc = getattr(lib, op.backward)(*op.inputs(*flags, route, *inputs), _ptr(grad_out), *[_ptr(g) for g in grads],
+                                           *workspace_args, *op.sizes(route), _stream(dev))
+        _lib.check(rc, op.name + 'Grad')
+        return (None,) * 3 + tuple(grads)
+
+
+def _restate(model, double_sided, route, normals, positions, colors, light, light_color, camera, shininess):
+    """The restatement on the op's own inputs (flattened per-point rows, per-item rows): its value has the op's output
+    shape, and autograd through it gives differentiable gradients (double backward)."""
+    p_light, p_color, *p_rest = route.per_item
+    n, k = _unflat_points(normals, route), _unflat_points(colors, route)
+    L, lc = _unflat_item(light, route, p_light), _unflat_item(light_color, route, p_color)
+    if model == _lib.LIGHT_DIFFUSE_DIRECTIONAL:
+        return _diffuse_directional(n, k, L, lc, double_sided)
+    if model == _lib.LIGHT_DIFFUSE_POINT:
+        return _diffuse_point(_unflat_points(positions, route), n, k, L, lc, double_sided)
+    return _specular_directional(_unflat_points(positions, route), n, k, L, lc, _unflat_item(camera, route, p_rest[0]),
+                                 _unflat_item(shininess, route, p_rest[1]), double_sided)
+
+
 def _inputs(model, double_sided, route, normals, positions, colors, light, light_color, camera, shininess):
     """The input arguments of dirt_lighting_forward / _backward, in their order."""
-    stride = lambda t: t.stride(0) if t is not None and t.shape[0] > 1 else 0
     per_item = list(route.per_item) + [False] * (4 - len(route.per_item))
-    return [model, int(bool(double_sided)), _ptr(normals), stride(normals), _ptr(positions), stride(positions),
-            _ptr(colors), stride(colors), _ptr(light), int(per_item[0]), _ptr(light_color), int(per_item[1]),
-            _ptr(camera), int(per_item[2]), _ptr(shininess), int(per_item[3])]
+    return [model, int(bool(double_sided)), _ptr(normals), _point_stride(normals), _ptr(positions),
+            _point_stride(positions), _ptr(colors), _point_stride(colors), _ptr(light), int(per_item[0]),
+            _ptr(light_color), int(per_item[1]), _ptr(camera), int(per_item[2]), _ptr(shininess), int(per_item[3])]
+
+
+_REFLECTANCE = {model: _PointOp(name, 'dirt_lighting_forward', 'dirt_lighting_backward', _inputs, _bvc, _restate,
+                                first_param=3, workspace_bytes='dirt_lighting_workspace_bytes')
+                for model, name in ((_lib.LIGHT_DIFFUSE_DIRECTIONAL, 'DiffuseDirectional'),
+                                    (_lib.LIGHT_SPECULAR_DIRECTIONAL, 'SpecularDirectional'),
+                                    (_lib.LIGHT_DIFFUSE_POINT, 'DiffusePoint'))}
 
 
 def _reflectance(model, double_sided, route, normals, colors, light, light_color, positions=None, camera=None,
                  shininess=None):
     """The CUDA path of a call that `cuda_route` accepted."""
-    C = route.C
-    item = lambda t, per_item: (t.reshape((route.B,) + t.shape[len(route.lead):]) if per_item else t).contiguous()
     flags = list(route.per_item) + [False] * (4 - len(route.per_item))
-    return _Reflectance.apply(model, double_sided, route, _rows(normals, 3),
-                              _rows(positions, 3) if positions is not None else None, _rows(colors, C),
-                              item(light, flags[0]), item(light_color, flags[1]),
-                              item(camera, flags[2]) if camera is not None else None,
-                              item(shininess, flags[3]) if shininess is not None else None)
+    items = [_flat_item(t, route, per_item) if t is not None else None
+             for t, per_item in zip((light, light_color, camera, shininess), flags)]
+    return _PointFunction.apply(_REFLECTANCE[model], (model, double_sided), route, _rows(normals, 3),
+                                _rows(positions, 3) if positions is not None else None, _rows(colors, route.C), *items)
 
 
 def diffuse_directional(vertex_normals, vertex_colors, light_direction, light_color, double_sided=True, name=None):
@@ -414,65 +448,21 @@ def diffuse_point(vertex_positions, vertex_normals, vertex_colors, light_positio
 
 def _ggx_inputs(point_light, double_sided, route, normals, positions, roughness, specular, light, light_color, camera):
     """The input arguments of dirt_ggx_lighting_forward / _backward, in their order."""
-    stride = lambda t: t.stride(0) if t.shape[0] > 1 else 0
-    return [int(bool(point_light)), int(bool(double_sided)), _ptr(normals), stride(normals), _ptr(positions),
-            stride(positions), _ptr(roughness), stride(roughness), _ptr(specular), stride(specular), _ptr(light),
-            int(route.per_item[0]), _ptr(light_color), int(route.per_item[1]), _ptr(camera), int(route.per_item[2])]
+    return [int(bool(point_light)), int(bool(double_sided)), _ptr(normals), _point_stride(normals), _ptr(positions),
+            _point_stride(positions), _ptr(roughness), _point_stride(roughness), _ptr(specular), _point_stride(specular),
+            _ptr(light), int(route.per_item[0]), _ptr(light_color), int(route.per_item[1]), _ptr(camera),
+            int(route.per_item[2])]
 
 
 def _restate_ggx(point_light, double_sided, route, normals, positions, roughness, specular, light, light_color, camera):
     """The restatement on the op's own inputs (flattened per-point rows, per-item rows)."""
-    lead, V, C = route.lead, route.V, route.C
-    point = lambda t, w: t.reshape(lead + (V, w))
-    item = lambda t, per_item, w: t.reshape(lead + (w,)) if per_item else t
-    return _specular_ggx(point(positions, 3), point(normals, 3), point(roughness, 1), point(specular, C),
-                         item(light, route.per_item[0], 3), item(light_color, route.per_item[1], C),
-                         item(camera, route.per_item[2], 3), point_light, double_sided)
+    points = [_unflat_points(t, route) for t in (positions, normals, roughness, specular)]
+    items = [_unflat_item(t, route, per_item) for t, per_item in zip((light, light_color, camera), route.per_item)]
+    return _specular_ggx(*points, *items, point_light, double_sided)
 
 
-class _SpecularGGX(torch.autograd.Function):
-    """dirt_ggx_lighting_forward with its gradient.  Per-point inputs are [rows, k] with unit stride along k; per-item
-    inputs contiguous [B, k] or shared [k].  The node keeps only its inputs: the backward kernel recomputes the forward
-    from them."""
-
-    @staticmethod
-    def forward(ctx, point_light, double_sided, route, normals, positions, roughness, specular, light, light_color,
-                camera):
-        out = torch.empty(route.lead + (route.V, route.C), dtype=torch.float32, device=normals.device)
-        inputs = (normals, positions, roughness, specular, light, light_color, camera)
-        with torch.cuda.device(normals.device):
-            rc = _lib.lib().dirt_ggx_lighting_forward(*_ggx_inputs(point_light, double_sided, route, *inputs), _ptr(out),
-                                                      route.B, route.V, route.C, _stream(normals.device))
-        _lib.check(rc, 'SpecularGGX')
-        ctx.save_for_backward(*inputs)
-        ctx.point_light, ctx.double_sided, ctx.route = point_light, double_sided, route
-        return out
-
-    @staticmethod
-    def backward(ctx, grad_out):
-        want = ctx.needs_input_grad[3:]
-        if not any(want):
-            return (None,) * 10
-        inputs = ctx.saved_tensors
-        if torch.is_grad_enabled():
-            # create_graph=True: differentiable gradients through the restatement
-            out = _restate_ggx(ctx.point_light, ctx.double_sided, ctx.route, *inputs)
-            wanted = [t for t, w in zip(inputs, want) if w]
-            grads = iter(torch.autograd.grad(out, wanted, grad_out, create_graph=True))
-            return (None,) * 3 + tuple(next(grads) if w else None for w in want)
-        route = ctx.route
-        dev = inputs[0].device
-        grads = [torch.empty(t.shape, dtype=torch.float32, device=dev) if w else None for t, w in zip(inputs, want)]
-        lib = _lib.lib()
-        ws_bytes = int(lib.dirt_lighting_workspace_bytes(route.B, route.V, route.C)) if any(want[4:]) else 0
-        workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=dev) if ws_bytes else None
-        grad_out = grad_out.to(torch.float32).contiguous()
-        with torch.cuda.device(dev):
-            rc = lib.dirt_ggx_lighting_backward(*_ggx_inputs(ctx.point_light, ctx.double_sided, route, *inputs),
-                                                _ptr(grad_out), *[_ptr(g) for g in grads], _ptr(workspace), ws_bytes,
-                                                route.B, route.V, route.C, _stream(dev))
-        _lib.check(rc, 'SpecularGGXGrad')
-        return (None,) * 3 + tuple(grads)
+_GGX = _PointOp('SpecularGGX', 'dirt_ggx_lighting_forward', 'dirt_ggx_lighting_backward', _ggx_inputs, _bvc,
+                _restate_ggx, first_param=4, workspace_bytes='dirt_lighting_workspace_bytes')
 
 
 def _specular_ggx_call(point_light, vertex_positions, vertex_normals, vertex_roughness, vertex_specular, light,
@@ -487,11 +477,10 @@ def _specular_ggx_call(point_light, vertex_positions, vertex_normals, vertex_rou
     if route is None:
         return _specular_ggx(vertex_positions, vertex_normals, vertex_roughness, vertex_specular, light, light_color,
                              camera_position, point_light, double_sided)
-    C = route.C
-    item = lambda t, per_item: (t.reshape((route.B,) + t.shape[len(route.lead):]) if per_item else t).contiguous()
-    return _SpecularGGX.apply(point_light, double_sided, route, _rows(vertex_normals, 3), _rows(vertex_positions, 3),
-                              _rows(vertex_roughness, 1), _rows(vertex_specular, C), item(light, route.per_item[0]),
-                              item(light_color, route.per_item[1]), item(camera_position, route.per_item[2]))
+    items = [_flat_item(t, route, per_item) for t, per_item in zip((light, light_color, camera_position), route.per_item)]
+    return _PointFunction.apply(_GGX, (point_light, double_sided), route, _rows(vertex_normals, 3),
+                                _rows(vertex_positions, 3), _rows(vertex_roughness, 1), _rows(vertex_specular, route.C),
+                                *items)
 
 
 def specular_ggx_directional(vertex_positions, vertex_normals, vertex_roughness, vertex_specular, light_direction,
@@ -645,53 +634,18 @@ def specular_ggx_environment(vertex_positions, vertex_normals, vertex_roughness,
 
 def _sh_inputs(route, normals, albedo, coefficients):
     """The input arguments of dirt_sh_lighting_forward / _backward, in their order."""
-    stride = lambda t: t.stride(0) if t.shape[0] > 1 else 0
-    return [_ptr(normals), stride(normals), _ptr(albedo), stride(albedo), _ptr(coefficients), int(route.per_item[0])]
+    return [_ptr(normals), _point_stride(normals), _ptr(albedo), _point_stride(albedo), _ptr(coefficients),
+            int(route.per_item[0])]
 
 
-class _SphericalHarmonics(torch.autograd.Function):
-    """dirt_sh_lighting_forward with its gradient.  normals [rows, 3] and albedo [rows, C] with unit stride along the row;
-    coefficients contiguous [B, 9, C] or shared [9, C].  The node keeps only its inputs: the backward kernel recomputes
-    the forward from them."""
+def _restate_sh(route, normals, albedo, coefficients):
+    """The restatement on the op's own inputs (flattened per-point rows, per-item coefficients)."""
+    return _diffuse_spherical_harmonics(_unflat_points(normals, route), _unflat_points(albedo, route),
+                                        _unflat_item(coefficients, route, route.per_item[0]))
 
-    @staticmethod
-    def forward(ctx, route, normals, albedo, coefficients):
-        out = torch.empty(route.lead + (route.V, route.C), dtype=torch.float32, device=normals.device)
-        with torch.cuda.device(normals.device):
-            rc = _lib.lib().dirt_sh_lighting_forward(*_sh_inputs(route, normals, albedo, coefficients), _ptr(out),
-                                                     route.B, route.V, route.C, _stream(normals.device))
-        _lib.check(rc, 'DiffuseSphericalHarmonics')
-        ctx.save_for_backward(normals, albedo, coefficients)
-        ctx.route = route
-        return out
 
-    @staticmethod
-    def backward(ctx, grad_out):
-        want = ctx.needs_input_grad[1:]
-        if not any(want):
-            return (None,) * 4
-        inputs = ctx.saved_tensors
-        route = ctx.route
-        if torch.is_grad_enabled():
-            # create_graph=True: differentiable gradients through the restatement
-            normals, albedo, coefficients = inputs
-            lead, V, C = route.lead, route.V, route.C
-            coef = coefficients.reshape(lead + (9, C)) if route.per_item[0] else coefficients
-            out = _diffuse_spherical_harmonics(normals.reshape(lead + (V, 3)), albedo.reshape(lead + (V, C)), coef)
-            wanted = [t for t, w in zip(inputs, want) if w]
-            grads = iter(torch.autograd.grad(out, wanted, grad_out, create_graph=True))
-            return (None,) + tuple(next(grads) if w else None for w in want)
-        dev = inputs[0].device
-        grads = [torch.empty(t.shape, dtype=torch.float32, device=dev) if w else None for t, w in zip(inputs, want)]
-        lib = _lib.lib()
-        ws_bytes = int(lib.dirt_sh_lighting_workspace_bytes(route.B, route.V, route.C)) if want[2] else 0
-        workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=dev) if ws_bytes else None
-        grad_out = grad_out.to(torch.float32).contiguous()
-        with torch.cuda.device(dev):
-            rc = lib.dirt_sh_lighting_backward(*_sh_inputs(route, *inputs), _ptr(grad_out), *[_ptr(g) for g in grads],
-                                               _ptr(workspace), ws_bytes, route.B, route.V, route.C, _stream(dev))
-        _lib.check(rc, 'DiffuseSphericalHarmonicsGrad')
-        return (None,) + tuple(grads)
+_SH = _PointOp('DiffuseSphericalHarmonics', 'dirt_sh_lighting_forward', 'dirt_sh_lighting_backward', _sh_inputs, _bvc,
+               _restate_sh, first_param=2, workspace_bytes='dirt_sh_lighting_workspace_bytes')
 
 
 def diffuse_spherical_harmonics(vertex_normals, vertex_colors, coefficients, name=None):
@@ -710,9 +664,8 @@ def diffuse_spherical_harmonics(vertex_normals, vertex_colors, coefficients, nam
     route = _route([vertex_normals, vertex_colors], [(coefficients, (9, 'C'))])
     if route is None:
         return _diffuse_spherical_harmonics(vertex_normals, vertex_colors, coefficients)
-    C = route.C
-    coefficients = (coefficients.reshape((route.B, 9, C)) if route.per_item[0] else coefficients).contiguous()
-    return _SphericalHarmonics.apply(route, _rows(vertex_normals, 3), _rows(vertex_colors, C), coefficients)
+    return _PointFunction.apply(_SH, (), route, _rows(vertex_normals, 3), _rows(vertex_colors, route.C),
+                                _flat_item(coefficients, route, route.per_item[0]))
 
 
 # ---- the CUDA path of the normals -----------------------------------------------------------------------------------
@@ -972,50 +925,20 @@ def vertex_tangents(vertices, uvs, faces, vertex_normals, name=None):
     return out.reshape(route.lead + (route.V, 4))
 
 
-class _NormalMap(torch.autograd.Function):
-    """dirt_normal_map_forward with its gradient.  normals [rows, 3], tangents [rows, 4] and samples [rows, 3] with unit
-    stride along the row.  The node keeps only its inputs: the backward kernel recomputes the forward from them."""
-
-    @staticmethod
-    def forward(ctx, route, normals, tangents, samples):
-        out = torch.empty(route.lead + (route.V, 3), dtype=torch.float32, device=normals.device)
-        with torch.cuda.device(normals.device):
-            rc = _lib.lib().dirt_normal_map_forward(*_normal_map_inputs(normals, tangents, samples), _ptr(out), route.B,
-                                                    route.V, _stream(normals.device))
-        _lib.check(rc, 'PerturbNormals')
-        ctx.save_for_backward(normals, tangents, samples)
-        ctx.route = route
-        return out
-
-    @staticmethod
-    def backward(ctx, grad_out):
-        want = ctx.needs_input_grad[1:]
-        if not any(want):
-            return (None,) * 4
-        inputs = ctx.saved_tensors
-        route = ctx.route
-        if torch.is_grad_enabled():
-            # create_graph=True: differentiable gradients through the restatement
-            lead, V = route.lead, route.V
-            out = _perturb_normals(*[t.reshape(lead + (V, t.shape[-1])) for t in inputs])
-            wanted = [t for t, w in zip(inputs, want) if w]
-            grads = iter(torch.autograd.grad(out, wanted, grad_out, create_graph=True))
-            return (None,) + tuple(next(grads) if w else None for w in want)
-        dev = inputs[0].device
-        grads = [torch.empty((t.shape[0], t.shape[1]), dtype=torch.float32, device=dev) if w else None
-                 for t, w in zip(inputs, want)]
-        grad_out = grad_out.to(torch.float32).contiguous()
-        with torch.cuda.device(dev):
-            rc = _lib.lib().dirt_normal_map_backward(*_normal_map_inputs(*inputs), _ptr(grad_out),
-                                                     *[_ptr(g) for g in grads], route.B, route.V, _stream(dev))
-        _lib.check(rc, 'PerturbNormalsGrad')
-        return (None,) + tuple(grads)
-
-
-def _normal_map_inputs(normals, tangents, samples):
+def _normal_map_inputs(route, normals, tangents, samples):
     """The input arguments of dirt_normal_map_forward / _backward, in their order."""
-    stride = lambda t: t.stride(0) if t.shape[0] > 1 else 0
-    return [_ptr(normals), stride(normals), _ptr(tangents), stride(tangents), _ptr(samples), stride(samples)]
+    return [_ptr(normals), _point_stride(normals), _ptr(tangents), _point_stride(tangents), _ptr(samples),
+            _point_stride(samples)]
+
+
+def _restate_normal_map(route, normals, tangents, samples):
+    """The restatement on the op's own inputs (flattened per-point rows)."""
+    return _perturb_normals(*[_unflat_points(t, route) for t in (normals, tangents, samples)])
+
+
+# its entry points take no channel count: the output rows are 3 wide
+_NORMAL_MAP = _PointOp('PerturbNormals', 'dirt_normal_map_forward', 'dirt_normal_map_backward', _normal_map_inputs,
+                       lambda route: (route.B, route.V), _restate_normal_map)
 
 
 def perturb_normals(normals, tangents, tangent_space_normals, name=None):
@@ -1035,4 +958,5 @@ def perturb_normals(normals, tangents, tangent_space_normals, name=None):
     route = _route([normals, tangents, tangent_space_normals], [], [3, 4, 3])
     if route is None:
         return _perturb_normals(normals, tangents, tangent_space_normals)
-    return _NormalMap.apply(route, _rows(normals, 3), _rows(tangents, 4), _rows(tangent_space_normals, 3))
+    return _PointFunction.apply(_NORMAL_MAP, (), route, _rows(normals, 3), _rows(tangents, 4),
+                                _rows(tangent_space_normals, 3))
