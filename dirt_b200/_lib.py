@@ -180,6 +180,17 @@ def load(path):
     L.dirt_normal_map_forward.argtypes = normal_map_inputs + [vp, i, ll, vp]
     L.dirt_normal_map_backward.restype = i
     L.dirt_normal_map_backward.argtypes = normal_map_inputs + [vp] * 4 + [i, ll, vp]
+    shadow_inputs = [vp, ll, vp, vp, i, i, i, i, ctypes.c_float, ctypes.c_float]
+    L.dirt_shadow_workspace_bytes.restype = sz
+    L.dirt_shadow_workspace_bytes.argtypes = [i, ll]
+    L.dirt_shadow_forward.restype = i
+    L.dirt_shadow_forward.argtypes = shadow_inputs + [vp, i, ll, vp]
+    L.dirt_shadow_backward.restype = i
+    L.dirt_shadow_backward.argtypes = shadow_inputs + [vp] * 5 + [sz, i, ll, vp]
+    L.dirt_shadow_backward_deterministic_bytes.restype = sz
+    L.dirt_shadow_backward_deterministic_bytes.argtypes = [i, ll, i, i, i]
+    L.dirt_shadow_backward_deterministic.restype = i
+    L.dirt_shadow_backward_deterministic.argtypes = shadow_inputs + [vp] * 5 + [sz, vp, sz, i, ll, vp]
     return L
 
 
@@ -204,7 +215,9 @@ EXPORTED_SYMBOLS = ['dirt_error_string', 'dirt_abi_version', 'dirt_workspace_byt
                     'dirt_cubemap_sh_project_bytes', 'dirt_cubemap_sh_project', 'dirt_cubemap_sh_project_backward',
                     'dirt_latlong_samples', 'dirt_latlong_to_cubemap', 'dirt_latlong_to_cubemap_backward',
                     'dirt_tangents_workspace_bytes', 'dirt_tangents_forward', 'dirt_tangents_backward',
-                    'dirt_normal_map_forward', 'dirt_normal_map_backward']
+                    'dirt_normal_map_forward', 'dirt_normal_map_backward', 'dirt_shadow_workspace_bytes',
+                    'dirt_shadow_forward', 'dirt_shadow_backward', 'dirt_shadow_backward_deterministic_bytes',
+                    'dirt_shadow_backward_deterministic']
 
 
 def error_string(code):

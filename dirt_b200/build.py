@@ -9,7 +9,7 @@ import subprocess
 _HERE = os.path.dirname(os.path.abspath(__file__))
 SO_PATH = os.path.join(_HERE, 'libdirt_b200.so')
 SOURCES = ['api.cu', 'setup.cu', 'raster.cu', 'backward.cu', 'exchange.cu', 'texture.cu', 'lighting.cu', 'normals.cu',
-           'deterministic.cu', 'derivatives.cu', 'ibl.cu', 'latlong.cu']
+           'deterministic.cu', 'derivatives.cu', 'ibl.cu', 'latlong.cu', 'shadow.cu']
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
               '-Xcompiler', '-fPIC', '-shared']
 

@@ -4,6 +4,7 @@
 #include "../../include/dirt_b200.h"
 #include "common.cuh"
 
+#include <cmath>
 #include <initializer_list>
 
 using namespace dirt;
@@ -1148,6 +1149,142 @@ extern "C" int dirt_sh_lighting_backward(const float* normals, long long normals
     }
     // with no points only the memset of a wanted coefficient gradient is enqueued
     CUDA_TRY(launch_sh_lighting_backward(a, (cudaStream_t)cuda_stream, &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
+// ---- shadow-map visibility (DESIGN.md §7.15) ------------------------------------------------------------------------
+
+// the points as the other per-point ops', a map of at most 2^62 texel floats, the lookup's parameters in range, and the
+// partial rows of the light-matrix gradient below 2^62 bytes
+static bool shadow_shape_ok(int B, long long V, long long sp, int SH, int SW, int radius, float softness, float bias)
+{
+    return points_shape_ok(B, V, 3, {sp}) && SH > 0 && SW > 0 && (double)(B > 1 ? B : 1) * SH * SW * 2 <= 4.0e18 &&
+           radius >= 0 && radius <= 3 && softness >= 0.f && bias >= 0.f && std::isfinite(softness) &&
+           std::isfinite(bias) && (double)B * light_chunks(V) * SHADOW_MATRIX * sizeof(float) <= 4.0e18;
+}
+
+extern "C" size_t dirt_shadow_workspace_bytes(int B, long long V)
+{
+    if (B <= 0 || V <= 0) return 0;
+    return sizeof(float) * (size_t)B * (size_t)light_chunks(V) * SHADOW_MATRIX;
+}
+
+static ShadowArgs make_shadow_args(const float* positions, long long sp, const float* light_matrix,
+                                   const float* shadow_map, int per_item, int SH, int SW, int radius, float softness,
+                                   float bias, int B, long long V)
+{
+    ShadowArgs a = {};
+    a.positions = positions; a.sp = sp; a.matrix = light_matrix; a.map = shadow_map; a.per_item = per_item != 0;
+    a.SH = SH; a.SW = SW; a.R = radius; a.softness = softness; a.bias = bias;
+    a.V = V; a.B = B; a.chunks = (int)light_chunks(V);
+    return a;
+}
+
+// the inputs, with the map's float2 texels 8-byte aligned
+static int shadow_inputs_check(const ShadowArgs& a)
+{
+    const int rc = required_check({a.positions, a.matrix, a.map});
+    if (rc != DIRT_OK) return rc;
+    return (uintptr_t)a.map % 8 ? DIRT_ERR_MISALIGNED : DIRT_OK;
+}
+
+extern "C" int dirt_shadow_forward(const float* positions, long long positions_stride, const float* light_matrix,
+                                   const float* shadow_map, int per_item, int SH, int SW, int radius, float softness,
+                                   float bias, float* out, int B, long long V, void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (!shadow_shape_ok(B, V, positions_stride, SH, SW, radius, softness, bias)) return DIRT_ERR_BAD_SHAPE;
+    if ((long long)B * V == 0) return DIRT_OK;
+    ShadowArgs a = make_shadow_args(positions, positions_stride, light_matrix, shadow_map, per_item, SH, SW, radius,
+                                    softness, bias, B, V);
+    a.out = out;
+    int rc = shadow_inputs_check(a);
+    if (rc == DIRT_OK) rc = required_check({out});
+    if (rc != DIRT_OK) return rc;
+    CUDA_TRY(launch_shadow_forward(a, (cudaStream_t)cuda_stream, &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
+extern "C" int dirt_shadow_backward(const float* positions, long long positions_stride, const float* light_matrix,
+                                    const float* shadow_map, int per_item, int SH, int SW, int radius, float softness,
+                                    float bias, const float* grad_out, float* grad_positions, float* grad_light_matrix,
+                                    float* grad_shadow_map, void* workspace, size_t workspace_bytes, int B, long long V,
+                                    void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (!shadow_shape_ok(B, V, positions_stride, SH, SW, radius, softness, bias)) return DIRT_ERR_BAD_SHAPE;
+    ShadowArgs a = make_shadow_args(positions, positions_stride, light_matrix, shadow_map, per_item, SH, SW, radius,
+                                    softness, bias, B, V);
+    a.grad_out = grad_out;
+    a.g_positions = grad_positions; a.g_matrix = grad_light_matrix; a.g_map = grad_shadow_map;
+    if (!aligned({grad_positions, grad_light_matrix, grad_shadow_map}) || (uintptr_t)grad_shadow_map % 8)
+        return DIRT_ERR_MISALIGNED;
+    if ((long long)B * V > 0 && (grad_positions || grad_light_matrix || grad_shadow_map)) {
+        int rc = shadow_inputs_check(a);
+        if (rc == DIRT_OK) rc = required_check({grad_out});
+        if (rc == DIRT_OK && grad_light_matrix)
+            rc = partials_check(workspace, workspace_bytes, dirt_shadow_workspace_bytes(B, V), &a.partial);
+        if (rc != DIRT_OK) return rc;
+    }
+    // with no points only the memsets of the wanted map and matrix gradients are enqueued
+    CUDA_TRY(launch_shadow_backward(a, (cudaStream_t)cuda_stream, &launches));
+    t_last_launches = launches;
+    return DIRT_OK;
+}
+
+// the deterministic backward's point ids and segment offsets are int32
+static bool shadow_det_shape_ok(int B, long long V, int per_item, int SH, int SW)
+{
+    return (long long)B * V <= 0x7fffffffll && SH > 0 && SW > 0 &&
+           shadow_det_keys(B, per_item != 0, SH, SW) + 2 <= 0x7fffffffll;
+}
+
+extern "C" size_t dirt_shadow_backward_deterministic_bytes(int B, long long V, int per_item, int SH, int SW)
+{
+    if (B <= 0 || V <= 0 || !shadow_det_shape_ok(B, V, per_item, SH, SW)) return 0;
+    ShadowArgs a = {};
+    a.B = B; a.V = V; a.per_item = per_item != 0; a.SH = SH; a.SW = SW;
+    return carve_shadow_det_scratch(nullptr, a).bytes;
+}
+
+extern "C" int dirt_shadow_backward_deterministic(const float* positions, long long positions_stride,
+                                                  const float* light_matrix, const float* shadow_map, int per_item,
+                                                  int SH, int SW, int radius, float softness, float bias,
+                                                  const float* grad_out, float* grad_positions,
+                                                  float* grad_light_matrix, float* grad_shadow_map, void* workspace,
+                                                  size_t workspace_bytes, void* scratch, size_t scratch_bytes, int B,
+                                                  long long V, void* cuda_stream)
+{
+    int launches = 0;
+    t_last_launches = 0;
+    if (!shadow_shape_ok(B, V, positions_stride, SH, SW, radius, softness, bias) ||
+        !shadow_det_shape_ok(B, V, per_item, SH, SW))
+        return DIRT_ERR_BAD_SHAPE;
+    ShadowArgs a = make_shadow_args(positions, positions_stride, light_matrix, shadow_map, per_item, SH, SW, radius,
+                                    softness, bias, B, V);
+    a.grad_out = grad_out;
+    a.g_positions = grad_positions; a.g_matrix = grad_light_matrix; a.g_map = grad_shadow_map;
+    if (!aligned({grad_positions, grad_light_matrix, grad_shadow_map}) || (uintptr_t)grad_shadow_map % 8)
+        return DIRT_ERR_MISALIGNED;
+    const bool sorts = grad_shadow_map && (long long)B * V > 0;
+    if ((long long)B * V > 0 && (grad_positions || grad_light_matrix || grad_shadow_map)) {
+        int rc = shadow_inputs_check(a);
+        if (rc == DIRT_OK) rc = required_check({grad_out});
+        if (rc == DIRT_OK && grad_light_matrix)
+            rc = partials_check(workspace, workspace_bytes, dirt_shadow_workspace_bytes(B, V), &a.partial);
+        if (rc == DIRT_OK && sorts) {
+            rc = required_check({scratch});
+            if (rc == DIRT_OK && scratch_bytes < dirt_shadow_backward_deterministic_bytes(B, V, per_item, SH, SW))
+                rc = DIRT_ERR_WORKSPACE_TOO_SMALL;
+        }
+        if (rc != DIRT_OK) return rc;
+    }
+    CUDA_TRY(launch_shadow_backward_deterministic(a, carve_shadow_det_scratch(sorts ? scratch : nullptr, a),
+                                                  (cudaStream_t)cuda_stream, &launches));
     t_last_launches = launches;
     return DIRT_OK;
 }

@@ -345,23 +345,18 @@ __global__ void __launch_bounds__(REDUCE_THREADS) lighting_reduce_kernel(const f
     }
 }
 
-inline dim3 point_grid(const LightArgs& a)
-{
-    return dim3((unsigned)a.chunks, (unsigned)(a.B < (int)MAX_ITEMS_PER_GRID ? a.B : (int)MAX_ITEMS_PER_GRID));
-}
-
 template <int MODEL, bool DS>
 void forward_md(const LightArgs& a, cudaStream_t stream)
 {
-    if (a.C == 3) lighting_forward_kernel<MODEL, DS, 3><<<point_grid(a), LIGHT_THREADS, 0, stream>>>(a);
-    else lighting_forward_kernel<MODEL, DS, 0><<<point_grid(a), LIGHT_THREADS, 0, stream>>>(a);
+    if (a.C == 3) lighting_forward_kernel<MODEL, DS, 3><<<light_grid(a.chunks, a.B), LIGHT_THREADS, 0, stream>>>(a);
+    else lighting_forward_kernel<MODEL, DS, 0><<<light_grid(a.chunks, a.B), LIGHT_THREADS, 0, stream>>>(a);
 }
 
 template <int MODEL, bool DS>
 void backward_md(const LightArgs& a, cudaStream_t stream)
 {
-    if (a.C == 3) lighting_backward_kernel<MODEL, DS, 3><<<point_grid(a), LIGHT_THREADS, 0, stream>>>(a);
-    else lighting_backward_kernel<MODEL, DS, 0><<<point_grid(a), LIGHT_THREADS, 0, stream>>>(a);
+    if (a.C == 3) lighting_backward_kernel<MODEL, DS, 3><<<light_grid(a.chunks, a.B), LIGHT_THREADS, 0, stream>>>(a);
+    else lighting_backward_kernel<MODEL, DS, 0><<<light_grid(a.chunks, a.B), LIGHT_THREADS, 0, stream>>>(a);
 }
 
 template <int MODEL>
@@ -423,6 +418,26 @@ cudaError_t reduce_params(const LightArgs& a, const ReduceJobs& jobs, cudaStream
 }
 
 }  // namespace
+
+dim3 light_grid(long long chunks, int B)
+{
+    return dim3((unsigned)chunks, (unsigned)(B < (int)MAX_ITEMS_PER_GRID ? B : (int)MAX_ITEMS_PER_GRID));
+}
+
+cudaError_t launch_partials_reduce(const float* partial, float* out, int width, bool per_item, long long chunks, int B,
+                                   cudaStream_t stream, int* launches)
+{
+    ReduceJobs jobs = {};
+    jobs.count = 1;
+    jobs.out[0] = out; jobs.offset[0] = 0; jobs.width[0] = width; jobs.per_item[0] = per_item;
+    const long long total = (per_item ? (long long)B : 1ll) * width;
+    jobs.first[0] = 0; jobs.first[1] = total;
+    const unsigned blocks = (unsigned)(total < REDUCE_MAX_BLOCKS ? total : REDUCE_MAX_BLOCKS);
+    lighting_reduce_kernel<<<blocks, REDUCE_THREADS, 0, stream>>>(partial, jobs, total, chunks, B, width);
+    const cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) ++*launches;
+    return e;
+}
 
 cudaError_t launch_lighting_forward(const LightArgs& a, cudaStream_t stream, int* launches)
 {
@@ -737,11 +752,11 @@ template <bool POINT, bool DS>
 void ggx_launch(const LightArgs& a, bool forward, cudaStream_t stream)
 {
     if (forward) {
-        if (a.C == 3) ggx_forward_kernel<POINT, DS, 3><<<point_grid(a), LIGHT_THREADS, 0, stream>>>(a);
-        else ggx_forward_kernel<POINT, DS, 0><<<point_grid(a), LIGHT_THREADS, 0, stream>>>(a);
+        if (a.C == 3) ggx_forward_kernel<POINT, DS, 3><<<light_grid(a.chunks, a.B), LIGHT_THREADS, 0, stream>>>(a);
+        else ggx_forward_kernel<POINT, DS, 0><<<light_grid(a.chunks, a.B), LIGHT_THREADS, 0, stream>>>(a);
     } else {
-        if (a.C == 3) ggx_backward_kernel<POINT, DS, 3><<<point_grid(a), LIGHT_THREADS, 0, stream>>>(a);
-        else ggx_backward_kernel<POINT, DS, 0><<<point_grid(a), LIGHT_THREADS, 0, stream>>>(a);
+        if (a.C == 3) ggx_backward_kernel<POINT, DS, 3><<<light_grid(a.chunks, a.B), LIGHT_THREADS, 0, stream>>>(a);
+        else ggx_backward_kernel<POINT, DS, 0><<<light_grid(a.chunks, a.B), LIGHT_THREADS, 0, stream>>>(a);
     }
 }
 
@@ -955,17 +970,12 @@ __global__ void __launch_bounds__(LIGHT_THREADS) sh_backward_kernel(ShArgs a)
     }
 }
 
-inline dim3 sh_grid(long long chunks, int B)
-{
-    return dim3((unsigned)chunks, (unsigned)(B < (int)MAX_ITEMS_PER_GRID ? B : (int)MAX_ITEMS_PER_GRID));
-}
-
 }  // namespace
 
 cudaError_t launch_sh_lighting_forward(const ShArgs& a, cudaStream_t stream, int* launches)
 {
     if ((long long)a.B * a.V == 0) return cudaSuccess;
-    const dim3 grid = sh_grid(light_chunks(a.V), a.B);
+    const dim3 grid = light_grid(light_chunks(a.V), a.B);
     if (a.C == 3) sh_forward_kernel<3><<<grid, LIGHT_THREADS, 0, stream>>>(a);
     else sh_forward_kernel<0><<<grid, LIGHT_THREADS, 0, stream>>>(a);
     const cudaError_t e = cudaGetLastError();
@@ -985,21 +995,14 @@ cudaError_t launch_sh_lighting_backward(const ShArgs& a, cudaStream_t stream, in
     if (!a.g_normals && !a.g_albedo && !a.g_coef) return cudaSuccess;
     ShArgs b = a;
     if (!a.g_coef) b.partial = nullptr;
-    const dim3 grid = sh_grid(a.chunks, a.B);
+    const dim3 grid = light_grid(a.chunks, a.B);
     if (a.C == 3) sh_backward_kernel<3><<<grid, LIGHT_THREADS, 0, stream>>>(b);
     else sh_backward_kernel<0><<<grid, LIGHT_THREADS, 0, stream>>>(b);
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     ++*launches;
     if (a.g_coef) {
         // one job: the [9, C] columns of the partials, per item or over every item
-        ReduceJobs jobs = {};
-        jobs.count = 1;
-        jobs.out[0] = a.g_coef; jobs.offset[0] = 0; jobs.width[0] = (int)width; jobs.per_item[0] = a.item_coef;
-        jobs.first[0] = 0; jobs.first[1] = total;
-        const unsigned blocks = (unsigned)(total < REDUCE_MAX_BLOCKS ? total : REDUCE_MAX_BLOCKS);
-        lighting_reduce_kernel<<<blocks, REDUCE_THREADS, 0, stream>>>(b.partial, jobs, total, a.chunks, a.B, (int)width);
-        if ((e = cudaGetLastError()) != cudaSuccess) return e;
-        ++*launches;
+        return launch_partials_reduce(b.partial, a.g_coef, (int)width, a.item_coef, a.chunks, a.B, stream, launches);
     }
     return cudaSuccess;
 }
@@ -1135,17 +1138,12 @@ __global__ void __launch_bounds__(LIGHT_THREADS) normal_map_backward_kernel(Norm
     }
 }
 
-inline dim3 normal_map_grid(const NormalMapArgs& a)
-{
-    return dim3((unsigned)light_chunks(a.V), (unsigned)(a.B < (int)MAX_ITEMS_PER_GRID ? a.B : (int)MAX_ITEMS_PER_GRID));
-}
-
 }  // namespace
 
 cudaError_t launch_normal_map_forward(const NormalMapArgs& a, cudaStream_t stream, int* launches)
 {
     if ((long long)a.B * a.V == 0) return cudaSuccess;
-    normal_map_forward_kernel<<<normal_map_grid(a), LIGHT_THREADS, 0, stream>>>(a);
+    normal_map_forward_kernel<<<light_grid(light_chunks(a.V), a.B), LIGHT_THREADS, 0, stream>>>(a);
     const cudaError_t e = cudaGetLastError();
     if (e == cudaSuccess) ++*launches;
     return e;
@@ -1154,7 +1152,7 @@ cudaError_t launch_normal_map_forward(const NormalMapArgs& a, cudaStream_t strea
 cudaError_t launch_normal_map_backward(const NormalMapArgs& a, cudaStream_t stream, int* launches)
 {
     if ((long long)a.B * a.V == 0 || (!a.g_normals && !a.g_tangents && !a.g_samples)) return cudaSuccess;
-    normal_map_backward_kernel<<<normal_map_grid(a), LIGHT_THREADS, 0, stream>>>(a);
+    normal_map_backward_kernel<<<light_grid(light_chunks(a.V), a.B), LIGHT_THREADS, 0, stream>>>(a);
     const cudaError_t e = cudaGetLastError();
     if (e == cudaSuccess) ++*launches;
     return e;

@@ -15,6 +15,7 @@
 // fixed-order float64 sums per texel; see the section below and DESIGN.md §7.5.
 #include "../../include/dirt_b200.h"
 #include "common.cuh"
+#include "sort.cuh"
 
 #include <type_traits>
 
@@ -312,74 +313,7 @@ __global__ void __launch_bounds__(TEX_THREADS) texture_forward_generic_kernel(co
 
 // ---- backward -------------------------------------------------------------------------------------------------------
 
-// How the lanes of a warp that share a key sum their values.  Lanes that contribute nothing carry a key of their own.
-struct Agg {
-    unsigned peers;     // lanes with this lane's key, this lane included
-    unsigned leaders;   // the lowest lane of every group of two or more
-    bool pull;          // each leader pulls its members one by one (else: one butterfly over the warp per group)
-};
-
-__device__ __forceinline__ Agg agg_plan(unsigned long long key, int lane)
-{
-    Agg a;
-    a.peers = __match_any_sync(FULL, key);
-    const unsigned size = __popc(a.peers);
-    const bool leader = __ffs(a.peers) - 1 == lane;
-    a.leaders = __ballot_sync(FULL, leader && size > 1);
-    // pulling costs (largest group - 1) shuffle rounds, the butterflies 5 per group of two or more
-    a.pull = __reduce_max_sync(FULL, size) - 1 <= 5u * __popc(a.leaders);
-    return a;
-}
-
-// On return the lowest lane of each group holds the group's sum in v (other lanes: unspecified).  Warp-uniform.
-template <int NV>
-__device__ __forceinline__ void agg_sum(const Agg& a, float v[NV], int lane)
-{
-    if (!a.leaders) return;
-    if (a.pull) {
-        float s[NV];
-#pragma unroll
-        for (int j = 0; j < NV; ++j) s[j] = v[j];
-        unsigned rest = __ffs(a.peers) - 1 == lane ? a.peers & (a.peers - 1) : 0u;
-        while (__any_sync(FULL, rest)) {
-            const int src = rest ? __ffs(rest) - 1 : lane;
-#pragma unroll
-            for (int j = 0; j < NV; ++j) {
-                const float x = __shfl_sync(FULL, v[j], src);
-                if (rest) s[j] += x;
-            }
-            rest &= rest - 1;
-        }
-#pragma unroll
-        for (int j = 0; j < NV; ++j) v[j] = s[j];
-    } else {
-        float s[NV];
-#pragma unroll
-        for (int j = 0; j < NV; ++j) s[j] = v[j];
-        for (unsigned todo = a.leaders; todo; todo &= todo - 1) {
-            const int L = __ffs(todo) - 1;
-            const bool member = (a.peers >> L) & 1u;
-#pragma unroll
-            for (int j = 0; j < NV; ++j) {
-                float x = member ? v[j] : 0.f;
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(FULL, x, o);
-                if (lane == L) s[j] = x;
-            }
-        }
-#pragma unroll
-        for (int j = 0; j < NV; ++j) v[j] = s[j];
-    }
-}
-
-__device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d)
-{
-    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
-__device__ __forceinline__ void red_add_v2(float* addr, float a, float b)
-{
-    asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
-}
+// warp aggregation (Agg, agg_plan, agg_sum) and the vector reductions: common.cuh
 
 template <int NV, bool VEC>
 __device__ __forceinline__ void red_row(float* dst, const float v[NV])
@@ -623,155 +557,23 @@ cudaError_t backward_ct(const float* texture, const float* pyramid, const float*
 //      butterfly 16, 8, 4, 2, 1, and the chunk sums are added in chunk order from +0.0.  The tree depends on L alone.
 //      A texel of at most DET_CHUNK terms is summed by one warp; a longer one is listed, each of its chunks is summed by
 //      a warp of its own into the scratch, and one thread per (texel, channel) adds its chunks.
-constexpr int RS_THREADS = 256;             // sort CTA: one thread per digit value
-constexpr int RS_RADIX = 256;
-constexpr int RS_WARPS = RS_THREADS / 32;
-constexpr int RS_TILE = 4096;               // lookups per sort tile, 16 per thread
 constexpr long long DET_CHUNK = 4096;       // terms per chunk of a texel's sum
 #ifndef DIRT_TEX_DET_GRID
 #define DIRT_TEX_DET_GRID 8192
 #endif
 constexpr unsigned DET_GRID = DIRT_TEX_DET_GRID;   // CTAs of the grid-stride passes
 
-__device__ __forceinline__ unsigned lookup_key(const float* indices, const TexDims& d, long long g, unsigned sentinel)
-{
-    const Taps t = taps_of(__ldg(indices + 2 * g), __ldg(indices + 2 * g + 1), d, g);
-    return t.valid ? (unsigned)(t.base + (long long)t.r0 * d.TW + t.c0) : sentinel;
-}
-
-// Exclusive scan of one value per thread over the RS_THREADS threads of the CTA; *total gets the sum.  Contains
-// __syncthreads(); warp_sums is RS_WARPS words of shared memory.
-__device__ __forceinline__ unsigned block_exclusive_scan(unsigned v, unsigned* warp_sums, unsigned* total)
-{
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    unsigned x = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const unsigned y = __shfl_up_sync(FULL, x, o);
-        if (lane >= o) x += y;
+// the sort key of lookup g: its base texel, or the sentinel for an invalid lookup
+struct LookupKey {
+    const float* indices;
+    TexDims d;
+    unsigned sentinel;
+    __device__ __forceinline__ unsigned operator()(long long g) const
+    {
+        const Taps t = taps_of(__ldg(indices + 2 * g), __ldg(indices + 2 * g + 1), d, g);
+        return t.valid ? (unsigned)(t.base + (long long)t.r0 * d.TW + t.c0) : sentinel;
     }
-    if (lane == 31) warp_sums[warp] = x;
-    __syncthreads();
-    unsigned before = 0, all = 0;
-#pragma unroll
-    for (int w = 0; w < RS_WARPS; ++w) {
-        const unsigned s = warp_sums[w];
-        before += w < warp ? s : 0u;
-        all += s;
-    }
-    __syncthreads();
-    *total = all;
-    return before + x - v;
-}
-
-// counts[digit][tile]: how many lookups of the tile have the digit (key >> shift) & 255
-template <bool FIRST>
-__global__ void __launch_bounds__(RS_THREADS) tex_sort_hist_kernel(const unsigned* __restrict__ keys,
-                                                                   const float* __restrict__ indices, TexDims d,
-                                                                   unsigned sentinel, int shift,
-                                                                   unsigned* __restrict__ counts, int tiles)
-{
-    __shared__ unsigned hist[RS_RADIX];
-    hist[threadIdx.x] = 0;
-    __syncthreads();
-    const long long first = (long long)blockIdx.x * RS_TILE;
-    for (int j = 0; j < RS_TILE / RS_THREADS; ++j) {
-        const long long i = first + j * RS_THREADS + threadIdx.x;
-        if (i < d.total) {
-            const unsigned key = FIRST ? lookup_key(indices, d, i, sentinel) : __ldg(keys + i);
-            atomicAdd(&hist[(key >> shift) & 255u], 1u);
-        }
-    }
-    __syncthreads();
-    counts[(size_t)threadIdx.x * tiles + blockIdx.x] = hist[threadIdx.x];
-}
-
-// one CTA per digit: its row of tile counts becomes the exclusive prefix, in place; the row's sum goes to digit_total
-__global__ void __launch_bounds__(RS_THREADS) tex_sort_scan_kernel(unsigned* __restrict__ counts,
-                                                                   unsigned* __restrict__ digit_total, int tiles)
-{
-    __shared__ unsigned warp_sums[RS_WARPS];
-    unsigned* row = counts + (size_t)blockIdx.x * tiles;
-    unsigned carry = 0;
-    for (int base = 0; base < tiles; base += RS_THREADS) {
-        const int i = base + threadIdx.x;
-        const unsigned v = i < tiles ? row[i] : 0u;
-        unsigned total;
-        const unsigned ex = block_exclusive_scan(v, warp_sums, &total);
-        if (i < tiles) row[i] = carry + ex;
-        carry += total;
-    }
-    if (threadIdx.x == 0) digit_total[blockIdx.x] = carry;
-}
-
-// Stable scatter of one tile.  Its lookups go in 16 rounds of RS_THREADS consecutive ones; in a round a lookup's slot is
-// the tile's running slot of its digit, plus the lookups of the lower warps with that digit, plus its rank among its
-// warp's lanes with that digit.  Thread dgt keeps the running slot of digit dgt.
-template <bool FIRST>
-__global__ void __launch_bounds__(RS_THREADS) tex_sort_scatter_kernel(const unsigned* __restrict__ keys_in,
-                                                                      const int* __restrict__ ids_in,
-                                                                      const float* __restrict__ indices, TexDims d,
-                                                                      unsigned sentinel, int shift,
-                                                                      const unsigned* __restrict__ counts,
-                                                                      const unsigned* __restrict__ digit_total, int tiles,
-                                                                      unsigned* __restrict__ keys_out,
-                                                                      int* __restrict__ ids_out)
-{
-    __shared__ unsigned warp_sums[RS_WARPS];
-    __shared__ unsigned wcount[RS_WARPS][RS_RADIX];
-    __shared__ unsigned woff[RS_WARPS][RS_RADIX];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, dgt = threadIdx.x;
-    unsigned all;
-    // the lookups of the smaller digits, then those of digit dgt in the earlier tiles
-    unsigned run = block_exclusive_scan(digit_total[dgt], warp_sums, &all) + counts[(size_t)dgt * tiles + blockIdx.x];
-#pragma unroll
-    for (int w = 0; w < RS_WARPS; ++w) wcount[w][dgt] = 0;
-    __syncthreads();
-    const long long first = (long long)blockIdx.x * RS_TILE;
-    for (int j = 0; j < RS_TILE / RS_THREADS; ++j) {
-        const long long i = first + j * RS_THREADS + threadIdx.x;
-        const bool live = i < d.total;
-        unsigned key = 0;
-        int id = 0;
-        if (live) {
-            key = FIRST ? lookup_key(indices, d, i, sentinel) : __ldg(keys_in + i);
-            id = FIRST ? (int)i : __ldg(ids_in + i);
-        }
-        const unsigned digit = live ? (key >> shift) & 255u : (unsigned)RS_RADIX;
-        const unsigned peers = __match_any_sync(FULL, digit);
-        const unsigned rank = __popc(peers & ((1u << lane) - 1u));
-        if (live && rank == 0) wcount[warp][digit] = __popc(peers);
-        __syncthreads();
-#pragma unroll
-        for (int w = 0; w < RS_WARPS; ++w) {
-            woff[w][dgt] = run;
-            run += wcount[w][dgt];
-            wcount[w][dgt] = 0;
-        }
-        __syncthreads();
-        if (live) {
-            const unsigned pos = woff[warp][digit] + rank;
-            keys_out[pos] = key;
-            ids_out[pos] = id;
-        }
-    }
-}
-
-// offsets[k] = the first position of the sorted keys that is >= k, k = 0 .. sentinel + 1
-__global__ void __launch_bounds__(TEX_THREADS) tex_segment_bounds_kernel(const unsigned* __restrict__ keys, long long n,
-                                                                         unsigned sentinel, int* __restrict__ offsets)
-{
-    const long long stride = (long long)gridDim.x * TEX_THREADS;
-    for (long long k = (long long)blockIdx.x * TEX_THREADS + threadIdx.x; k <= (long long)sentinel + 1; k += stride) {
-        long long lo = 0, hi = n;
-        while (lo < hi) {
-            const long long mid = (lo + hi) >> 1;
-            if (__ldg(keys + mid) < (unsigned)k) lo = mid + 1;
-            else hi = mid;
-        }
-        offsets[k] = (int)lo;
-    }
-}
+};
 
 // The term sequence of one texel: segment k (corner k) starts at sorted position s_k and holds terms [e_k, e_{k+1}) of
 // the sequence (e_0 = 0, e_4 = L).  Scalars, not arrays, so that nothing is indexed dynamically.
@@ -928,14 +730,6 @@ inline unsigned det_blocks(long long work, long long per_block)
     return (unsigned)(b < 1 ? 1 : (b < DET_GRID ? b : DET_GRID));
 }
 
-// sort passes: one per 8 bits of the largest key, the sentinel
-inline int sort_passes(unsigned sentinel)
-{
-    int bits = 0;
-    while (bits < 32 && (sentinel >> bits) != 0) ++bits;
-    return (bits + 7) / 8;
-}
-
 }  // namespace
 
 TexDetScratch carve_texture_det_scratch(void* base, const TexDims& d)
@@ -979,32 +773,16 @@ cudaError_t launch_texture_backward_deterministic(const float* texture, const fl
         return e;
     if ((e = cudaMemsetAsync(s.counters, 0, 2 * sizeof(int), stream)) != cudaSuccess) return e;
     const unsigned sentinel = (unsigned)(d.TB * d.texels);
-    const int tiles = (int)((d.total + RS_TILE - 1) / RS_TILE), passes = sort_passes(sentinel);
-    for (int p = 0; p < passes; ++p) {
-        const unsigned* kin = s.keys[(p + 1) & 1];
-        const int* iin = s.ids[(p + 1) & 1];
-        unsigned* kout = s.keys[p & 1];
-        int* iout = s.ids[p & 1];
-        if (p == 0) tex_sort_hist_kernel<true><<<tiles, RS_THREADS, 0, stream>>>(kin, indices, d, sentinel, 0, s.counts, tiles);
-        else tex_sort_hist_kernel<false><<<tiles, RS_THREADS, 0, stream>>>(kin, indices, d, sentinel, 8 * p, s.counts, tiles);
-        if ((e = cudaGetLastError()) != cudaSuccess) return e;
-        tex_sort_scan_kernel<<<RS_RADIX, RS_THREADS, 0, stream>>>(s.counts, s.digit_total, tiles);
-        if ((e = cudaGetLastError()) != cudaSuccess) return e;
-        if (p == 0)
-            tex_sort_scatter_kernel<true><<<tiles, RS_THREADS, 0, stream>>>(kin, iin, indices, d, sentinel, 0, s.counts,
-                                                                             s.digit_total, tiles, kout, iout);
-        else
-            tex_sort_scatter_kernel<false><<<tiles, RS_THREADS, 0, stream>>>(kin, iin, indices, d, sentinel, 8 * p, s.counts,
-                                                                              s.digit_total, tiles, kout, iout);
-        if ((e = cudaGetLastError()) != cudaSuccess) return e;
-        *launches += 3;
-    }
-    const unsigned* keys = s.keys[(passes - 1) & 1];
+    int last;
+    if ((e = sort_by_key(LookupKey{indices, d, sentinel}, d.total, sentinel, s.keys, s.ids, s.counts, s.digit_total, stream,
+                         launches, &last)) != cudaSuccess)
+        return e;
+    const unsigned* keys = s.keys[last];
     tex_segment_bounds_kernel<<<det_blocks((long long)sentinel + 2, TEX_THREADS), TEX_THREADS, 0, stream>>>(keys, d.total,
                                                                                                            sentinel, s.offsets);
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     TexDetArgs a;
-    a.indices = indices; a.grad_out = grad_out; a.ids = s.ids[(passes - 1) & 1]; a.offsets = s.offsets;
+    a.indices = indices; a.grad_out = grad_out; a.ids = s.ids[last]; a.offsets = s.offsets;
     a.grad_texture = grad_texture; a.counters = s.counters; a.long_list = s.long_list; a.owner = s.owner;
     a.partial = s.partial; a.d = d;
     const unsigned gather_blocks = det_blocks(sentinel, TEX_THREADS / 32);

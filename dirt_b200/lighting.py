@@ -14,6 +14,9 @@ the CUDA cube-map lookup; `cubemap_spherical_harmonics` projects a cube map onto
 `vertex_tangents` and `perturb_normals` (tangent-space normal mapping, DESIGN.md §7.14) run CUDA kernels
 (dirt_tangents_* and dirt_normal_map_*) in the shapes `tangents_route` and `cuda_route` accept, and their torch
 restatements (`_vertex_tangents`, `_perturb_normals`) otherwise.
+`shadow_map` rasterises a light-view map of (occupancy, depth) with `rasterise_batch`, and `shadow_visibility` looks it
+up with percentage-closer filtering: CUDA kernels (dirt_shadow_forward / _backward) in the shapes `shadow_route`
+accepts, its torch restatement `_shadow_visibility` otherwise; see DESIGN.md §7.15.
 """
 import math
 from collections import namedtuple
@@ -292,10 +295,13 @@ def _bvc(route):
 #   sizes(route): their size arguments;
 #   restate(*flags, route, *inputs): the torch restatement on the op's own inputs, in the output's shape;
 #   first_param: the index of the first per-item parameter.  The gradients of these parameters need a partials
-#     workspace of workspace_bytes(B, V, C) bytes, where workspace_bytes is an entry point; both are None for an op
-#     without such parameters, whose backward then takes no workspace.
-_PointOp = namedtuple('_PointOp', 'name forward backward inputs sizes restate first_param workspace_bytes',
-                      defaults=(None, None))
+#     workspace of workspace_bytes(*sizes(route)) bytes, where workspace_bytes is an entry point; both are None for an
+#     op without such parameters, whose backward then takes no workspace.
+#   deterministic: for an op whose backward uses float atomics, (entry point, scratch_bytes) of its deterministic
+#     backward, which takes the backward's arguments plus (scratch, scratch bytes) before the sizes and runs under
+#     torch.use_deterministic_algorithms(True); scratch_bytes(lib, route, want, *inputs) gives the bytes, 0 for none.
+_PointOp = namedtuple('_PointOp', 'name forward backward inputs sizes restate first_param workspace_bytes deterministic',
+                      defaults=(None, None, None))
 
 
 class _PointFunction(torch.autograd.Function):
@@ -334,13 +340,19 @@ class _PointFunction(torch.autograd.Function):
         lib = _lib.lib()
         workspace_args = ()
         if op.workspace_bytes is not None:
-            ws_bytes = int(getattr(lib, op.workspace_bytes)(*_bvc(route))) if any(want[op.first_param:]) else 0
+            ws_bytes = int(getattr(lib, op.workspace_bytes)(*op.sizes(route))) if any(want[op.first_param:]) else 0
             workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=dev) if ws_bytes else None
             workspace_args = (_ptr(workspace), ws_bytes)
+        entry, scratch_args = op.backward, ()
+        if op.deterministic is not None and torch.are_deterministic_algorithms_enabled():
+            entry, scratch_bytes = op.deterministic
+            sc_bytes = int(scratch_bytes(lib, route, want, *inputs))
+            scratch = torch.empty(sc_bytes, dtype=torch.uint8, device=dev) if sc_bytes else None
+            scratch_args = (_ptr(scratch), sc_bytes)
         grad_out = grad_out.to(torch.float32).contiguous()
         with torch.cuda.device(dev):
-            rc = getattr(lib, op.backward)(*op.inputs(*flags, route, *inputs), _ptr(grad_out), *[_ptr(g) for g in grads],
-                                           *workspace_args, *op.sizes(route), _stream(dev))
+            rc = getattr(lib, entry)(*op.inputs(*flags, route, *inputs), _ptr(grad_out), *[_ptr(g) for g in grads],
+                                     *workspace_args, *scratch_args, *op.sizes(route), _stream(dev))
         _lib.check(rc, op.name + 'Grad')
         return (None,) * 3 + tuple(grads)
 
@@ -960,3 +972,157 @@ def perturb_normals(normals, tangents, tangent_space_normals, name=None):
         return _perturb_normals(normals, tangents, tangent_space_normals)
     return _PointFunction.apply(_NORMAL_MAP, (), route, _rows(normals, 3), _rows(tangents, 4),
                                 _rows(tangent_space_normals, 3))
+
+
+# ---- shadow mapping (DESIGN.md §7.15) --------------------------------------------------------------------------------
+
+SHADOW_MAX_RADIUS = 3
+
+
+def shadow_map(vertices, faces, light_matrix, height, width):
+    """A shadow map: the mesh rasterised from the light, [*, height, width, 2] = (occupancy, depth) per texel.
+
+    vertices [*, V, 3|4] world positions (a w column is ignored), faces [F, 3] or [*, F, 3], light_matrix [*, 4, 4] or
+    [4, 4] world -> light clip (row vectors, as in `matrices`, e.g. a view matrix composed with
+    `orthographic_projection` for a directional light).  One `rasterise_batch` call over a zero background, with clip
+    vertices (p, 1) @ light_matrix and vertex colours (1, clip z): occupancy is exactly 1 on covered texels and 0
+    elsewhere, and depth is the interpolated clip z (0 where nothing is covered), exact for orthographic and perspective
+    lights alike because clip z is affine in the light's view space.  Gradients reach `vertices` and `light_matrix`
+    through the rasteriser's backward pass; the occupancy channel's carries the occluders' gradient (DESIGN.md §7.15).
+    This is the map format `shadow_visibility` reads.  Needs CUDA, as `rasterise_batch` does."""
+    from .rasterise_ops import rasterise_batch
+    vertices = torch.as_tensor(vertices, dtype=torch.float32)
+    dev = vertices.device
+    light_matrix = torch.as_tensor(light_matrix, dtype=torch.float32, device=dev)
+    faces = torch.as_tensor(faces, device=dev)
+    lead, V, F = vertices.shape[:-2], vertices.shape[-2], faces.shape[-2]
+    B = math.prod(lead)
+    p = vertices[..., :3]
+    clip = torch.matmul(torch.cat([p, torch.ones_like(p[..., :1])], -1), light_matrix)   # [*, V, 4]
+    colors = torch.stack([torch.ones_like(clip[..., 2]), clip[..., 2]], -1)
+    faces = faces.expand(lead + (F, 3)) if faces.dim() == 2 else faces
+    background = torch.zeros((B, height, width, 2), dtype=torch.float32, device=dev)
+    out = rasterise_batch(background, clip.reshape(B, V, 4), colors.reshape(B, V, 2), faces.reshape(B, F, 3))
+    return out.reshape(lead + (height, width, 2))
+
+
+def _shadow_visibility(positions, light_matrix, shadow_map, radius=1, softness=0., bias=0.):
+    """The torch restatement of `shadow_visibility`: its CPU implementation and its specification.  Keeps the dtype of
+    its inputs (the tests evaluate it in float64).  Points that are not looked up take safe values inside the `where`s,
+    so that their gradients are exactly 0 and not NaN."""
+    p = positions
+    SH, SW = shadow_map.shape[-3], shadow_map.shape[-2]
+    ones = torch.ones_like(p[..., :1])
+    with torch.no_grad():
+        h0 = torch.matmul(torch.cat([p, ones], -1), light_matrix)
+        ok = torch.isfinite(h0).all(-1) & (h0[..., 3] > 0)
+    p = torch.where(ok[..., None], p, 0.)
+    h = torch.matmul(torch.cat([p, ones], -1), light_matrix)
+    h = torch.where(ok[..., None], h, torch.tensor([0., 0., 0., 1.], dtype=h.dtype, device=h.device))
+    x, y, z, w = h.unbind(-1)
+    X = (x / w + 1.) * (0.5 * SW)
+    Yd = (1. - y / w) * (0.5 * SH)
+    valid = ok & (X >= 0) & (X < SW) & (Yd >= 0) & (Yd < SH)
+    u, v = torch.where(valid, X, 0.5) - 0.5, torch.where(valid, Yd, 0.5) - 0.5
+    c0, r0 = u.detach().floor(), v.detach().floor()
+    fc, fr = u - c0, v - r0
+    flat = shadow_map.reshape(shadow_map.shape[:-3] + (SH * SW, 2))
+
+    def texel(r, c):
+        idx = (r * SW + c).long()
+        if flat.dim() == 2:
+            return flat[idx]
+        return torch.gather(flat, -2, idx[..., None].expand(idx.shape + (2,)))
+
+    def weight(i, f):
+        return 1. - f if i == 0 else (f if i == 2 * radius + 1 else torch.ones_like(f))
+
+    vis = torch.zeros_like(fc)
+    for i in range(2 * radius + 2):
+        r = (r0 - radius + i).clamp(0, SH - 1)
+        for k in range(2 * radius + 2):
+            t = texel(r, (c0 - radius + k).clamp(0, SW - 1))
+            d = z - t[..., 1] - bias
+            step = torch.sigmoid(d / softness) if softness > 0 else (d > 0).to(d.dtype)
+            vis = vis + weight(i, fr) * weight(k, fc) * (1. - t[..., 0] * step)
+    vis = vis / (2 * radius + 1) ** 2
+    return torch.where(valid, vis, 1.)[..., None]
+
+
+def shadow_route(position_shape, matrix_shape, map_shape, devices):
+    """Whether a `shadow_visibility` call runs the CUDA kernels, decided from shapes and devices alone: positions
+    [*, N, 3], and light_matrix [*, 4, 4] with shadow_map [*, SH, SW, 2] (one per item) or [4, 4] with [SH, SW, 2]
+    (shared), all on one CUDA device.  Returns a Route (C = 1, the output's width; per_item = (matrix, map)) or None."""
+    map_shape = tuple(map_shape)
+    if len(map_shape) < 3 or map_shape[-1] != 2:
+        return None
+    route = cuda_route([position_shape], [(matrix_shape, (4, 4)), (map_shape, map_shape[-3:])], devices, [3])
+    if route is None or route.per_item[0] != route.per_item[1]:
+        return None
+    return route._replace(C=1)
+
+
+def _shadow_inputs(radius, softness, bias, route, positions, light_matrix, shadow_map):
+    """The input arguments of dirt_shadow_forward / _backward, in their order."""
+    return [_ptr(positions), _point_stride(positions), _ptr(light_matrix), _ptr(shadow_map), int(route.per_item[0]),
+            shadow_map.shape[-3], shadow_map.shape[-2], radius, softness, bias]
+
+
+def _restate_shadow(radius, softness, bias, route, positions, light_matrix, shadow_map):
+    """The restatement on the op's own inputs (flattened per-point rows, per-item matrix and map)."""
+    return _shadow_visibility(_unflat_points(positions, route), _unflat_item(light_matrix, route, route.per_item[0]),
+                              _unflat_item(shadow_map, route, route.per_item[1]), radius, softness, bias)
+
+
+def _shadow_scratch_bytes(lib, route, want, positions, light_matrix, shadow_map):
+    """The deterministic backward's scratch: needed only for the map gradient."""
+    if not want[2]:
+        return 0
+    return lib.dirt_shadow_backward_deterministic_bytes(route.B, route.V, int(route.per_item[0]), shadow_map.shape[-3],
+                                                        shadow_map.shape[-2])
+
+
+_SHADOW = _PointOp('ShadowVisibility', 'dirt_shadow_forward', 'dirt_shadow_backward', _shadow_inputs,
+                   lambda route: (route.B, route.V), _restate_shadow, first_param=1,
+                   workspace_bytes='dirt_shadow_workspace_bytes',
+                   deterministic=('dirt_shadow_backward_deterministic', _shadow_scratch_bytes))
+
+
+def shadow_visibility(positions, light_matrix, shadow_map, radius=1, softness=0., bias=0., name=None):
+    """The fraction of a light that reaches each point past the occluders of a shadow map, by percentage-closer
+    filtering.
+
+    positions [*, N, 3] world points; light_matrix [*, 4, 4] with shadow_map [*, SH, SW, 2] (one per item), or [4, 4]
+    with [SH, SW, 2] (shared): the matrix and the `shadow_map` output it was rendered with -> visibility [*, N, 1] in
+    [0, 1].  With (x, y, z, w) = (p, 1) @ light_matrix, the point falls at X = (x/w + 1) SW/2, Yd = (1 - y/w) SH/2 (the
+    texel the rasteriser covers there); the (2R+2)^2 texels around it, clamped into the map, each give
+    s = 1 - occupancy * step((z - depth - bias) / softness), and V is their box-of-bilinear average with 1-D weights
+    (1 - f, 1, ..., 1, f) / (2R+1) (radius R = 0: bilinear).  step is the logistic sigmoid for softness > 0 and the
+    Heaviside step (step(0) = 0) for softness = 0.  A point behind the light (w <= 0), with a non-finite coordinate or
+    outside the map is lit: V = 1, with no gradient.  Gradients reach the positions, the light matrix and both channels
+    of the map (none through the step for softness = 0; the occupancy gradient is what carries the occluders'
+    gradient); softness and bias are plain floats without gradient.
+
+    radius in 0..3, softness >= 0, bias >= 0.  On CUDA in the shapes `shadow_route` accepts fused kernels compute it,
+    reading G-buffer channel slices in place, with a bit-reproducible light-matrix gradient.  The map gradient is summed
+    with float atomics, or, under torch.use_deterministic_algorithms(True), by a sort of the points by texel and
+    fixed-order float64 sums, bit-reproducible.  Any other call runs the torch restatement `_shadow_visibility`
+    (DESIGN.md §7.15)."""
+    radius, softness, bias = int(radius), float(softness), float(bias)
+    if not 0 <= radius <= SHADOW_MAX_RADIUS:
+        raise ValueError('shadow_visibility: radius must be in 0..%d, got %d' % (SHADOW_MAX_RADIUS, radius))
+    if not (softness >= 0 and bias >= 0 and math.isfinite(softness) and math.isfinite(bias)):
+        raise ValueError('shadow_visibility: softness and bias must be finite and >= 0')
+    positions = torch.as_tensor(positions, dtype=torch.float32)
+    dev = positions.device
+    light_matrix = torch.as_tensor(light_matrix, dtype=torch.float32, device=dev)
+    shadow_map = torch.as_tensor(shadow_map, dtype=torch.float32, device=dev)
+    route = shadow_route(positions.shape, light_matrix.shape, shadow_map.shape,
+                         [t.device for t in (positions, light_matrix, shadow_map)])
+    if route is None:
+        return _shadow_visibility(positions, light_matrix, shadow_map, radius, softness, bias)
+    flat_map = _flat_item(shadow_map, route, route.per_item[1])
+    if flat_map.data_ptr() % 8:
+        flat_map = flat_map.clone()   # the kernels read float2 texels
+    return _PointFunction.apply(_SHADOW, (radius, softness, bias), route, _rows(positions, 3),
+                                _flat_item(light_matrix, route, route.per_item[0]), flat_map)

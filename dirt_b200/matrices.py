@@ -68,6 +68,23 @@ def perspective_projection(near, far, right, aspect, name=None):
     return out
 
 
+def orthographic_projection(left, right, bottom, top, near, far, name=None):
+    """OpenGL-convention orthographic matrices [A1..An,4,4] (glOrtho), in the [in, out] layout of
+    `perspective_projection`: view-space x in [left, right], y in [bottom, top] and z in [-near, -far] map to clip x, y,
+    z in [-1, 1], with w = 1.  The view looks along -z; a directional light's shadow map uses one."""
+    left, right, bottom, top, near, far = torch.broadcast_tensors(_t(left), _t(right), _t(bottom), _t(top), _t(near),
+                                                                  _t(far))
+    out = torch.zeros(near.shape + (4, 4), dtype=near.dtype, device=near.device)
+    out[..., 0, 0] = 2. / (right - left)
+    out[..., 1, 1] = 2. / (top - bottom)
+    out[..., 2, 2] = -2. / (far - near)
+    out[..., 3, 0] = -(right + left) / (right - left)
+    out[..., 3, 1] = -(top + bottom) / (top - bottom)
+    out[..., 3, 2] = -(far + near) / (far - near)
+    out[..., 3, 3] = 1.
+    return out
+
+
 def compose(*matrices):
     """Product of the given matrices, the first applied first (dirt/matrices.py:183-207)."""
     if len(matrices) == 0:

@@ -629,6 +629,50 @@ int dirt_normal_map_backward(const float* normals, long long normals_stride, con
                              const float* grad_out, float* grad_normals, float* grad_tangents, float* grad_samples,
                              int B, long long V, void* cuda_stream);
 
+/* Shadow-map visibility: a percentage-closer lookup of a light-view map, one value per point.  B items of V points:
+ *   positions            float32 [B*V, 3] world points, row stride positions_stride, unit stride along the row
+ *   light_matrix         float32 [B, 4, 4] (per_item) or [4, 4]: world -> light clip, row vectors ((p, 1) @ M)
+ *   shadow_map           float32 [B, SH, SW, 2] (per_item) or [SH, SW, 2], contiguous and 8-byte aligned: per texel
+ *                        (occupancy, depth), e.g. a rasterisation from the light with vertex colours (1, clip z)
+ *   out, grad_out        float32 [B*V], contiguous
+ * With (x, y, z, w) = (p, 1) @ M, X = (x/w + 1) (0.5 SW) and Yd = (1 - y/w) (0.5 SH) (the rasteriser's pixel rule;
+ * this chain is evaluated in double precision), u = X - 0.5, c0 = floor(u), fc = u - c0, and r0, fr the same of
+ * Yd - 0.5:
+ *   out = sum_i sum_k a_i b_k s_ik / (2R+1)^2 over rows r0-R+i and columns c0-R+k, i, k = 0 .. 2R+1, each clamped into
+ *   the map; a = (1 - fr, 1, ..., 1, fr), b = (1 - fc, 1, ..., 1, fc);
+ *   s_ik = 1 - o_ik step((z - z_ik - bias) / softness), step the logistic sigmoid for softness > 0, and for
+ *   softness = 0 the Heaviside step with step(0) = 0.
+ * A non-finite (x, y, z, w), w <= 0, or (X, Yd) outside [0, SW) x [0, SH) gives out = 1 and no gradient.
+ * Backward: the gradients torch autograd gives the same expressions (none through the step for softness = 0).
+ * grad_positions [B*V, 3] is contiguous, grad_light_matrix and grad_shadow_map (8-byte aligned) have the shapes of
+ * their inputs; each may be NULL, and its work is skipped.  The light-matrix gradient is summed in a fixed order
+ * (per-CTA partials in the workspace, of at least dirt_shadow_workspace_bytes(B, V) bytes, needed only when it is
+ * wanted), so repeated calls give bit-identical results.  The map gradient is summed with float atomics after
+ * aggregation inside each warp: its last bits may differ between calls (see dirt_shadow_backward_deterministic).
+ * B = 0 or V = 0: nothing is launched (the backward call still zeroes wanted map and matrix gradients).
+ * 0 <= radius <= 3, softness and bias finite and >= 0, SH, SW > 0; all pointers 4-byte aligned; row stride >= 0.
+ * dirt_shadow_backward_deterministic: the same gradients with the map gradient summed without float atomics, so that
+ * repeated calls give bit-identical results.  The points are sorted by base texel (r0, c0), and each texel sums, in
+ * float64 from +0.0 and rounded once, the backward call's fp32 terms in this order: tap row i, the base rows whose tap
+ * row i clamps onto it (ascending), tap column k, the base columns likewise, then the points of that base in ascending
+ * id b*V + n (DESIGN.md §7.15).  Its scratch, of at least dirt_shadow_backward_deterministic_bytes(B, V, per_item, SH,
+ * SW) bytes, is needed only when grad_shadow_map is wanted; B*V and (B | 1)(SH + 1)(SW + 1) below 2^31. */
+size_t dirt_shadow_workspace_bytes(int B, long long V);
+size_t dirt_shadow_backward_deterministic_bytes(int B, long long V, int per_item, int SH, int SW);
+int dirt_shadow_forward(const float* positions, long long positions_stride, const float* light_matrix,
+                        const float* shadow_map, int per_item, int SH, int SW, int radius, float softness, float bias,
+                        float* out, int B, long long V, void* cuda_stream);
+int dirt_shadow_backward(const float* positions, long long positions_stride, const float* light_matrix,
+                         const float* shadow_map, int per_item, int SH, int SW, int radius, float softness, float bias,
+                         const float* grad_out, float* grad_positions, float* grad_light_matrix, float* grad_shadow_map,
+                         void* workspace, size_t workspace_bytes, int B, long long V, void* cuda_stream);
+int dirt_shadow_backward_deterministic(const float* positions, long long positions_stride, const float* light_matrix,
+                                       const float* shadow_map, int per_item, int SH, int SW, int radius,
+                                       float softness, float bias, const float* grad_out, float* grad_positions,
+                                       float* grad_light_matrix, float* grad_shadow_map, void* workspace,
+                                       size_t workspace_bytes, void* scratch, size_t scratch_bytes, int B, long long V,
+                                       void* cuda_stream);
+
 /* Number of kernels the last call on this thread launched (bench.py's gpu_launches). */
 int dirt_last_launch_count(void);
 
