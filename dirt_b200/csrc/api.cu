@@ -69,6 +69,32 @@ extern "C" float dirt_kernel_timer_elapsed_ms(void)
 
 extern "C" int dirt_last_launch_count(void) { return t_last_launches; }
 
+// gradient outputs may be NULL (not wanted), but not misaligned
+static bool aligned(std::initializer_list<const void*> ptrs)
+{
+    for (const void* p : ptrs)
+        if ((uintptr_t)p % 4) return false;
+    return true;
+}
+
+// buffers a call reads or writes: DIRT_ERR_NULL_POINTER if one is NULL, else DIRT_ERR_MISALIGNED if one is not 4-byte
+// aligned
+static int required_check(std::initializer_list<const void*> ptrs)
+{
+    for (const void* p : ptrs)
+        if (!p) return DIRT_ERR_NULL_POINTER;
+    return aligned(ptrs) ? DIRT_OK : DIRT_ERR_MISALIGNED;
+}
+
+// a caller-owned workspace or scratch of `bytes` bytes that a call needs `need` of: DIRT_ERR_NULL_POINTER if it is NULL,
+// else DIRT_ERR_MISALIGNED if it is not 256-byte aligned, else DIRT_ERR_WORKSPACE_TOO_SMALL if it is too small
+static int scratch_check(void* scratch, size_t bytes, size_t need)
+{
+    if (!scratch) return DIRT_ERR_NULL_POINTER;
+    if ((uintptr_t)scratch % 256) return DIRT_ERR_MISALIGNED;
+    return bytes < need ? DIRT_ERR_WORKSPACE_TOO_SMALL : DIRT_OK;
+}
+
 static bool shape_ok(int B, int H, int W, int C, int V, int F)
 {
     if (B < 0 || H <= 0 || W <= 0 || C <= 0 || V < 0 || F < 0) return false;
@@ -125,11 +151,8 @@ extern "C" size_t dirt_workspace_bytes_min(int B, int H, int W, int C, int V, in
 static int check_workspace(void* workspace, size_t workspace_bytes, int B, int H, int W, int C, int V, int F,
                            bool needs_face_id_scratch = false)
 {
-    if (!workspace) return DIRT_ERR_NULL_POINTER;
-    if ((uintptr_t)workspace % 256 != 0) return DIRT_ERR_MISALIGNED;
-    const size_t need = needs_face_id_scratch ? dirt_workspace_bytes(B, H, W, C, V, F) : dirt_workspace_bytes_min(B, H, W, C, V, F);
-    if (workspace_bytes < need) return DIRT_ERR_WORKSPACE_TOO_SMALL;
-    return DIRT_OK;
+    return scratch_check(workspace, workspace_bytes, needs_face_id_scratch ? dirt_workspace_bytes(B, H, W, C, V, F)
+                                                                           : dirt_workspace_bytes_min(B, H, W, C, V, F));
 }
 
 #define CUDA_TRY(expr)                                   \
@@ -213,9 +236,8 @@ static int backward_impl(const float* vertices, const int32_t* faces, const floa
     rc = check_workspace(workspace, workspace_bytes, B, H, W, C, V, F, face_ids == nullptr);
     if (rc != DIRT_OK) return rc;
     if (deterministic) {
-        if (!scratch) return DIRT_ERR_NULL_POINTER;
-        if ((uintptr_t)scratch % 256 != 0) return DIRT_ERR_MISALIGNED;
-        if (scratch_bytes < dirt_rasterise_backward_deterministic_bytes(B, H, W, C, V, F)) return DIRT_ERR_WORKSPACE_TOO_SMALL;
+        rc = scratch_check(scratch, scratch_bytes, dirt_rasterise_backward_deterministic_bytes(B, H, W, C, V, F));
+        if (rc != DIRT_OK) return rc;
     }
     cudaStream_t stream = (cudaStream_t)cuda_stream;
     const Workspace ws = carve_workspace(workspace, B, H, W, C, V, F);
@@ -351,8 +373,8 @@ extern "C" int dirt_texture_sample(const float* texture, const float* indices, f
     t_last_launches = 0;
     if (!texture_shape_ok(TB, TH, TW, C, B, N, mode)) return DIRT_ERR_BAD_SHAPE;
     if (B == 0 || N == 0) return DIRT_OK;
-    if (!texture || !indices || !out) return DIRT_ERR_NULL_POINTER;
-    if ((uintptr_t)texture % 4 || (uintptr_t)indices % 4 || (uintptr_t)out % 4) return DIRT_ERR_MISALIGNED;
+    const int rc = required_check({texture, indices, out});
+    if (rc != DIRT_OK) return rc;
     CUDA_TRY(launch_texture_forward(texture, indices, out, make_tex_dims(TB, TH, TW, C, B, N, mode), (cudaStream_t)cuda_stream,
                                     &launches));
     t_last_launches = launches;
@@ -371,9 +393,7 @@ extern "C" int dirt_texture_sample_backward(const float* texture, const float* i
         if (!indices || !grad_out) return DIRT_ERR_NULL_POINTER;
         if (grad_indices && mode == DIRT_TEXTURE_BILINEAR && !texture) return DIRT_ERR_NULL_POINTER;
     }
-    if ((uintptr_t)texture % 4 || (uintptr_t)indices % 4 || (uintptr_t)grad_out % 4 || (uintptr_t)grad_texture % 4 ||
-        (uintptr_t)grad_indices % 4)
-        return DIRT_ERR_MISALIGNED;
+    if (!aligned({texture, indices, grad_out, grad_texture, grad_indices})) return DIRT_ERR_MISALIGNED;
     // with no lookups only the memset of grad_texture is enqueued
     CUDA_TRY(launch_texture_backward(texture, indices, grad_out, grad_texture, grad_indices, d, (cudaStream_t)cuda_stream,
                                      &launches));
@@ -407,16 +427,13 @@ extern "C" int dirt_texture_sample_backward_deterministic(const float* texture, 
         if (!indices || !grad_out) return DIRT_ERR_NULL_POINTER;
         if (grad_indices && mode == DIRT_TEXTURE_BILINEAR && !texture) return DIRT_ERR_NULL_POINTER;
     }
-    if ((uintptr_t)texture % 4 || (uintptr_t)indices % 4 || (uintptr_t)grad_out % 4 || (uintptr_t)grad_texture % 4 ||
-        (uintptr_t)grad_indices % 4)
-        return DIRT_ERR_MISALIGNED;
+    if (!aligned({texture, indices, grad_out, grad_texture, grad_indices})) return DIRT_ERR_MISALIGNED;
     // only the texture gradient of a call with lookups sorts them
     const bool sorts = grad_texture && d.total > 0;
     if (sorts) {
-        if (!scratch) return DIRT_ERR_NULL_POINTER;
-        if ((uintptr_t)scratch % 256) return DIRT_ERR_MISALIGNED;
-        if (scratch_bytes < dirt_texture_sample_backward_deterministic_bytes(TB, TH, TW, C, B, N, mode))
-            return DIRT_ERR_WORKSPACE_TOO_SMALL;
+        const int rc = scratch_check(scratch, scratch_bytes,
+                                     dirt_texture_sample_backward_deterministic_bytes(TB, TH, TW, C, B, N, mode));
+        if (rc != DIRT_OK) return rc;
     }
     CUDA_TRY(launch_texture_backward_deterministic(texture, indices, grad_out, grad_texture, grad_indices, d,
                                                    carve_texture_det_scratch(sorts ? scratch : nullptr, d),
@@ -448,8 +465,8 @@ extern "C" int dirt_texture_mip_build(const float* texture, float* pyramid, int 
     t_last_launches = 0;
     if (TB < 0 || !texture_shape_ok(TB, TH, TW, C, TB, 0, DIRT_TEXTURE_BILINEAR)) return DIRT_ERR_BAD_SHAPE;
     if (TB == 0 || mip_levels(TH, TW) == 1) return DIRT_OK;
-    if (!texture || !pyramid) return DIRT_ERR_NULL_POINTER;
-    if ((uintptr_t)texture % 4 || (uintptr_t)pyramid % 4) return DIRT_ERR_MISALIGNED;
+    const int rc = required_check({texture, pyramid});
+    if (rc != DIRT_OK) return rc;
     CUDA_TRY(launch_texture_mip_build(texture, pyramid, make_tex_dims(TB, TH, TW, C, TB, 0, DIRT_TEXTURE_BILINEAR),
                                       (cudaStream_t)cuda_stream, &launches));
     t_last_launches = launches;
@@ -465,9 +482,7 @@ extern "C" int dirt_texture_sample_trilinear(const float* texture, const float* 
     if (!mip_shape_ok(TB, TH, TW, C, B, N)) return DIRT_ERR_BAD_SHAPE;
     if (B == 0 || N == 0) return DIRT_OK;
     if (!texture || !indices || !derivatives || !out || (!pyramid && mip_levels(TH, TW) > 1)) return DIRT_ERR_NULL_POINTER;
-    if ((uintptr_t)texture % 4 || (uintptr_t)pyramid % 4 || (uintptr_t)indices % 4 || (uintptr_t)derivatives % 4 ||
-        (uintptr_t)out % 4)
-        return DIRT_ERR_MISALIGNED;
+    if (!aligned({texture, pyramid, indices, derivatives, out})) return DIRT_ERR_MISALIGNED;
     CUDA_TRY(launch_texture_trilinear_forward(texture, pyramid, indices, derivatives, out,
                                               make_tex_dims(TB, TH, TW, C, B, N, DIRT_TEXTURE_BILINEAR),
                                               (cudaStream_t)cuda_stream, &launches));
@@ -502,16 +517,14 @@ extern "C" int dirt_texture_sample_trilinear_backward(const float* texture, cons
         if (!indices || !derivatives || !grad_out) return DIRT_ERR_NULL_POINTER;
         if (grad_indices && (!texture || (!pyramid && L > 1))) return DIRT_ERR_NULL_POINTER;
     }
-    if ((uintptr_t)texture % 4 || (uintptr_t)pyramid % 4 || (uintptr_t)indices % 4 || (uintptr_t)derivatives % 4 ||
-        (uintptr_t)grad_out % 4 || (uintptr_t)grad_texture % 4 || (uintptr_t)grad_indices % 4)
-        return DIRT_ERR_MISALIGNED;
+    if (!aligned({texture, pyramid, indices, derivatives, grad_out, grad_texture, grad_indices})) return DIRT_ERR_MISALIGNED;
     // the scratch holds the pyramid's gradients (default) or the per-level passes (deterministic)
     const bool det = deterministic && grad_texture && d.total > 0;
     const bool uses_scratch = grad_texture && d.total > 0 && (det || L > 1);
     if (uses_scratch) {
-        if (!scratch) return DIRT_ERR_NULL_POINTER;
-        if ((uintptr_t)scratch % 256) return DIRT_ERR_MISALIGNED;
-        if (scratch_bytes < dirt_texture_sample_trilinear_backward_bytes(TB, TH, TW, C, B, N, det)) return DIRT_ERR_WORKSPACE_TOO_SMALL;
+        const int rc = scratch_check(scratch, scratch_bytes,
+                                     dirt_texture_sample_trilinear_backward_bytes(TB, TH, TW, C, B, N, det));
+        if (rc != DIRT_OK) return rc;
     }
     CUDA_TRY(launch_texture_trilinear_backward(texture, pyramid, indices, derivatives, grad_out, grad_texture, grad_indices, d,
                                                det, carve_texture_mip_scratch(uses_scratch ? scratch : nullptr, d, det),
@@ -548,9 +561,8 @@ extern "C" int dirt_cubemap_sample(const float* cubemap, const float* directions
     t_last_launches = 0;
     if (!cubemap_shape_ok(TB, S, C, B, N, mode)) return DIRT_ERR_BAD_SHAPE;
     if (B == 0 || N == 0) return DIRT_OK;
-    if (!cubemap || !directions || !atlas || !out) return DIRT_ERR_NULL_POINTER;
-    if ((uintptr_t)cubemap % 4 || (uintptr_t)directions % 4 || (uintptr_t)atlas % 4 || (uintptr_t)out % 4)
-        return DIRT_ERR_MISALIGNED;
+    const int rc = required_check({cubemap, directions, atlas, out});
+    if (rc != DIRT_OK) return rc;
     CUDA_TRY(launch_cubemap_forward(cubemap, directions, atlas, out, cubemap_dims(TB, S, C, B, N, mode),
                                     (cudaStream_t)cuda_stream, &launches));
     t_last_launches = launches;
@@ -578,16 +590,13 @@ extern "C" int dirt_cubemap_sample_backward(const float* atlas, const float* dir
         if (!directions || !grad_out) return DIRT_ERR_NULL_POINTER;
         if (grad_directions && mode == DIRT_TEXTURE_BILINEAR && !atlas) return DIRT_ERR_NULL_POINTER;
     }
-    if ((uintptr_t)atlas % 4 || (uintptr_t)directions % 4 || (uintptr_t)grad_out % 4 || (uintptr_t)grad_cubemap % 4 ||
-        (uintptr_t)grad_directions % 4)
-        return DIRT_ERR_MISALIGNED;
+    if (!aligned({atlas, directions, grad_out, grad_cubemap, grad_directions})) return DIRT_ERR_MISALIGNED;
     // the scratch holds the atlas's gradient (and the deterministic path's per-face passes)
     const bool det = deterministic && grad_cubemap && d.total > 0;
     const bool uses_scratch = grad_cubemap && d.total > 0;
     if (uses_scratch) {
-        if (!scratch) return DIRT_ERR_NULL_POINTER;
-        if ((uintptr_t)scratch % 256) return DIRT_ERR_MISALIGNED;
-        if (scratch_bytes < dirt_cubemap_sample_backward_bytes(TB, S, C, B, N, mode, det)) return DIRT_ERR_WORKSPACE_TOO_SMALL;
+        const int rc = scratch_check(scratch, scratch_bytes, dirt_cubemap_sample_backward_bytes(TB, S, C, B, N, mode, det));
+        if (rc != DIRT_OK) return rc;
     }
     CUDA_TRY(launch_cubemap_backward(atlas, directions, grad_out, grad_cubemap, grad_directions, d, det,
                                      carve_cubemap_scratch(uses_scratch ? scratch : nullptr, d, det),
@@ -617,10 +626,8 @@ extern "C" int dirt_cubemap_sample_trilinear(const float* cubemap, const float* 
     t_last_launches = 0;
     if (!cubemap_mip_shape_ok(TB, S, C, B, N)) return DIRT_ERR_BAD_SHAPE;
     if (B == 0 || N == 0) return DIRT_OK;
-    if (!cubemap || !directions || !lod || !atlas || !out) return DIRT_ERR_NULL_POINTER;
-    if ((uintptr_t)cubemap % 4 || (uintptr_t)directions % 4 || (uintptr_t)lod % 4 || (uintptr_t)atlas % 4 ||
-        (uintptr_t)out % 4)
-        return DIRT_ERR_MISALIGNED;
+    const int rc = required_check({cubemap, directions, lod, atlas, out});
+    if (rc != DIRT_OK) return rc;
     CUDA_TRY(launch_cubemap_mip_forward(cubemap, directions, lod, atlas, out,
                                         cubemap_dims(TB, S, C, B, N, DIRT_TEXTURE_BILINEAR), (cudaStream_t)cuda_stream,
                                         &launches));
@@ -651,17 +658,13 @@ extern "C" int dirt_cubemap_sample_trilinear_backward(const float* atlas, const 
         if (!directions || !lod || !grad_out) return DIRT_ERR_NULL_POINTER;
         if ((grad_directions || grad_lod) && !atlas) return DIRT_ERR_NULL_POINTER;
     }
-    if ((uintptr_t)atlas % 4 || (uintptr_t)directions % 4 || (uintptr_t)lod % 4 || (uintptr_t)grad_out % 4 ||
-        (uintptr_t)grad_cubemap % 4 || (uintptr_t)grad_directions % 4 || (uintptr_t)grad_lod % 4)
-        return DIRT_ERR_MISALIGNED;
+    if (!aligned({atlas, directions, lod, grad_out, grad_cubemap, grad_directions, grad_lod})) return DIRT_ERR_MISALIGNED;
     // the scratch holds the atlas's and the pyramid's gradients (and the deterministic path's per-level passes)
     const bool det = deterministic && grad_cubemap && d.total > 0;
     const bool uses_scratch = grad_cubemap && d.total > 0;
     if (uses_scratch) {
-        if (!scratch) return DIRT_ERR_NULL_POINTER;
-        if ((uintptr_t)scratch % 256) return DIRT_ERR_MISALIGNED;
-        if (scratch_bytes < dirt_cubemap_sample_trilinear_backward_bytes(TB, S, C, B, N, det))
-            return DIRT_ERR_WORKSPACE_TOO_SMALL;
+        const int rc = scratch_check(scratch, scratch_bytes, dirt_cubemap_sample_trilinear_backward_bytes(TB, S, C, B, N, det));
+        if (rc != DIRT_OK) return rc;
     }
     CUDA_TRY(launch_cubemap_mip_backward(atlas, directions, lod, grad_out, grad_cubemap, grad_directions, grad_lod, d, det,
                                          carve_cubemap_mip_scratch(uses_scratch ? scratch : nullptr, d, det),
@@ -691,8 +694,9 @@ extern "C" int dirt_cubemap_ggx_prefilter(const float* cubemap, float* atlas, in
     t_last_launches = 0;
     if (TB < 0 || !cubemap_ggx_shape_ok(TB, S, C, TB, 0)) return DIRT_ERR_BAD_SHAPE;
     if (TB == 0) return DIRT_OK;
-    if (!cubemap || !atlas) return DIRT_ERR_NULL_POINTER;
-    if ((uintptr_t)cubemap % 4 || (uintptr_t)atlas % 16) return DIRT_ERR_MISALIGNED;
+    const int rc = required_check({cubemap, atlas});
+    if (rc != DIRT_OK) return rc;
+    if ((uintptr_t)atlas % 16) return DIRT_ERR_MISALIGNED;
     CUDA_TRY(launch_ggx_prefilter(cubemap, atlas, cubemap_dims(TB, S, C, TB, 0, DIRT_TEXTURE_BILINEAR),
                                   (cudaStream_t)cuda_stream, &launches));
     t_last_launches = launches;
@@ -706,10 +710,9 @@ extern "C" int dirt_cubemap_sample_ggx(const float* cubemap, const float* direct
     t_last_launches = 0;
     if (!cubemap_ggx_shape_ok(TB, S, C, B, N)) return DIRT_ERR_BAD_SHAPE;
     if (B == 0 || N == 0) return DIRT_OK;
-    if (!cubemap || !directions || !lod || !atlas || !out) return DIRT_ERR_NULL_POINTER;
-    if ((uintptr_t)cubemap % 4 || (uintptr_t)directions % 4 || (uintptr_t)lod % 4 || (uintptr_t)atlas % 16 ||
-        (uintptr_t)out % 4)
-        return DIRT_ERR_MISALIGNED;
+    const int rc = required_check({cubemap, directions, lod, atlas, out});
+    if (rc != DIRT_OK) return rc;
+    if ((uintptr_t)atlas % 16) return DIRT_ERR_MISALIGNED;
     CUDA_TRY(launch_cubemap_ggx_forward(cubemap, directions, lod, atlas, out,
                                         cubemap_dims(TB, S, C, B, N, DIRT_TEXTURE_BILINEAR), (cudaStream_t)cuda_stream,
                                         &launches));
@@ -740,15 +743,13 @@ extern "C" int dirt_cubemap_sample_ggx_backward(const float* atlas, const float*
         // the lookups read the atlas; the prefilter's adjoint reads its normalisers and texel table
         if ((grad_directions || grad_lod || grad_cubemap) && !atlas) return DIRT_ERR_NULL_POINTER;
     }
-    if ((uintptr_t)atlas % 16 || (uintptr_t)directions % 4 || (uintptr_t)lod % 4 || (uintptr_t)grad_out % 4 ||
-        (uintptr_t)grad_cubemap % 4 || (uintptr_t)grad_directions % 4 || (uintptr_t)grad_lod % 4)
+    if (!aligned({directions, lod, grad_out, grad_cubemap, grad_directions, grad_lod}) || (uintptr_t)atlas % 16)
         return DIRT_ERR_MISALIGNED;
     const bool det = deterministic && grad_cubemap && d.total > 0;
     const bool uses_scratch = grad_cubemap && d.total > 0;
     if (uses_scratch) {
-        if (!scratch) return DIRT_ERR_NULL_POINTER;
-        if ((uintptr_t)scratch % 256) return DIRT_ERR_MISALIGNED;
-        if (scratch_bytes < dirt_cubemap_sample_ggx_backward_bytes(TB, S, C, B, N, det)) return DIRT_ERR_WORKSPACE_TOO_SMALL;
+        const int rc = scratch_check(scratch, scratch_bytes, dirt_cubemap_sample_ggx_backward_bytes(TB, S, C, B, N, det));
+        if (rc != DIRT_OK) return rc;
     }
     CUDA_TRY(launch_cubemap_ggx_backward(atlas, directions, lod, grad_out, grad_cubemap, grad_directions, grad_lod, d, det,
                                          carve_cubemap_ggx_scratch(uses_scratch ? scratch : nullptr, d, det),
@@ -823,8 +824,8 @@ extern "C" int dirt_latlong_to_cubemap(const float* panorama, float* cubemap, in
     t_last_launches = 0;
     if (!latlong_shape_ok(TB, H, W, S, C)) return DIRT_ERR_BAD_SHAPE;
     if (TB == 0) return DIRT_OK;
-    if (!panorama || !cubemap) return DIRT_ERR_NULL_POINTER;
-    if ((uintptr_t)panorama % 4 || (uintptr_t)cubemap % 4) return DIRT_ERR_MISALIGNED;
+    const int rc = required_check({panorama, cubemap});
+    if (rc != DIRT_OK) return rc;
     CUDA_TRY(launch_latlong_forward(panorama, cubemap, TB, H, W, S, C, (cudaStream_t)cuda_stream, &launches));
     t_last_launches = launches;
     return DIRT_OK;
@@ -837,8 +838,8 @@ extern "C" int dirt_latlong_to_cubemap_backward(const float* grad_cubemap, float
     t_last_launches = 0;
     if (!latlong_shape_ok(TB, H, W, S, C)) return DIRT_ERR_BAD_SHAPE;
     if (TB == 0) return DIRT_OK;
-    if (!grad_cubemap || !grad_panorama) return DIRT_ERR_NULL_POINTER;
-    if ((uintptr_t)grad_cubemap % 4 || (uintptr_t)grad_panorama % 4) return DIRT_ERR_MISALIGNED;
+    const int rc = required_check({grad_cubemap, grad_panorama});
+    if (rc != DIRT_OK) return rc;
     CUDA_TRY(launch_latlong_backward(grad_cubemap, grad_panorama, TB, H, W, S, C, (cudaStream_t)cuda_stream, &launches));
     t_last_launches = launches;
     return DIRT_OK;
@@ -850,8 +851,8 @@ extern "C" int dirt_ggx_brdf_table(float* table, int N, void* cuda_stream)
     t_last_launches = 0;
     if (N < 0 || N > 4096) return DIRT_ERR_BAD_SHAPE;
     if (N == 0) return DIRT_OK;
-    if (!table) return DIRT_ERR_NULL_POINTER;
-    if ((uintptr_t)table % 4) return DIRT_ERR_MISALIGNED;
+    const int rc = required_check({table});
+    if (rc != DIRT_OK) return rc;
     CUDA_TRY(launch_ggx_brdf_table(table, N, (cudaStream_t)cuda_stream, &launches));
     t_last_launches = launches;
     return DIRT_OK;
@@ -875,23 +876,6 @@ static bool points_shape_ok(int B, long long V, double width, std::initializer_l
 static bool light_partials_ok(int B, long long V, int C)
 {
     return (double)B * light_chunks(V) * (LIGHT_FIXED_PARAMS + (double)C) * sizeof(float) <= 4.0e18;
-}
-
-// gradient outputs may be NULL (not wanted), but not misaligned
-static bool aligned(std::initializer_list<const void*> ptrs)
-{
-    for (const void* p : ptrs)
-        if ((uintptr_t)p % 4) return false;
-    return true;
-}
-
-// buffers a call reads or writes: DIRT_ERR_NULL_POINTER if one is NULL, else DIRT_ERR_MISALIGNED if one is not 4-byte
-// aligned
-static int required_check(std::initializer_list<const void*> ptrs)
-{
-    for (const void* p : ptrs)
-        if (!p) return DIRT_ERR_NULL_POINTER;
-    return aligned(ptrs) ? DIRT_OK : DIRT_ERR_MISALIGNED;
 }
 
 // the partials workspace of the per-item parameter gradients, `need` bytes, set as *partial when it passes

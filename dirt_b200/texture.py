@@ -33,6 +33,23 @@ def uvs_to_pixel_indices(uvs, texture_shape, mode='repeat'):
     raise NotImplementedError(mode)
 
 
+def _backward(device, want_table, entry, size, op, too_large):
+    """Runs a lookup's backward entry point, `entry(deterministic, scratch, scratch_bytes, stream)`, on `device`, with
+    the scratch of `size(deterministic)` bytes it asks for.  The deterministic (sorted) path is taken when the gradient
+    of the texture or cube map is wanted under torch.use_deterministic_algorithms(True); the gradients of the lookup
+    coordinates alone are per lookup and already reproducible.  `too_large` names the shapes a deterministic call
+    refuses with ERR_BAD_SHAPE, for the RuntimeError that then names the flag."""
+    deterministic = bool(want_table and torch.are_deterministic_algorithms_enabled())
+    scratch_bytes = int(size(deterministic))
+    scratch = torch.empty(scratch_bytes, dtype=torch.uint8, device=device) if scratch_bytes else None
+    with torch.cuda.device(device):
+        rc = entry(deterministic, _ptr(scratch), scratch_bytes, _stream_ptr(device))
+    if deterministic and rc == _lib.ERR_BAD_SHAPE:
+        # the shapes passed the forward call: what fails are the sorted path's 32-bit limits
+        raise RuntimeError(too_large + ', but torch.use_deterministic_algorithms(True) is set')
+    _lib.check(rc, op)
+
+
 class _SampleTexture(torch.autograd.Function):
     """dirt_texture_sample, or for mode 'trilinear' dirt_texture_mip_build then dirt_texture_sample_trilinear, with the
     gradient.  texture [TB, TH, TW, C], indices [B, N, 2], derivatives [B, N, 4] ('trilinear' only), contiguous fp32
@@ -75,32 +92,23 @@ class _SampleTexture(torch.autograd.Function):
         grad_out = grad_out.contiguous().to(torch.float32)
         grad_texture = torch.empty_like(texture) if want_texture else None
         grad_indices = torch.empty_like(indices) if want_indices else None
-        # grad_indices alone is per lookup and already reproducible; grad_texture needs the sorted path
-        deterministic = bool(want_texture and torch.are_deterministic_algorithms_enabled())
-        with torch.cuda.device(indices.device):
-            stream = _stream_ptr(indices.device)
-            if ctx.mode == 'trilinear':
-                scratch_bytes = int(L.dirt_texture_sample_trilinear_backward_bytes(TB, TH, TW, C, B, N, int(deterministic)))
-                scratch = torch.empty(scratch_bytes, dtype=torch.uint8, device=indices.device) if scratch_bytes else None
-                rc = L.dirt_texture_sample_trilinear_backward(
-                    _ptr(texture), _ptr(pyramid), _ptr(indices), _ptr(derivatives), _ptr(grad_out), _ptr(grad_texture),
-                    _ptr(grad_indices), TB, TH, TW, C, B, N, int(deterministic), _ptr(scratch), scratch_bytes, stream)
-            elif deterministic:
-                scratch_bytes = max(int(L.dirt_texture_sample_backward_deterministic_bytes(TB, TH, TW, C, B, N, ctx.mode)), 256)
-                scratch = torch.empty(scratch_bytes, dtype=torch.uint8, device=indices.device)
-                rc = L.dirt_texture_sample_backward_deterministic(
-                    _ptr(texture), _ptr(indices), _ptr(grad_out), _ptr(grad_texture), _ptr(grad_indices), TB, TH, TW, C, B, N,
-                    ctx.mode, _ptr(scratch), scratch_bytes, stream)
-            else:
-                rc = L.dirt_texture_sample_backward(_ptr(texture), _ptr(indices), _ptr(grad_out), _ptr(grad_texture),
-                                                    _ptr(grad_indices), TB, TH, TW, C, B, N, ctx.mode, stream)
-        if deterministic and rc == _lib.ERR_BAD_SHAPE:
-            # the shapes passed the forward call: what fails are the sorted path's 32-bit limits
-            raise RuntimeError(
-                'sample_texture backward: the texture gradient has no deterministic implementation for %d lookups '
-                'into %d x %d x %d texels (it needs fewer than 2^31 of each), but '
-                'torch.use_deterministic_algorithms(True) is set' % (B * N, TB, TH, TW))
-        _lib.check(rc, 'SampleTextureGrad')
+        if ctx.mode == 'trilinear':
+            ptrs = [_ptr(t) for t in (texture, pyramid, indices, derivatives, grad_out, grad_texture, grad_indices)]
+            dims = (TB, TH, TW, C, B, N)
+            entry = lambda det, scratch, nbytes, stream: L.dirt_texture_sample_trilinear_backward(
+                *ptrs, *dims, int(det), scratch, nbytes, stream)
+            size = lambda det: L.dirt_texture_sample_trilinear_backward_bytes(*dims, int(det))
+        else:
+            # bilinear and nearest: the default entry point takes no scratch, the deterministic one has its own
+            ptrs = [_ptr(t) for t in (texture, indices, grad_out, grad_texture, grad_indices)]
+            dims = (TB, TH, TW, C, B, N, ctx.mode)
+            entry = lambda det, scratch, nbytes, stream: (
+                L.dirt_texture_sample_backward_deterministic(*ptrs, *dims, scratch, nbytes, stream) if det
+                else L.dirt_texture_sample_backward(*ptrs, *dims, stream))
+            size = lambda det: L.dirt_texture_sample_backward_deterministic_bytes(*dims) if det else 0
+        _backward(indices.device, want_texture, entry, size, 'SampleTextureGrad',
+                  'sample_texture backward: the texture gradient has no deterministic implementation for %d lookups '
+                  'into %d x %d x %d texels (it needs fewer than 2^31 of each)' % (B * N, TB, TH, TW))
         return grad_texture, grad_indices, None, None, None
 
 
@@ -145,6 +153,20 @@ def index_derivatives(indices, texture_shape):
         return torch.cat([along(indices.dim() - 2), along(indices.dim() - 3)], -1)
 
 
+def _batched(table, coords, item_dims, per_item_error):
+    """The lookups of sample_texture and sample_cubemap as one batch.  A table of `item_dims` dimensions is shared by
+    every lookup; one with a leading batch axis holds one table per batch item, and the coordinates then lead with the
+    same axis (else ValueError(per_item_error)).  Returns the table [TB, ...] and the coordinates [B, N, K], both
+    contiguous, B, N and the lookup's output shape coords.shape[:-1] + (C,)."""
+    per_item = table.dim() == item_dims + 1
+    if per_item and (coords.dim() < 2 or coords.shape[0] != table.shape[0]):
+        raise ValueError(per_item_error)
+    B = int(coords.shape[0]) if per_item else 1
+    N = math.prod(int(n) for n in coords.shape[(1 if per_item else 0):-1])
+    return ((table if per_item else table[None]).contiguous(), coords.reshape(B, N, coords.shape[-1]).contiguous(), B, N,
+            tuple(coords.shape[:-1]) + (int(table.shape[-1]),))
+
+
 def sample_texture(texture, indices, mode='bilinear', derivatives=None):
     """Reads `texture` at fractional (row, column) texel indices, with gradients to the texture and to the indices.
 
@@ -183,101 +205,57 @@ def sample_texture(texture, indices, mode='bilinear', derivatives=None):
         raise ValueError('SampleTexture expects a texture with positive height, width and channels')
     if indices.dim() < 1 or indices.shape[-1] != 2:
         raise ValueError('SampleTexture expects indices.shape[-1] == 2')
-    per_item = texture.dim() == 4
-    if per_item and (indices.dim() < 2 or indices.shape[0] != texture.shape[0]):
-        raise ValueError('SampleTexture expects indices of per-item textures to be at least 2D, and indices.shape[0] == '
-                         'texture.shape[0]')
+    tex, flat, B, N, out_shape = _batched(
+        texture, indices, 3, 'SampleTexture expects indices of per-item textures to be at least 2D, and indices.shape[0] '
+        '== texture.shape[0]')
     if mode == 'trilinear':
         derivatives = _as_f32(derivatives, device)
         if tuple(derivatives.shape) != tuple(indices.shape[:-1]) + (4,):
             raise ValueError('SampleTexture expects derivatives.shape == indices.shape[:-1] + (4,), got %s for indices %s'
                              % (tuple(derivatives.shape), tuple(indices.shape)))
         _require_cuda(texture, indices, derivatives)
-    else:
-        _require_cuda(texture, indices)
-    out_shape = tuple(indices.shape[:-1]) + (int(texture.shape[-1]),)
-    B = int(indices.shape[0]) if per_item else 1
-    N = 1
-    for n in indices.shape[(1 if per_item else 0):-1]:
-        N *= int(n)
-    flat = indices.reshape(B, N, 2).contiguous()
-    tex = (texture if per_item else texture[None]).contiguous()
-    if mode == 'trilinear':
         return _SampleTexture.apply(tex, flat, mode, out_shape, derivatives.detach().reshape(B, N, 4).contiguous())
+    _require_cuda(texture, indices)
     return _SampleTexture.apply(tex, flat, _MODES[mode], out_shape)
 
 
+# per sample_cubemap mode: the atlas size query, the lookup, the backward scratch size query, the backward pass and the
+# op's name in errors
+_CUBEMAP_ENTRIES = {
+    'bilinear': ('dirt_cubemap_atlas_bytes', 'dirt_cubemap_sample', 'dirt_cubemap_sample_backward_bytes',
+                 'dirt_cubemap_sample_backward', 'SampleCubemap'),
+    'trilinear': ('dirt_cubemap_mip_atlas_bytes', 'dirt_cubemap_sample_trilinear',
+                  'dirt_cubemap_sample_trilinear_backward_bytes', 'dirt_cubemap_sample_trilinear_backward',
+                  'SampleCubemapTrilinear'),
+    'ggx': ('dirt_cubemap_ggx_atlas_bytes', 'dirt_cubemap_sample_ggx', 'dirt_cubemap_sample_ggx_backward_bytes',
+            'dirt_cubemap_sample_ggx_backward', 'SampleCubemapGGX'),
+}
+_CUBEMAP_ENTRIES['nearest'] = _CUBEMAP_ENTRIES['bilinear']
+
+
 class _SampleCubemap(torch.autograd.Function):
-    """dirt_cubemap_sample / dirt_cubemap_sample_backward.  cubemap [TB, 6, S, S, C], directions [B, N, 3], contiguous
-    fp32 CUDA.  The atlas of padded faces is built per call and kept for the backward pass in place of the cube map."""
+    """dirt_cubemap_sample / dirt_cubemap_sample_backward, or for mode 'trilinear' and 'ggx' the
+    dirt_cubemap_sample_trilinear and dirt_cubemap_sample_ggx pairs.  cubemap [TB, 6, S, S, C], directions [B, N, 3],
+    lod [B, N] ('trilinear' and 'ggx' only, else None), contiguous fp32 CUDA.  The atlas of padded faces ('trilinear':
+    every level's; 'ggx': also the prefiltered levels, their normalisers and the texel table) is built per call and kept
+    for the backward pass in place of the cube map."""
 
     @staticmethod
-    def forward(ctx, cubemap, directions, mode, out_shape):
+    def forward(ctx, cubemap, directions, lod, mode, out_shape):
         TB, _, S, _, C = cubemap.shape
         B, N = directions.shape[0], directions.shape[1]
         L = _lib.lib()
+        atlas_bytes, sample, _, _, op = _CUBEMAP_ENTRIES[mode]
         out = torch.empty(out_shape, dtype=torch.float32, device=directions.device)
-        atlas = torch.empty(int(L.dirt_cubemap_atlas_bytes(TB, S, C)) // 4, dtype=torch.float32, device=directions.device)
+        atlas = torch.empty(int(getattr(L, atlas_bytes)(TB, S, C)) // 4, dtype=torch.float32, device=directions.device)
+        # bilinear and nearest take the mode, trilinear and ggx the level of detail
+        lod_arg, mode_arg = ((), (_MODES[mode],)) if lod is None else ((_ptr(lod),), ())
         with torch.cuda.device(directions.device):
-            rc = L.dirt_cubemap_sample(_ptr(cubemap), _ptr(directions), _ptr(atlas), _ptr(out), TB, S, C, B, N, mode,
-                                       _stream_ptr(directions.device))
-        _lib.check(rc, 'SampleCubemap')
-        ctx.save_for_backward(atlas, directions)
-        ctx.mode, ctx.shape = mode, (TB, S, C)
-        return out
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, grad_out):
-        want_cubemap, want_directions = ctx.needs_input_grad[:2]
-        if not (want_cubemap or want_directions):
-            return None, None, None, None
-        atlas, directions = ctx.saved_tensors
-        TB, S, C = ctx.shape
-        B, N = directions.shape[0], directions.shape[1]
-        L = _lib.lib()
-        grad_out = grad_out.contiguous().to(torch.float32)
-        grad_cubemap = torch.empty((TB, 6, S, S, C), dtype=torch.float32, device=directions.device) if want_cubemap else None
-        grad_directions = torch.empty_like(directions) if want_directions else None
-        # grad_directions alone is per lookup and already reproducible; grad_cubemap needs the sorted path
-        deterministic = bool(want_cubemap and torch.are_deterministic_algorithms_enabled())
-        scratch_bytes = int(L.dirt_cubemap_sample_backward_bytes(TB, S, C, B, N, ctx.mode, int(deterministic)))
-        scratch = torch.empty(scratch_bytes, dtype=torch.uint8, device=directions.device) if scratch_bytes else None
-        with torch.cuda.device(directions.device):
-            rc = L.dirt_cubemap_sample_backward(
-                _ptr(atlas), _ptr(directions), _ptr(grad_out), _ptr(grad_cubemap), _ptr(grad_directions), TB, S, C, B, N,
-                ctx.mode, int(deterministic), _ptr(scratch), scratch_bytes, _stream_ptr(directions.device))
-        if deterministic and rc == _lib.ERR_BAD_SHAPE:
-            # the shapes passed the forward call: what fails are the sorted path's 32-bit limits
-            raise RuntimeError(
-                'sample_cubemap backward: the cube-map gradient has no deterministic implementation for %d lookups '
-                'into %d x 6 x %d x %d texels (it needs fewer than 2^31 lookups and padded texels per face), but '
-                'torch.use_deterministic_algorithms(True) is set' % (B * N, TB, S, S))
-        _lib.check(rc, 'SampleCubemapGrad')
-        return grad_cubemap, grad_directions, None, None
-
-
-class _SampleCubemapMip(torch.autograd.Function):
-    """dirt_cubemap_sample_trilinear / dirt_cubemap_sample_trilinear_backward, or with ggx the dirt_cubemap_sample_ggx
-    pair.  cubemap [TB, 6, S, S, C], directions [B, N, 3], lod [B, N], contiguous fp32 CUDA.  The mip atlas (every
-    level's padded faces; with ggx also the prefiltered levels, their normalisers and the texel table) is built per
-    call and kept for the backward pass in place of the cube map."""
-
-    @staticmethod
-    def forward(ctx, cubemap, directions, lod, out_shape, ggx=False):
-        TB, _, S, _, C = cubemap.shape
-        B, N = directions.shape[0], directions.shape[1]
-        L = _lib.lib()
-        out = torch.empty(out_shape, dtype=torch.float32, device=directions.device)
-        atlas_bytes = L.dirt_cubemap_ggx_atlas_bytes if ggx else L.dirt_cubemap_mip_atlas_bytes
-        atlas = torch.empty(int(atlas_bytes(TB, S, C)) // 4, dtype=torch.float32, device=directions.device)
-        sample = L.dirt_cubemap_sample_ggx if ggx else L.dirt_cubemap_sample_trilinear
-        with torch.cuda.device(directions.device):
-            rc = sample(_ptr(cubemap), _ptr(directions), _ptr(lod), _ptr(atlas), _ptr(out), TB, S, C, B, N,
-                        _stream_ptr(directions.device))
-        _lib.check(rc, 'SampleCubemapGGX' if ggx else 'SampleCubemapTrilinear')
+            rc = getattr(L, sample)(_ptr(cubemap), _ptr(directions), *lod_arg, _ptr(atlas), _ptr(out), TB, S, C, B, N,
+                                    *mode_arg, _stream_ptr(directions.device))
+        _lib.check(rc, op)
         ctx.save_for_backward(atlas, directions, lod)
-        ctx.shape, ctx.ggx = (TB, S, C), ggx
+        ctx.mode, ctx.shape = mode, (TB, S, C)
         return out
 
     @staticmethod
@@ -290,29 +268,25 @@ class _SampleCubemapMip(torch.autograd.Function):
         TB, S, C = ctx.shape
         B, N = directions.shape[0], directions.shape[1]
         L = _lib.lib()
+        _, _, size, entry, op = _CUBEMAP_ENTRIES[ctx.mode]
         grad_out = grad_out.contiguous().to(torch.float32)
         dev = directions.device
         grad_cubemap = torch.empty((TB, 6, S, S, C), dtype=torch.float32, device=dev) if want_cubemap else None
         grad_directions = torch.empty_like(directions) if want_directions else None
         grad_lod = torch.empty_like(lod) if want_lod else None
-        # grad_directions and grad_lod are per lookup and already reproducible; grad_cubemap needs the sorted path
-        deterministic = bool(want_cubemap and torch.are_deterministic_algorithms_enabled())
-        backward_bytes, backward = ((L.dirt_cubemap_sample_ggx_backward_bytes, L.dirt_cubemap_sample_ggx_backward) if ctx.ggx
-                                    else (L.dirt_cubemap_sample_trilinear_backward_bytes,
-                                          L.dirt_cubemap_sample_trilinear_backward))
-        scratch_bytes = int(backward_bytes(TB, S, C, B, N, int(deterministic)))
-        scratch = torch.empty(scratch_bytes, dtype=torch.uint8, device=dev) if scratch_bytes else None
-        with torch.cuda.device(dev):
-            rc = backward(
-                _ptr(atlas), _ptr(directions), _ptr(lod), _ptr(grad_out), _ptr(grad_cubemap), _ptr(grad_directions),
-                _ptr(grad_lod), TB, S, C, B, N, int(deterministic), _ptr(scratch), scratch_bytes, _stream_ptr(dev))
-        if deterministic and rc == _lib.ERR_BAD_SHAPE:
-            # the shapes passed the forward call: what fails are the sorted path's 32-bit limits
-            raise RuntimeError(
-                'sample_cubemap backward: the cube-map gradient has no deterministic implementation for %d lookups '
-                'into %d x 6 x %d x %d texels (it needs fewer than 2^31 lookups and padded texels per face), but '
-                'torch.use_deterministic_algorithms(True) is set' % (B * N, TB, S, S))
-        _lib.check(rc, 'SampleCubemapGGXGrad' if ctx.ggx else 'SampleCubemapTrilinearGrad')
+        # bilinear and nearest take the mode, trilinear and ggx the level of detail and its gradient
+        if lod is None:
+            ptrs = [_ptr(t) for t in (atlas, directions, grad_out, grad_cubemap, grad_directions)]
+            dims = (TB, S, C, B, N, _MODES[ctx.mode])
+        else:
+            ptrs = [_ptr(t) for t in (atlas, directions, lod, grad_out, grad_cubemap, grad_directions, grad_lod)]
+            dims = (TB, S, C, B, N)
+        _backward(dev, want_cubemap,
+                  lambda det, scratch, nbytes, stream: getattr(L, entry)(*ptrs, *dims, int(det), scratch, nbytes, stream),
+                  lambda det: getattr(L, size)(*dims, int(det)), op + 'Grad',
+                  'sample_cubemap backward: the cube-map gradient has no deterministic implementation for %d lookups '
+                  'into %d x 6 x %d x %d texels (it needs fewer than 2^31 lookups and padded texels per face)'
+                  % (B * N, TB, S, S))
         return grad_cubemap, grad_directions, grad_lod, None, None
 
 
@@ -371,10 +345,9 @@ def sample_cubemap(cubemap, directions, mode='bilinear', lod=None, roughness=Non
         raise ValueError('SampleCubemap expects a cube map with positive size and channels')
     if directions.dim() < 1 or directions.shape[-1] != 3:
         raise ValueError('SampleCubemap expects directions.shape[-1] == 3')
-    per_item = cubemap.dim() == 5
-    if per_item and (directions.dim() < 2 or directions.shape[0] != cubemap.shape[0]):
-        raise ValueError('SampleCubemap expects directions of per-item cube maps to be at least 2D, and '
-                         'directions.shape[0] == cubemap.shape[0]')
+    cube, flat, B, N, out_shape = _batched(
+        cubemap, directions, 4, 'SampleCubemap expects directions of per-item cube maps to be at least 2D, and '
+        'directions.shape[0] == cubemap.shape[0]')
     if mode == 'ggx':
         S = int(cubemap.shape[-2])
         if S % 2:
@@ -391,18 +364,10 @@ def sample_cubemap(cubemap, directions, mode='bilinear', lod=None, roughness=Non
             raise ValueError('SampleCubemap expects lod broadcastable to directions.shape[:-1] = %s, got %s'
                              % (tuple(directions.shape[:-1]), tuple(lod.shape)))
         _require_cuda(cubemap, directions, lod)
+        lod = lod.reshape(B, N).contiguous()
     else:
         _require_cuda(cubemap, directions)
-    out_shape = tuple(directions.shape[:-1]) + (int(cubemap.shape[-1]),)
-    B = int(directions.shape[0]) if per_item else 1
-    N = 1
-    for n in directions.shape[(1 if per_item else 0):-1]:
-        N *= int(n)
-    flat = directions.reshape(B, N, 3).contiguous()
-    cube = (cubemap if per_item else cubemap[None]).contiguous()
-    if mode in ('trilinear', 'ggx'):
-        return _SampleCubemapMip.apply(cube, flat, lod.reshape(B, N).contiguous(), out_shape, mode == 'ggx')
-    return _SampleCubemap.apply(cube, flat, _MODES[mode], out_shape)
+    return _SampleCubemap.apply(cube, flat, lod, mode, out_shape)
 
 
 def _mip_level_count(S):
