@@ -12,8 +12,6 @@ using namespace dirt;
 static_assert(BWD_SHARED_GEOMETRY == DIRT_BWD_SHARED_GEOMETRY && BWD_SKIP_POSITION == DIRT_BWD_SKIP_POSITION &&
               BWD_SKIP_COLOUR == DIRT_BWD_SKIP_COLOUR, "flag values of common.cuh and dirt_b200.h differ");
 
-static thread_local int t_last_launches = 0;
-
 extern "C" const char* dirt_error_string(int code)
 {
     switch (code) {
@@ -39,6 +37,12 @@ KernelTimer& kernel_timer()
 {
     static thread_local KernelTimer t;
     return t;
+}
+
+int& launch_count()
+{
+    static thread_local int n = 0;
+    return n;
 }
 }  // namespace dirt
 
@@ -67,7 +71,7 @@ extern "C" float dirt_kernel_timer_elapsed_ms(void)
     return ms;
 }
 
-extern "C" int dirt_last_launch_count(void) { return t_last_launches; }
+extern "C" int dirt_last_launch_count(void) { return launch_count(); }
 
 // gradient outputs may be NULL (not wanted), but not misaligned
 static bool aligned(std::initializer_list<const void*> ptrs)
@@ -157,16 +161,14 @@ static int check_workspace(void* workspace, size_t workspace_bytes, int B, int H
 
 #define CUDA_TRY(expr)                                   \
     do {                                                 \
-        cudaError_t e__ = (expr);                        \
-        if (e__ != cudaSuccess) { t_last_launches = launches; return DIRT_ERR_CUDA; } \
+        if ((expr) != cudaSuccess) return DIRT_ERR_CUDA; \
     } while (0)
 
 extern "C" int dirt_rasterise_forward(const float* background, const float* vertices, const float* vertex_colors,
                                       const int32_t* faces, float* pixels, int32_t* face_ids_out, int B, int H, int W,
                                       int C, int V, int F, void* workspace, size_t workspace_bytes, void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!shape_ok(B, H, W, C, V, F)) return DIRT_ERR_BAD_SHAPE;
     if (B == 0) return DIRT_OK;
     if (!background || !pixels) return DIRT_ERR_NULL_POINTER;
@@ -180,11 +182,10 @@ extern "C" int dirt_rasterise_forward(const float* background, const float* vert
     cudaStream_t stream = (cudaStream_t)cuda_stream;
     const Workspace ws = carve_workspace(workspace, B, H, W, C, V, F);
     const Dims d = make_dims(B, H, W, C, V, F);
-    CUDA_TRY(launch_setup_and_bin(vertices, faces, vertex_colors, ws, d, stream, &launches));
+    CUDA_TRY(launch_setup_and_bin(vertices, faces, vertex_colors, ws, d, stream));
 #if !defined(DIRT_SETUP_ABLATE) || DIRT_SETUP_ABLATE == 0   // a setup timing build leaves the records undefined
-    CUDA_TRY(launch_raster_forward(vertices, background, vertex_colors, pixels, face_ids_out, ws, d, stream, &launches));
+    CUDA_TRY(launch_raster_forward(vertices, background, vertex_colors, pixels, face_ids_out, ws, d, stream));
 #endif
-    t_last_launches = launches;
     return DIRT_OK;
 }
 
@@ -192,8 +193,7 @@ extern "C" int dirt_rasterise_visibility(const float* vertices, const int32_t* f
                                          int B, int H, int W, int V, int F, void* workspace, size_t workspace_bytes,
                                          void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!shape_ok(B, H, W, 1, V, F)) return DIRT_ERR_BAD_SHAPE;
     if (B == 0) return DIRT_OK;
     if ((V > 0 && !vertices) || (F > 0 && !faces)) return DIRT_ERR_NULL_POINTER;
@@ -204,9 +204,8 @@ extern "C" int dirt_rasterise_visibility(const float* vertices, const int32_t* f
     cudaStream_t stream = (cudaStream_t)cuda_stream;
     const Workspace ws = carve_workspace(workspace, B, H, W, 1, V, F);
     const Dims d = make_dims(B, H, W, 1, V, F);
-    CUDA_TRY(launch_setup_and_bin(vertices, faces, nullptr, ws, d, stream, &launches));
-    CUDA_TRY(launch_raster_visibility(vertices, face_ids, gbuffer, ws, d, stream, &launches));
-    t_last_launches = launches;
+    CUDA_TRY(launch_setup_and_bin(vertices, faces, nullptr, ws, d, stream));
+    CUDA_TRY(launch_raster_visibility(vertices, face_ids, gbuffer, ws, d, stream));
     return DIRT_OK;
 }
 
@@ -216,8 +215,7 @@ static int backward_impl(const float* vertices, const int32_t* faces, const floa
                          int workspace_holds_setup, int flags, void* workspace, size_t workspace_bytes, void* cuda_stream,
                          bool deterministic = false, void* scratch = nullptr, size_t scratch_bytes = 0)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!shape_ok(B, H, W, C, V, F)) return DIRT_ERR_BAD_SHAPE;
     if (V > (1 << 24)) return DIRT_ERR_TOO_MANY_VERTICES;
     if (flags & ~(DIRT_BWD_SHARED_GEOMETRY | DIRT_BWD_SKIP_POSITION | DIRT_BWD_SKIP_COLOUR)) return DIRT_ERR_BAD_SHAPE;
@@ -248,11 +246,11 @@ static int backward_impl(const float* vertices, const int32_t* faces, const floa
     unsigned long long expect_tag = 0;
     if (!ids) {
         // no cached visibility: re-derive it exactly as the forward pass does
-        CUDA_TRY(launch_setup_and_bin(vertices, faces, nullptr, ws, d, stream, &launches));
-        CUDA_TRY(launch_raster_visibility(vertices, ws.face_ids, nullptr, ws, d, stream, &launches));
+        CUDA_TRY(launch_setup_and_bin(vertices, faces, nullptr, ws, d, stream));
+        CUDA_TRY(launch_raster_visibility(vertices, ws.face_ids, nullptr, ws, d, stream));
         ids = ws.face_ids;
     } else if (!workspace_holds_setup) {
-        CUDA_TRY(launch_setup_only(vertices, faces, ws, d, stream, &launches));
+        CUDA_TRY(launch_setup_only(vertices, faces, ws, d, stream));
     } else {
         // a promise: checked on the device against the tag the setup pass left in the workspace
         expect_tag = workspace_tag(vertices, faces, B, H, W, V, F);
@@ -260,11 +258,10 @@ static int backward_impl(const float* vertices, const int32_t* faces, const floa
     if (deterministic)
         CUDA_TRY(launch_backward_deterministic(vertices, faces, pixels, grad_pixels, ids, grad_background, grad_vertices,
                                                grad_vertex_colors, ws, d, groups, flags, expect_tag,
-                                               carve_det_scratch(scratch, B, H, W, C, V, F), stream, &launches));
+                                               carve_det_scratch(scratch, B, H, W, C, V, F), stream));
     else
         CUDA_TRY(launch_backward(vertices, pixels, grad_pixels, ids, grad_background, grad_vertices, grad_vertex_colors, ws, d,
-                                 groups, flags_valid, flags, expect_tag, stream, &launches));
-    t_last_launches = launches;
+                                 groups, flags_valid, flags, expect_tag, stream));
     return DIRT_OK;
 }
 
@@ -293,8 +290,7 @@ extern "C" int dirt_rasterise_derivatives(const float* vertices, const int32_t* 
                                           int F, int first_channel, int channel_count, int workspace_holds_setup,
                                           void* workspace, size_t workspace_bytes, void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!shape_ok(B, H, W, C, V, F)) return DIRT_ERR_BAD_SHAPE;
     if (first_channel < 0 || channel_count <= 0 || first_channel >= C || channel_count > C - first_channel)
         return DIRT_ERR_BAD_SHAPE;
@@ -311,12 +307,11 @@ extern "C" int dirt_rasterise_derivatives(const float* vertices, const int32_t* 
     const Dims d = make_dims(B, H, W, C, V, F);
     unsigned long long expect_tag = 0;
     if (!workspace_holds_setup)
-        CUDA_TRY(launch_setup_only(vertices, faces, ws, d, stream, &launches));
+        CUDA_TRY(launch_setup_only(vertices, faces, ws, d, stream));
     else
         expect_tag = workspace_tag(vertices, faces, B, H, W, V, F);   // checked on the device, as backward_impl does
     CUDA_TRY(launch_gbuffer_derivatives(face_ids, attributes, derivatives, ws, d, first_channel, channel_count, expect_tag,
-                                        stream, &launches));
-    t_last_launches = launches;
+                                        stream));
     return DIRT_OK;
 }
 
@@ -340,7 +335,7 @@ extern "C" int dirt_rasterise_backward_deterministic(const float* vertices, cons
                                                      size_t workspace_bytes, void* scratch, size_t scratch_bytes,
                                                      void* cuda_stream)
 {
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!deterministic_shape_ok(B, H, W, C, V, F)) return DIRT_ERR_BAD_SHAPE;
     return backward_impl(vertices, faces, pixels, grad_pixels, face_ids, grad_background, grad_vertices, grad_vertex_colors, B, H,
                          W, C, V, F, channel_groups, n_groups, workspace_holds_setup, flags, workspace, workspace_bytes,
@@ -369,15 +364,12 @@ static TexDims make_tex_dims(int TB, int TH, int TW, int C, int B, long long N, 
 extern "C" int dirt_texture_sample(const float* texture, const float* indices, float* out, int TB, int TH, int TW, int C,
                                    int B, long long N, int mode, void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!texture_shape_ok(TB, TH, TW, C, B, N, mode)) return DIRT_ERR_BAD_SHAPE;
     if (B == 0 || N == 0) return DIRT_OK;
     const int rc = required_check({texture, indices, out});
     if (rc != DIRT_OK) return rc;
-    CUDA_TRY(launch_texture_forward(texture, indices, out, make_tex_dims(TB, TH, TW, C, B, N, mode), (cudaStream_t)cuda_stream,
-                                    &launches));
-    t_last_launches = launches;
+    CUDA_TRY(launch_texture_forward(texture, indices, out, make_tex_dims(TB, TH, TW, C, B, N, mode), (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
@@ -385,8 +377,7 @@ extern "C" int dirt_texture_sample_backward(const float* texture, const float* i
                                             float* grad_texture, float* grad_indices, int TB, int TH, int TW, int C, int B,
                                             long long N, int mode, void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!texture_shape_ok(TB, TH, TW, C, B, N, mode)) return DIRT_ERR_BAD_SHAPE;
     const TexDims d = make_tex_dims(TB, TH, TW, C, B, N, mode);
     if (d.total > 0) {
@@ -395,9 +386,7 @@ extern "C" int dirt_texture_sample_backward(const float* texture, const float* i
     }
     if (!aligned({texture, indices, grad_out, grad_texture, grad_indices})) return DIRT_ERR_MISALIGNED;
     // with no lookups only the memset of grad_texture is enqueued
-    CUDA_TRY(launch_texture_backward(texture, indices, grad_out, grad_texture, grad_indices, d, (cudaStream_t)cuda_stream,
-                                     &launches));
-    t_last_launches = launches;
+    CUDA_TRY(launch_texture_backward(texture, indices, grad_out, grad_texture, grad_indices, d, (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
@@ -419,8 +408,7 @@ extern "C" int dirt_texture_sample_backward_deterministic(const float* texture, 
                                                           int C, int B, long long N, int mode, void* scratch,
                                                           size_t scratch_bytes, void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!texture_det_shape_ok(TB, TH, TW, C, B, N, mode)) return DIRT_ERR_BAD_SHAPE;
     const TexDims d = make_tex_dims(TB, TH, TW, C, B, N, mode);
     if (d.total > 0) {
@@ -437,8 +425,7 @@ extern "C" int dirt_texture_sample_backward_deterministic(const float* texture, 
     }
     CUDA_TRY(launch_texture_backward_deterministic(texture, indices, grad_out, grad_texture, grad_indices, d,
                                                    carve_texture_det_scratch(sorts ? scratch : nullptr, d),
-                                                   (cudaStream_t)cuda_stream, &launches));
-    t_last_launches = launches;
+                                                   (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
@@ -461,15 +448,13 @@ extern "C" size_t dirt_texture_mip_pyramid_bytes(int TB, int TH, int TW, int C)
 
 extern "C" int dirt_texture_mip_build(const float* texture, float* pyramid, int TB, int TH, int TW, int C, void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (TB < 0 || !texture_shape_ok(TB, TH, TW, C, TB, 0, DIRT_TEXTURE_BILINEAR)) return DIRT_ERR_BAD_SHAPE;
     if (TB == 0 || mip_levels(TH, TW) == 1) return DIRT_OK;
     const int rc = required_check({texture, pyramid});
     if (rc != DIRT_OK) return rc;
     CUDA_TRY(launch_texture_mip_build(texture, pyramid, make_tex_dims(TB, TH, TW, C, TB, 0, DIRT_TEXTURE_BILINEAR),
-                                      (cudaStream_t)cuda_stream, &launches));
-    t_last_launches = launches;
+                                      (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
@@ -477,16 +462,14 @@ extern "C" int dirt_texture_sample_trilinear(const float* texture, const float* 
                                              const float* derivatives, float* out, int TB, int TH, int TW, int C, int B,
                                              long long N, void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!mip_shape_ok(TB, TH, TW, C, B, N)) return DIRT_ERR_BAD_SHAPE;
     if (B == 0 || N == 0) return DIRT_OK;
     if (!texture || !indices || !derivatives || !out || (!pyramid && mip_levels(TH, TW) > 1)) return DIRT_ERR_NULL_POINTER;
     if (!aligned({texture, pyramid, indices, derivatives, out})) return DIRT_ERR_MISALIGNED;
     CUDA_TRY(launch_texture_trilinear_forward(texture, pyramid, indices, derivatives, out,
                                               make_tex_dims(TB, TH, TW, C, B, N, DIRT_TEXTURE_BILINEAR),
-                                              (cudaStream_t)cuda_stream, &launches));
-    t_last_launches = launches;
+                                              (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
@@ -506,8 +489,7 @@ extern "C" int dirt_texture_sample_trilinear_backward(const float* texture, cons
                                                       int deterministic, void* scratch, size_t scratch_bytes,
                                                       void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!mip_shape_ok(TB, TH, TW, C, B, N)) return DIRT_ERR_BAD_SHAPE;
     if (deterministic && grad_texture && !texture_det_shape_ok(TB, TH, TW, C, B, N, DIRT_TEXTURE_BILINEAR))
         return DIRT_ERR_BAD_SHAPE;
@@ -528,8 +510,7 @@ extern "C" int dirt_texture_sample_trilinear_backward(const float* texture, cons
     }
     CUDA_TRY(launch_texture_trilinear_backward(texture, pyramid, indices, derivatives, grad_out, grad_texture, grad_indices, d,
                                                det, carve_texture_mip_scratch(uses_scratch ? scratch : nullptr, d, det),
-                                               (cudaStream_t)cuda_stream, &launches));
-    t_last_launches = launches;
+                                               (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
@@ -557,15 +538,13 @@ extern "C" size_t dirt_cubemap_atlas_bytes(int TB, int S, int C)
 extern "C" int dirt_cubemap_sample(const float* cubemap, const float* directions, float* atlas, float* out, int TB, int S,
                                    int C, int B, long long N, int mode, void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!cubemap_shape_ok(TB, S, C, B, N, mode)) return DIRT_ERR_BAD_SHAPE;
     if (B == 0 || N == 0) return DIRT_OK;
     const int rc = required_check({cubemap, directions, atlas, out});
     if (rc != DIRT_OK) return rc;
     CUDA_TRY(launch_cubemap_forward(cubemap, directions, atlas, out, cubemap_dims(TB, S, C, B, N, mode),
-                                    (cudaStream_t)cuda_stream, &launches));
-    t_last_launches = launches;
+                                    (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
@@ -581,8 +560,7 @@ extern "C" int dirt_cubemap_sample_backward(const float* atlas, const float* dir
                                             long long N, int mode, int deterministic, void* scratch, size_t scratch_bytes,
                                             void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!cubemap_shape_ok(TB, S, C, B, N, mode)) return DIRT_ERR_BAD_SHAPE;
     if (deterministic && grad_cubemap && !texture_det_shape_ok(TB, S + 2, S + 2, C, B, N, mode)) return DIRT_ERR_BAD_SHAPE;
     const TexDims d = cubemap_dims(TB, S, C, B, N, mode);
@@ -600,8 +578,7 @@ extern "C" int dirt_cubemap_sample_backward(const float* atlas, const float* dir
     }
     CUDA_TRY(launch_cubemap_backward(atlas, directions, grad_out, grad_cubemap, grad_directions, d, det,
                                      carve_cubemap_scratch(uses_scratch ? scratch : nullptr, d, det),
-                                     (cudaStream_t)cuda_stream, &launches));
-    t_last_launches = launches;
+                                     (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
@@ -622,16 +599,13 @@ extern "C" size_t dirt_cubemap_mip_atlas_bytes(int TB, int S, int C)
 extern "C" int dirt_cubemap_sample_trilinear(const float* cubemap, const float* directions, const float* lod, float* atlas,
                                              float* out, int TB, int S, int C, int B, long long N, void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!cubemap_mip_shape_ok(TB, S, C, B, N)) return DIRT_ERR_BAD_SHAPE;
     if (B == 0 || N == 0) return DIRT_OK;
     const int rc = required_check({cubemap, directions, lod, atlas, out});
     if (rc != DIRT_OK) return rc;
     CUDA_TRY(launch_cubemap_mip_forward(cubemap, directions, lod, atlas, out,
-                                        cubemap_dims(TB, S, C, B, N, DIRT_TEXTURE_BILINEAR), (cudaStream_t)cuda_stream,
-                                        &launches));
-    t_last_launches = launches;
+                                        cubemap_dims(TB, S, C, B, N, DIRT_TEXTURE_BILINEAR), (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
@@ -648,8 +622,7 @@ extern "C" int dirt_cubemap_sample_trilinear_backward(const float* atlas, const 
                                                       int deterministic, void* scratch, size_t scratch_bytes,
                                                       void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!cubemap_mip_shape_ok(TB, S, C, B, N)) return DIRT_ERR_BAD_SHAPE;
     if (deterministic && grad_cubemap && !texture_det_shape_ok(TB, S + 2, S + 2, C, B, N, DIRT_TEXTURE_BILINEAR))
         return DIRT_ERR_BAD_SHAPE;
@@ -668,8 +641,7 @@ extern "C" int dirt_cubemap_sample_trilinear_backward(const float* atlas, const 
     }
     CUDA_TRY(launch_cubemap_mip_backward(atlas, directions, lod, grad_out, grad_cubemap, grad_directions, grad_lod, d, det,
                                          carve_cubemap_mip_scratch(uses_scratch ? scratch : nullptr, d, det),
-                                         (cudaStream_t)cuda_stream, &launches));
-    t_last_launches = launches;
+                                         (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
@@ -690,33 +662,28 @@ extern "C" size_t dirt_cubemap_ggx_atlas_bytes(int TB, int S, int C)
 
 extern "C" int dirt_cubemap_ggx_prefilter(const float* cubemap, float* atlas, int TB, int S, int C, void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (TB < 0 || !cubemap_ggx_shape_ok(TB, S, C, TB, 0)) return DIRT_ERR_BAD_SHAPE;
     if (TB == 0) return DIRT_OK;
     const int rc = required_check({cubemap, atlas});
     if (rc != DIRT_OK) return rc;
     if ((uintptr_t)atlas % 16) return DIRT_ERR_MISALIGNED;
     CUDA_TRY(launch_ggx_prefilter(cubemap, atlas, cubemap_dims(TB, S, C, TB, 0, DIRT_TEXTURE_BILINEAR),
-                                  (cudaStream_t)cuda_stream, &launches));
-    t_last_launches = launches;
+                                  (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
 extern "C" int dirt_cubemap_sample_ggx(const float* cubemap, const float* directions, const float* lod, float* atlas,
                                        float* out, int TB, int S, int C, int B, long long N, void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!cubemap_ggx_shape_ok(TB, S, C, B, N)) return DIRT_ERR_BAD_SHAPE;
     if (B == 0 || N == 0) return DIRT_OK;
     const int rc = required_check({cubemap, directions, lod, atlas, out});
     if (rc != DIRT_OK) return rc;
     if ((uintptr_t)atlas % 16) return DIRT_ERR_MISALIGNED;
     CUDA_TRY(launch_cubemap_ggx_forward(cubemap, directions, lod, atlas, out,
-                                        cubemap_dims(TB, S, C, B, N, DIRT_TEXTURE_BILINEAR), (cudaStream_t)cuda_stream,
-                                        &launches));
-    t_last_launches = launches;
+                                        cubemap_dims(TB, S, C, B, N, DIRT_TEXTURE_BILINEAR), (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
@@ -732,8 +699,7 @@ extern "C" int dirt_cubemap_sample_ggx_backward(const float* atlas, const float*
                                                 float* grad_lod, int TB, int S, int C, int B, long long N, int deterministic,
                                                 void* scratch, size_t scratch_bytes, void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!cubemap_ggx_shape_ok(TB, S, C, B, N)) return DIRT_ERR_BAD_SHAPE;
     if (deterministic && grad_cubemap && !texture_det_shape_ok(TB, S + 2, S + 2, C, B, N, DIRT_TEXTURE_BILINEAR))
         return DIRT_ERR_BAD_SHAPE;
@@ -753,8 +719,7 @@ extern "C" int dirt_cubemap_sample_ggx_backward(const float* atlas, const float*
     }
     CUDA_TRY(launch_cubemap_ggx_backward(atlas, directions, lod, grad_out, grad_cubemap, grad_directions, grad_lod, d, det,
                                          carve_cubemap_ggx_scratch(uses_scratch ? scratch : nullptr, d, det),
-                                         (cudaStream_t)cuda_stream, &launches));
-    t_last_launches = launches;
+                                         (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
@@ -772,31 +737,26 @@ extern "C" size_t dirt_cubemap_sh_project_bytes(int TB, int S, int C)
 extern "C" int dirt_cubemap_sh_project(const float* cubemap, float* coeffs, void* scratch, size_t scratch_bytes, int TB,
                                        int S, int C, void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!cubemap_sh_shape_ok(TB, S, C)) return DIRT_ERR_BAD_SHAPE;
     if (TB == 0) return DIRT_OK;
     if (!cubemap || !coeffs || !scratch) return DIRT_ERR_NULL_POINTER;
     if ((uintptr_t)cubemap % 4 || (uintptr_t)coeffs % 4 || (uintptr_t)scratch % 256) return DIRT_ERR_MISALIGNED;
     if (scratch_bytes < sh_project_scratch_bytes(TB, S, C)) return DIRT_ERR_WORKSPACE_TOO_SMALL;
-    CUDA_TRY(launch_sh_project(cubemap, coeffs, scratch, TB, S, C, (cudaStream_t)cuda_stream, &launches));
-    t_last_launches = launches;
+    CUDA_TRY(launch_sh_project(cubemap, coeffs, scratch, TB, S, C, (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
 extern "C" int dirt_cubemap_sh_project_backward(const float* grad_coeffs, float* grad_cubemap, void* scratch,
                                                 size_t scratch_bytes, int TB, int S, int C, void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!cubemap_sh_shape_ok(TB, S, C)) return DIRT_ERR_BAD_SHAPE;
     if (TB == 0) return DIRT_OK;
     if (!grad_coeffs || !grad_cubemap || !scratch) return DIRT_ERR_NULL_POINTER;
     if ((uintptr_t)grad_coeffs % 4 || (uintptr_t)grad_cubemap % 4 || (uintptr_t)scratch % 256) return DIRT_ERR_MISALIGNED;
     if (scratch_bytes < sh_project_scratch_bytes(TB, S, C)) return DIRT_ERR_WORKSPACE_TOO_SMALL;
-    CUDA_TRY(launch_sh_project_backward(grad_coeffs, grad_cubemap, scratch, TB, S, C, (cudaStream_t)cuda_stream,
-                                        &launches));
-    t_last_launches = launches;
+    CUDA_TRY(launch_sh_project_backward(grad_coeffs, grad_cubemap, scratch, TB, S, C, (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
@@ -820,41 +780,35 @@ extern "C" int dirt_latlong_samples(int H, int W, int S)
 extern "C" int dirt_latlong_to_cubemap(const float* panorama, float* cubemap, int TB, int H, int W, int S, int C,
                                        void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!latlong_shape_ok(TB, H, W, S, C)) return DIRT_ERR_BAD_SHAPE;
     if (TB == 0) return DIRT_OK;
     const int rc = required_check({panorama, cubemap});
     if (rc != DIRT_OK) return rc;
-    CUDA_TRY(launch_latlong_forward(panorama, cubemap, TB, H, W, S, C, (cudaStream_t)cuda_stream, &launches));
-    t_last_launches = launches;
+    CUDA_TRY(launch_latlong_forward(panorama, cubemap, TB, H, W, S, C, (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
 extern "C" int dirt_latlong_to_cubemap_backward(const float* grad_cubemap, float* grad_panorama, int TB, int H, int W,
                                                 int S, int C, void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!latlong_shape_ok(TB, H, W, S, C)) return DIRT_ERR_BAD_SHAPE;
     if (TB == 0) return DIRT_OK;
     const int rc = required_check({grad_cubemap, grad_panorama});
     if (rc != DIRT_OK) return rc;
-    CUDA_TRY(launch_latlong_backward(grad_cubemap, grad_panorama, TB, H, W, S, C, (cudaStream_t)cuda_stream, &launches));
-    t_last_launches = launches;
+    CUDA_TRY(launch_latlong_backward(grad_cubemap, grad_panorama, TB, H, W, S, C, (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
 extern "C" int dirt_ggx_brdf_table(float* table, int N, void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (N < 0 || N > 4096) return DIRT_ERR_BAD_SHAPE;
     if (N == 0) return DIRT_OK;
     const int rc = required_check({table});
     if (rc != DIRT_OK) return rc;
-    CUDA_TRY(launch_ggx_brdf_table(table, N, (cudaStream_t)cuda_stream, &launches));
-    t_last_launches = launches;
+    CUDA_TRY(launch_ggx_brdf_table(table, N, (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
@@ -934,8 +888,7 @@ extern "C" int dirt_lighting_forward(int model, int double_sided, const float* n
                                      int camera_per_item, const float* shininess, int shininess_per_item, float* out,
                                      int B, long long V, int C, void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!lighting_shape_ok(model, B, V, C, normals_stride, positions_stride, colors_stride)) return DIRT_ERR_BAD_SHAPE;
     if ((long long)B * V == 0) return DIRT_OK;
     LightArgs a = make_light_args(model, double_sided, normals, normals_stride, positions, positions_stride, colors,
@@ -945,8 +898,7 @@ extern "C" int dirt_lighting_forward(int model, int double_sided, const float* n
     int rc = lighting_inputs_check(a);
     if (rc == DIRT_OK) rc = required_check({out});
     if (rc != DIRT_OK) return rc;
-    CUDA_TRY(launch_lighting_forward(a, (cudaStream_t)cuda_stream, &launches));
-    t_last_launches = launches;
+    CUDA_TRY(launch_lighting_forward(a, (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
@@ -960,8 +912,7 @@ extern "C" int dirt_lighting_backward(int model, int double_sided, const float* 
                                       float* grad_shininess, void* workspace, size_t workspace_bytes, int B, long long V,
                                       int C, void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!lighting_shape_ok(model, B, V, C, normals_stride, positions_stride, colors_stride)) return DIRT_ERR_BAD_SHAPE;
     LightArgs a = make_light_args(model, double_sided, normals, normals_stride, positions, positions_stride, colors,
                                   colors_stride, light, light_per_item, light_color, light_color_per_item, camera,
@@ -983,8 +934,7 @@ extern "C" int dirt_lighting_backward(int model, int double_sided, const float* 
         if (rc != DIRT_OK) return rc;
     }
     // with no points only the memsets of the wanted parameter gradients are enqueued
-    CUDA_TRY(launch_lighting_backward(a, (cudaStream_t)cuda_stream, &launches));
-    t_last_launches = launches;
+    CUDA_TRY(launch_lighting_backward(a, (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
@@ -1015,8 +965,7 @@ extern "C" int dirt_ggx_lighting_forward(int point_light, int double_sided, cons
                                          const float* light_color, int light_color_per_item, const float* camera,
                                          int camera_per_item, float* out, int B, long long V, int C, void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!ggx_shape_ok(B, V, C, normals_stride, positions_stride, roughness_stride, specular_stride))
         return DIRT_ERR_BAD_SHAPE;
     if ((long long)B * V == 0) return DIRT_OK;
@@ -1027,8 +976,7 @@ extern "C" int dirt_ggx_lighting_forward(int point_light, int double_sided, cons
     int rc = required_check({normals, positions, roughness, specular, light, light_color, camera});
     if (rc == DIRT_OK) rc = required_check({out});
     if (rc != DIRT_OK) return rc;
-    CUDA_TRY(launch_ggx_forward(a, (cudaStream_t)cuda_stream, &launches));
-    t_last_launches = launches;
+    CUDA_TRY(launch_ggx_forward(a, (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
@@ -1043,8 +991,7 @@ extern "C" int dirt_ggx_lighting_backward(int point_light, int double_sided, con
                                           void* workspace, size_t workspace_bytes, int B, long long V, int C,
                                           void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!ggx_shape_ok(B, V, C, normals_stride, positions_stride, roughness_stride, specular_stride))
         return DIRT_ERR_BAD_SHAPE;
     LightArgs a = make_ggx_args(point_light, double_sided, normals, normals_stride, positions, positions_stride,
@@ -1064,8 +1011,7 @@ extern "C" int dirt_ggx_lighting_backward(int point_light, int double_sided, con
         if (rc != DIRT_OK) return rc;
     }
     // with no points only the memsets of the wanted parameter gradients are enqueued
-    CUDA_TRY(launch_ggx_backward(a, (cudaStream_t)cuda_stream, &launches));
-    t_last_launches = launches;
+    CUDA_TRY(launch_ggx_backward(a, (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
@@ -1097,8 +1043,7 @@ extern "C" int dirt_sh_lighting_forward(const float* normals, long long normals_
                                         long long albedo_stride, const float* coefficients, int coefficients_per_item,
                                         float* out, int B, long long V, int C, void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!sh_shape_ok(B, V, C, normals_stride, albedo_stride)) return DIRT_ERR_BAD_SHAPE;
     if ((long long)B * V == 0) return DIRT_OK;
     ShArgs a = make_sh_args(normals, normals_stride, albedo, albedo_stride, coefficients, coefficients_per_item, B, V, C);
@@ -1106,8 +1051,7 @@ extern "C" int dirt_sh_lighting_forward(const float* normals, long long normals_
     int rc = required_check({normals, albedo, coefficients});
     if (rc == DIRT_OK) rc = required_check({out});
     if (rc != DIRT_OK) return rc;
-    CUDA_TRY(launch_sh_lighting_forward(a, (cudaStream_t)cuda_stream, &launches));
-    t_last_launches = launches;
+    CUDA_TRY(launch_sh_lighting_forward(a, (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
@@ -1117,8 +1061,7 @@ extern "C" int dirt_sh_lighting_backward(const float* normals, long long normals
                                          float* grad_coefficients, void* workspace, size_t workspace_bytes, int B,
                                          long long V, int C, void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!sh_shape_ok(B, V, C, normals_stride, albedo_stride)) return DIRT_ERR_BAD_SHAPE;
     ShArgs a = make_sh_args(normals, normals_stride, albedo, albedo_stride, coefficients, coefficients_per_item, B, V, C);
     a.grad_out = grad_out;
@@ -1132,8 +1075,7 @@ extern "C" int dirt_sh_lighting_backward(const float* normals, long long normals
         if (rc != DIRT_OK) return rc;
     }
     // with no points only the memset of a wanted coefficient gradient is enqueued
-    CUDA_TRY(launch_sh_lighting_backward(a, (cudaStream_t)cuda_stream, &launches));
-    t_last_launches = launches;
+    CUDA_TRY(launch_sh_lighting_backward(a, (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
@@ -1177,8 +1119,7 @@ extern "C" int dirt_shadow_forward(const float* positions, long long positions_s
                                    const float* shadow_map, int per_item, int SH, int SW, int radius, float softness,
                                    float bias, float* out, int B, long long V, void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!shadow_shape_ok(B, V, positions_stride, SH, SW, radius, softness, bias)) return DIRT_ERR_BAD_SHAPE;
     if ((long long)B * V == 0) return DIRT_OK;
     ShadowArgs a = make_shadow_args(positions, positions_stride, light_matrix, shadow_map, per_item, SH, SW, radius,
@@ -1187,8 +1128,7 @@ extern "C" int dirt_shadow_forward(const float* positions, long long positions_s
     int rc = shadow_inputs_check(a);
     if (rc == DIRT_OK) rc = required_check({out});
     if (rc != DIRT_OK) return rc;
-    CUDA_TRY(launch_shadow_forward(a, (cudaStream_t)cuda_stream, &launches));
-    t_last_launches = launches;
+    CUDA_TRY(launch_shadow_forward(a, (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
@@ -1198,8 +1138,7 @@ extern "C" int dirt_shadow_backward(const float* positions, long long positions_
                                     float* grad_shadow_map, void* workspace, size_t workspace_bytes, int B, long long V,
                                     void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!shadow_shape_ok(B, V, positions_stride, SH, SW, radius, softness, bias)) return DIRT_ERR_BAD_SHAPE;
     ShadowArgs a = make_shadow_args(positions, positions_stride, light_matrix, shadow_map, per_item, SH, SW, radius,
                                     softness, bias, B, V);
@@ -1215,8 +1154,7 @@ extern "C" int dirt_shadow_backward(const float* positions, long long positions_
         if (rc != DIRT_OK) return rc;
     }
     // with no points only the memsets of the wanted map and matrix gradients are enqueued
-    CUDA_TRY(launch_shadow_backward(a, (cudaStream_t)cuda_stream, &launches));
-    t_last_launches = launches;
+    CUDA_TRY(launch_shadow_backward(a, (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
@@ -1243,8 +1181,7 @@ extern "C" int dirt_shadow_backward_deterministic(const float* positions, long l
                                                   size_t workspace_bytes, void* scratch, size_t scratch_bytes, int B,
                                                   long long V, void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!shadow_shape_ok(B, V, positions_stride, SH, SW, radius, softness, bias) ||
         !shadow_det_shape_ok(B, V, per_item, SH, SW))
         return DIRT_ERR_BAD_SHAPE;
@@ -1268,8 +1205,7 @@ extern "C" int dirt_shadow_backward_deterministic(const float* positions, long l
         if (rc != DIRT_OK) return rc;
     }
     CUDA_TRY(launch_shadow_backward_deterministic(a, carve_shadow_det_scratch(sorts ? scratch : nullptr, a),
-                                                  (cudaStream_t)cuda_stream, &launches));
-    t_last_launches = launches;
+                                                  (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
@@ -1310,8 +1246,7 @@ extern "C" int dirt_normals_forward(int mode, const float* vertices, long long v
                                     float* normals, void* workspace, size_t workspace_bytes, int B, long long V, long long F,
                                     void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!normals_shape_ok(mode, B, V, F, vertex_stride)) return DIRT_ERR_BAD_SHAPE;
     if ((long long)B * V == 0) return DIRT_OK;
     const int rc = normals_check(vertices, faces, workspace, workspace_bytes, B, V, F);
@@ -1321,8 +1256,7 @@ extern "C" int dirt_normals_forward(int mode, const float* vertices, long long v
     NormalsArgs a = make_normals_args(mode, vertices, vertex_stride, faces, B, V, F);
     a.out = normals;
     CUDA_TRY(launch_normals_forward(a, carve_normals_workspace(F > 0 ? workspace : nullptr, B, V, F),
-                                    (cudaStream_t)cuda_stream, &launches));
-    t_last_launches = launches;
+                                    (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
@@ -1330,8 +1264,7 @@ extern "C" int dirt_normals_backward(int mode, const float* vertices, long long 
                                      const float* grad_normals, float* grad_vertices, void* workspace,
                                      size_t workspace_bytes, int B, long long V, long long F, void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!normals_shape_ok(mode, B, V, F, vertex_stride)) return DIRT_ERR_BAD_SHAPE;
     if ((long long)B * V == 0) return DIRT_OK;
     const int rc = normals_check(vertices, faces, workspace, workspace_bytes, B, V, F);
@@ -1342,8 +1275,7 @@ extern "C" int dirt_normals_backward(int mode, const float* vertices, long long 
     a.grad = grad_normals;
     a.g_vertices = grad_vertices;
     CUDA_TRY(launch_normals_backward(a, carve_normals_workspace(F > 0 ? workspace : nullptr, B, V, F),
-                                     (cudaStream_t)cuda_stream, &launches));
-    t_last_launches = launches;
+                                     (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
@@ -1388,8 +1320,7 @@ extern "C" int dirt_tangents_forward(const float* vertices, long long vertex_str
                                      const int32_t* faces, float* tangents, void* workspace, size_t workspace_bytes, int B,
                                      long long V, long long F, void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!tangents_shape_ok(B, V, F, vertex_stride, uv_stride, uv_item_stride, normals_stride)) return DIRT_ERR_BAD_SHAPE;
     if ((long long)B * V == 0) return DIRT_OK;
     const int rc = tangents_check(vertices, uvs, normals, faces, workspace, workspace_bytes, B, V, F);
@@ -1400,8 +1331,7 @@ extern "C" int dirt_tangents_forward(const float* vertices, long long vertex_str
                                       faces, B, V, F);
     a.out = tangents;
     CUDA_TRY(launch_tangents_forward(a, carve_normals_workspace(F > 0 ? workspace : nullptr, B, V, F),
-                                     (cudaStream_t)cuda_stream, &launches));
-    t_last_launches = launches;
+                                     (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
@@ -1411,8 +1341,7 @@ extern "C" int dirt_tangents_backward(const float* vertices, long long vertex_st
                                       float* grad_uvs, float* grad_normals, void* workspace, size_t workspace_bytes, int B,
                                       long long V, long long F, void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!tangents_shape_ok(B, V, F, vertex_stride, uv_stride, uv_item_stride, normals_stride)) return DIRT_ERR_BAD_SHAPE;
     if ((uintptr_t)grad_vertices % 4 || (uintptr_t)grad_uvs % 4 || (uintptr_t)grad_normals % 4) return DIRT_ERR_MISALIGNED;
     if ((long long)B * V == 0 || (!grad_vertices && !grad_uvs && !grad_normals)) return DIRT_OK;
@@ -1425,8 +1354,7 @@ extern "C" int dirt_tangents_backward(const float* vertices, long long vertex_st
     a.grad = grad_tangents;
     a.g_vertices = grad_vertices; a.g_uvs = grad_uvs; a.g_normals = grad_normals;
     CUDA_TRY(launch_tangents_backward(a, carve_normals_workspace(F > 0 ? workspace : nullptr, B, V, F),
-                                      (cudaStream_t)cuda_stream, &launches));
-    t_last_launches = launches;
+                                      (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
@@ -1444,8 +1372,7 @@ extern "C" int dirt_normal_map_forward(const float* normals, long long normals_s
                                        long long tangents_stride, const float* samples, long long samples_stride,
                                        float* out, int B, long long V, void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!points_shape_ok(B, V, 4, {normals_stride, tangents_stride, samples_stride})) return DIRT_ERR_BAD_SHAPE;
     if ((long long)B * V == 0) return DIRT_OK;
     NormalMapArgs a = make_normal_map_args(normals, normals_stride, tangents, tangents_stride, samples, samples_stride, B, V);
@@ -1453,8 +1380,7 @@ extern "C" int dirt_normal_map_forward(const float* normals, long long normals_s
     if (rc == DIRT_OK) rc = required_check({out});
     if (rc != DIRT_OK) return rc;
     a.out = out;
-    CUDA_TRY(launch_normal_map_forward(a, (cudaStream_t)cuda_stream, &launches));
-    t_last_launches = launches;
+    CUDA_TRY(launch_normal_map_forward(a, (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
@@ -1463,8 +1389,7 @@ extern "C" int dirt_normal_map_backward(const float* normals, long long normals_
                                         const float* grad_out, float* grad_normals, float* grad_tangents,
                                         float* grad_samples, int B, long long V, void* cuda_stream)
 {
-    int launches = 0;
-    t_last_launches = 0;
+    launch_count() = 0;
     if (!points_shape_ok(B, V, 4, {normals_stride, tangents_stride, samples_stride})) return DIRT_ERR_BAD_SHAPE;
     if (!aligned({grad_normals, grad_tangents, grad_samples})) return DIRT_ERR_MISALIGNED;
     if ((long long)B * V == 0 || (!grad_normals && !grad_tangents && !grad_samples)) return DIRT_OK;
@@ -1474,8 +1399,7 @@ extern "C" int dirt_normal_map_backward(const float* normals, long long normals_
     if (rc != DIRT_OK) return rc;
     a.grad_out = grad_out;
     a.g_normals = grad_normals; a.g_tangents = grad_tangents; a.g_samples = grad_samples;
-    CUDA_TRY(launch_normal_map_backward(a, (cudaStream_t)cuda_stream, &launches));
-    t_last_launches = launches;
+    CUDA_TRY(launch_normal_map_backward(a, (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 

@@ -885,13 +885,13 @@ static cudaError_t launch_tile_kernel(const CUtensorMap& px_map, const CUtensorM
         kernel<<<grid, NW * 32, smem, stream>>>(px_map, ids_map, vertices, pixels, grad_pixels, face_ids, grad_background,
                                                 grad_vertices, grad_vertex_colors, ws, d, tflags, cs, c0, gstride, flags, expect_tag, b_base);
     }
-    return cudaGetLastError();
+    return launched();   // one logical launch, however many image slices it took
 }
 
 cudaError_t launch_backward(const float* vertices, const float* pixels, const float* grad_pixels,
                             const int32_t* face_ids, float* grad_background, float* grad_vertices,
                             float* grad_vertex_colors, const Workspace& ws, const Dims& d, const GroupSpec& groups,
-                            bool tile_flags_valid, int flags, unsigned long long expect_tag, cudaStream_t stream, int* launches)
+                            bool tile_flags_valid, int flags, unsigned long long expect_tag, cudaStream_t stream)
 {
     cudaError_t e;
     const size_t rows = (size_t)((flags & BWD_SHARED_GEOMETRY) ? 1 : d.B) * d.V;
@@ -911,8 +911,7 @@ cudaError_t launch_backward(const float* vertices, const float* pixels, const fl
         if (!padded) return cudaSuccess;
         const long long n = (long long)rows * 3;
         unpad_rows_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(grad_vertex_colors, gc_out, (long long)rows);
-        ++*launches;
-        return cudaGetLastError();
+        return launched();
     };
     const long long total_tiles = (long long)d.B * d.btiles;
     if (total_tiles == 0) return finish();
@@ -940,7 +939,6 @@ cudaError_t launch_backward(const float* vertices, const float* pixels, const fl
          : launch_tile_kernel<CC, NSLOT, false>(px_map, ids_map, vertices, pixels, grad_pixels, face_ids, grad_background,      \
                                                 grad_vertices, grad_vertex_colors, ws, d, tflags, d.C, c0, gstride, flags, expect_tag, stream))
     if (fused4) {
-        ++*launches;
         const cudaError_t le = DIRT_LAUNCH(4, DIRT_BWD_SLOTS_C4, 0);
         return le != cudaSuccess ? le : finish();
     }
@@ -948,7 +946,6 @@ cudaError_t launch_backward(const float* vertices, const float* pixels, const fl
     for (int g = 0; g < groups.n; ++g) {
         const cudaError_t le = groups.width[g] == 3 ? DIRT_LAUNCH(3, DIRT_BWD_SLOTS_C3, c0) : DIRT_LAUNCH(1, DIRT_BWD_SLOTS_C3, c0);
         c0 += groups.width[g];
-        ++*launches;
         if (le != cudaSuccess) return le;
     }
 #undef DIRT_LAUNCH

@@ -116,7 +116,7 @@ __global__ void __launch_bounds__(DERIV_THREADS) derivatives_kernel(DerivArgs a)
 
 cudaError_t launch_gbuffer_derivatives(const int32_t* face_ids, const float* attributes, float* out, const Workspace& ws,
                                        const Dims& d, int first_channel, int count, unsigned long long expect_tag,
-                                       cudaStream_t stream, int* launches)
+                                       cudaStream_t stream)
 {
     DerivArgs a;
     a.face_ids = face_ids; a.attributes = attributes; a.out = out; a.itp = ws.itp; a.header = ws.header;
@@ -144,8 +144,7 @@ cudaError_t launch_gbuffer_derivatives(const int32_t* face_ids, const float* att
         derivatives_kernel<4, false><<<blocks, DERIV_THREADS, 0, stream>>>(a);
     else
         derivatives_kernel<0, false><<<blocks, DERIV_THREADS, 0, stream>>>(a);
-    ++*launches;
-    return cudaGetLastError();
+    return launched();
 }
 
 }  // namespace dirt

@@ -355,7 +355,7 @@ cudaError_t launch_backward_deterministic(const float* vertices, const int32_t* 
                                           const float* grad_pixels, const int32_t* face_ids, float* grad_background,
                                           float* grad_vertices, float* grad_vertex_colors, const Workspace& ws, const Dims& d,
                                           const GroupSpec& groups, int flags, unsigned long long expect_tag,
-                                          const DetScratch& s, cudaStream_t stream, int* launches)
+                                          const DetScratch& s, cudaStream_t stream)
 {
     cudaError_t e;
     const long long px = (long long)d.B * d.H * d.W, faces_n = (long long)d.B * d.F;
@@ -376,32 +376,26 @@ cudaError_t launch_backward_deterministic(const float* vertices, const int32_t* 
         const bool three = groups.width[g] == 3;
         if (three) det_record_kernel<3><<<det_blocks(px, DET_THREADS), DET_THREADS, 0, stream>>>(a);
         else det_record_kernel<1><<<det_blocks(px, DET_THREADS), DET_THREADS, 0, stream>>>(a);
-        if ((e = cudaGetLastError()) != cudaSuccess) return e;
-        ++*launches;
+        if ((e = launched()) != cudaSuccess) return e;
         if (faces_n > 0) {
             if (three) det_face_warp_kernel<3><<<det_blocks(faces_n, DET_WARPS), DET_THREADS, 0, stream>>>(a);
             else det_face_warp_kernel<1><<<det_blocks(faces_n, DET_WARPS), DET_THREADS, 0, stream>>>(a);
-            if ((e = cudaGetLastError()) != cudaSuccess) return e;
-            ++*launches;
+            if ((e = launched()) != cudaSuccess) return e;
             if (three) det_face_cta_kernel<3><<<large_ctas, DET_THREADS, 0, stream>>>(a);
             else det_face_cta_kernel<1><<<large_ctas, DET_THREADS, 0, stream>>>(a);
-            if ((e = cudaGetLastError()) != cudaSuccess) return e;
-            ++*launches;
+            if ((e = launched()) != cudaSuccess) return e;
         }
         c0 += groups.width[g];
     }
     const bool shared = (flags & BWD_SHARED_GEOMETRY) != 0;
     const long long rows = shared ? (long long)d.V : (long long)d.B * d.V;
     if (rows == 0) return cudaSuccess;
-    if ((e = launch_corner_adjacency(faces, 3ll * d.F, d.B, d.V, d.F, s.counts, s.offsets, s.unsorted, s.inc, stream, launches)) !=
-        cudaSuccess)
+    if ((e = launch_corner_adjacency(faces, 3ll * d.F, d.B, d.V, d.F, s.counts, s.offsets, s.unsorted, s.inc, stream)) != cudaSuccess)
         return e;
     det_vertex_kernel<<<det_blocks(rows, DET_THREADS), DET_THREADS, 0, stream>>>(s.offsets, s.inc, s.partial, grad_vertices,
                                                                                  grad_vertex_colors, d.B, d.V, d.F, d.C, shared,
                                                                                  ws.header, expect_tag);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    ++*launches;
-    return cudaSuccess;
+    return launched();
 }
 
 }  // namespace dirt

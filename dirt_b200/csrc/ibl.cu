@@ -614,7 +614,7 @@ GgxLayout ggx_layout(const TexDims& d)
     return g;
 }
 
-cudaError_t launch_ggx_prefilter(const float* cubemap, float* atlas, const TexDims& d, cudaStream_t stream, int* launches)
+cudaError_t launch_ggx_prefilter(const float* cubemap, float* atlas, const TexDims& d, cudaStream_t stream)
 {
     const IblLevels p0 = ibl_levels(d);
     if (p0.L == 1 || d.TB == 0) return cudaSuccess;
@@ -628,14 +628,12 @@ cudaError_t launch_ggx_prefilter(const float* cubemap, float* atlas, const TexDi
     pd.texels = (long long)p0.S * p0.S;
     pd.total = 0;
     pd.mode = DIRT_TEXTURE_BILINEAR;
-    if (p0.ss > 0 && (e = launch_texture_mip_build(cubemap, atlas, pd, stream, launches)) != cudaSuccess) return e;
+    if (p0.ss > 0 && (e = launch_texture_mip_build(cubemap, atlas, pd, stream)) != cudaSuccess) return e;
     float4* cones = reinterpret_cast<float4*>(atlas + g.cones);
     ggx_texel_table_kernel<<<ibl_blocks(p0.table[p0.L]), IBL_THREADS, 0, stream>>>(table, p0);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    ++*launches;
+    if ((e = launched()) != cudaSuccess) return e;
     ggx_cone_table_kernel<<<ibl_blocks(p0.cone[p0.L]), IBL_THREADS, 0, stream>>>(cones, p0);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    ++*launches;
+    if ((e = launched()) != cudaSuccess) return e;
     IblLevels p = p0;
     int levels[MIP_MAX_LEVELS];
     for (int k = 1; k < p.L; ++k) levels[k - 1] = k;
@@ -645,16 +643,15 @@ cudaError_t launch_ggx_prefilter(const float* cubemap, float* atlas, const TexDi
         e = with_nv(d.C - c0, [&](auto nv) {
             ggx_prefilter_kernel<decltype(nv)::value><<<grid, IBL_THREADS, 0, stream>>>(
                 cubemap, atlas, table, cones, atlas + g.levels, atlas + g.weights, p, c0, c0 == 0);
-            return cudaGetLastError();
+            return launched();
         });
         if (e != cudaSuccess) return e;
-        ++*launches;
     }
     return cudaSuccess;
 }
 
 cudaError_t launch_ggx_prefilter_adjoint(const float* atlas, const float* level_grad, float* src_grad, float* grad_cubemap,
-                                         const TexDims& d, cudaStream_t stream, int* launches)
+                                         const TexDims& d, cudaStream_t stream)
 {
     IblLevels p = ibl_levels(d);
     if (p.L == 1 || d.TB == 0) return cudaSuccess;
@@ -668,20 +665,17 @@ cudaError_t launch_ggx_prefilter_adjoint(const float* atlas, const float* level_
             ggx_prefilter_adjoint_kernel<decltype(nv)::value><<<grid, IBL_THREADS, 0, stream>>>(
                 level_grad, atlas + g.weights, reinterpret_cast<const float4*>(atlas + g.table),
                 reinterpret_cast<const float4*>(atlas + g.cones), src_grad, grad_cubemap, p, c0);
-            return cudaGetLastError();
+            return launched();
         });
         if (e != cudaSuccess) return e;
-        ++*launches;
     }
     return cudaSuccess;
 }
 
-cudaError_t launch_ggx_brdf_table(float* table, int N, cudaStream_t stream, int* launches)
+cudaError_t launch_ggx_brdf_table(float* table, int N, cudaStream_t stream)
 {
     ggx_brdf_table_kernel<<<(N * N + 127) / 128, 128, 0, stream>>>(table, N);
-    const cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) ++*launches;
-    return e;
+    return launched();
 }
 
 // the SH projection's scratch: level 0's texel table, then the partial sums
@@ -703,8 +697,7 @@ size_t sh_project_scratch_bytes(int TB, int S, int C)
     return align_up(sizeof(float4) * 6 * (size_t)S * S, 256) + sizeof(double) * (size_t)TB * cube_sh_chunks(S) * 9 * C;
 }
 
-cudaError_t launch_sh_project(const float* cubemap, float* coeffs, void* scratch, int TB, int S, int C, cudaStream_t stream,
-                              int* launches)
+cudaError_t launch_sh_project(const float* cubemap, float* coeffs, void* scratch, int TB, int S, int C, cudaStream_t stream)
 {
     const IblLevels p = sh_levels(TB, S, C);
     float4* table = static_cast<float4*>(scratch);
@@ -712,32 +705,25 @@ cudaError_t launch_sh_project(const float* cubemap, float* coeffs, void* scratch
     const int chunks = cube_sh_chunks(S);
     cudaError_t e;
     ggx_texel_table_kernel<<<ibl_blocks(p.table[1]), IBL_THREADS, 0, stream>>>(table, p);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    ++*launches;
+    if ((e = launched()) != cudaSuccess) return e;
     const dim3 grid((unsigned)(chunks < IBL_MAX_BLOCKS ? chunks : IBL_MAX_BLOCKS), TB < IBL_MAX_ITEMS ? TB : IBL_MAX_ITEMS);
     sh_project_partial_kernel<<<grid, IBL_THREADS, 0, stream>>>(cubemap, table, partial, p.table[1], TB, C, chunks);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    ++*launches;
+    if ((e = launched()) != cudaSuccess) return e;
     sh_project_final_kernel<<<ibl_blocks((long long)TB * 9 * C), IBL_THREADS, 0, stream>>>(partial, coeffs, TB, C, chunks);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    ++*launches;
-    return cudaSuccess;
+    return launched();
 }
 
 cudaError_t launch_sh_project_backward(const float* grad_coeffs, float* grad_cubemap, void* scratch, int TB, int S, int C,
-                                       cudaStream_t stream, int* launches)
+                                       cudaStream_t stream)
 {
     const IblLevels p = sh_levels(TB, S, C);
     float4* table = static_cast<float4*>(scratch);
     cudaError_t e;
     ggx_texel_table_kernel<<<ibl_blocks(p.table[1]), IBL_THREADS, 0, stream>>>(table, p);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    ++*launches;
+    if ((e = launched()) != cudaSuccess) return e;
     sh_project_backward_kernel<<<ibl_blocks((long long)TB * p.table[1] * C), IBL_THREADS, 0, stream>>>(
         table, grad_coeffs, grad_cubemap, p.table[1], TB, C);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    ++*launches;
-    return cudaSuccess;
+    return launched();
 }
 
 }  // namespace dirt

@@ -286,7 +286,7 @@ cudaError_t latlong_forward_ct(const float* panorama, float* cubemap, const LlDi
     } else {
         latlong_forward_kernel<CT, false><<<blocks, LL_THREADS, 0, stream>>>(panorama, cubemap, d);
     }
-    return cudaGetLastError();
+    return launched();
 }
 
 }  // namespace
@@ -299,23 +299,20 @@ int latlong_samples(int H, int W, int S)
 }
 
 cudaError_t launch_latlong_forward(const float* panorama, float* cubemap, int TB, int H, int W, int S, int C,
-                                   cudaStream_t stream, int* launches)
+                                   cudaStream_t stream)
 {
     const LlDims d = {TB, H, W, S, C, latlong_samples(H, W, S)};
-    cudaError_t e;
     switch (C) {
-        case 1: e = latlong_forward_ct<1>(panorama, cubemap, d, stream); break;
-        case 2: e = latlong_forward_ct<2>(panorama, cubemap, d, stream); break;
-        case 3: e = latlong_forward_ct<3>(panorama, cubemap, d, stream); break;
-        case 4: e = latlong_forward_ct<4>(panorama, cubemap, d, stream); break;
-        default: e = latlong_forward_ct<0>(panorama, cubemap, d, stream); break;
+        case 1: return latlong_forward_ct<1>(panorama, cubemap, d, stream);
+        case 2: return latlong_forward_ct<2>(panorama, cubemap, d, stream);
+        case 3: return latlong_forward_ct<3>(panorama, cubemap, d, stream);
+        case 4: return latlong_forward_ct<4>(panorama, cubemap, d, stream);
+        default: return latlong_forward_ct<0>(panorama, cubemap, d, stream);
     }
-    if (e == cudaSuccess) ++*launches;
-    return e;
 }
 
 cudaError_t launch_latlong_backward(const float* grad_cubemap, float* grad_panorama, int TB, int H, int W, int S, int C,
-                                    cudaStream_t stream, int* launches)
+                                    cudaStream_t stream)
 {
     const LlDims d = {TB, H, W, S, C, latlong_samples(H, W, S)};
     const dim3 grid(ll_blocks((long long)H * W), TB < LL_MAX_ITEMS ? TB : LL_MAX_ITEMS);
@@ -326,9 +323,8 @@ cudaError_t launch_latlong_backward(const float* grad_cubemap, float* grad_panor
             case 3: latlong_backward_kernel<3><<<grid, LL_THREADS, 0, stream>>>(grad_cubemap, grad_panorama, d, c0); break;
             default: latlong_backward_kernel<4><<<grid, LL_THREADS, 0, stream>>>(grad_cubemap, grad_panorama, d, c0); break;
         }
-        const cudaError_t e = cudaGetLastError();
+        const cudaError_t e = launched();
         if (e != cudaSuccess) return e;
-        ++*launches;
     }
     return cudaSuccess;
 }

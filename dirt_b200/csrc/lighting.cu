@@ -405,16 +405,14 @@ cudaError_t zero_params(const ReduceJobs& jobs, cudaStream_t stream)
 }
 
 // after the point kernel: adds the partial rows of every job in a fixed order
-cudaError_t reduce_params(const LightArgs& a, const ReduceJobs& jobs, cudaStream_t stream, int* launches)
+cudaError_t reduce_params(const LightArgs& a, const ReduceJobs& jobs, cudaStream_t stream)
 {
     if (!jobs.count) return cudaSuccess;
     const long long total = jobs.first[jobs.count];
     const unsigned blocks = (unsigned)(total < REDUCE_MAX_BLOCKS ? total : REDUCE_MAX_BLOCKS);
     lighting_reduce_kernel<<<blocks, REDUCE_THREADS, 0, stream>>>(a.partial, jobs, total, a.chunks, a.B,
                                                                   LIGHT_FIXED_PARAMS + a.C);
-    const cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) ++*launches;
-    return e;
+    return launched();
 }
 
 }  // namespace
@@ -425,7 +423,7 @@ dim3 light_grid(long long chunks, int B)
 }
 
 cudaError_t launch_partials_reduce(const float* partial, float* out, int width, bool per_item, long long chunks, int B,
-                                   cudaStream_t stream, int* launches)
+                                   cudaStream_t stream)
 {
     ReduceJobs jobs = {};
     jobs.count = 1;
@@ -434,12 +432,10 @@ cudaError_t launch_partials_reduce(const float* partial, float* out, int width, 
     jobs.first[0] = 0; jobs.first[1] = total;
     const unsigned blocks = (unsigned)(total < REDUCE_MAX_BLOCKS ? total : REDUCE_MAX_BLOCKS);
     lighting_reduce_kernel<<<blocks, REDUCE_THREADS, 0, stream>>>(partial, jobs, total, chunks, B, width);
-    const cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) ++*launches;
-    return e;
+    return launched();
 }
 
-cudaError_t launch_lighting_forward(const LightArgs& a, cudaStream_t stream, int* launches)
+cudaError_t launch_lighting_forward(const LightArgs& a, cudaStream_t stream)
 {
     if ((long long)a.B * a.V == 0) return cudaSuccess;
     switch (a.model) {
@@ -447,12 +443,10 @@ cudaError_t launch_lighting_forward(const LightArgs& a, cudaStream_t stream, int
         case SP: forward_m<SP>(a, stream); break;
         default: forward_m<DP>(a, stream);
     }
-    const cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) ++*launches;
-    return e;
+    return launched();
 }
 
-cudaError_t launch_lighting_backward(const LightArgs& a, cudaStream_t stream, int* launches)
+cudaError_t launch_lighting_backward(const LightArgs& a, cudaStream_t stream)
 {
     const bool sp = a.model == SP;
     const ReduceJobs jobs = param_jobs(a, sp, sp);
@@ -467,9 +461,8 @@ cudaError_t launch_lighting_backward(const LightArgs& a, cudaStream_t stream, in
         case SP: backward_m<SP>(b, stream); break;
         default: backward_m<DP>(b, stream);
     }
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    ++*launches;
-    return reduce_params(b, jobs, stream, launches);
+    if ((e = launched()) != cudaSuccess) return e;
+    return reduce_params(b, jobs, stream);
 }
 
 // ---- GGX microfacet specular reflectance (dirt_ggx_lighting_*, DESIGN.md §7.9) ---------------------------------------
@@ -773,16 +766,14 @@ void ggx_dispatch(const LightArgs& a, bool forward, cudaStream_t stream)
 
 }  // namespace
 
-cudaError_t launch_ggx_forward(const LightArgs& a, cudaStream_t stream, int* launches)
+cudaError_t launch_ggx_forward(const LightArgs& a, cudaStream_t stream)
 {
     if ((long long)a.B * a.V == 0) return cudaSuccess;
     ggx_dispatch(a, true, stream);
-    const cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) ++*launches;
-    return e;
+    return launched();
 }
 
-cudaError_t launch_ggx_backward(const LightArgs& a, cudaStream_t stream, int* launches)
+cudaError_t launch_ggx_backward(const LightArgs& a, cudaStream_t stream)
 {
     const ReduceJobs jobs = param_jobs(a, true, false);
     if ((long long)a.B * a.V == 0) return zero_params(jobs, stream);
@@ -790,10 +781,9 @@ cudaError_t launch_ggx_backward(const LightArgs& a, cudaStream_t stream, int* la
     LightArgs b = a;
     if (!jobs.count) b.partial = nullptr;
     ggx_dispatch(b, false, stream);
-    const cudaError_t e = cudaGetLastError();
+    const cudaError_t e = launched();
     if (e != cudaSuccess) return e;
-    ++*launches;
-    return reduce_params(b, jobs, stream, launches);
+    return reduce_params(b, jobs, stream);
 }
 
 // ---- spherical-harmonics environment lighting (dirt_sh_lighting_*, DESIGN.md §7.8) ------------------------------------
@@ -972,18 +962,16 @@ __global__ void __launch_bounds__(LIGHT_THREADS) sh_backward_kernel(ShArgs a)
 
 }  // namespace
 
-cudaError_t launch_sh_lighting_forward(const ShArgs& a, cudaStream_t stream, int* launches)
+cudaError_t launch_sh_lighting_forward(const ShArgs& a, cudaStream_t stream)
 {
     if ((long long)a.B * a.V == 0) return cudaSuccess;
     const dim3 grid = light_grid(light_chunks(a.V), a.B);
     if (a.C == 3) sh_forward_kernel<3><<<grid, LIGHT_THREADS, 0, stream>>>(a);
     else sh_forward_kernel<0><<<grid, LIGHT_THREADS, 0, stream>>>(a);
-    const cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) ++*launches;
-    return e;
+    return launched();
 }
 
-cudaError_t launch_sh_lighting_backward(const ShArgs& a, cudaStream_t stream, int* launches)
+cudaError_t launch_sh_lighting_backward(const ShArgs& a, cudaStream_t stream)
 {
     const long long width = 9ll * a.C, total = (a.item_coef ? (long long)a.B : 1ll) * width;
     cudaError_t e;
@@ -998,11 +986,10 @@ cudaError_t launch_sh_lighting_backward(const ShArgs& a, cudaStream_t stream, in
     const dim3 grid = light_grid(a.chunks, a.B);
     if (a.C == 3) sh_backward_kernel<3><<<grid, LIGHT_THREADS, 0, stream>>>(b);
     else sh_backward_kernel<0><<<grid, LIGHT_THREADS, 0, stream>>>(b);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    ++*launches;
+    if ((e = launched()) != cudaSuccess) return e;
     if (a.g_coef) {
         // one job: the [9, C] columns of the partials, per item or over every item
-        return launch_partials_reduce(b.partial, a.g_coef, (int)width, a.item_coef, a.chunks, a.B, stream, launches);
+        return launch_partials_reduce(b.partial, a.g_coef, (int)width, a.item_coef, a.chunks, a.B, stream);
     }
     return cudaSuccess;
 }
@@ -1140,22 +1127,18 @@ __global__ void __launch_bounds__(LIGHT_THREADS) normal_map_backward_kernel(Norm
 
 }  // namespace
 
-cudaError_t launch_normal_map_forward(const NormalMapArgs& a, cudaStream_t stream, int* launches)
+cudaError_t launch_normal_map_forward(const NormalMapArgs& a, cudaStream_t stream)
 {
     if ((long long)a.B * a.V == 0) return cudaSuccess;
     normal_map_forward_kernel<<<light_grid(light_chunks(a.V), a.B), LIGHT_THREADS, 0, stream>>>(a);
-    const cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) ++*launches;
-    return e;
+    return launched();
 }
 
-cudaError_t launch_normal_map_backward(const NormalMapArgs& a, cudaStream_t stream, int* launches)
+cudaError_t launch_normal_map_backward(const NormalMapArgs& a, cudaStream_t stream)
 {
     if ((long long)a.B * a.V == 0 || (!a.g_normals && !a.g_tangents && !a.g_samples)) return cudaSuccess;
     normal_map_backward_kernel<<<light_grid(light_chunks(a.V), a.B), LIGHT_THREADS, 0, stream>>>(a);
-    const cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) ++*launches;
-    return e;
+    return launched();
 }
 
 }  // namespace dirt

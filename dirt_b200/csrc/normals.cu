@@ -524,32 +524,27 @@ NormalsWorkspace carve_normals_workspace(void* base, int B, long long V, long lo
 }
 
 cudaError_t launch_corner_adjacency(const int* faces, long long face_stride, int items, int V, int F, int* counts, int* offsets,
-                                    int* unsorted, int* inc, cudaStream_t stream, int* launches)
+                                    int* unsorted, int* inc, cudaStream_t stream)
 {
     cudaError_t e;
     const long long rows = (long long)items * V, corners = 3ll * items * F;
     if ((e = cudaMemsetAsync(counts, 0, sizeof(int) * (size_t)rows, stream)) != cudaSuccess) return e;
     count_kernel<<<blocks_for(corners / 3), NORMALS_THREADS, 0, stream>>>(faces, face_stride, items, F, V, counts);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    ++*launches;
+    if ((e = launched()) != cudaSuccess) return e;
     scan_kernel<<<1, SCAN_THREADS, 0, stream>>>(counts, rows, offsets);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    ++*launches;
+    if ((e = launched()) != cudaSuccess) return e;
     fill_kernel<<<blocks_for(corners / 3), NORMALS_THREADS, 0, stream>>>(faces, face_stride, items, F, V, offsets, counts, unsorted);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    ++*launches;
+    if ((e = launched()) != cudaSuccess) return e;
     rank_kernel<<<blocks_for(corners), NORMALS_THREADS, 0, stream>>>(faces, face_stride, items, F, offsets, unsorted, inc, V);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    ++*launches;
-    return cudaSuccess;
+    return launched();
 }
 
-cudaError_t launch_normals_forward(NormalsArgs a, const NormalsWorkspace& w, cudaStream_t stream, int* launches)
+cudaError_t launch_normals_forward(NormalsArgs a, const NormalsWorkspace& w, cudaStream_t stream)
 {
     cudaError_t e;
     if (a.total == 0) return cudaSuccess;
     if (a.F == 0) return cudaMemsetAsync(a.out, 0, sizeof(float) * 3 * (size_t)a.total, stream);
-    if ((e = launch_corner_adjacency(a.faces, 0, 1, a.V, a.F, w.counts, w.offsets, w.unsorted, w.inc, stream, launches)) != cudaSuccess)
+    if ((e = launch_corner_adjacency(a.faces, 0, 1, a.V, a.F, w.counts, w.offsets, w.unsorted, w.inc, stream)) != cudaSuccess)
         return e;
     a.offsets = w.offsets;
     a.inc = w.inc;
@@ -557,12 +552,10 @@ cudaError_t launch_normals_forward(NormalsArgs a, const NormalsWorkspace& w, cud
         normals_forward_kernel<DIRT_NORMALS_AVERAGE><<<blocks_for(a.total), NORMALS_THREADS, 0, stream>>>(a);
     else
         normals_forward_kernel<DIRT_NORMALS_PRE_SPLIT><<<blocks_for(a.total), NORMALS_THREADS, 0, stream>>>(a);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    ++*launches;
-    return cudaSuccess;
+    return launched();
 }
 
-cudaError_t launch_normals_backward(NormalsArgs a, const NormalsWorkspace& w, cudaStream_t stream, int* launches)
+cudaError_t launch_normals_backward(NormalsArgs a, const NormalsWorkspace& w, cudaStream_t stream)
 {
     cudaError_t e;
     if (a.total == 0) return cudaSuccess;
@@ -572,34 +565,28 @@ cudaError_t launch_normals_backward(NormalsArgs a, const NormalsWorkspace& w, cu
     a.gs = w.gs;
     if (a.mode == DIRT_NORMALS_AVERAGE) {
         normals_sum_grad_kernel<<<blocks_for(a.total), NORMALS_THREADS, 0, stream>>>(a);
-        if ((e = cudaGetLastError()) != cudaSuccess) return e;
-        ++*launches;
+        if ((e = launched()) != cudaSuccess) return e;
         normals_position_grad_kernel<DIRT_NORMALS_AVERAGE><<<blocks_for(a.total), NORMALS_THREADS, 0, stream>>>(a);
     } else {
         normals_position_grad_kernel<DIRT_NORMALS_PRE_SPLIT><<<blocks_for(a.total), NORMALS_THREADS, 0, stream>>>(a);
     }
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    ++*launches;
-    return cudaSuccess;
+    return launched();
 }
 
-cudaError_t launch_tangents_forward(TangentArgs a, const NormalsWorkspace& w, cudaStream_t stream, int* launches)
+cudaError_t launch_tangents_forward(TangentArgs a, const NormalsWorkspace& w, cudaStream_t stream)
 {
     cudaError_t e;
     if (a.m.total == 0) return cudaSuccess;
     if (a.m.F > 0 &&
-        (e = launch_corner_adjacency(a.m.faces, 0, 1, a.m.V, a.m.F, w.counts, w.offsets, w.unsorted, w.inc, stream,
-                                     launches)) != cudaSuccess)
+        (e = launch_corner_adjacency(a.m.faces, 0, 1, a.m.V, a.m.F, w.counts, w.offsets, w.unsorted, w.inc, stream)) != cudaSuccess)
         return e;
     a.m.offsets = w.offsets;
     a.m.inc = w.inc;
     tangents_forward_kernel<<<blocks_for(a.m.total), NORMALS_THREADS, 0, stream>>>(a);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    ++*launches;
-    return cudaSuccess;
+    return launched();
 }
 
-cudaError_t launch_tangents_backward(TangentArgs a, const NormalsWorkspace& w, cudaStream_t stream, int* launches)
+cudaError_t launch_tangents_backward(TangentArgs a, const NormalsWorkspace& w, cudaStream_t stream)
 {
     cudaError_t e;
     if (a.m.total == 0) return cudaSuccess;
@@ -617,12 +604,10 @@ cudaError_t launch_tangents_backward(TangentArgs a, const NormalsWorkspace& w, c
     a.m.inc = w.inc;
     a.gt = corner ? w.gs : nullptr;
     tangents_vertex_grad_kernel<<<blocks_for(a.m.total), NORMALS_THREADS, 0, stream>>>(a);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    ++*launches;
+    if ((e = launched()) != cudaSuccess) return e;
     if (corner) {
         tangents_corner_grad_kernel<<<blocks_for(a.m.total), NORMALS_THREADS, 0, stream>>>(a);
-        if ((e = cudaGetLastError()) != cudaSuccess) return e;
-        ++*launches;
+        if ((e = launched()) != cudaSuccess) return e;
     }
     return cudaSuccess;
 }

@@ -463,8 +463,7 @@ __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32, DIRT_RASTER_MIN_BLOCKS) 
 }
 
 cudaError_t launch_raster_forward(const float* vertices, const float* background, const float* vertex_colors, float* pixels,
-                                  int32_t* face_ids_out, const Workspace& ws, const Dims& d, cudaStream_t stream,
-                                  int* launches)
+                                  int32_t* face_ids_out, const Workspace& ws, const Dims& d, cudaStream_t stream)
 {
     if ((long long)d.B * d.tiles == 0) return cudaSuccess;
     const dim3 grid((unsigned)((d.tiles_x + WARPS_PER_BLOCK * TILES_PER_WARP - 1) / (WARPS_PER_BLOCK * TILES_PER_WARP)), (unsigned)d.tiles_y, (unsigned)min(d.B, 65535));
@@ -486,18 +485,16 @@ cudaError_t launch_raster_forward(const float* vertices, const float* background
     else   // more than four channels (or a frame beyond the records' 16-bit reference pixel): barycentrics + colour gathers
         raster_kernel<0, 0, false><<<grid, WARPS_PER_BLOCK * 32, 0, stream>>>(vertices, background, vertex_colors, pixels,
                                                                               face_ids_out, nullptr, ws, d);
-    ++*launches;
-    return cudaGetLastError();
+    return launched();
 }
 
 cudaError_t launch_raster_visibility(const float* vertices, int32_t* face_ids, float* gbuffer, const Workspace& ws, const Dims& d,
-                                     cudaStream_t stream, int* launches)
+                                     cudaStream_t stream)
 {
     if ((long long)d.B * d.tiles == 0) return cudaSuccess;
     const dim3 grid((unsigned)((d.tiles_x + WARPS_PER_BLOCK * TILES_PER_WARP - 1) / (WARPS_PER_BLOCK * TILES_PER_WARP)), (unsigned)d.tiles_y, (unsigned)min(d.B, 65535));
     raster_kernel<1, 0, false><<<grid, WARPS_PER_BLOCK * 32, 0, stream>>>(vertices, nullptr, nullptr, nullptr, face_ids, gbuffer, ws, d);
-    ++*launches;
-    return cudaGetLastError();
+    return launched();
 }
 
 }  // namespace dirt

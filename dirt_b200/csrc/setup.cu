@@ -398,7 +398,7 @@ static unsigned setup_blocks(long long total)
 }
 
 cudaError_t launch_setup_and_bin(const float* vertices, const int32_t* faces, const float* vertex_colors, const Workspace& ws,
-                                 const Dims& d, cudaStream_t stream, int* launches)
+                                 const Dims& d, cudaStream_t stream)
 {
     if (!shade_records_ok(d)) vertex_colors = nullptr;
     const long long total = (long long)d.B * d.F;
@@ -407,20 +407,18 @@ cudaError_t launch_setup_and_bin(const float* vertices, const int32_t* faces, co
     // at least one block, even without faces: its first thread leaves the tag, which a later call reusing the workspace checks
     ScopedKernelTimer timer(3, stream);
     setup_kernel<true><<<setup_blocks(total), DIRT_SETUP_THREADS, 0, stream>>>(vertices, faces, vertex_colors, ws, d);
-    ++*launches;
-    return cudaGetLastError();
+    return launched();
 }
 
 cudaError_t launch_setup_only(const float* vertices, const int32_t* faces, const Workspace& ws, const Dims& d,
-                              cudaStream_t stream, int* launches)
+                              cudaStream_t stream)
 {
     const long long total = (long long)d.B * d.F;
     cudaError_t e;
     if ((e = cudaMemsetAsync(ws.header, 0, sizeof(Header), stream)) != cudaSuccess) return e;
     ScopedKernelTimer timer(3, stream);
     setup_kernel<false><<<setup_blocks(total), DIRT_SETUP_THREADS, 0, stream>>>(vertices, faces, nullptr, ws, d);
-    ++*launches;
-    return cudaGetLastError();
+    return launched();
 }
 
 }  // namespace dirt

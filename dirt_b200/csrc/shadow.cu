@@ -366,7 +366,7 @@ cudaError_t launch_rs(const ShadowArgs& a, ShadowKernel kind, const int* ids, co
         shadow_det_gather_kernel<R, SOFT><<<(unsigned)(blocks < DET_GRID ? blocks : DET_GRID), LIGHT_THREADS, 0, stream>>>(
             a, ids, offsets);
     }
-    return cudaGetLastError();
+    return launched();
 }
 
 template <int R>
@@ -389,15 +389,13 @@ cudaError_t launch_shadow(const ShadowArgs& a, ShadowKernel kind, cudaStream_t s
 
 }  // namespace
 
-cudaError_t launch_shadow_forward(const ShadowArgs& a, cudaStream_t stream, int* launches)
+cudaError_t launch_shadow_forward(const ShadowArgs& a, cudaStream_t stream)
 {
     if ((long long)a.B * a.V == 0) return cudaSuccess;
-    const cudaError_t e = launch_shadow(a, SHADOW_FORWARD, stream);
-    if (e == cudaSuccess) ++*launches;
-    return e;
+    return launch_shadow(a, SHADOW_FORWARD, stream);
 }
 
-cudaError_t launch_shadow_backward(const ShadowArgs& a, cudaStream_t stream, int* launches)
+cudaError_t launch_shadow_backward(const ShadowArgs& a, cudaStream_t stream)
 {
     const long long items = a.per_item ? a.B : 1;
     cudaError_t e;
@@ -411,9 +409,8 @@ cudaError_t launch_shadow_backward(const ShadowArgs& a, cudaStream_t stream, int
     ShadowArgs b = a;
     if (!a.g_matrix) b.partial = nullptr;
     if ((e = launch_shadow(b, SHADOW_BACKWARD, stream)) != cudaSuccess) return e;
-    ++*launches;
     if (!a.g_matrix) return cudaSuccess;
-    return launch_partials_reduce(b.partial, a.g_matrix, SHADOW_MATRIX, a.per_item, a.chunks, a.B, stream, launches);
+    return launch_partials_reduce(b.partial, a.g_matrix, SHADOW_MATRIX, a.per_item, a.chunks, a.B, stream);
 }
 
 ShadowDetScratch carve_shadow_det_scratch(void* base, const ShadowArgs& a)
@@ -437,26 +434,23 @@ ShadowDetScratch carve_shadow_det_scratch(void* base, const ShadowArgs& a)
     return s;
 }
 
-cudaError_t launch_shadow_backward_deterministic(const ShadowArgs& a, const ShadowDetScratch& s, cudaStream_t stream,
-                                                 int* launches)
+cudaError_t launch_shadow_backward_deterministic(const ShadowArgs& a, const ShadowDetScratch& s, cudaStream_t stream)
 {
     // the position and matrix gradients have no atomics: the default kernel writes them
-    if (!a.g_map || (long long)a.B * a.V == 0) return launch_shadow_backward(a, stream, launches);
+    if (!a.g_map || (long long)a.B * a.V == 0) return launch_shadow_backward(a, stream);
     cudaError_t e;
     ShadowArgs b = a;
     b.g_map = nullptr;
-    if ((a.g_positions || a.g_matrix) && (e = launch_shadow_backward(b, stream, launches)) != cudaSuccess) return e;
+    if ((a.g_positions || a.g_matrix) && (e = launch_shadow_backward(b, stream)) != cudaSuccess) return e;
     int last;
     if ((e = sort_by_key(ShadowKey{a, s.sentinel}, (long long)a.B * a.V, s.sentinel, s.keys, s.ids, s.counts,
-                         s.digit_total, stream, launches, &last)) != cudaSuccess)
+                         s.digit_total, stream, &last)) != cudaSuccess)
         return e;
     const long long bounds = ((long long)s.sentinel + 2 + RS_THREADS - 1) / RS_THREADS;
     tex_segment_bounds_kernel<<<(unsigned)(bounds < DET_GRID ? bounds : DET_GRID), RS_THREADS, 0, stream>>>(
         s.keys[last], (long long)a.B * a.V, s.sentinel, s.offsets);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    if ((e = launch_shadow(a, SHADOW_GATHER, stream, s.ids[last], s.offsets)) != cudaSuccess) return e;
-    *launches += 2;
-    return cudaSuccess;
+    if ((e = launched()) != cudaSuccess) return e;
+    return launch_shadow(a, SHADOW_GATHER, stream, s.ids[last], s.offsets);
 }
 
 }  // namespace dirt

@@ -163,7 +163,7 @@ inline int sort_passes(unsigned sentinel)
 // ids[*last].  n > 0.
 template <class Key>
 cudaError_t sort_by_key(const Key& key, long long n, unsigned sentinel, unsigned* const keys[2], int* const ids[2],
-                        unsigned* counts, unsigned* digit_total, cudaStream_t stream, int* launches, int* last)
+                        unsigned* counts, unsigned* digit_total, cudaStream_t stream, int* last)
 {
     cudaError_t e;
     const int tiles = (int)((n + RS_TILE - 1) / RS_TILE), passes = sort_passes(sentinel);
@@ -174,17 +174,16 @@ cudaError_t sort_by_key(const Key& key, long long n, unsigned sentinel, unsigned
         int* iout = ids[p & 1];
         if (p == 0) tex_sort_hist_kernel<true><<<tiles, RS_THREADS, 0, stream>>>(kin, key, n, 0, counts, tiles);
         else tex_sort_hist_kernel<false><<<tiles, RS_THREADS, 0, stream>>>(kin, key, n, 8 * p, counts, tiles);
-        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+        if ((e = launched()) != cudaSuccess) return e;
         tex_sort_scan_kernel<<<RS_RADIX, RS_THREADS, 0, stream>>>(counts, digit_total, tiles);
-        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+        if ((e = launched()) != cudaSuccess) return e;
         if (p == 0)
             tex_sort_scatter_kernel<true><<<tiles, RS_THREADS, 0, stream>>>(kin, iin, key, n, 0, counts, digit_total, tiles,
                                                                              kout, iout);
         else
             tex_sort_scatter_kernel<false><<<tiles, RS_THREADS, 0, stream>>>(kin, iin, key, n, 8 * p, counts, digit_total,
                                                                               tiles, kout, iout);
-        if ((e = cudaGetLastError()) != cudaSuccess) return e;
-        *launches += 3;
+        if ((e = launched()) != cudaSuccess) return e;
     }
     *last = (passes - 1) & 1;
     return cudaSuccess;

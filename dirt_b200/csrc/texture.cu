@@ -515,7 +515,7 @@ cudaError_t forward_ct(const float* texture, const float* pyramid, const float* 
                 kernel = texture_forward_kernel<CT, true, MIP>;
         kernel<<<blocks_for(d.total), TEX_THREADS, 0, stream>>>(texture, indices, out, d, pyramid, derivatives, L);
     }
-    return cudaGetLastError();
+    return launched();
 }
 
 // The vector path needs 8-byte index pairs and grad_indices pairs, 16-byte derivatives, and the rows of grad_out,
@@ -535,7 +535,7 @@ cudaError_t backward_ct(const float* texture, const float* pyramid, const float*
             kernel = texture_backward_kernel<CT, true, MIP>;
     kernel<<<blocks_for(d.total), TEX_THREADS, 0, stream>>>(texture, indices, grad_out, grad_texture, grad_indices, d,
                                                             pyramid, derivatives, level_grad, L);
-    return cudaGetLastError();
+    return launched();
 }
 
 // ---- deterministic backward (DESIGN.md §7.5) ------------------------------------------------------------------------
@@ -718,10 +718,10 @@ template <int CT>
 cudaError_t det_gather_ct(const TexDetArgs& a, unsigned gather_blocks, unsigned chunk_blocks, cudaStream_t stream)
 {
     tex_det_gather_kernel<CT><<<gather_blocks, TEX_THREADS, 0, stream>>>(a);
-    cudaError_t e = cudaGetLastError();
+    cudaError_t e = launched();
     if (e != cudaSuccess) return e;
     tex_det_chunk_kernel<CT><<<chunk_blocks, TEX_THREADS, 0, stream>>>(a);
-    return cudaGetLastError();
+    return launched();
 }
 
 inline unsigned det_blocks(long long work, long long per_block)
@@ -762,25 +762,25 @@ TexDetScratch carve_texture_det_scratch(void* base, const TexDims& d)
 
 cudaError_t launch_texture_backward_deterministic(const float* texture, const float* indices, const float* grad_out,
                                                   float* grad_texture, float* grad_indices, const TexDims& d,
-                                                  const TexDetScratch& s, cudaStream_t stream, int* launches)
+                                                  const TexDetScratch& s, cudaStream_t stream)
 {
     // grad_indices is per lookup and has no atomics: the default kernel writes it
     if (!grad_texture || d.total == 0) return launch_texture_backward(texture, indices, grad_out, grad_texture, grad_indices, d,
-                                                                      stream, launches);
+                                                                      stream);
     cudaError_t e;
-    if (grad_indices && (e = launch_texture_backward(texture, indices, grad_out, nullptr, grad_indices, d, stream, launches)) !=
+    if (grad_indices && (e = launch_texture_backward(texture, indices, grad_out, nullptr, grad_indices, d, stream)) !=
                             cudaSuccess)
         return e;
     if ((e = cudaMemsetAsync(s.counters, 0, 2 * sizeof(int), stream)) != cudaSuccess) return e;
     const unsigned sentinel = (unsigned)(d.TB * d.texels);
     int last;
     if ((e = sort_by_key(LookupKey{indices, d, sentinel}, d.total, sentinel, s.keys, s.ids, s.counts, s.digit_total, stream,
-                         launches, &last)) != cudaSuccess)
+                         &last)) != cudaSuccess)
         return e;
     const unsigned* keys = s.keys[last];
     tex_segment_bounds_kernel<<<det_blocks((long long)sentinel + 2, TEX_THREADS), TEX_THREADS, 0, stream>>>(keys, d.total,
                                                                                                            sentinel, s.offsets);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    if ((e = launched()) != cudaSuccess) return e;
     TexDetArgs a;
     a.indices = indices; a.grad_out = grad_out; a.ids = s.ids[last]; a.offsets = s.offsets;
     a.grad_texture = grad_texture; a.counters = s.counters; a.long_list = s.long_list; a.owner = s.owner;
@@ -797,35 +797,29 @@ cudaError_t launch_texture_backward_deterministic(const float* texture, const fl
     }
     if (e != cudaSuccess) return e;
     tex_det_finish_kernel<<<det_blocks((terms / (DET_CHUNK + 1) + 1) * d.C, TEX_THREADS), TEX_THREADS, 0, stream>>>(a);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    *launches += 4;
-    return cudaSuccess;
+    return launched();
 }
 
 cudaError_t launch_texture_forward(const float* texture, const float* indices, float* out, const TexDims& d,
-                                   cudaStream_t stream, int* launches)
+                                   cudaStream_t stream)
 {
-    const cudaError_t e = with_ct(d.C, [&](auto ct) {
+    return with_ct(d.C, [&](auto ct) {
         return forward_ct<decltype(ct)::value, false>(texture, nullptr, indices, nullptr, out, d, 1, stream);
     });
-    if (e == cudaSuccess) ++*launches;
-    return e;
 }
 
 cudaError_t launch_texture_backward(const float* texture, const float* indices, const float* grad_out, float* grad_texture,
-                                    float* grad_indices, const TexDims& d, cudaStream_t stream, int* launches)
+                                    float* grad_indices, const TexDims& d, cudaStream_t stream)
 {
     cudaError_t e;
     if (grad_texture &&
         (e = cudaMemsetAsync(grad_texture, 0, sizeof(float) * (size_t)d.TB * d.texels * d.C, stream)) != cudaSuccess)
         return e;
     if (d.total == 0 || (!grad_texture && !grad_indices)) return cudaSuccess;
-    e = with_ct(d.C, [&](auto ct) {
+    return with_ct(d.C, [&](auto ct) {
         return backward_ct<decltype(ct)::value, false>(texture, nullptr, indices, nullptr, grad_out, grad_texture, nullptr,
                                                         grad_indices, d, 1, stream);
     });
-    if (e == cudaSuccess) ++*launches;
-    return e;
 }
 
 // ---- mipmapped (trilinear) lookup (DESIGN.md §7.6): the pyramid, its adjoint and the deterministic level terms ------
@@ -912,8 +906,7 @@ MipScratch carve_texture_mip_scratch(void* base, const TexDims& d, bool determin
     return s;
 }
 
-cudaError_t launch_texture_mip_build(const float* texture, float* pyramid, const TexDims& d, cudaStream_t stream,
-                                     int* launches)
+cudaError_t launch_texture_mip_build(const float* texture, float* pyramid, const TexDims& d, cudaStream_t stream)
 {
     const int L = mip_levels(d.TH, d.TW);
     for (int k = 1; k < L; ++k) {
@@ -921,29 +914,25 @@ cudaError_t launch_texture_mip_build(const float* texture, float* pyramid, const
         mip_build_kernel<<<blocks_for(n), TEX_THREADS, 0, stream>>>(level_base(texture, (const float*)pyramid, d, k - 1),
                                                                     pyramid + mip_offset(d, k) * d.C, n, d.TH >> k,
                                                                     d.TW >> k, d.C);
-        const cudaError_t e = cudaGetLastError();
+        const cudaError_t e = launched();
         if (e != cudaSuccess) return e;
-        ++*launches;
     }
     return cudaSuccess;
 }
 
 cudaError_t launch_texture_trilinear_forward(const float* texture, const float* pyramid, const float* indices,
-                                             const float* derivatives, float* out, const TexDims& d, cudaStream_t stream,
-                                             int* launches)
+                                             const float* derivatives, float* out, const TexDims& d, cudaStream_t stream)
 {
     const int L = mip_levels(d.TH, d.TW);
-    const cudaError_t e = with_ct(d.C, [&](auto ct) {
+    return with_ct(d.C, [&](auto ct) {
         return forward_ct<decltype(ct)::value, true>(texture, pyramid, indices, derivatives, out, d, L, stream);
     });
-    if (e == cudaSuccess) ++*launches;
-    return e;
 }
 
 cudaError_t launch_texture_trilinear_backward(const float* texture, const float* pyramid, const float* indices,
                                               const float* derivatives, const float* grad_out, float* grad_texture,
                                               float* grad_indices, const TexDims& d, bool deterministic,
-                                              const MipScratch& s, cudaStream_t stream, int* launches)
+                                              const MipScratch& s, cudaStream_t stream)
 {
     const int L = mip_levels(d.TH, d.TW);
     const size_t texture_bytes = sizeof(float) * (size_t)d.TB * d.texels * d.C;
@@ -965,7 +954,6 @@ cudaError_t launch_texture_trilinear_backward(const float* texture, const float*
                                                            grad_indices, d, L, stream);
         });
         if (e != cudaSuccess) return e;
-        ++*launches;
     }
     if (!grad_texture) return cudaSuccess;
     if (deterministic) {
@@ -973,13 +961,12 @@ cudaError_t launch_texture_trilinear_backward(const float* texture, const float*
         for (int k = 0; k < L; ++k) {
             mip_level_terms_kernel<<<blocks_for(d.total), TEX_THREADS, 0, stream>>>(indices, derivatives, grad_out, d, L, k,
                                                                                      s.indices, s.grad_out);
-            if ((e = cudaGetLastError()) != cudaSuccess) return e;
-            ++*launches;
+            if ((e = launched()) != cudaSuccess) return e;
             TexDims dk = d;
             dk.TH = d.TH >> k; dk.TW = d.TW >> k; dk.texels = d.texels >> (2 * k);
             float* gk = k == 0 ? grad_texture : s.level_grad + mip_offset(d, k) * d.C;
             if ((e = launch_texture_backward_deterministic(nullptr, s.indices, s.grad_out, gk, nullptr, dk,
-                                                           carve_texture_det_scratch(s.det, dk), stream, launches)) !=
+                                                           carve_texture_det_scratch(s.det, dk), stream)) !=
                 cudaSuccess)
                 return e;
         }
@@ -987,8 +974,7 @@ cudaError_t launch_texture_trilinear_backward(const float* texture, const float*
     if (L > 1) {
         mip_collapse_kernel<<<blocks_for((long long)d.TB * d.texels * d.C), TEX_THREADS, 0, stream>>>(grad_texture, s.level_grad,
                                                                                                       d, L);
-        if ((e = cudaGetLastError()) != cudaSuccess) return e;
-        ++*launches;
+        if ((e = launched()) != cudaSuccess) return e;
     }
     return cudaSuccess;
 }
@@ -1530,7 +1516,7 @@ cudaError_t cube_forward_ct(const float* atlas, const float* directions, float* 
     if constexpr (CT != 0)
         if (aligned(out, CT == 3 ? 16 : row) && aligned(atlas, row)) kernel = cube_forward_kernel<CT, true, MIP>;
     kernel<<<blocks_for(d.total), TEX_THREADS, 0, stream>>>(atlas, directions, out, d, m);
-    return cudaGetLastError();
+    return launched();
 }
 
 // MIP: the shared-memory levels (smem_first < m.L) take (offset[L] - offset[smem_first]) * C floats of dynamic shared
@@ -1558,7 +1544,7 @@ cudaError_t cube_backward_ct(const float* atlas, const float* directions, const 
     }
     kernel<<<blocks, TEX_THREADS, smem, stream>>>(atlas, directions, grad_out, grad_atlas, grad_directions, d, m, grad_lod,
                                                   smem_first);
-    return cudaGetLastError();
+    return launched();
 }
 
 // the mip atlas's levels: offset[k], k = 0 .. L, of level k's first texel
@@ -1606,23 +1592,19 @@ CubeScratch carve_cubemap_scratch(void* base, const TexDims& d, bool determinist
 }
 
 cudaError_t launch_cubemap_forward(const float* cubemap, const float* directions, float* atlas, float* out,
-                                   const TexDims& d, cudaStream_t stream, int* launches)
+                                   const TexDims& d, cudaStream_t stream)
 {
     cube_atlas_kernel<<<blocks_for(6ll * d.TB * d.texels * d.C), TEX_THREADS, 0, stream>>>(cubemap, atlas, d);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
-    ++*launches;
-    if (d.total == 0) return cudaSuccess;
-    e = with_ct(d.C, [&](auto ct) {
+    const cudaError_t e = launched();
+    if (e != cudaSuccess || d.total == 0) return e;
+    return with_ct(d.C, [&](auto ct) {
         return cube_forward_ct<decltype(ct)::value, false>(atlas, directions, out, d, CubeMip{}, stream);
     });
-    if (e == cudaSuccess) ++*launches;
-    return e;
 }
 
 cudaError_t launch_cubemap_backward(const float* atlas, const float* directions, const float* grad_out, float* grad_cubemap,
                                     float* grad_directions, const TexDims& d, bool deterministic, const CubeScratch& s,
-                                    cudaStream_t stream, int* launches)
+                                    cudaStream_t stream)
 {
     const int S = d.TW - 2;
     cudaError_t e;
@@ -1644,26 +1626,22 @@ cudaError_t launch_cubemap_backward(const float* atlas, const float* directions,
                                                                  CubeMip{}, nullptr, 0, stream);
         });
         if (e != cudaSuccess) return e;
-        ++*launches;
     }
     if (!grad_cubemap) return cudaSuccess;
     if (deterministic) {
         // face f's block of grad_atlas, every texel written, by the §7.5 path over the lookups on face f
         for (int f = 0; f < 6; ++f) {
             cube_face_indices_kernel<<<blocks_for(d.total), TEX_THREADS, 0, stream>>>(directions, d, f, s.indices);
-            if ((e = cudaGetLastError()) != cudaSuccess) return e;
-            ++*launches;
+            if ((e = launched()) != cudaSuccess) return e;
             if ((e = launch_texture_backward_deterministic(nullptr, s.indices, grad_out,
                                                            s.grad_atlas + (size_t)f * d.TB * d.texels * d.C, nullptr, d,
-                                                           carve_texture_det_scratch(s.det, d), stream, launches)) !=
+                                                           carve_texture_det_scratch(s.det, d), stream)) !=
                 cudaSuccess)
                 return e;
         }
     }
     cube_adjoint_kernel<<<blocks_for(6ll * d.TB * S * S * d.C), TEX_THREADS, 0, stream>>>(s.grad_atlas, grad_cubemap, d);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    ++*launches;
-    return cudaSuccess;
+    return launched();
 }
 
 // ---- mipmapped cube-map lookup (DESIGN.md §7.11) ----
@@ -1710,8 +1688,7 @@ CubeMipScratch carve_cubemap_mip_scratch(void* base, const TexDims& d, bool dete
 // every level's atlas from level 0 (cubemap) and levels 1 .. L-1 (the pyramid layout at levels), coarsest first, then
 // the lookups
 static cudaError_t cube_mip_atlas_lookup(const float* cubemap, const float* levels, const float* directions,
-                                         const float* lod, float* atlas, float* out, const TexDims& d, cudaStream_t stream,
-                                         int* launches)
+                                         const float* lod, float* atlas, float* out, const TexDims& d, cudaStream_t stream)
 {
     const TexDims pd = cube_faces_dims(d);
     const CubeMip m = cube_mip_of(d, lod);
@@ -1720,20 +1697,17 @@ static cudaError_t cube_mip_atlas_lookup(const float* cubemap, const float* leve
         const TexDims dk = cube_level_dims(d, k);
         cube_atlas_kernel<<<blocks_for(6ll * d.TB * dk.texels * d.C), TEX_THREADS, 0, stream>>>(
             k == 0 ? cubemap : levels + mip_offset(pd, k) * d.C, atlas + m.offset[k] * d.C, dk);
-        if ((e = cudaGetLastError()) != cudaSuccess) return e;
-        ++*launches;
+        if ((e = launched()) != cudaSuccess) return e;
     }
-    e = with_ct(d.C, [&](auto ct) { return cube_forward_ct<decltype(ct)::value, true>(atlas, directions, out, d, m, stream); });
-    if (e == cudaSuccess) ++*launches;
-    return e;
+    return with_ct(d.C, [&](auto ct) { return cube_forward_ct<decltype(ct)::value, true>(atlas, directions, out, d, m, stream); });
 }
 
 cudaError_t launch_cubemap_mip_forward(const float* cubemap, const float* directions, const float* lod, float* atlas,
-                                       float* out, const TexDims& d, cudaStream_t stream, int* launches)
+                                       float* out, const TexDims& d, cudaStream_t stream)
 {
-    const cudaError_t e = launch_texture_mip_build(cubemap, atlas, cube_faces_dims(d), stream, launches);
+    const cudaError_t e = launch_texture_mip_build(cubemap, atlas, cube_faces_dims(d), stream);
     if (e != cudaSuccess) return e;
-    return cube_mip_atlas_lookup(cubemap, atlas, directions, lod, atlas, out, d, stream, launches);
+    return cube_mip_atlas_lookup(cubemap, atlas, directions, lod, atlas, out, d, stream);
 }
 
 // the lookups' gradients, and the cube map's by level: level 0 to grad_cubemap, levels 1 .. L-1 to s.level_grad; *done
@@ -1741,7 +1715,7 @@ cudaError_t launch_cubemap_mip_forward(const float* cubemap, const float* direct
 static cudaError_t cube_mip_level_grads(const float* atlas, const float* directions, const float* lod,
                                         const float* grad_out, float* grad_cubemap, float* grad_directions, float* grad_lod,
                                         const TexDims& d, bool deterministic, const CubeMipScratch& s, cudaStream_t stream,
-                                        int* launches, bool* done)
+                                        bool* done)
 {
     *done = true;
     const TexDims pd = cube_faces_dims(d);
@@ -1766,7 +1740,6 @@ static cudaError_t cube_mip_level_grads(const float* atlas, const float* directi
                                                                 grad_lod, smem_first, stream);
         });
         if (e != cudaSuccess) return e;
-        ++*launches;
     }
     if (!grad_cubemap) return cudaSuccess;
     if (deterministic) {
@@ -1776,11 +1749,10 @@ static cudaError_t cube_mip_level_grads(const float* atlas, const float* directi
             for (int f = 0; f < 6; ++f) {
                 cube_mip_terms_kernel<<<blocks_for(d.total), TEX_THREADS, 0, stream>>>(directions, d, m, grad_out, k, f, f == 0,
                                                                                         s.indices, s.grad_out);
-                if ((e = cudaGetLastError()) != cudaSuccess) return e;
-                ++*launches;
+                if ((e = launched()) != cudaSuccess) return e;
                 float* gk = s.grad_atlas + (m.offset[k] + (size_t)f * d.TB * dk.texels) * d.C;
                 if ((e = launch_texture_backward_deterministic(nullptr, s.indices, s.grad_out, gk, nullptr, dk,
-                                                               carve_texture_det_scratch(s.det, dk), stream, launches)) !=
+                                                               carve_texture_det_scratch(s.det, dk), stream)) !=
                     cudaSuccess)
                     return e;
             }
@@ -1792,8 +1764,7 @@ static cudaError_t cube_mip_level_grads(const float* atlas, const float* directi
         const long long S = dk.TW - 2;
         cube_adjoint_kernel<<<blocks_for(6ll * d.TB * S * S * d.C), TEX_THREADS, 0, stream>>>(
             s.grad_atlas + m.offset[k] * d.C, k == 0 ? grad_cubemap : s.level_grad + mip_offset(pd, k) * d.C, dk);
-        if ((e = cudaGetLastError()) != cudaSuccess) return e;
-        ++*launches;
+        if ((e = launched()) != cudaSuccess) return e;
     }
     *done = false;
     return cudaSuccess;
@@ -1801,19 +1772,18 @@ static cudaError_t cube_mip_level_grads(const float* atlas, const float* directi
 
 cudaError_t launch_cubemap_mip_backward(const float* atlas, const float* directions, const float* lod, const float* grad_out,
                                         float* grad_cubemap, float* grad_directions, float* grad_lod, const TexDims& d,
-                                        bool deterministic, const CubeMipScratch& s, cudaStream_t stream, int* launches)
+                                        bool deterministic, const CubeMipScratch& s, cudaStream_t stream)
 {
     const TexDims pd = cube_faces_dims(d);
     const CubeMip m = cube_mip_of(d, lod);
     bool done;
     cudaError_t e = cube_mip_level_grads(atlas, directions, lod, grad_out, grad_cubemap, grad_directions, grad_lod, d,
-                                         deterministic, s, stream, launches, &done);
+                                         deterministic, s, stream, &done);
     if (e != cudaSuccess || done) return e;
     if (m.L > 1) {
         mip_collapse_kernel<<<blocks_for((long long)pd.TB * pd.texels * d.C), TEX_THREADS, 0, stream>>>(grad_cubemap,
                                                                                                        s.level_grad, pd, m.L);
-        if ((e = cudaGetLastError()) != cudaSuccess) return e;
-        ++*launches;
+        if ((e = launched()) != cudaSuccess) return e;
     }
     return cudaSuccess;
 }
@@ -1832,35 +1802,32 @@ CubeGgxScratch carve_cubemap_ggx_scratch(void* base, const TexDims& d, bool dete
 }
 
 cudaError_t launch_cubemap_ggx_forward(const float* cubemap, const float* directions, const float* lod, float* atlas,
-                                       float* out, const TexDims& d, cudaStream_t stream, int* launches)
+                                       float* out, const TexDims& d, cudaStream_t stream)
 {
-    const cudaError_t e = launch_ggx_prefilter(cubemap, atlas, d, stream, launches);
+    const cudaError_t e = launch_ggx_prefilter(cubemap, atlas, d, stream);
     if (e != cudaSuccess) return e;
-    return cube_mip_atlas_lookup(cubemap, atlas + ggx_layout(d).levels, directions, lod, atlas, out, d, stream, launches);
+    return cube_mip_atlas_lookup(cubemap, atlas + ggx_layout(d).levels, directions, lod, atlas, out, d, stream);
 }
 
 // the lookups' backward pass and border adjoints as §7.11's, then the prefilter's adjoint into the box levels (level 0
 // straight into grad_cubemap) and the box pyramid's adjoint
 cudaError_t launch_cubemap_ggx_backward(const float* atlas, const float* directions, const float* lod, const float* grad_out,
                                         float* grad_cubemap, float* grad_directions, float* grad_lod, const TexDims& d,
-                                        bool deterministic, const CubeGgxScratch& s, cudaStream_t stream, int* launches)
+                                        bool deterministic, const CubeGgxScratch& s, cudaStream_t stream)
 {
     const TexDims pd = cube_faces_dims(d);
     const int L = mip_levels(pd.TW, pd.TW);
     bool done;
     cudaError_t e = cube_mip_level_grads(atlas, directions, lod, grad_out, grad_cubemap, grad_directions, grad_lod, d,
-                                         deterministic, s.mip, stream, launches, &done);
+                                         deterministic, s.mip, stream, &done);
     if (e != cudaSuccess || done || L == 1) return e;
     if ((e = cudaMemsetAsync(s.src_grad, 0, sizeof(float) * (size_t)mip_pyramid_texels(pd, L) * d.C, stream)) != cudaSuccess)
         return e;
-    if ((e = launch_ggx_prefilter_adjoint(atlas, s.mip.level_grad, s.src_grad, grad_cubemap, d, stream, launches)) !=
-        cudaSuccess)
+    if ((e = launch_ggx_prefilter_adjoint(atlas, s.mip.level_grad, s.src_grad, grad_cubemap, d, stream)) != cudaSuccess)
         return e;
     mip_collapse_kernel<<<blocks_for((long long)pd.TB * pd.texels * d.C), TEX_THREADS, 0, stream>>>(grad_cubemap, s.src_grad,
                                                                                                    pd, L);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    ++*launches;
-    return cudaSuccess;
+    return launched();
 }
 
 }  // namespace dirt

@@ -673,7 +673,9 @@ int dirt_shadow_backward_deterministic(const float* positions, long long positio
                                        size_t workspace_bytes, void* scratch, size_t scratch_bytes, int B, long long V,
                                        void* cuda_stream);
 
-/* Number of kernels the last call on this thread launched (bench.py's gpu_launches). */
+/* Number of kernels the last launching call on this thread launched successfully (bench.py's gpu_launches).  A
+ * launch that fails is not counted; the call then returns DIRT_ERR_CUDA.  The size queries, the kernel-timer hooks and
+ * dirt_peer_exchange leave the count as it was. */
 int dirt_last_launch_count(void);
 
 /* Profiling hooks (replace the reference's compile-time TIME_SECTIONS stamps,
