@@ -1132,32 +1132,6 @@ extern "C" int dirt_shadow_forward(const float* positions, long long positions_s
     return DIRT_OK;
 }
 
-extern "C" int dirt_shadow_backward(const float* positions, long long positions_stride, const float* light_matrix,
-                                    const float* shadow_map, int per_item, int SH, int SW, int radius, float softness,
-                                    float bias, const float* grad_out, float* grad_positions, float* grad_light_matrix,
-                                    float* grad_shadow_map, void* workspace, size_t workspace_bytes, int B, long long V,
-                                    void* cuda_stream)
-{
-    launch_count() = 0;
-    if (!shadow_shape_ok(B, V, positions_stride, SH, SW, radius, softness, bias)) return DIRT_ERR_BAD_SHAPE;
-    ShadowArgs a = make_shadow_args(positions, positions_stride, light_matrix, shadow_map, per_item, SH, SW, radius,
-                                    softness, bias, B, V);
-    a.grad_out = grad_out;
-    a.g_positions = grad_positions; a.g_matrix = grad_light_matrix; a.g_map = grad_shadow_map;
-    if (!aligned({grad_positions, grad_light_matrix, grad_shadow_map}) || (uintptr_t)grad_shadow_map % 8)
-        return DIRT_ERR_MISALIGNED;
-    if ((long long)B * V > 0 && (grad_positions || grad_light_matrix || grad_shadow_map)) {
-        int rc = shadow_inputs_check(a);
-        if (rc == DIRT_OK) rc = required_check({grad_out});
-        if (rc == DIRT_OK && grad_light_matrix)
-            rc = partials_check(workspace, workspace_bytes, dirt_shadow_workspace_bytes(B, V), &a.partial);
-        if (rc != DIRT_OK) return rc;
-    }
-    // with no points only the memsets of the wanted map and matrix gradients are enqueued
-    CUDA_TRY(launch_shadow_backward(a, (cudaStream_t)cuda_stream));
-    return DIRT_OK;
-}
-
 // the deterministic backward's point ids and segment offsets are int32
 static bool shadow_det_shape_ok(int B, long long V, int per_item, int SH, int SW)
 {
@@ -1173,17 +1147,18 @@ extern "C" size_t dirt_shadow_backward_deterministic_bytes(int B, long long V, i
     return carve_shadow_det_scratch(nullptr, a).bytes;
 }
 
-extern "C" int dirt_shadow_backward_deterministic(const float* positions, long long positions_stride,
-                                                  const float* light_matrix, const float* shadow_map, int per_item,
-                                                  int SH, int SW, int radius, float softness, float bias,
-                                                  const float* grad_out, float* grad_positions,
-                                                  float* grad_light_matrix, float* grad_shadow_map, void* workspace,
-                                                  size_t workspace_bytes, void* scratch, size_t scratch_bytes, int B,
-                                                  long long V, void* cuda_stream)
+// Both shadow backward entries.  The deterministic one adds its int32 rule (shadow_det_shape_ok, a second
+// DIRT_ERR_BAD_SHAPE check) and, when it sorts (a wanted map gradient and points), a scratch: NULL, then 4-byte
+// alignment (not scratch_check's 256), then its size.
+static int shadow_backward_impl(const float* positions, long long positions_stride, const float* light_matrix,
+                                const float* shadow_map, int per_item, int SH, int SW, int radius, float softness,
+                                float bias, const float* grad_out, float* grad_positions, float* grad_light_matrix,
+                                float* grad_shadow_map, void* workspace, size_t workspace_bytes, bool deterministic,
+                                void* scratch, size_t scratch_bytes, int B, long long V, void* cuda_stream)
 {
     launch_count() = 0;
     if (!shadow_shape_ok(B, V, positions_stride, SH, SW, radius, softness, bias) ||
-        !shadow_det_shape_ok(B, V, per_item, SH, SW))
+        (deterministic && !shadow_det_shape_ok(B, V, per_item, SH, SW)))
         return DIRT_ERR_BAD_SHAPE;
     ShadowArgs a = make_shadow_args(positions, positions_stride, light_matrix, shadow_map, per_item, SH, SW, radius,
                                     softness, bias, B, V);
@@ -1191,7 +1166,7 @@ extern "C" int dirt_shadow_backward_deterministic(const float* positions, long l
     a.g_positions = grad_positions; a.g_matrix = grad_light_matrix; a.g_map = grad_shadow_map;
     if (!aligned({grad_positions, grad_light_matrix, grad_shadow_map}) || (uintptr_t)grad_shadow_map % 8)
         return DIRT_ERR_MISALIGNED;
-    const bool sorts = grad_shadow_map && (long long)B * V > 0;
+    const bool sorts = deterministic && grad_shadow_map && (long long)B * V > 0;
     if ((long long)B * V > 0 && (grad_positions || grad_light_matrix || grad_shadow_map)) {
         int rc = shadow_inputs_check(a);
         if (rc == DIRT_OK) rc = required_check({grad_out});
@@ -1204,9 +1179,37 @@ extern "C" int dirt_shadow_backward_deterministic(const float* positions, long l
         }
         if (rc != DIRT_OK) return rc;
     }
-    CUDA_TRY(launch_shadow_backward_deterministic(a, carve_shadow_det_scratch(sorts ? scratch : nullptr, a),
-                                                  (cudaStream_t)cuda_stream));
+    // with no points only the memsets of the wanted map and matrix gradients are enqueued
+    if (deterministic)
+        CUDA_TRY(launch_shadow_backward_deterministic(a, carve_shadow_det_scratch(sorts ? scratch : nullptr, a),
+                                                      (cudaStream_t)cuda_stream));
+    else
+        CUDA_TRY(launch_shadow_backward(a, (cudaStream_t)cuda_stream));
     return DIRT_OK;
+}
+
+extern "C" int dirt_shadow_backward(const float* positions, long long positions_stride, const float* light_matrix,
+                                    const float* shadow_map, int per_item, int SH, int SW, int radius, float softness,
+                                    float bias, const float* grad_out, float* grad_positions, float* grad_light_matrix,
+                                    float* grad_shadow_map, void* workspace, size_t workspace_bytes, int B, long long V,
+                                    void* cuda_stream)
+{
+    return shadow_backward_impl(positions, positions_stride, light_matrix, shadow_map, per_item, SH, SW, radius,
+                                softness, bias, grad_out, grad_positions, grad_light_matrix, grad_shadow_map, workspace,
+                                workspace_bytes, false, nullptr, 0, B, V, cuda_stream);
+}
+
+extern "C" int dirt_shadow_backward_deterministic(const float* positions, long long positions_stride,
+                                                  const float* light_matrix, const float* shadow_map, int per_item,
+                                                  int SH, int SW, int radius, float softness, float bias,
+                                                  const float* grad_out, float* grad_positions,
+                                                  float* grad_light_matrix, float* grad_shadow_map, void* workspace,
+                                                  size_t workspace_bytes, void* scratch, size_t scratch_bytes, int B,
+                                                  long long V, void* cuda_stream)
+{
+    return shadow_backward_impl(positions, positions_stride, light_matrix, shadow_map, per_item, SH, SW, radius,
+                                softness, bias, grad_out, grad_positions, grad_light_matrix, grad_shadow_map, workspace,
+                                workspace_bytes, true, scratch, scratch_bytes, B, V, cuda_stream);
 }
 
 // element offsets of the vertex rows stay below 2^62; vertex ids and incidence ids (k*F + f) are int32
@@ -1224,13 +1227,22 @@ extern "C" size_t dirt_normals_workspace_bytes(int B, long long V, long long F)
     return carve_normals_workspace(nullptr, B, V, F).bytes;
 }
 
-static int normals_check(const float* vertices, const int32_t* faces, const void* workspace, size_t workspace_bytes,
-                         int B, long long V, long long F)
+// The checks the four mesh entries share, in order: the vertices, faces and workspace, NULL (the faces and workspace
+// only when F > 0) then 4-byte alignment (the workspace holds int32 adjacency, so not scratch_check's 256 bytes); the
+// workspace's size; the other inputs and then `outs` (the output, or the incoming gradient and the gradients a backward
+// requires), each by required_check.  Before it each entry makes its shape check and its early return, which differ:
+// - the forwards and the normals backward return DIRT_OK for B*V == 0 before they check anything else;
+// - the tangents backward first checks the alignment of its gradients, which may be NULL, then returns DIRT_OK for
+//   B*V == 0 or when no gradient is wanted.
+static int mesh_check(const float* vertices, const int32_t* faces, const void* workspace, size_t workspace_bytes, int B,
+                      long long V, long long F, std::initializer_list<const void*> inputs,
+                      std::initializer_list<const void*> outs)
 {
     if (!vertices || (F > 0 && (!faces || !workspace))) return DIRT_ERR_NULL_POINTER;
-    if ((uintptr_t)vertices % 4 || (uintptr_t)faces % 4 || (uintptr_t)workspace % 4) return DIRT_ERR_MISALIGNED;
+    if (!aligned({vertices, faces, workspace})) return DIRT_ERR_MISALIGNED;
     if (workspace_bytes < dirt_normals_workspace_bytes(B, V, F)) return DIRT_ERR_WORKSPACE_TOO_SMALL;
-    return DIRT_OK;
+    const int rc = required_check(inputs);
+    return rc != DIRT_OK ? rc : required_check(outs);
 }
 
 static NormalsArgs make_normals_args(int mode, const float* vertices, long long stride, const int32_t* faces, int B,
@@ -1249,10 +1261,8 @@ extern "C" int dirt_normals_forward(int mode, const float* vertices, long long v
     launch_count() = 0;
     if (!normals_shape_ok(mode, B, V, F, vertex_stride)) return DIRT_ERR_BAD_SHAPE;
     if ((long long)B * V == 0) return DIRT_OK;
-    const int rc = normals_check(vertices, faces, workspace, workspace_bytes, B, V, F);
+    const int rc = mesh_check(vertices, faces, workspace, workspace_bytes, B, V, F, {}, {normals});
     if (rc != DIRT_OK) return rc;
-    if (!normals) return DIRT_ERR_NULL_POINTER;
-    if ((uintptr_t)normals % 4) return DIRT_ERR_MISALIGNED;
     NormalsArgs a = make_normals_args(mode, vertices, vertex_stride, faces, B, V, F);
     a.out = normals;
     CUDA_TRY(launch_normals_forward(a, carve_normals_workspace(F > 0 ? workspace : nullptr, B, V, F),
@@ -1267,10 +1277,8 @@ extern "C" int dirt_normals_backward(int mode, const float* vertices, long long 
     launch_count() = 0;
     if (!normals_shape_ok(mode, B, V, F, vertex_stride)) return DIRT_ERR_BAD_SHAPE;
     if ((long long)B * V == 0) return DIRT_OK;
-    const int rc = normals_check(vertices, faces, workspace, workspace_bytes, B, V, F);
+    const int rc = mesh_check(vertices, faces, workspace, workspace_bytes, B, V, F, {}, {grad_normals, grad_vertices});
     if (rc != DIRT_OK) return rc;
-    if (!grad_normals || !grad_vertices) return DIRT_ERR_NULL_POINTER;
-    if ((uintptr_t)grad_normals % 4 || (uintptr_t)grad_vertices % 4) return DIRT_ERR_MISALIGNED;
     NormalsArgs a = make_normals_args(mode, vertices, vertex_stride, faces, B, V, F);
     a.grad = grad_normals;
     a.g_vertices = grad_vertices;
@@ -1294,16 +1302,6 @@ extern "C" size_t dirt_tangents_workspace_bytes(int B, long long V, long long F)
     return dirt_normals_workspace_bytes(B, V, F);
 }
 
-static int tangents_check(const float* vertices, const float* uvs, const float* normals, const int32_t* faces,
-                          const void* workspace, size_t workspace_bytes, int B, long long V, long long F)
-{
-    const int rc = normals_check(vertices, faces, workspace, workspace_bytes, B, V, F);
-    if (rc != DIRT_OK) return rc;
-    if (!uvs || !normals) return DIRT_ERR_NULL_POINTER;
-    if ((uintptr_t)uvs % 4 || (uintptr_t)normals % 4) return DIRT_ERR_MISALIGNED;
-    return DIRT_OK;
-}
-
 static TangentArgs make_tangent_args(const float* vertices, long long vertex_stride, const float* uvs, long long uv_stride,
                                      long long uv_item_stride, const float* normals, long long normals_stride,
                                      const int32_t* faces, int B, long long V, long long F)
@@ -1323,10 +1321,8 @@ extern "C" int dirt_tangents_forward(const float* vertices, long long vertex_str
     launch_count() = 0;
     if (!tangents_shape_ok(B, V, F, vertex_stride, uv_stride, uv_item_stride, normals_stride)) return DIRT_ERR_BAD_SHAPE;
     if ((long long)B * V == 0) return DIRT_OK;
-    const int rc = tangents_check(vertices, uvs, normals, faces, workspace, workspace_bytes, B, V, F);
+    const int rc = mesh_check(vertices, faces, workspace, workspace_bytes, B, V, F, {uvs, normals}, {tangents});
     if (rc != DIRT_OK) return rc;
-    if (!tangents) return DIRT_ERR_NULL_POINTER;
-    if ((uintptr_t)tangents % 4) return DIRT_ERR_MISALIGNED;
     TangentArgs a = make_tangent_args(vertices, vertex_stride, uvs, uv_stride, uv_item_stride, normals, normals_stride,
                                       faces, B, V, F);
     a.out = tangents;
@@ -1343,12 +1339,10 @@ extern "C" int dirt_tangents_backward(const float* vertices, long long vertex_st
 {
     launch_count() = 0;
     if (!tangents_shape_ok(B, V, F, vertex_stride, uv_stride, uv_item_stride, normals_stride)) return DIRT_ERR_BAD_SHAPE;
-    if ((uintptr_t)grad_vertices % 4 || (uintptr_t)grad_uvs % 4 || (uintptr_t)grad_normals % 4) return DIRT_ERR_MISALIGNED;
+    if (!aligned({grad_vertices, grad_uvs, grad_normals})) return DIRT_ERR_MISALIGNED;
     if ((long long)B * V == 0 || (!grad_vertices && !grad_uvs && !grad_normals)) return DIRT_OK;
-    const int rc = tangents_check(vertices, uvs, normals, faces, workspace, workspace_bytes, B, V, F);
+    const int rc = mesh_check(vertices, faces, workspace, workspace_bytes, B, V, F, {uvs, normals}, {grad_tangents});
     if (rc != DIRT_OK) return rc;
-    if (!grad_tangents) return DIRT_ERR_NULL_POINTER;
-    if ((uintptr_t)grad_tangents % 4) return DIRT_ERR_MISALIGNED;
     TangentArgs a = make_tangent_args(vertices, vertex_stride, uvs, uv_stride, uv_item_stride, normals, normals_stride,
                                       faces, B, V, F);
     a.grad = grad_tangents;

@@ -20,6 +20,7 @@ accepts, its torch restatement `_shadow_visibility` otherwise; see DESIGN.md §7
 """
 import math
 from collections import namedtuple
+from functools import partial
 
 import torch
 
@@ -68,7 +69,7 @@ def vertex_normals(vertices, faces, name=None):
     route = _normals_route(vertices, faces)
     if route is None:
         return _vertex_normals(vertices, faces)
-    return _normals(_lib.NORMALS_AVERAGE, route, vertices, faces)
+    return _mesh(_NORMALS, route, faces, _point_rows(vertices[..., :3], 3))
 
 
 def vertex_normals_pre_split(vertices, faces, name=None, static=False):
@@ -78,7 +79,7 @@ def vertex_normals_pre_split(vertices, faces, name=None, static=False):
     route = _normals_route(vertices, faces)
     if route is None:
         return _vertex_normals_pre_split(vertices, faces)
-    return _normals(_lib.NORMALS_PRE_SPLIT, route, vertices, faces)
+    return _mesh(_NORMALS_PRE_SPLIT, route, faces, _point_rows(vertices[..., :3], 3))
 
 
 def split_vertices_by_face(vertices, faces, name=None):
@@ -680,7 +681,7 @@ def diffuse_spherical_harmonics(vertex_normals, vertex_colors, coefficients, nam
                                 _flat_item(coefficients, route, route.per_item[0]))
 
 
-# ---- the CUDA path of the normals -----------------------------------------------------------------------------------
+# ---- the CUDA path of the normals and of every mesh op -------------------------------------------------------------
 
 NormalsRoute = namedtuple('NormalsRoute', 'lead B V F')
 
@@ -708,69 +709,97 @@ def _normals_route(vertices, faces):
     return normals_route(vertices.shape, vertices.dtype, vertices.device, faces.shape, faces.dtype)
 
 
-_NORMALS_NAMES = {_lib.NORMALS_AVERAGE: 'VertexNormals', _lib.NORMALS_PRE_SPLIT: 'VertexNormalsPreSplit'}
+def _point_rows(t, k):
+    """`_rows`, with a row stride of at least k (the C ABI's requirement for these rows)."""
+    r = _rows(t, k)
+    return r.contiguous() if r.shape[0] > 1 and r.stride(0) < k else r
 
 
-class _Normals(torch.autograd.Function):
-    """dirt_normals_forward with its gradient.  rows: the vertices' positions as [B*V, 3] with unit stride along the row
-    and one row stride >= 3; faces: int32 [F, 3] on their device.  The node keeps its inputs and the forward's
-    workspace, whose adjacency the backward kernels read."""
+def _stride(rows, k):
+    return rows.stride(0) if rows.shape[0] > 1 else k
+
+
+# A mesh op: vertex normals (either mode) or vertex tangents.  Its forward builds a corner-adjacency workspace of
+# workspace_bytes(B, V, F) bytes, where workspace_bytes is an entry point, and its backward reads that adjacency.
+#   name: the op's name in errors (its backward's is name + 'Grad');
+#   forward, backward: its entry points in the library;
+#   inputs(route, faces, *inputs): their input arguments, in their order;
+#   width: the width of the output rows; input_widths: the width of each input's gradient rows, B*V of them;
+#   restate(route, faces, *inputs): the torch restatement on the op's own inputs and the faces the kernels use, in the
+#     output's shape;
+#   finish(route, grads): turns the backward's gradient rows into the inputs' gradients; None where they are the same.
+_MeshOp = namedtuple('_MeshOp', 'name forward backward workspace_bytes inputs width input_widths restate finish',
+                     defaults=(None,))
+
+
+class _MeshFunction(torch.autograd.Function):
+    """The forward entry point of a _MeshOp with its gradient.  faces: int32 [F, 3] on the inputs' device; inputs: the
+    op's per-vertex rows, [B*V, k] ([V, k] for shared uvs) with unit stride along k and a row stride of at least k.  The
+    node keeps its inputs and the forward's workspace, whose adjacency the backward kernels read."""
 
     @staticmethod
-    def forward(ctx, mode, route, rows, faces):
-        dev = rows.device
+    def forward(ctx, op, route, faces, *inputs):
+        dev = inputs[0].device
         lib = _lib.lib()
-        out = torch.empty((route.B * route.V, 3), dtype=torch.float32, device=dev)
-        ws_bytes = int(lib.dirt_normals_workspace_bytes(route.B, route.V, route.F))
+        out = torch.empty((route.B * route.V, op.width), dtype=torch.float32, device=dev)
+        ws_bytes = int(getattr(lib, op.workspace_bytes)(route.B, route.V, route.F))
         workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=dev) if ws_bytes else None
         with torch.cuda.device(dev):
-            rc = lib.dirt_normals_forward(mode, _ptr(rows), _row_stride(rows), _ptr(faces), _ptr(out), _ptr(workspace),
-                                          ws_bytes, route.B, route.V, route.F, _stream(dev))
-        _lib.check(rc, _NORMALS_NAMES[mode])
-        ctx.save_for_backward(rows, faces)
-        ctx.mode, ctx.route, ctx.workspace, ctx.ws_bytes = mode, route, workspace, ws_bytes
+            rc = getattr(lib, op.forward)(*op.inputs(route, faces, *inputs), _ptr(out), _ptr(workspace), ws_bytes,
+                                          route.B, route.V, route.F, _stream(dev))
+        _lib.check(rc, op.name)
+        ctx.save_for_backward(faces, *inputs)
+        ctx.op, ctx.route, ctx.workspace, ctx.ws_bytes = op, route, workspace, ws_bytes
         return out
 
     @staticmethod
     def backward(ctx, grad_out):
-        if not ctx.needs_input_grad[2]:
-            return None, None, None, None
-        rows, faces = ctx.saved_tensors
-        route = ctx.route
+        op, route = ctx.op, ctx.route
+        want = ctx.needs_input_grad[3:]
+        if not any(want):
+            return (None,) * (3 + len(want))
+        faces, *inputs = ctx.saved_tensors
         if torch.is_grad_enabled():
             # create_graph=True: differentiable gradients through the restatement, on the faces the kernels used
-            valid = faces[((faces >= 0) & (faces < route.V)).all(1)]
-            restate = _vertex_normals if ctx.mode == _lib.NORMALS_AVERAGE else _vertex_normals_pre_split
-            out = restate(rows.reshape(route.lead + (route.V, 3)), valid)
-            grad, = torch.autograd.grad(out, rows, grad_out.reshape(out.shape), create_graph=True)
-            return None, None, grad, None
-        dev = rows.device
+            out = op.restate(route, faces[((faces >= 0) & (faces < route.V)).all(1)], *inputs)
+            wanted = [t for t, w in zip(inputs, want) if w]
+            grads = iter(torch.autograd.grad(out, wanted, grad_out.reshape(out.shape), create_graph=True))
+            return (None,) * 3 + tuple(next(grads) if w else None for w in want)
+        dev = inputs[0].device
+        grads = [torch.empty((route.B * route.V, k), dtype=torch.float32, device=dev) if w else None
+                 for k, w in zip(op.input_widths, want)]
         grad_out = grad_out.to(torch.float32).contiguous()
-        grad = torch.empty((route.B * route.V, 3), dtype=torch.float32, device=dev)
-        lib = _lib.lib()
         with torch.cuda.device(dev):
-            rc = lib.dirt_normals_backward(ctx.mode, _ptr(rows), _row_stride(rows), _ptr(faces), _ptr(grad_out),
-                                           _ptr(grad), _ptr(ctx.workspace), ctx.ws_bytes, route.B, route.V, route.F,
-                                           _stream(dev))
-        _lib.check(rc, _NORMALS_NAMES[ctx.mode] + 'Grad')
-        return None, None, grad, None
+            rc = getattr(_lib.lib(), op.backward)(*op.inputs(route, faces, *inputs), _ptr(grad_out),
+                                                  *[_ptr(g) for g in grads], _ptr(ctx.workspace), ctx.ws_bytes,
+                                                  route.B, route.V, route.F, _stream(dev))
+        _lib.check(rc, op.name + 'Grad')
+        return (None,) * 3 + tuple(op.finish(route, grads) if op.finish else grads)
 
 
-def _row_stride(rows):
-    return rows.stride(0) if rows.shape[0] > 1 else 3
-
-
-def _normals(mode, route, vertices, faces):
-    """The CUDA path of a call that `normals_route` accepted."""
-    faces = torch.as_tensor(faces).to(device=vertices.device)
+def _mesh(op, route, faces, *inputs):
+    """The CUDA path of a mesh op's call that its route accepted, on its per-vertex rows (`_point_rows`)."""
+    faces = torch.as_tensor(faces).to(device=inputs[0].device)
     if faces.dtype == torch.int64:
         faces = faces.clamp(-1, (1 << 31) - 1)   # above int32: >= V, so left out like any other invalid index
-    faces = faces.to(torch.int32).contiguous()
-    rows = _rows(vertices[..., :3], 3)
-    if rows.shape[0] > 1 and rows.stride(0) < 3:
-        rows = rows.contiguous()
-    out = _Normals.apply(mode, route, rows, faces)
-    return out.reshape(route.lead + (route.V, 3))
+    out = _MeshFunction.apply(op, route, faces.to(torch.int32).contiguous(), *inputs)
+    return out.reshape(route.lead + (route.V, op.width))
+
+
+def _normals_inputs(mode, route, faces, rows):
+    """The input arguments of dirt_normals_forward / _backward, in their order."""
+    return [mode, _ptr(rows), _stride(rows, 3), _ptr(faces)]
+
+
+def _restate_normals(restate, route, faces, rows):
+    return restate(_unflat_points(rows, route), faces)
+
+
+_NORMALS = _MeshOp('VertexNormals', 'dirt_normals_forward', 'dirt_normals_backward', 'dirt_normals_workspace_bytes',
+                   partial(_normals_inputs, _lib.NORMALS_AVERAGE), 3, (3,), partial(_restate_normals, _vertex_normals))
+_NORMALS_PRE_SPLIT = _NORMALS._replace(name='VertexNormalsPreSplit',
+                                       inputs=partial(_normals_inputs, _lib.NORMALS_PRE_SPLIT),
+                                       restate=partial(_restate_normals, _vertex_normals_pre_split))
 
 
 # ---- tangent-space normal mapping (DESIGN.md §7.14) -------------------------------------------------------------------
@@ -845,73 +874,28 @@ def _tangents_route(vertices, uvs, vertex_normals, faces):
     return tangents_route(meta(vertices), meta(uvs), meta(vertex_normals), faces.shape, faces.dtype)
 
 
-def _point_rows(t, k):
-    """`_rows`, with a row stride of at least k (the C ABI's requirement for these rows)."""
-    r = _rows(t, k)
-    return r.contiguous() if r.shape[0] > 1 and r.stride(0) < k else r
-
-
-def _stride(rows, k):
-    return rows.stride(0) if rows.shape[0] > 1 else k
-
-
-class _Tangents(torch.autograd.Function):
-    """dirt_tangents_forward with its gradient.  rows, normals: [B*V, 3]; uvs: [B*V, 2] (per item) or [V, 2] (shared), all
-    with unit stride along the row; faces: int32 [F, 3] on their device.  The node keeps its inputs and the forward's
-    workspace, whose adjacency the backward kernels read."""
-
-    @staticmethod
-    def forward(ctx, route, rows, uvs, normals, faces):
-        dev = rows.device
-        lib = _lib.lib()
-        out = torch.empty((route.B * route.V, 4), dtype=torch.float32, device=dev)
-        ws_bytes = int(lib.dirt_tangents_workspace_bytes(route.B, route.V, route.F))
-        workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=dev) if ws_bytes else None
-        with torch.cuda.device(dev):
-            rc = lib.dirt_tangents_forward(*_tangent_inputs(route, rows, uvs, normals, faces), _ptr(out), _ptr(workspace),
-                                           ws_bytes, route.B, route.V, route.F, _stream(dev))
-        _lib.check(rc, 'VertexTangents')
-        ctx.save_for_backward(rows, uvs, normals, faces)
-        ctx.route, ctx.workspace, ctx.ws_bytes = route, workspace, ws_bytes
-        return out
-
-    @staticmethod
-    def backward(ctx, grad_out):
-        want = ctx.needs_input_grad[1:4]
-        if not any(want):
-            return (None,) * 5
-        rows, uvs, normals, faces = ctx.saved_tensors
-        route = ctx.route
-        inputs = (rows, uvs, normals)
-        if torch.is_grad_enabled():
-            # create_graph=True: differentiable gradients through the restatement, on the faces the kernels used
-            valid = faces[((faces >= 0) & (faces < route.V)).all(1)]
-            lead, V = route.lead, route.V
-            out = _vertex_tangents(rows.reshape(lead + (V, 3)), uvs.reshape(lead + (V, 2)) if route.uv_per_item else uvs,
-                                   valid, normals.reshape(lead + (V, 3)))
-            wanted = [t for t, w in zip(inputs, want) if w]
-            grads = iter(torch.autograd.grad(out, wanted, grad_out.reshape(out.shape), create_graph=True))
-            return (None,) + tuple(next(grads) if w else None for w in want) + (None,)
-        dev = rows.device
-        n = route.B * route.V
-        grads = [torch.empty((n, k), dtype=torch.float32, device=dev) if w else None for k, w in zip((3, 2, 3), want)]
-        grad_out = grad_out.to(torch.float32).contiguous()
-        lib = _lib.lib()
-        with torch.cuda.device(dev):
-            rc = lib.dirt_tangents_backward(*_tangent_inputs(route, rows, uvs, normals, faces), _ptr(grad_out),
-                                            *[_ptr(g) for g in grads], _ptr(ctx.workspace), ctx.ws_bytes, route.B,
-                                            route.V, route.F, _stream(dev))
-        _lib.check(rc, 'VertexTangentsGrad')
-        if grads[1] is not None and not route.uv_per_item:
-            grads[1] = grads[1].reshape(route.B, route.V, 2).sum(0)   # shared uvs: one fixed-order sum over the items
-        return (None,) + tuple(grads) + (None,)
-
-
-def _tangent_inputs(route, rows, uvs, normals, faces):
+def _tangent_inputs(route, faces, rows, uvs, normals):
     """The input arguments of dirt_tangents_forward / _backward, in their order."""
     uv_stride = _stride(uvs, 2)
     return [_ptr(rows), _stride(rows, 3), _ptr(uvs), uv_stride, route.V * uv_stride if route.uv_per_item else 0,
             _ptr(normals), _stride(normals, 3), _ptr(faces)]
+
+
+def _restate_tangents(route, faces, rows, uvs, normals):
+    return _vertex_tangents(_unflat_points(rows, route), _unflat_points(uvs, route) if route.uv_per_item else uvs,
+                            faces, _unflat_points(normals, route))
+
+
+def _sum_shared_uvs(route, grads):
+    """Shared uvs: their gradient rows [B*V, 2] as [V, 2], by one fixed-order sum over the items."""
+    g_rows, g_uvs, g_normals = grads
+    if g_uvs is not None and not route.uv_per_item:
+        g_uvs = g_uvs.reshape(route.B, route.V, 2).sum(0)
+    return g_rows, g_uvs, g_normals
+
+
+_TANGENTS = _MeshOp('VertexTangents', 'dirt_tangents_forward', 'dirt_tangents_backward',
+                    'dirt_tangents_workspace_bytes', _tangent_inputs, 4, (3, 2, 3), _restate_tangents, _sum_shared_uvs)
 
 
 def vertex_tangents(vertices, uvs, faces, vertex_normals, name=None):
@@ -928,13 +912,8 @@ def vertex_tangents(vertices, uvs, faces, vertex_normals, name=None):
     route = _tangents_route(vertices, uvs, vertex_normals, faces)
     if route is None:
         return _vertex_tangents(vertices, uvs, faces, vertex_normals)
-    faces = torch.as_tensor(faces).to(device=vertices.device)
-    if faces.dtype == torch.int64:
-        faces = faces.clamp(-1, (1 << 31) - 1)   # above int32: >= V, so left out like any other invalid index
-    faces = faces.to(torch.int32).contiguous()
-    out = _Tangents.apply(route, _point_rows(vertices[..., :3], 3), _point_rows(uvs, 2),
-                          _point_rows(vertex_normals, 3), faces)
-    return out.reshape(route.lead + (route.V, 4))
+    return _mesh(_TANGENTS, route, faces, _point_rows(vertices[..., :3], 3), _point_rows(uvs, 2),
+                 _point_rows(vertex_normals, 3))
 
 
 def _normal_map_inputs(route, normals, tangents, samples):
