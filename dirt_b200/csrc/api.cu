@@ -92,7 +92,7 @@ static int required_check(std::initializer_list<const void*> ptrs)
 
 // a caller-owned workspace or scratch of `bytes` bytes that a call needs `need` of: DIRT_ERR_NULL_POINTER if it is NULL,
 // else DIRT_ERR_MISALIGNED if it is not 256-byte aligned, else DIRT_ERR_WORKSPACE_TOO_SMALL if it is too small
-static int scratch_check(void* scratch, size_t bytes, size_t need)
+static int scratch_check(const void* scratch, size_t bytes, size_t need)
 {
     if (!scratch) return DIRT_ERR_NULL_POINTER;
     if ((uintptr_t)scratch % 256) return DIRT_ERR_MISALIGNED;
@@ -151,18 +151,41 @@ extern "C" size_t dirt_workspace_bytes_min(int B, int H, int W, int C, int V, in
     return ws.bytes_without_face_ids + 256;
 }
 
-// needs_face_id_scratch: only a backward call without face ids derives them into the workspace's last block
-static int check_workspace(void* workspace, size_t workspace_bytes, int B, int H, int W, int C, int V, int F,
-                           bool needs_face_id_scratch = false)
-{
-    return scratch_check(workspace, workspace_bytes, needs_face_id_scratch ? dirt_workspace_bytes(B, H, W, C, V, F)
-                                                                           : dirt_workspace_bytes_min(B, H, W, C, V, F));
-}
-
 #define CUDA_TRY(expr)                                   \
     do {                                                 \
         if ((expr) != cudaSuccess) return DIRT_ERR_CUDA; \
     } while (0)
+
+// The checks the rasteriser entries share, in order: NULL (DIRT_ERR_NULL_POINTER) for `required`, for `per_vertex` when
+// V > 0 and for `faces` when F > 0; 16-byte alignment of `aligned16`, then 4-byte alignment of `aligned4`
+// (DIRT_ERR_MISALIGNED); the workspace against `need`.  Before it each entry makes its shape check, its own checks
+// (backward: vertex limit, flags, channel groups; derivatives: channel range) and its DIRT_OK return for B == 0.
+// What stays per entry:
+// - visibility NULL-checks only vertices and faces, and aligns its face ids but not the faces; its G-buffer may be NULL;
+// - backward first requires pixels unless DIRT_BWD_SKIP_POSITION and grad_background unless DIRT_BWD_SKIP_COLOUR; without
+//   face ids it needs dirt_workspace_bytes (room to derive them), and the deterministic entry then checks its scratch.
+static int raster_check(int V, int F, const int32_t* faces, std::initializer_list<const void*> required,
+                        std::initializer_list<const void*> per_vertex, std::initializer_list<const void*> aligned16,
+                        std::initializer_list<const void*> aligned4, const void* workspace, size_t bytes, size_t need)
+{
+    for (const void* p : required)
+        if (!p) return DIRT_ERR_NULL_POINTER;
+    for (const void* p : per_vertex)
+        if (V > 0 && !p) return DIRT_ERR_NULL_POINTER;
+    if (F > 0 && !faces) return DIRT_ERR_NULL_POINTER;
+    for (const void* p : aligned16)
+        if ((uintptr_t)p % 16) return DIRT_ERR_MISALIGNED;
+    return aligned(aligned4) ? scratch_check(workspace, bytes, need) : DIRT_ERR_MISALIGNED;
+}
+
+// the workspace blocks, launch sizes and stream of one rasteriser call
+struct RasterCall { Workspace ws; Dims d; cudaStream_t stream; };
+
+static RasterCall raster_call(const void* workspace, int B, int H, int W, int C, int V, int F, void* cuda_stream)
+{
+    return {carve_workspace(const_cast<void*>(workspace), B, H, W, C, V, F), make_dims(B, H, W, C, V, F),
+            (cudaStream_t)cuda_stream};
+}
 
 extern "C" int dirt_rasterise_forward(const float* background, const float* vertices, const float* vertex_colors,
                                       const int32_t* faces, float* pixels, int32_t* face_ids_out, int B, int H, int W,
@@ -171,20 +194,14 @@ extern "C" int dirt_rasterise_forward(const float* background, const float* vert
     launch_count() = 0;
     if (!shape_ok(B, H, W, C, V, F)) return DIRT_ERR_BAD_SHAPE;
     if (B == 0) return DIRT_OK;
-    if (!background || !pixels) return DIRT_ERR_NULL_POINTER;
-    if ((V > 0 && (!vertices || !vertex_colors)) || (F > 0 && !faces)) return DIRT_ERR_NULL_POINTER;
-    if ((uintptr_t)vertices % 16 != 0) return DIRT_ERR_MISALIGNED;
-    if ((uintptr_t)background % 4 || (uintptr_t)pixels % 4 || (uintptr_t)vertex_colors % 4 || (uintptr_t)faces % 4 ||
-        (uintptr_t)face_ids_out % 4)
-        return DIRT_ERR_MISALIGNED;
-    int rc = check_workspace(workspace, workspace_bytes, B, H, W, C, V, F);
+    const int rc = raster_check(V, F, faces, {background, pixels}, {vertices, vertex_colors}, {vertices},
+                                {background, pixels, vertex_colors, faces, face_ids_out}, workspace, workspace_bytes,
+                                dirt_workspace_bytes_min(B, H, W, C, V, F));
     if (rc != DIRT_OK) return rc;
-    cudaStream_t stream = (cudaStream_t)cuda_stream;
-    const Workspace ws = carve_workspace(workspace, B, H, W, C, V, F);
-    const Dims d = make_dims(B, H, W, C, V, F);
-    CUDA_TRY(launch_setup_and_bin(vertices, faces, vertex_colors, ws, d, stream));
+    const RasterCall r = raster_call(workspace, B, H, W, C, V, F, cuda_stream);
+    CUDA_TRY(launch_setup_and_bin(vertices, faces, vertex_colors, r.ws, r.d, r.stream));
 #if !defined(DIRT_SETUP_ABLATE) || DIRT_SETUP_ABLATE == 0   // a setup timing build leaves the records undefined
-    CUDA_TRY(launch_raster_forward(vertices, background, vertex_colors, pixels, face_ids_out, ws, d, stream));
+    CUDA_TRY(launch_raster_forward(vertices, background, vertex_colors, pixels, face_ids_out, r.ws, r.d, r.stream));
 #endif
     return DIRT_OK;
 }
@@ -196,19 +213,17 @@ extern "C" int dirt_rasterise_visibility(const float* vertices, const int32_t* f
     launch_count() = 0;
     if (!shape_ok(B, H, W, 1, V, F)) return DIRT_ERR_BAD_SHAPE;
     if (B == 0) return DIRT_OK;
-    if ((V > 0 && !vertices) || (F > 0 && !faces)) return DIRT_ERR_NULL_POINTER;
-    if ((uintptr_t)vertices % 16 != 0 || (uintptr_t)gbuffer % 16 != 0 || (uintptr_t)face_ids % 4 != 0)
-        return DIRT_ERR_MISALIGNED;
-    int rc = check_workspace(workspace, workspace_bytes, B, H, W, 1, V, F);
+    const int rc = raster_check(V, F, faces, {}, {vertices}, {vertices, gbuffer}, {face_ids}, workspace, workspace_bytes,
+                                dirt_workspace_bytes_min(B, H, W, 1, V, F));
     if (rc != DIRT_OK) return rc;
-    cudaStream_t stream = (cudaStream_t)cuda_stream;
-    const Workspace ws = carve_workspace(workspace, B, H, W, 1, V, F);
-    const Dims d = make_dims(B, H, W, 1, V, F);
-    CUDA_TRY(launch_setup_and_bin(vertices, faces, nullptr, ws, d, stream));
-    CUDA_TRY(launch_raster_visibility(vertices, face_ids, gbuffer, ws, d, stream));
+    const RasterCall r = raster_call(workspace, B, H, W, 1, V, F, cuda_stream);
+    CUDA_TRY(launch_setup_and_bin(vertices, faces, nullptr, r.ws, r.d, r.stream));
+    CUDA_TRY(launch_raster_visibility(vertices, face_ids, gbuffer, r.ws, r.d, r.stream));
     return DIRT_OK;
 }
 
+// The three backward entries.  The deterministic one adds its int32 rule (the adjacency's corner ids b*3F + k*F + f, a
+// second DIRT_ERR_BAD_SHAPE check) and its scratch.
 static int backward_impl(const float* vertices, const int32_t* faces, const float* pixels, const float* grad_pixels,
                          const int32_t* face_ids, float* grad_background, float* grad_vertices, float* grad_vertex_colors,
                          int B, int H, int W, int C, int V, int F, const int* channel_groups, int n_groups,
@@ -216,52 +231,44 @@ static int backward_impl(const float* vertices, const int32_t* faces, const floa
                          bool deterministic = false, void* scratch = nullptr, size_t scratch_bytes = 0)
 {
     launch_count() = 0;
-    if (!shape_ok(B, H, W, C, V, F)) return DIRT_ERR_BAD_SHAPE;
+    if (!shape_ok(B, H, W, C, V, F) || (deterministic && 3ll * B * F > (1ll << 31) - 1)) return DIRT_ERR_BAD_SHAPE;
     if (V > (1 << 24)) return DIRT_ERR_TOO_MANY_VERTICES;
     if (flags & ~(DIRT_BWD_SHARED_GEOMETRY | DIRT_BWD_SKIP_POSITION | DIRT_BWD_SKIP_COLOUR)) return DIRT_ERR_BAD_SHAPE;
     GroupSpec groups;
     int rc = make_groups(C, channel_groups, n_groups, &groups);
     if (rc != DIRT_OK) return rc;
     if (B == 0) return DIRT_OK;
-    if (!grad_pixels) return DIRT_ERR_NULL_POINTER;
-    if (!(flags & DIRT_BWD_SKIP_POSITION) && !pixels) return DIRT_ERR_NULL_POINTER;
-    if (!(flags & DIRT_BWD_SKIP_COLOUR) && !grad_background) return DIRT_ERR_NULL_POINTER;
-    if ((V > 0 && (!vertices || !grad_vertices || !grad_vertex_colors)) || (F > 0 && !faces)) return DIRT_ERR_NULL_POINTER;
-    if ((uintptr_t)vertices % 16 != 0 || (uintptr_t)grad_vertices % 16 != 0) return DIRT_ERR_MISALIGNED;
-    if ((uintptr_t)pixels % 4 || (uintptr_t)grad_pixels % 4 || (uintptr_t)grad_background % 4 ||
-        (uintptr_t)grad_vertex_colors % 4 || (uintptr_t)faces % 4 || (uintptr_t)face_ids % 4)
-        return DIRT_ERR_MISALIGNED;
-    rc = check_workspace(workspace, workspace_bytes, B, H, W, C, V, F, face_ids == nullptr);
-    if (rc != DIRT_OK) return rc;
-    if (deterministic) {
+    if ((!(flags & DIRT_BWD_SKIP_POSITION) && !pixels) || (!(flags & DIRT_BWD_SKIP_COLOUR) && !grad_background))
+        return DIRT_ERR_NULL_POINTER;
+    rc = raster_check(V, F, faces, {grad_pixels}, {vertices, grad_vertices, grad_vertex_colors}, {vertices, grad_vertices},
+                      {pixels, grad_pixels, grad_background, grad_vertex_colors, faces, face_ids}, workspace, workspace_bytes,
+                      face_ids ? dirt_workspace_bytes_min(B, H, W, C, V, F) : dirt_workspace_bytes(B, H, W, C, V, F));
+    if (rc == DIRT_OK && deterministic)
         rc = scratch_check(scratch, scratch_bytes, dirt_rasterise_backward_deterministic_bytes(B, H, W, C, V, F));
-        if (rc != DIRT_OK) return rc;
-    }
-    cudaStream_t stream = (cudaStream_t)cuda_stream;
-    const Workspace ws = carve_workspace(workspace, B, H, W, C, V, F);
-    const Dims d = make_dims(B, H, W, C, V, F);
+    if (rc != DIRT_OK) return rc;
+    const RasterCall r = raster_call(workspace, B, H, W, C, V, F, cuda_stream);
     const int32_t* ids = face_ids;
     // the tile coverage flags in the workspace describe `ids` when the raster kernel that produced them ran on this workspace
     const bool flags_valid = !ids || workspace_holds_setup;
     unsigned long long expect_tag = 0;
     if (!ids) {
         // no cached visibility: re-derive it exactly as the forward pass does
-        CUDA_TRY(launch_setup_and_bin(vertices, faces, nullptr, ws, d, stream));
-        CUDA_TRY(launch_raster_visibility(vertices, ws.face_ids, nullptr, ws, d, stream));
-        ids = ws.face_ids;
+        CUDA_TRY(launch_setup_and_bin(vertices, faces, nullptr, r.ws, r.d, r.stream));
+        CUDA_TRY(launch_raster_visibility(vertices, r.ws.face_ids, nullptr, r.ws, r.d, r.stream));
+        ids = r.ws.face_ids;
     } else if (!workspace_holds_setup) {
-        CUDA_TRY(launch_setup_only(vertices, faces, ws, d, stream));
+        CUDA_TRY(launch_setup_only(vertices, faces, r.ws, r.d, r.stream));
     } else {
         // a promise: checked on the device against the tag the setup pass left in the workspace
         expect_tag = workspace_tag(vertices, faces, B, H, W, V, F);
     }
     if (deterministic)
         CUDA_TRY(launch_backward_deterministic(vertices, faces, pixels, grad_pixels, ids, grad_background, grad_vertices,
-                                               grad_vertex_colors, ws, d, groups, flags, expect_tag,
-                                               carve_det_scratch(scratch, B, H, W, C, V, F), stream));
+                                               grad_vertex_colors, r.ws, r.d, groups, flags, expect_tag,
+                                               carve_det_scratch(scratch, B, H, W, C, V, F), r.stream));
     else
-        CUDA_TRY(launch_backward(vertices, pixels, grad_pixels, ids, grad_background, grad_vertices, grad_vertex_colors, ws, d,
-                                 groups, flags_valid, flags, expect_tag, stream));
+        CUDA_TRY(launch_backward(vertices, pixels, grad_pixels, ids, grad_background, grad_vertices, grad_vertex_colors, r.ws,
+                                 r.d, groups, flags_valid, flags, expect_tag, r.stream));
     return DIRT_OK;
 }
 
@@ -285,42 +292,6 @@ extern "C" int dirt_rasterise_backward_ex(const float* vertices, const int32_t* 
                          W, C, V, F, channel_groups, n_groups, workspace_holds_setup, flags, workspace, workspace_bytes, cuda_stream);
 }
 
-extern "C" int dirt_rasterise_derivatives(const float* vertices, const int32_t* faces, const float* attributes,
-                                          const int32_t* face_ids, float* derivatives, int B, int H, int W, int C, int V,
-                                          int F, int first_channel, int channel_count, int workspace_holds_setup,
-                                          void* workspace, size_t workspace_bytes, void* cuda_stream)
-{
-    launch_count() = 0;
-    if (!shape_ok(B, H, W, C, V, F)) return DIRT_ERR_BAD_SHAPE;
-    if (first_channel < 0 || channel_count <= 0 || first_channel >= C || channel_count > C - first_channel)
-        return DIRT_ERR_BAD_SHAPE;
-    if (B == 0) return DIRT_OK;
-    if (!face_ids || !derivatives) return DIRT_ERR_NULL_POINTER;
-    if ((V > 0 && (!vertices || !attributes)) || (F > 0 && !faces)) return DIRT_ERR_NULL_POINTER;
-    if ((uintptr_t)vertices % 16 != 0) return DIRT_ERR_MISALIGNED;
-    if ((uintptr_t)attributes % 4 || (uintptr_t)faces % 4 || (uintptr_t)face_ids % 4 || (uintptr_t)derivatives % 4)
-        return DIRT_ERR_MISALIGNED;
-    int rc = check_workspace(workspace, workspace_bytes, B, H, W, C, V, F);
-    if (rc != DIRT_OK) return rc;
-    cudaStream_t stream = (cudaStream_t)cuda_stream;
-    const Workspace ws = carve_workspace(workspace, B, H, W, C, V, F);
-    const Dims d = make_dims(B, H, W, C, V, F);
-    unsigned long long expect_tag = 0;
-    if (!workspace_holds_setup)
-        CUDA_TRY(launch_setup_only(vertices, faces, ws, d, stream));
-    else
-        expect_tag = workspace_tag(vertices, faces, B, H, W, V, F);   // checked on the device, as backward_impl does
-    CUDA_TRY(launch_gbuffer_derivatives(face_ids, attributes, derivatives, ws, d, first_channel, channel_count, expect_tag,
-                                        stream));
-    return DIRT_OK;
-}
-
-// the adjacency's corner ids b*3F + k*F + f are int32
-static bool deterministic_shape_ok(int B, int H, int W, int C, int V, int F)
-{
-    return shape_ok(B, H, W, C, V, F) && 3ll * B * F <= (1ll << 31) - 1;
-}
-
 extern "C" size_t dirt_rasterise_backward_deterministic_bytes(int B, int H, int W, int C, int V, int F)
 {
     if (!shape_ok(B, H, W, C > 0 ? C : 1, V, F) || B == 0) return 0;
@@ -335,11 +306,34 @@ extern "C" int dirt_rasterise_backward_deterministic(const float* vertices, cons
                                                      size_t workspace_bytes, void* scratch, size_t scratch_bytes,
                                                      void* cuda_stream)
 {
-    launch_count() = 0;
-    if (!deterministic_shape_ok(B, H, W, C, V, F)) return DIRT_ERR_BAD_SHAPE;
     return backward_impl(vertices, faces, pixels, grad_pixels, face_ids, grad_background, grad_vertices, grad_vertex_colors, B, H,
                          W, C, V, F, channel_groups, n_groups, workspace_holds_setup, flags, workspace, workspace_bytes,
                          cuda_stream, true, scratch, scratch_bytes);
+}
+
+extern "C" int dirt_rasterise_derivatives(const float* vertices, const int32_t* faces, const float* attributes,
+                                          const int32_t* face_ids, float* derivatives, int B, int H, int W, int C, int V,
+                                          int F, int first_channel, int channel_count, int workspace_holds_setup,
+                                          void* workspace, size_t workspace_bytes, void* cuda_stream)
+{
+    launch_count() = 0;
+    if (!shape_ok(B, H, W, C, V, F)) return DIRT_ERR_BAD_SHAPE;
+    if (first_channel < 0 || channel_count <= 0 || first_channel >= C || channel_count > C - first_channel)
+        return DIRT_ERR_BAD_SHAPE;
+    if (B == 0) return DIRT_OK;
+    const int rc = raster_check(V, F, faces, {face_ids, derivatives}, {vertices, attributes}, {vertices},
+                                {attributes, faces, face_ids, derivatives}, workspace, workspace_bytes,
+                                dirt_workspace_bytes_min(B, H, W, C, V, F));
+    if (rc != DIRT_OK) return rc;
+    const RasterCall r = raster_call(workspace, B, H, W, C, V, F, cuda_stream);
+    unsigned long long expect_tag = 0;
+    if (!workspace_holds_setup)
+        CUDA_TRY(launch_setup_only(vertices, faces, r.ws, r.d, r.stream));
+    else
+        expect_tag = workspace_tag(vertices, faces, B, H, W, V, F);   // checked on the device, as backward_impl does
+    CUDA_TRY(launch_gbuffer_derivatives(face_ids, attributes, derivatives, r.ws, r.d, first_channel, channel_count, expect_tag,
+                                        r.stream));
+    return DIRT_OK;
 }
 
 // texel indices (and the warp keys built from them) stay below 2^62, element offsets of every buffer below 2^62
@@ -1402,12 +1396,11 @@ extern "C" int dirt_workspace_status(const void* workspace, size_t workspace_byt
 {
     if (!shape_ok(B, H, W, C, V, F)) return DIRT_ERR_BAD_SHAPE;
     if (B == 0) return DIRT_OK;
-    int rc = check_workspace(const_cast<void*>(workspace), workspace_bytes, B, H, W, C, V, F);
+    const int rc = scratch_check(workspace, workspace_bytes, dirt_workspace_bytes_min(B, H, W, C, V, F));
     if (rc != DIRT_OK) return rc;
-    const Workspace ws = carve_workspace(const_cast<void*>(workspace), B, H, W, C, V, F);
+    const RasterCall r = raster_call(workspace, B, H, W, C, V, F, cuda_stream);
     Header h;
-    cudaStream_t stream = (cudaStream_t)cuda_stream;
-    if (cudaMemcpyAsync(&h, ws.header, sizeof(h), cudaMemcpyDeviceToHost, stream) != cudaSuccess) return DIRT_ERR_CUDA;
-    if (cudaStreamSynchronize(stream) != cudaSuccess) return DIRT_ERR_CUDA;
+    if (cudaMemcpyAsync(&h, r.ws.header, sizeof(h), cudaMemcpyDeviceToHost, r.stream) != cudaSuccess) return DIRT_ERR_CUDA;
+    if (cudaStreamSynchronize(r.stream) != cudaSuccess) return DIRT_ERR_CUDA;
     return h.error ? DIRT_ERR_STALE_WORKSPACE : DIRT_OK;
 }

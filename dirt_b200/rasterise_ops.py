@@ -21,7 +21,8 @@ from . import _lib
 
 def default_channel_groups(channels):
     """The reference's split of `channels` into op calls: one group if channels is 1 or 3, else greedily
-    groups of 3 while at least 3 remain, then groups of 1 (dirt/rasterise_ops.py:80-108)."""
+    groups of 3 while at least 3 remain, then groups of 1 (dirt/rasterise_ops.py:80-108).  The library makes the same
+    split (make_groups, csrc/api.cu) for a backward call given no groups, as the autograd nodes here are."""
     if channels <= 0:
         raise ValueError('channels must be positive')
     if channels == 1 or channels == 3:
@@ -103,6 +104,13 @@ def _geometry_identity(vertices, faces, H, W):
     return (vertices.data_ptr(), vertices._version, tuple(vertices.shape), faces.data_ptr(), faces._version, tuple(faces.shape), H, W)
 
 
+def _holds_setup(workspace, vertices, faces, B, H, W, C, V, F):
+    """Whether the setup records in `workspace` (a forward call's, or None) can be reused by a call on these tensors: it
+    is big enough for the call and still describes exactly these tensors (storage, version counters, sizes)."""
+    return (workspace is not None and workspace.numel() >= int(_lib.lib().dirt_workspace_bytes_min(B, H, W, C, V, F)) and
+            getattr(workspace, '_dirt_setup_of', None) == _geometry_identity(vertices, faces, H, W))
+
+
 def rasterise_backward_raw(vertices, faces, pixels, grad_pixels, face_ids=None, channel_groups=None, setup_workspace=None,
                            shared_geometry=False, want_position=True, want_colour=True, deterministic=None):
     """One call of dirt_rasterise_backward (the RasteriseGrad op, csrc/rasterise_grad_egl.cpp:33-53).
@@ -111,6 +119,7 @@ def rasterise_backward_raw(vertices, faces, pixels, grad_pixels, face_ids=None, 
     recomputed.  `shared_geometry`: accumulate the vertex gradients over the batch (DIRT_BWD_SHARED_GEOMETRY):
     grad_vertices [V,4] and grad_vertex_colors [V,C] instead of [B,V,.].  want_position / want_colour = False skip
     the position terms (grad_vertices comes back zero) / the colour terms (grad_vertex_colors zero, grad_background None).
+    `pixels` and `grad_pixels` are made contiguous float32 here.
     `deterministic`: run dirt_rasterise_backward_deterministic, whose outputs are bit-reproducible (float64 sums in a
     fixed order, no float atomics); None follows torch.are_deterministic_algorithms_enabled().  Its scratch is allocated
     per call.
@@ -126,6 +135,7 @@ def rasterise_backward_raw(vertices, faces, pixels, grad_pixels, face_ids=None, 
         raise ValueError('RasteriseGrad expects grad_pixels to be 4D, and grad_pixels.shape == [None, height, width, channels]')
     if faces.shape[0] != B or vertices.shape[0] != B:
         raise ValueError('RasteriseGrad expects all arguments to have same leading (batch) dimension')
+    pixels, grad_pixels = pixels.contiguous().to(torch.float32), grad_pixels.contiguous().to(torch.float32)
     device = pixels.device
     grad_background = torch.empty_like(pixels) if want_colour else None
     lead = () if shared_geometry else (B,)
@@ -136,9 +146,7 @@ def rasterise_backward_raw(vertices, faces, pixels, grad_pixels, face_ids=None, 
     else:
         groups_arr = (ctypes.c_int * len(channel_groups))(*[int(g) for g in channel_groups])
         groups_ptr, n_groups = groups_arr, len(channel_groups)
-    need = int(_lib.lib().dirt_workspace_bytes_min(B, H, W, C, V, F))
-    reuse = int(setup_workspace is not None and face_ids is not None and setup_workspace.numel() >= need and
-                getattr(setup_workspace, '_dirt_setup_of', None) == _geometry_identity(vertices, faces, H, W))
+    reuse = int(face_ids is not None and _holds_setup(setup_workspace, vertices, faces, B, H, W, C, V, F))
     ws = setup_workspace if reuse else _workspace(B, H, W, C, V, F, device, face_id_scratch=face_ids is None)[0]
     nbytes = int(ws.numel())
     flags = ((_lib.BWD_SHARED_GEOMETRY if shared_geometry else 0) | (0 if want_position else _lib.BWD_SKIP_POSITION) |
@@ -172,9 +180,7 @@ def rasterise_derivatives_raw(vertices, faces, attributes, face_ids, first_chann
     B, H, W = face_ids.shape
     V, F, C = vertices.shape[1], faces.shape[1], attributes.shape[2]
     device = face_ids.device
-    need = int(_lib.lib().dirt_workspace_bytes_min(B, H, W, C, V, F))
-    reuse = int(setup_workspace is not None and setup_workspace.numel() >= need and
-                getattr(setup_workspace, '_dirt_setup_of', None) == _geometry_identity(vertices, faces, H, W))
+    reuse = int(_holds_setup(setup_workspace, vertices, faces, B, H, W, C, V, F))
     ws = setup_workspace if reuse else _workspace(B, H, W, C, V, F, device)[0]
     out = torch.empty((B, H, W, 2, channel_count), dtype=torch.float32, device=device)
     with torch.cuda.device(device):
@@ -212,12 +218,11 @@ class _Rasterise(torch.autograd.Function):
     """The Rasterise op with its registered gradient (dirt/rasterise_ops.py:111-129)."""
 
     @staticmethod
-    def forward(ctx, background, vertices, vertex_colors, faces, channel_groups):
+    def forward(ctx, background, vertices, vertex_colors, faces):
         pixels, face_ids, ws = rasterise_forward_raw(background, vertices, vertex_colors, faces, want_face_ids=True,
                                                      return_workspace=True)
         ctx.save_for_backward(vertices, faces, pixels, face_ids)
         ctx.setup_workspace = ws   # per-face setup records of this (vertices, faces): backward reuses them
-        ctx.channel_groups = channel_groups
         ctx.mark_non_differentiable(face_ids)
         return pixels, face_ids
 
@@ -225,25 +230,18 @@ class _Rasterise(torch.autograd.Function):
     def backward(ctx, grad_pixels, _grad_face_ids):
         want_background, want_vertices, want_colours = ctx.needs_input_grad[:3]
         if not (want_background or want_vertices or want_colours):
-            return None, None, None, None, None
+            return None, None, None, None
         vertices, faces, pixels, face_ids = ctx.saved_tensors
-        grad_pixels = grad_pixels.contiguous().to(torch.float32)
+        # channel_groups=None: the library's own split of the channels, the reference's greedy 3/1 grouping
         grad_background, grad_vertices, grad_vertex_colors = rasterise_backward_raw(
-            vertices, faces, pixels, grad_pixels, face_ids, ctx.channel_groups, ctx.setup_workspace,
+            vertices, faces, pixels, grad_pixels, face_ids, None, ctx.setup_workspace,
             want_position=want_vertices, want_colour=want_background or want_colours)
         return (grad_background if want_background else None, grad_vertices if want_vertices else None,
-                grad_vertex_colors if want_colours else None, None, None)  # None: wrt faces
+                grad_vertex_colors if want_colours else None, None)  # None: wrt faces
 
 
-def _as_f32(x, device=None):
-    t = torch.as_tensor(x, dtype=torch.float32) if not isinstance(x, torch.Tensor) else x.to(torch.float32)
-    if device is not None and t.device != device:
-        t = t.to(device)
-    return t
-
-
-def _as_i32(x, device=None):
-    t = torch.as_tensor(x, dtype=torch.int32) if not isinstance(x, torch.Tensor) else x.to(torch.int32)
+def _as(x, dtype, device=None):
+    t = torch.as_tensor(x, dtype=dtype) if not isinstance(x, torch.Tensor) else x.to(dtype)
     if device is not None and t.device != device:
         t = t.to(device)
     return t
@@ -260,6 +258,38 @@ def _pick_device(*xs):
     return None
 
 
+def _inputs(background, vertices, vertex_colors, faces, single, check):
+    """The four inputs of one rasterise call as contiguous float32 tensors (faces int32) on one CUDA device, with a leading
+    batch axis added when `single`.  Once the background is known to be 4-D, `check(background, vertices, vertex_colors,
+    faces)` makes the caller's shape checks; its result is returned after the four tensors.  The inputs must be on a CUDA
+    device only after that, so a malformed call raises its shape error on a machine without a GPU too."""
+    device = _pick_device(background, vertices, vertex_colors, faces)
+    inputs = [_as(x, torch.float32, device) for x in (background, vertices, vertex_colors)] + [_as(faces, torch.int32, device)]
+    if single:
+        inputs = [t[None] for t in inputs]
+    if inputs[0].dim() != 4:
+        raise ValueError('Rasterise expects background_tensor to be 4D, and bgcolor.shape == [None, height, width, channels]')
+    checked = check(*inputs)
+    _require_cuda(*inputs)
+    return [t.contiguous() for t in inputs] + [checked]
+
+
+def _rasterise(background, vertices, vertex_colors, faces, height, width, channels, single):
+    def check(background, vertices, vertex_colors, faces):
+        h = int(background.shape[1]) if height is None else height
+        w = int(background.shape[2]) if width is None else width
+        c = int(background.shape[3]) if channels is None else channels
+        if not (c > 0):
+            raise ValueError('channels must be positive')  # `assert channels > 0`, rasterise_ops.py:87
+        if not (w > 0 and h > 0):
+            raise ValueError('width and height must be positive')  # csrc/hwc.h:28
+        _check_shapes('Rasterise', background, vertices, vertex_colors, faces, h, w, c)
+
+    background, vertices, vertex_colors, faces, _ = _inputs(background, vertices, vertex_colors, faces, single, check)
+    pixels, _ = _Rasterise.apply(background, vertices, vertex_colors, faces)
+    return pixels[0] if single else pixels
+
+
 def rasterise(background, vertices, vertex_colors, faces, height=None, width=None, channels=None, name=None):
     """Rasterises the given `vertices` and `faces` over `background` (dirt/rasterise_ops.py:13-48).
 
@@ -274,12 +304,7 @@ def rasterise(background, vertices, vertex_colors, faces, height=None, width=Non
     Returns:
         float32 tensor [height, width, channels]
     """
-    device = _pick_device(background, vertices, vertex_colors, faces)
-    background = _as_f32(background, device)
-    vertices = _as_f32(vertices, device)
-    vertex_colors = _as_f32(vertex_colors, device)
-    faces = _as_i32(faces, device)
-    return rasterise_batch(background[None], vertices[None], vertex_colors[None], faces[None], height, width, channels, name)[0]
+    return _rasterise(background, vertices, vertex_colors, faces, height, width, channels, single=True)
 
 
 def rasterise_batch(background, vertices, vertex_colors, faces, height=None, width=None, channels=None, name=None):
@@ -287,52 +312,7 @@ def rasterise_batch(background, vertices, vertex_colors, faces, height=None, wid
 
     As `rasterise`, with a leading batch dimension on every argument.
     """
-    device = _pick_device(background, vertices, vertex_colors, faces)
-    background = _as_f32(background, device)
-    vertices = _as_f32(vertices, device)
-    vertex_colors = _as_f32(vertex_colors, device)
-    faces = _as_i32(faces, device)
-    if background.dim() != 4:
-        raise ValueError('Rasterise expects background_tensor to be 4D, and bgcolor.shape == [None, height, width, channels]')
-    if height is None:
-        height = int(background.shape[1])
-    if width is None:
-        width = int(background.shape[2])
-    if channels is None:
-        channels = int(background.shape[3])
-    if not (channels > 0):
-        raise ValueError('channels must be positive')  # `assert channels > 0`, rasterise_ops.py:87
-    if not (width > 0 and height > 0):
-        raise ValueError('width and height must be positive')  # csrc/hwc.h:28
-    _check_shapes('Rasterise', background, vertices, vertex_colors, faces, height, width, channels)
-    _require_cuda(background, vertices, vertex_colors, faces)
-    groups = default_channel_groups(channels)
-    pixels, _ = _Rasterise.apply(background.contiguous(), vertices.contiguous(), vertex_colors.contiguous(),
-                                 faces.contiguous(), groups)
-    return pixels
-
-
-def _rasterise_grad_multichannel(vertices, faces, pixels, d_loss_by_pixels, single_or_batch, face_ids=None,
-                                 setup_workspace=None, want_position=True, want_colour=True):
-    """dirt/rasterise_ops.py:132-177: RasteriseGrad over the greedy channel groups of `pixels`, summing
-    grad_vertices over groups and concatenating the others -- here one fused backward call (no slicing, no copies).
-    Deferred shading uses only one half of each of its two calls (:206-237): want_position / want_colour = False
-    skip the other half inside the kernel."""
-    assert single_or_batch in ['single', 'batch']
-    if single_or_batch == 'single':
-        vertices, faces, pixels, d_loss_by_pixels = vertices[None], faces[None], pixels[None], d_loss_by_pixels[None]
-        if face_ids is not None:
-            face_ids = face_ids[None]
-    assert pixels.dim() == 4
-    groups = default_channel_groups(int(pixels.shape[3]))
-    grad_background, grad_vertices, grad_vertex_colors = rasterise_backward_raw(
-        vertices.contiguous(), faces.contiguous(), pixels.contiguous().to(torch.float32),
-        d_loss_by_pixels.contiguous().to(torch.float32), face_ids, groups, setup_workspace,
-        want_position=want_position, want_colour=want_colour)
-    if single_or_batch == 'single':
-        return {'grad_vertices': grad_vertices[0], 'grad_vertex_colors': grad_vertex_colors[0],
-                'grad_background': None if grad_background is None else grad_background[0]}
-    return {'grad_vertices': grad_vertices, 'grad_vertex_colors': grad_vertex_colors, 'grad_background': grad_background}
+    return _rasterise(background, vertices, vertex_colors, faces, height, width, channels, single=False)
 
 
 class _SetupHolder(object):
@@ -363,9 +343,9 @@ class _RasteriseAttributes(torch.autograd.Function):
             return None, None, None, None, None
         vertices, faces, gbuffer, face_ids = ctx.saved_tensors
         # the vertex gradient of THIS call (filtering the G-buffer) is the one the reference discards (:233-237)
-        grads = _rasterise_grad_multichannel(vertices, faces, gbuffer, d_loss_by_gbuffer, 'batch', face_ids,
-                                             ctx.holder.workspace, want_position=False)
-        return grads['grad_background'], None, grads['grad_vertex_colors'], None, None
+        grad_background, _, grad_attributes = rasterise_backward_raw(vertices, faces, gbuffer, d_loss_by_gbuffer, face_ids,
+                                                                     None, ctx.holder.workspace, want_position=False)
+        return grad_background, None, grad_attributes, None, None
 
 
 class _InjectVertexGradient(torch.autograd.Function):
@@ -383,8 +363,8 @@ class _InjectVertexGradient(torch.autograd.Function):
         if not ctx.needs_input_grad[1]:
             return d_loss_by_pixels, None, None, None, None
         pixels, vertices, faces, face_ids = ctx.saved_tensors
-        d_loss_by_vertices = _rasterise_grad_multichannel(vertices, faces, pixels, d_loss_by_pixels, 'batch', face_ids,
-                                                          ctx.holder.workspace, want_colour=False)['grad_vertices']
+        _, d_loss_by_vertices, _ = rasterise_backward_raw(vertices, faces, pixels, d_loss_by_pixels, face_ids, None,
+                                                          ctx.holder.workspace, want_colour=False)
         return d_loss_by_pixels, d_loss_by_vertices, None, None, None
 
 
@@ -401,42 +381,33 @@ def _channel_run(derivative_channels, channels):
     return run[0], len(run)
 
 
-def _rasterise_deferred_internal(background, vertices, attributes, faces, shader_fn, shader_additional_inputs, single_or_batch, name,
+def _rasterise_deferred_internal(background, vertices, attributes, faces, shader_fn, shader_additional_inputs, single,
                                  derivative_channels=None):
     # dirt/rasterise_ops.py:180-257.  The reference wraps everything in one tf.custom_gradient; here the same
     # three gradient paths are expressed as two autograd nodes around an ordinary call of shader_fn, so tensors
     # and parameters that shader_fn uses receive their gradients from plain autograd.
-    assert single_or_batch in ['single', 'batch']
-    device = _pick_device(background, vertices, attributes, faces)
-    background = _as_f32(background, device)
-    vertices = _as_f32(vertices, device)
-    attributes = _as_f32(attributes, device)
-    faces = _as_i32(faces, device)
-    if single_or_batch == 'single':
-        background, vertices, attributes, faces = background[None], vertices[None], attributes[None], faces[None]
-    if background.dim() != 4:
-        raise ValueError('Rasterise expects background_tensor to be 4D, and bgcolor.shape == [None, height, width, channels]')
-    _check_shapes('Rasterise', background, vertices, attributes, faces, int(background.shape[1]), int(background.shape[2]),
-                  int(background.shape[3]))
-    if derivative_channels is not None:
-        first, count = _channel_run(derivative_channels, int(attributes.shape[2]))
-    _require_cuda(background, vertices, attributes, faces)
-    background, vertices, attributes, faces = background.contiguous(), vertices.contiguous(), attributes.contiguous(), faces.contiguous()
+    def check(background, vertices, attributes, faces):
+        _check_shapes('Rasterise', background, vertices, attributes, faces, int(background.shape[1]),
+                      int(background.shape[2]), int(background.shape[3]))
+        if derivative_channels is not None:
+            return _channel_run(derivative_channels, int(attributes.shape[2]))
+
+    background, vertices, attributes, faces, run = _inputs(background, vertices, attributes, faces, single, check)
     holder = _SetupHolder(None)
     gbuffer, face_ids = _RasteriseAttributes.apply(background, vertices, attributes, faces, holder)
     extra = {}
-    if derivative_channels is not None:
+    if run is not None:
         with torch.no_grad():
-            derivatives = rasterise_derivatives_raw(vertices, faces, attributes, face_ids, first, count, holder.workspace)
-        extra['gbuffer_derivatives'] = derivatives[0] if single_or_batch == 'single' else derivatives
-    if single_or_batch == 'single':
+            derivatives = rasterise_derivatives_raw(vertices, faces, attributes, face_ids, *run, holder.workspace)
+        extra['gbuffer_derivatives'] = derivatives[0] if single else derivatives
+    if single:
         pixels = shader_fn(gbuffer[0], *shader_additional_inputs, **extra)[None]
     else:
         pixels = shader_fn(gbuffer, *shader_additional_inputs, **extra)
     if pixels.dim() != 4 or pixels.shape[:3] != gbuffer.shape[:3]:
         raise ValueError('shader_fn must return pixels of shape [height, width, channels] per image')
     pixels = _InjectVertexGradient.apply(pixels.to(torch.float32), vertices, faces, face_ids, holder)
-    return pixels[0] if single_or_batch == 'single' else pixels
+    return pixels[0] if single else pixels
 
 
 def rasterise_deferred(background_attributes, vertices, vertex_attributes, faces, shader_fn, shader_additional_inputs=[], name=None,
@@ -459,7 +430,7 @@ def rasterise_deferred(background_attributes, vertices, vertex_attributes, faces
     = (d row / dx, d col / dx, d row / dy, d col / dy).  Without it nothing else is computed or passed.
     """
     return _rasterise_deferred_internal(background_attributes, vertices, vertex_attributes, faces, shader_fn,
-                                        list(shader_additional_inputs), 'single', name, derivative_channels)
+                                        list(shader_additional_inputs), True, derivative_channels)
 
 
 def rasterise_batch_deferred(background_attributes, vertices, vertex_attributes, faces, shader_fn, shader_additional_inputs=[], name=None,
@@ -467,4 +438,4 @@ def rasterise_batch_deferred(background_attributes, vertices, vertex_attributes,
     """Batched `rasterise_deferred` (dirt/rasterise_ops.py:313-333).  With `derivative_channels`, `gbuffer_derivatives`
     is [B, H, W, 2, K]."""
     return _rasterise_deferred_internal(background_attributes, vertices, vertex_attributes, faces, shader_fn,
-                                        list(shader_additional_inputs), 'batch', name, derivative_channels)
+                                        list(shader_additional_inputs), False, derivative_channels)

@@ -15,7 +15,7 @@ import torch
 from torch.autograd.function import once_differentiable
 
 from . import _lib
-from .rasterise_ops import _as_f32, _pick_device, _ptr, _require_cuda, _stream_ptr
+from .rasterise_ops import _as, _pick_device, _ptr, _require_cuda, _stream_ptr
 
 _MODES = {'bilinear': _lib.TEXTURE_BILINEAR, 'nearest': _lib.TEXTURE_NEAREST}
 
@@ -196,8 +196,8 @@ def sample_texture(texture, indices, mode='bilinear', derivatives=None):
     if mode != 'trilinear' and derivatives is not None:
         raise ValueError("sample_texture: derivatives are only used by mode 'trilinear', not by %r" % (mode,))
     device = _pick_device(texture, indices)
-    texture = _as_f32(texture, device)
-    indices = _as_f32(indices, device)
+    texture = _as(texture, torch.float32, device)
+    indices = _as(indices, torch.float32, device)
     if texture.dim() not in (3, 4):
         raise ValueError('SampleTexture expects texture to be 3D or 4D, and texture.shape == [height, width, channels] '
                          'or [None, height, width, channels]')
@@ -209,7 +209,7 @@ def sample_texture(texture, indices, mode='bilinear', derivatives=None):
         texture, indices, 3, 'SampleTexture expects indices of per-item textures to be at least 2D, and indices.shape[0] '
         '== texture.shape[0]')
     if mode == 'trilinear':
-        derivatives = _as_f32(derivatives, device)
+        derivatives = _as(derivatives, torch.float32, device)
         if tuple(derivatives.shape) != tuple(indices.shape[:-1]) + (4,):
             raise ValueError('SampleTexture expects derivatives.shape == indices.shape[:-1] + (4,), got %s for indices %s'
                              % (tuple(derivatives.shape), tuple(indices.shape)))
@@ -336,8 +336,8 @@ def sample_cubemap(cubemap, directions, mode='bilinear', lod=None, roughness=Non
     if mode != 'ggx' and roughness is not None:
         raise ValueError("sample_cubemap: roughness is only used by mode 'ggx', not by %r" % (mode,))
     device = _pick_device(cubemap, directions)
-    cubemap = _as_f32(cubemap, device)
-    directions = _as_f32(directions, device)
+    cubemap = _as(cubemap, torch.float32, device)
+    directions = _as(directions, torch.float32, device)
     if cubemap.dim() not in (4, 5) or cubemap.shape[-4] != 6 or cubemap.shape[-3] != cubemap.shape[-2]:
         raise ValueError('SampleCubemap expects cubemap.shape == [6, size, size, channels] or '
                          '[None, 6, size, size, channels]')
@@ -354,9 +354,9 @@ def sample_cubemap(cubemap, directions, mode='bilinear', lod=None, roughness=Non
             raise ValueError("sample_cubemap: mode 'ggx' needs an even cube-map size (a mip chain of at least two "
                              "levels), got %d; with one level the roughness would be ignored" % S)
         # lod = roughness * (L-1) in torch, so that autograd carries lod's gradient to the roughness
-        lod = _as_f32(roughness, device) * float(_mip_level_count(S) - 1)
+        lod = _as(roughness, torch.float32, device) * float(_mip_level_count(S) - 1)
     if mode in ('trilinear', 'ggx'):
-        lod = _as_f32(lod, device)
+        lod = _as(lod, torch.float32, device)
         try:
             # broadcast before the autograd Function, so that autograd sums the gradient of a broadcast lod
             lod = lod.expand(directions.shape[:-1])
@@ -430,7 +430,7 @@ def latlong_to_cubemap(panorama, size):
     Needs CUDA tensors (there is no CPU kernel); anything else array-like is moved to the current CUDA device.
     """
     device = _pick_device(panorama)
-    panorama = _as_f32(panorama, device)
+    panorama = _as(panorama, torch.float32, device)
     if panorama.dim() not in (3, 4):
         raise ValueError('LatlongToCubemap expects panorama.shape == [height, width, channels] or '
                          '[None, height, width, channels]')
