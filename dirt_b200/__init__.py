@@ -5,8 +5,8 @@
 from .rasterise_ops import rasterise, rasterise_batch, rasterise_deferred, rasterise_batch_deferred
 from .texture import (index_derivatives, latlong_directions, latlong_to_cubemap, sample_cubemap, sample_texture,
                       uvs_to_pixel_indices)
-from . import matrices, lighting, projection
+from . import matrices, lighting, mesh, projection
 
 __all__ = ['rasterise', 'rasterise_batch', 'rasterise_deferred', 'rasterise_batch_deferred',
            'sample_texture', 'sample_cubemap', 'latlong_to_cubemap', 'latlong_directions', 'uvs_to_pixel_indices',
-           'index_derivatives', 'matrices', 'lighting', 'projection']
+           'index_derivatives', 'matrices', 'lighting', 'mesh', 'projection']

@@ -29,6 +29,8 @@ LIGHT_SPECULAR_DIRECTIONAL = 1
 LIGHT_DIFFUSE_POINT = 2
 NORMALS_AVERAGE = 0
 NORMALS_PRE_SPLIT = 1
+LAPLACIAN_UNIFORM = 0
+LAPLACIAN_COTANGENT = 1
 
 
 def lib():
@@ -168,6 +170,12 @@ def load(path):
     L.dirt_normals_forward.argtypes = [i, vp, ll, vp, vp, vp, sz, i, ll, ll, vp]
     L.dirt_normals_backward.restype = i
     L.dirt_normals_backward.argtypes = [i, vp, ll, vp, vp, vp, vp, sz, i, ll, ll, vp]
+    L.dirt_laplacian_workspace_bytes.restype = sz
+    L.dirt_laplacian_workspace_bytes.argtypes = [i, ll, ll]
+    L.dirt_laplacian_forward.restype = i
+    L.dirt_laplacian_forward.argtypes = [i, vp, ll, vp, vp, vp, sz, i, ll, ll, vp]
+    L.dirt_laplacian_backward.restype = i
+    L.dirt_laplacian_backward.argtypes = [i, vp, ll, vp, vp, vp, vp, sz, i, ll, ll, vp]
     tangent_inputs = [vp, ll, vp, ll, ll, vp, ll, vp]
     L.dirt_tangents_workspace_bytes.restype = sz
     L.dirt_tangents_workspace_bytes.argtypes = [i, ll, ll]
@@ -217,7 +225,8 @@ EXPORTED_SYMBOLS = ['dirt_error_string', 'dirt_abi_version', 'dirt_workspace_byt
                     'dirt_tangents_workspace_bytes', 'dirt_tangents_forward', 'dirt_tangents_backward',
                     'dirt_normal_map_forward', 'dirt_normal_map_backward', 'dirt_shadow_workspace_bytes',
                     'dirt_shadow_forward', 'dirt_shadow_backward', 'dirt_shadow_backward_deterministic_bytes',
-                    'dirt_shadow_backward_deterministic']
+                    'dirt_shadow_backward_deterministic', 'dirt_laplacian_workspace_bytes', 'dirt_laplacian_forward',
+                    'dirt_laplacian_backward']
 
 
 def error_string(code):

@@ -1221,20 +1221,21 @@ extern "C" size_t dirt_normals_workspace_bytes(int B, long long V, long long F)
     return carve_normals_workspace(nullptr, B, V, F).bytes;
 }
 
-// The checks the four mesh entries share, in order: the vertices, faces and workspace, NULL (the faces and workspace
-// only when F > 0) then 4-byte alignment (the workspace holds int32 adjacency, so not scratch_check's 256 bytes); the
-// workspace's size; the other inputs and then `outs` (the output, or the incoming gradient and the gradients a backward
-// requires), each by required_check.  Before it each entry makes its shape check and its early return, which differ:
-// - the forwards and the normals backward return DIRT_OK for B*V == 0 before they check anything else;
+// The checks the six mesh entries share, in order: the vertices, faces and workspace, NULL (the faces and workspace
+// only when a workspace is needed: `need`, the entry's workspace size, is 0 exactly when F = 0 once B*V > 0) then
+// 4-byte alignment (the workspace holds int32 adjacency and float gradients, read and written one element at a time, so
+// not scratch_check's 256 bytes); the workspace's size; the other inputs and then `outs` (the output, or the incoming
+// gradient and the gradients a backward requires), each by required_check.  Before it each entry makes its shape check
+// and its early return, which differ:
+// - the forwards and the normals and Laplacian backwards return DIRT_OK for B*V == 0 before they check anything else;
 // - the tangents backward first checks the alignment of its gradients, which may be NULL, then returns DIRT_OK for
 //   B*V == 0 or when no gradient is wanted.
-static int mesh_check(const float* vertices, const int32_t* faces, const void* workspace, size_t workspace_bytes, int B,
-                      long long V, long long F, std::initializer_list<const void*> inputs,
-                      std::initializer_list<const void*> outs)
+static int mesh_check(const float* vertices, const int32_t* faces, const void* workspace, size_t workspace_bytes,
+                      size_t need, std::initializer_list<const void*> inputs, std::initializer_list<const void*> outs)
 {
-    if (!vertices || (F > 0 && (!faces || !workspace))) return DIRT_ERR_NULL_POINTER;
+    if (!vertices || (need > 0 && (!faces || !workspace))) return DIRT_ERR_NULL_POINTER;
     if (!aligned({vertices, faces, workspace})) return DIRT_ERR_MISALIGNED;
-    if (workspace_bytes < dirt_normals_workspace_bytes(B, V, F)) return DIRT_ERR_WORKSPACE_TOO_SMALL;
+    if (workspace_bytes < need) return DIRT_ERR_WORKSPACE_TOO_SMALL;
     const int rc = required_check(inputs);
     return rc != DIRT_OK ? rc : required_check(outs);
 }
@@ -1255,7 +1256,8 @@ extern "C" int dirt_normals_forward(int mode, const float* vertices, long long v
     launch_count() = 0;
     if (!normals_shape_ok(mode, B, V, F, vertex_stride)) return DIRT_ERR_BAD_SHAPE;
     if ((long long)B * V == 0) return DIRT_OK;
-    const int rc = mesh_check(vertices, faces, workspace, workspace_bytes, B, V, F, {}, {normals});
+    const int rc = mesh_check(vertices, faces, workspace, workspace_bytes, dirt_normals_workspace_bytes(B, V, F), {},
+                              {normals});
     if (rc != DIRT_OK) return rc;
     NormalsArgs a = make_normals_args(mode, vertices, vertex_stride, faces, B, V, F);
     a.out = normals;
@@ -1271,13 +1273,63 @@ extern "C" int dirt_normals_backward(int mode, const float* vertices, long long 
     launch_count() = 0;
     if (!normals_shape_ok(mode, B, V, F, vertex_stride)) return DIRT_ERR_BAD_SHAPE;
     if ((long long)B * V == 0) return DIRT_OK;
-    const int rc = mesh_check(vertices, faces, workspace, workspace_bytes, B, V, F, {}, {grad_normals, grad_vertices});
+    const int rc = mesh_check(vertices, faces, workspace, workspace_bytes, dirt_normals_workspace_bytes(B, V, F), {},
+                              {grad_normals, grad_vertices});
     if (rc != DIRT_OK) return rc;
     NormalsArgs a = make_normals_args(mode, vertices, vertex_stride, faces, B, V, F);
     a.grad = grad_normals;
     a.g_vertices = grad_vertices;
     CUDA_TRY(launch_normals_backward(a, carve_normals_workspace(F > 0 ? workspace : nullptr, B, V, F),
                                      (cudaStream_t)cuda_stream));
+    return DIRT_OK;
+}
+
+// ---- the mesh Laplacian (DESIGN.md §7.16): the normals' arguments, checks and early returns ------------------------
+
+static bool laplacian_shape_ok(int mode, int B, long long V, long long F, long long stride)
+{
+    return (mode == DIRT_LAPLACIAN_UNIFORM || mode == DIRT_LAPLACIAN_COTANGENT) &&
+           normals_shape_ok(DIRT_NORMALS_AVERAGE, B, V, F, stride);
+}
+
+extern "C" size_t dirt_laplacian_workspace_bytes(int B, long long V, long long F)
+{
+    if (!normals_shape_ok(DIRT_NORMALS_AVERAGE, B, V, F, 3) || B == 0 || V == 0 || F == 0) return 0;
+    return carve_normals_workspace(nullptr, B, V, F, 4).bytes;
+}
+
+extern "C" int dirt_laplacian_forward(int mode, const float* vertices, long long vertex_stride, const int32_t* faces,
+                                      float* out, void* workspace, size_t workspace_bytes, int B, long long V, long long F,
+                                      void* cuda_stream)
+{
+    launch_count() = 0;
+    if (!laplacian_shape_ok(mode, B, V, F, vertex_stride)) return DIRT_ERR_BAD_SHAPE;
+    if ((long long)B * V == 0) return DIRT_OK;
+    const int rc = mesh_check(vertices, faces, workspace, workspace_bytes, dirt_laplacian_workspace_bytes(B, V, F), {},
+                              {out});
+    if (rc != DIRT_OK) return rc;
+    NormalsArgs a = make_normals_args(mode, vertices, vertex_stride, faces, B, V, F);
+    a.out = out;
+    CUDA_TRY(launch_laplacian_forward(a, carve_normals_workspace(F > 0 ? workspace : nullptr, B, V, F, 4),
+                                      (cudaStream_t)cuda_stream));
+    return DIRT_OK;
+}
+
+extern "C" int dirt_laplacian_backward(int mode, const float* vertices, long long vertex_stride, const int32_t* faces,
+                                       const float* grad_out, float* grad_vertices, void* workspace,
+                                       size_t workspace_bytes, int B, long long V, long long F, void* cuda_stream)
+{
+    launch_count() = 0;
+    if (!laplacian_shape_ok(mode, B, V, F, vertex_stride)) return DIRT_ERR_BAD_SHAPE;
+    if ((long long)B * V == 0) return DIRT_OK;
+    const int rc = mesh_check(vertices, faces, workspace, workspace_bytes, dirt_laplacian_workspace_bytes(B, V, F), {},
+                              {grad_out, grad_vertices});
+    if (rc != DIRT_OK) return rc;
+    NormalsArgs a = make_normals_args(mode, vertices, vertex_stride, faces, B, V, F);
+    a.grad = grad_out;
+    a.g_vertices = grad_vertices;
+    CUDA_TRY(launch_laplacian_backward(a, carve_normals_workspace(F > 0 ? workspace : nullptr, B, V, F, 4),
+                                       (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 
@@ -1315,7 +1367,8 @@ extern "C" int dirt_tangents_forward(const float* vertices, long long vertex_str
     launch_count() = 0;
     if (!tangents_shape_ok(B, V, F, vertex_stride, uv_stride, uv_item_stride, normals_stride)) return DIRT_ERR_BAD_SHAPE;
     if ((long long)B * V == 0) return DIRT_OK;
-    const int rc = mesh_check(vertices, faces, workspace, workspace_bytes, B, V, F, {uvs, normals}, {tangents});
+    const int rc = mesh_check(vertices, faces, workspace, workspace_bytes, dirt_tangents_workspace_bytes(B, V, F),
+                              {uvs, normals}, {tangents});
     if (rc != DIRT_OK) return rc;
     TangentArgs a = make_tangent_args(vertices, vertex_stride, uvs, uv_stride, uv_item_stride, normals, normals_stride,
                                       faces, B, V, F);
@@ -1335,7 +1388,8 @@ extern "C" int dirt_tangents_backward(const float* vertices, long long vertex_st
     if (!tangents_shape_ok(B, V, F, vertex_stride, uv_stride, uv_item_stride, normals_stride)) return DIRT_ERR_BAD_SHAPE;
     if (!aligned({grad_vertices, grad_uvs, grad_normals})) return DIRT_ERR_MISALIGNED;
     if ((long long)B * V == 0 || (!grad_vertices && !grad_uvs && !grad_normals)) return DIRT_OK;
-    const int rc = mesh_check(vertices, faces, workspace, workspace_bytes, B, V, F, {uvs, normals}, {grad_tangents});
+    const int rc = mesh_check(vertices, faces, workspace, workspace_bytes, dirt_tangents_workspace_bytes(B, V, F),
+                              {uvs, normals}, {grad_tangents});
     if (rc != DIRT_OK) return rc;
     TangentArgs a = make_tangent_args(vertices, vertex_stride, uvs, uv_stride, uv_item_stride, normals, normals_stride,
                                       faces, B, V, F);

@@ -15,8 +15,8 @@
 // vertex does not hold up its warp's other 31 lanes.  Either way each sum has one fixed order for given faces, and two
 // calls give bit-identical results.
 //
-// The file also holds the vertex tangents (dirt_tangents_forward / _backward, DESIGN.md §7.14), which use the same
-// adjacency, workspace and per-vertex passes.
+// The file also holds the vertex tangents (dirt_tangents_forward / _backward, DESIGN.md §7.14) and the mesh Laplacian
+// (dirt_laplacian_forward / _backward, DESIGN.md §7.16), which use the same adjacency, workspace and per-vertex passes.
 #include <cub/block/block_scan.cuh>
 
 #include "../../include/dirt_b200.h"
@@ -77,6 +77,18 @@ __device__ __forceinline__ void add_xor(Frame& p, int o)
 __device__ __forceinline__ float3 scale3(float3 a, float k)
 {
     return make_float3(__fmul_rn(a.x, k), __fmul_rn(a.y, k), __fmul_rn(a.z, k));
+}
+// A float3 and a scalar summed side by side: the Laplacian's (S_v, D_v).
+__device__ __forceinline__ float4 add3(float4 a, float4 b)
+{
+    return make_float4(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y), __fadd_rn(a.z, b.z), __fadd_rn(a.w, b.w));
+}
+__device__ __forceinline__ float4 zero_of(float4) { return make_float4(0.f, 0.f, 0.f, 0.f); }
+__device__ __forceinline__ void add_xor(float4& p, int o)
+{
+    float3 q = make_float3(p.x, p.y, p.z);
+    add_xor(q, o);
+    p = make_float4(q.x, q.y, q.z, __fadd_rn(p.w, __shfl_xor_sync(FULL, p.w, o)));
 }
 
 // x / (|x| + 1e-12)
@@ -498,9 +510,177 @@ __global__ void __launch_bounds__(NORMALS_THREADS) tangents_corner_grad_kernel(T
     }
 }
 
+// ---- the mesh Laplacian (DESIGN.md §7.16) ---------------------------------------------------------------------------------
+//
+// laplacian_v = S_v / (D_v + 1e-12), S_v and D_v sums over the corners that name v.  Each corner is seen from its
+// vertex: q0 = p_k, q1 = p_{k+1}, q2 = p_{k+2} (mod 3), a rotation that keeps the face's n = (q1 - q0) x (q2 - q0).
+// Uniform: S += (q1 - q0) + (q2 - q0), D += 2.  Cotangent: with c_j the cotangent at q_j, S += c2 (q1 - q0) +
+// c1 (q2 - q0), D += |n| / 3.  The modes' enum values are a.mode.
+
+// The corner of incidence i = k*F + f, rotated to q0: its vertices and its edges.
+struct Wedge {
+    int v[3];
+    float3 e01, e02, e12;
+};
+
+__device__ __forceinline__ Wedge wedge(const NormalsArgs& a, long long b, int i)
+{
+    const int k = i / a.F, f = i - k * a.F;
+    Wedge w;
+    w.v[0] = __ldg(a.faces + 3ll * f + k);
+    w.v[1] = __ldg(a.faces + 3ll * f + (k == 2 ? 0 : k + 1));
+    w.v[2] = __ldg(a.faces + 3ll * f + (k == 0 ? 2 : k - 1));
+    const float* base = a.vertices + b * a.V * a.stride;
+    const float3 q0 = ld3(base + w.v[0] * a.stride), q1 = ld3(base + w.v[1] * a.stride);
+    const float3 q2 = ld3(base + w.v[2] * a.stride);
+    w.e01 = sub3(q1, q0);
+    w.e02 = sub3(q2, q0);
+    w.e12 = sub3(q2, q1);
+    return w;
+}
+
+// The face's normal n, |n|, |n| + 1e-12 and the cotangents c_j = ((q_{j+1} - q_j) . (q_{j+2} - q_j)) / (|n| + 1e-12).
+struct Cotangents {
+    float3 n;
+    float nn, den, c0, c1, c2;
+};
+
+__device__ __forceinline__ Cotangents cotangents(const Wedge& w)
+{
+    Cotangents c;
+    c.n = cross3(w.e01, w.e02);
+    c.nn = __fsqrt_rn(dot3(c.n, c.n));
+    c.den = __fadd_rn(c.nn, 1.e-12f);
+    c.c0 = __fdiv_rn(dot3(w.e01, w.e02), c.den);
+    c.c1 = -__fdiv_rn(dot3(w.e12, w.e01), c.den);
+    c.c2 = __fdiv_rn(dot3(w.e02, w.e12), c.den);
+    return c;
+}
+
+// (S, D) of the corner of incidence i
+template <int MODE>
+struct LaplacianTerm {
+    const NormalsArgs& a;
+    __device__ __forceinline__ float4 operator()(long long b, int i) const
+    {
+        const Wedge w = wedge(a, b, i);
+        if (MODE == DIRT_LAPLACIAN_UNIFORM) {
+            const float3 s = add3(w.e01, w.e02);
+            return make_float4(s.x, s.y, s.z, 2.f);
+        }
+        const Cotangents c = cotangents(w);
+        const float3 s = add3(scale3(w.e01, c.c2), scale3(w.e02, c.c1));
+        return make_float4(s.x, s.y, s.z, __fdiv_rn(c.nn, 3.f));
+    }
+};
+
+__device__ __forceinline__ float3 xyz(float4 a) { return make_float3(a.x, a.y, a.z); }
+
+// The workspace's gradient region holds (g_S, g_D) of row t at gs + 4t, four floats read and written one at a time:
+// the C ABI asks the workspace for 4-byte alignment only.
+
+template <int MODE>
+__global__ void __launch_bounds__(NORMALS_THREADS) laplacian_forward_kernel(NormalsArgs a)
+{
+    FOR_EACH_ROW(a) {
+        const Row r = row_of(a, t0);
+        const float4 s = row_sum(a.inc, r.lo, r.hi, r.b, LaplacianTerm<MODE>{a});
+        const float d = __fadd_rn(s.w, 1.e-12f);
+        if (r.active) st3(a.out + 3 * r.t, make_float3(__fdiv_rn(s.x, d), __fdiv_rn(s.y, d), __fdiv_rn(s.z, d)));
+    }
+}
+
+// D_u + 1e-12 of the uniform mode, from the length of u's row
+__device__ __forceinline__ float uniform_den(const NormalsArgs& a, int u)
+{
+    return __fadd_rn(2.f * (float)(__ldg(a.offsets + u + 1) - __ldg(a.offsets + u)), 1.e-12f);
+}
+
+// Uniform: the gradient that reaches vertex j through the corners of the face of incidence i = k*F + f that are not
+// corner k, each of which sums p_j with weight 1: g_u / (D_u + 1e-12) of their vertices u.
+struct UniformNeighbourGrad {
+    const NormalsArgs& a;
+    __device__ __forceinline__ float3 operator()(long long b, int i) const
+    {
+        const int k = i / a.F, f = i - k * a.F;
+        float3 g = make_float3(0.f, 0.f, 0.f);
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+            if (j == k) continue;
+            const int u = __ldg(a.faces + 3ll * f + j);
+            const float3 gu = ld3(a.grad + 3 * (b * a.V + u));
+            const float d = uniform_den(a, u);
+            g = add3(g, make_float3(__fdiv_rn(gu.x, d), __fdiv_rn(gu.y, d), __fdiv_rn(gu.z, d)));
+        }
+        return g;
+    }
+};
+
+// uniform: the neighbours' terms, then vertex j's own -D_j p_j in S_j
+__global__ void __launch_bounds__(NORMALS_THREADS) laplacian_uniform_grad_kernel(NormalsArgs a)
+{
+    FOR_EACH_ROW(a) {
+        const Row r = row_of(a, t0);
+        const float3 s = row_sum(a.inc, r.lo, r.hi, r.b, UniformNeighbourGrad{a});
+        if (!r.active) continue;
+        const float D = 2.f * (float)(r.hi - r.lo), d = __fadd_rn(D, 1.e-12f);
+        const float3 g = ld3(a.grad + 3 * r.t);
+        const float3 gs = make_float3(__fdiv_rn(g.x, d), __fdiv_rn(g.y, d), __fdiv_rn(g.z, d));
+        st3(a.g_vertices + 3 * r.t, sub3(s, scale3(gs, D)));
+    }
+}
+
+// cotangent, pass 1: gs[t] = (g_S, g_D) of vertex t, g_S = g / (D + 1e-12) and g_D = -(g . S) / (D + 1e-12)^2
+__global__ void __launch_bounds__(NORMALS_THREADS) laplacian_sum_grad_kernel(NormalsArgs a)
+{
+    FOR_EACH_ROW(a) {
+        const Row r = row_of(a, t0);
+        const float4 s = row_sum(a.inc, r.lo, r.hi, r.b, LaplacianTerm<DIRT_LAPLACIAN_COTANGENT>{a});
+        if (!r.active) continue;
+        const float3 g = ld3(a.grad + 3 * r.t);
+        const float d = __fadd_rn(s.w, 1.e-12f);
+        const float gd = -__fdiv_rn(dot3(g, xyz(s)), __fmul_rn(d, d));
+        st3(a.gs + 4 * r.t, make_float3(__fdiv_rn(g.x, d), __fdiv_rn(g.y, d), __fdiv_rn(g.z, d)));
+        a.gs[4 * r.t + 3] = gd;
+    }
+}
+
+// cotangent, pass 2: the gradient to q0 of the face's sum over its corners m of g_S(m) . S_m + g_D(m) |n| / 3, where
+// S_m is corner m's term.  Grouped by cotangent, that sum is sum_j c_j w_j + (sum_m g_D(m)) |n| / 3 with
+// w_j = (g_S(j+1) - g_S(j+2)) . (q_{j+2} - q_{j+1}); its gradient runs through the dot products d_j = c_j (|n| + 1e-12),
+// through w_j, and through |n| (none through the norm of a zero n).
+struct CotangentCornerGrad {
+    const NormalsArgs& a;
+    __device__ __forceinline__ float3 operator()(long long b, int i) const
+    {
+        const Wedge w = wedge(a, b, i);
+        const Cotangents c = cotangents(w);
+        const float* gs = a.gs + 4 * b * a.V;
+        const float *g0 = gs + 4 * w.v[0], *g1 = gs + 4 * w.v[1], *g2 = gs + 4 * w.v[2];
+        const float3 s0 = ld3(g0), s1 = ld3(g1), s2 = ld3(g2);
+        const float gd = __fadd_rn(__fadd_rn(__ldg(g0 + 3), __ldg(g1 + 3)), __ldg(g2 + 3));
+        const float w0 = dot3(sub3(s1, s2), w.e12), w1 = -dot3(sub3(s2, s0), w.e02), w2 = dot3(sub3(s0, s1), w.e01);
+        const float wc = __fmaf_rn(w2, c.c2, __fmaf_rn(w1, c.c1, __fmul_rn(w0, c.c0)));
+        const float gnn = __fsub_rn(__fdiv_rn(gd, 3.f), __fdiv_rn(wc, c.den));
+        const float3 gn = scale3(c.n, c.nn == 0.f ? 0.f : __fdiv_rn(gnn, c.nn));
+        float3 g = add3(scale3(add3(w.e01, w.e02), -__fdiv_rn(w0, c.den)), scale3(w.e12, __fdiv_rn(__fsub_rn(w1, w2), c.den)));
+        g = add3(g, sub3(scale3(sub3(s2, s0), c.c1), scale3(sub3(s0, s1), c.c2)));
+        return add3(g, cross3(gn, w.e12));
+    }
+};
+
+__global__ void __launch_bounds__(NORMALS_THREADS) laplacian_cotangent_grad_kernel(NormalsArgs a)
+{
+    FOR_EACH_ROW(a) {
+        const Row r = row_of(a, t0);
+        const float3 g = row_sum(a.inc, r.lo, r.hi, r.b, CotangentCornerGrad{a});
+        if (r.active) st3(a.g_vertices + 3 * r.t, g);
+    }
+}
+
 }  // namespace
 
-NormalsWorkspace carve_normals_workspace(void* base, int B, long long V, long long F)
+NormalsWorkspace carve_normals_workspace(void* base, int B, long long V, long long F, int grad_width)
 {
     NormalsWorkspace w = {};
     char* p = static_cast<char*>(base);
@@ -514,7 +694,7 @@ NormalsWorkspace carve_normals_workspace(void* base, int B, long long V, long lo
     w.inc = reinterpret_cast<int*>(take(sizeof(int) * (size_t)(3 * F)));
     // the build's scratch (counts, unsorted ids) and the backward's per-vertex gradients share one region
     const size_t build = ((sizeof(int) * (size_t)V + 255) & ~size_t(255)) + sizeof(int) * (size_t)(3 * F);
-    const size_t grads = sizeof(float) * 3 * (size_t)B * (size_t)V;
+    const size_t grads = sizeof(float) * grad_width * (size_t)B * (size_t)V;
     char* scratch = take(build > grads ? build : grads);
     w.counts = reinterpret_cast<int*>(scratch);
     w.unsorted = scratch ? reinterpret_cast<int*>(scratch + ((sizeof(int) * (size_t)V + 255) & ~size_t(255))) : nullptr;
@@ -610,6 +790,40 @@ cudaError_t launch_tangents_backward(TangentArgs a, const NormalsWorkspace& w, c
         if ((e = launched()) != cudaSuccess) return e;
     }
     return cudaSuccess;
+}
+
+cudaError_t launch_laplacian_forward(NormalsArgs a, const NormalsWorkspace& w, cudaStream_t stream)
+{
+    cudaError_t e;
+    if (a.total == 0) return cudaSuccess;
+    if (a.F == 0) return cudaMemsetAsync(a.out, 0, sizeof(float) * 3 * (size_t)a.total, stream);
+    if ((e = launch_corner_adjacency(a.faces, 0, 1, a.V, a.F, w.counts, w.offsets, w.unsorted, w.inc, stream)) != cudaSuccess)
+        return e;
+    a.offsets = w.offsets;
+    a.inc = w.inc;
+    if (a.mode == DIRT_LAPLACIAN_UNIFORM)
+        laplacian_forward_kernel<DIRT_LAPLACIAN_UNIFORM><<<blocks_for(a.total), NORMALS_THREADS, 0, stream>>>(a);
+    else
+        laplacian_forward_kernel<DIRT_LAPLACIAN_COTANGENT><<<blocks_for(a.total), NORMALS_THREADS, 0, stream>>>(a);
+    return launched();
+}
+
+cudaError_t launch_laplacian_backward(NormalsArgs a, const NormalsWorkspace& w, cudaStream_t stream)
+{
+    cudaError_t e;
+    if (a.total == 0) return cudaSuccess;
+    if (a.F == 0) return cudaMemsetAsync(a.g_vertices, 0, sizeof(float) * 3 * (size_t)a.total, stream);
+    a.offsets = w.offsets;
+    a.inc = w.inc;
+    a.gs = w.gs;
+    if (a.mode == DIRT_LAPLACIAN_UNIFORM) {
+        laplacian_uniform_grad_kernel<<<blocks_for(a.total), NORMALS_THREADS, 0, stream>>>(a);
+    } else {
+        laplacian_sum_grad_kernel<<<blocks_for(a.total), NORMALS_THREADS, 0, stream>>>(a);
+        if ((e = launched()) != cudaSuccess) return e;
+        laplacian_cotangent_grad_kernel<<<blocks_for(a.total), NORMALS_THREADS, 0, stream>>>(a);
+    }
+    return launched();
 }
 
 }  // namespace dirt

@@ -578,6 +578,38 @@ int dirt_normals_backward(int mode, const float* vertices, long long vertex_stri
                           const float* grad_normals, float* grad_vertices, void* workspace, size_t workspace_bytes,
                           int B, long long V, long long F, void* cuda_stream);
 
+/* The mesh Laplacian, a smoothness term for fitting shapes, for B items of V vertices sharing the faces:
+ *   vertices             float32 [B*V, 3], row stride vertex_stride >= 3 floats, unit stride along the row
+ *   faces                int32 [F, 3], shared by the batch
+ *   out, grad_out, grad_vertices   float32 [B*V, 3], contiguous
+ * For corner k of face f that names v, with corners p0, p1, p2, a = k+1 mod 3 and b = k+2 mod 3:
+ *   DIRT_LAPLACIAN_UNIFORM    S_v = sum (p_a - p_v) + (p_b - p_v),  D_v = sum 2
+ *   DIRT_LAPLACIAN_COTANGENT  S_v = sum c_b (p_a - p_v) + c_a (p_b - p_v),  D_v = sum |n_f| / 3, with
+ *                             n_f = (p1 - p0) x (p2 - p0) and c_j = ((p_{j+1} - p_j) . (p_{j+2} - p_j)) / (|n_f| + 1e-12)
+ *   out_v = S_v / (D_v + 1e-12)
+ * the sums running over every corner that names v (a vertex no face names gets 0).  Uniform: on a closed manifold
+ * mesh, the mean of p_u - p_v over the neighbours u; on a boundary, boundary edges weigh half.  Cotangent: the
+ * discrete mean-curvature normal, about -(2/r) n on a sphere of radius r.  A face with an index outside [0, V) is
+ * left out: it adds nothing and receives no gradient.
+ * Backward: grad_vertices = the gradient torch autograd gives the same expressions, through the cotangents and the
+ * areas (none through the norm of a zero n_f; a zero-area face passes the 1e12-scale values its division implies).
+ * Workspace: at least dirt_laplacian_workspace_bytes(B, V, F) bytes (0 when B, V or F is 0), a function of the sizes
+ * alone; the forward call writes the vertex -> face-corner adjacency into it and the backward call reads it there, as
+ * for the normals, and uses the rest as scratch.
+ * Every sum has one fixed order (no float atomics): repeated calls give bit-identical values and gradients.
+ * B = 0 or V = 0: nothing is launched; F = 0: the outputs are zeroed.  V < 2^31, 3F < 2^31; all pointers, the
+ * workspace included, 4-byte aligned. */
+enum {
+    DIRT_LAPLACIAN_UNIFORM = 0,
+    DIRT_LAPLACIAN_COTANGENT = 1
+};
+size_t dirt_laplacian_workspace_bytes(int B, long long V, long long F);
+int dirt_laplacian_forward(int mode, const float* vertices, long long vertex_stride, const int32_t* faces, float* out,
+                           void* workspace, size_t workspace_bytes, int B, long long V, long long F, void* cuda_stream);
+int dirt_laplacian_backward(int mode, const float* vertices, long long vertex_stride, const int32_t* faces,
+                            const float* grad_out, float* grad_vertices, void* workspace, size_t workspace_bytes,
+                            int B, long long V, long long F, void* cuda_stream);
+
 /* Vertex tangents for tangent-space normal mapping, for B items of V vertices sharing the faces:
  *   vertices             float32 [B*V, 3], row stride vertex_stride >= 3 floats, unit stride along the row
  *   uvs                  float32, the uv of vertex v of item b at uvs + b*uv_item_stride + v*uv_stride, uv_stride >= 2,
