@@ -376,7 +376,11 @@ def read_scratch(buf, B, H, W, C, V, F):
     return dict(codes=view('codes', np.uint8, (C, B, H, W)), rec=view('rec', np.float32, (B, H, W, 2)),
                 boxes=view('boxes', np.uint32, (B * F, 4)), large=view('large', np.int32, (B * F,)),
                 large_count=int(view('large_count', np.int32, (1,))[0]),
-                partial=view('partial', np.float64, (B * F, 3, 3 + C)))
+                partial=view('partial', np.float64, (B * F, 3, 3 + C)),
+                # the corner adjacency of the B face tables (tests/mesh_order.adjacency with items = B): offsets [B*V + 1],
+                # counts [B*V] (back to 0 after the build), inc and the unsorted ids [3*B*F] (the first offsets[B*V] used)
+                offsets=view('offsets', np.int32, (B * V + 1,)), counts=view('counts', np.int32, (B * V,)),
+                inc=view('inc', np.int32, (3 * B * F,)), unsorted=view('unsorted', np.int32, (3 * B * F,)))
 
 
 def large_faces(group, shape, F):
