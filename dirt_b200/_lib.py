@@ -31,6 +31,8 @@ NORMALS_AVERAGE = 0
 NORMALS_PRE_SPLIT = 1
 LAPLACIAN_UNIFORM = 0
 LAPLACIAN_COTANGENT = 1
+EDGE_LENGTH = 0
+NORMAL_CONSISTENCY = 1
 
 
 def lib():
@@ -176,6 +178,12 @@ def load(path):
     L.dirt_laplacian_forward.argtypes = [i, vp, ll, vp, vp, vp, sz, i, ll, ll, vp]
     L.dirt_laplacian_backward.restype = i
     L.dirt_laplacian_backward.argtypes = [i, vp, ll, vp, vp, vp, vp, sz, i, ll, ll, vp]
+    L.dirt_edge_terms_workspace_bytes.restype = sz
+    L.dirt_edge_terms_workspace_bytes.argtypes = [i, ll, ll]
+    L.dirt_edge_terms_forward.restype = i
+    L.dirt_edge_terms_forward.argtypes = [i, vp, ll, vp, vp, vp, sz, i, ll, ll, vp]
+    L.dirt_edge_terms_backward.restype = i
+    L.dirt_edge_terms_backward.argtypes = [i, vp, ll, vp, vp, vp, vp, sz, i, ll, ll, vp]
     tangent_inputs = [vp, ll, vp, ll, ll, vp, ll, vp]
     L.dirt_tangents_workspace_bytes.restype = sz
     L.dirt_tangents_workspace_bytes.argtypes = [i, ll, ll]
@@ -226,7 +234,8 @@ EXPORTED_SYMBOLS = ['dirt_error_string', 'dirt_abi_version', 'dirt_workspace_byt
                     'dirt_normal_map_forward', 'dirt_normal_map_backward', 'dirt_shadow_workspace_bytes',
                     'dirt_shadow_forward', 'dirt_shadow_backward', 'dirt_shadow_backward_deterministic_bytes',
                     'dirt_shadow_backward_deterministic', 'dirt_laplacian_workspace_bytes', 'dirt_laplacian_forward',
-                    'dirt_laplacian_backward']
+                    'dirt_laplacian_backward', 'dirt_edge_terms_workspace_bytes', 'dirt_edge_terms_forward',
+                    'dirt_edge_terms_backward']
 
 
 def error_string(code):

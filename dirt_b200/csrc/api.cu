@@ -1221,7 +1221,7 @@ extern "C" size_t dirt_normals_workspace_bytes(int B, long long V, long long F)
     return carve_normals_workspace(nullptr, B, V, F).bytes;
 }
 
-// The checks the six mesh entries share, in order: the vertices, faces and workspace, NULL (the faces and workspace
+// The checks the eight mesh entries share, in order: the vertices, faces and workspace, NULL (the faces and workspace
 // only when a workspace is needed: `need`, the entry's workspace size, is 0 exactly when F = 0 once B*V > 0) then
 // 4-byte alignment (the workspace holds int32 adjacency and float gradients, read and written one element at a time, so
 // not scratch_check's 256 bytes); the workspace's size; the other inputs and then `outs` (the output, or the incoming
@@ -1229,7 +1229,8 @@ extern "C" size_t dirt_normals_workspace_bytes(int B, long long V, long long F)
 // and its early return, which differ:
 // - the forwards and the normals and Laplacian backwards return DIRT_OK for B*V == 0 before they check anything else;
 // - the tangents backward first checks the alignment of its gradients, which may be NULL, then returns DIRT_OK for
-//   B*V == 0 or when no gradient is wanted.
+//   B*V == 0 or when no gradient is wanted;
+// - the edge-term entries return DIRT_OK for B*F == 0, and handle V == 0 themselves (see below).
 static int mesh_check(const float* vertices, const int32_t* faces, const void* workspace, size_t workspace_bytes,
                       size_t need, std::initializer_list<const void*> inputs, std::initializer_list<const void*> outs)
 {
@@ -1330,6 +1331,68 @@ extern "C" int dirt_laplacian_backward(int mode, const float* vertices, long lon
     a.g_vertices = grad_vertices;
     CUDA_TRY(launch_laplacian_backward(a, carve_normals_workspace(F > 0 ? workspace : nullptr, B, V, F, 4),
                                        (cudaStream_t)cuda_stream));
+    return DIRT_OK;
+}
+
+// ---- edge lengths and normal consistency (DESIGN.md §7.17): the Laplacian's arguments and checks ---------------------
+// The output is per face, so the early returns differ: the forward launches nothing for B*F == 0, and V == 0 with
+// F > 0 makes every face invalid, so it zeroes out.  The backward writes nothing for B*V == 0 and zeroes grad_vertices
+// for F == 0.  All are decided before mesh_check, which requires a workspace whenever F > 0.
+
+static bool edge_terms_shape_ok(int mode, int B, long long V, long long F, long long stride)
+{
+    return (mode == DIRT_EDGE_LENGTH || mode == DIRT_NORMAL_CONSISTENCY) &&
+           normals_shape_ok(DIRT_NORMALS_AVERAGE, B, V, F, stride);
+}
+
+extern "C" size_t dirt_edge_terms_workspace_bytes(int B, long long V, long long F)
+{
+    if (!normals_shape_ok(DIRT_NORMALS_AVERAGE, B, V, F, 3) || B == 0 || V == 0 || F == 0) return 0;
+    return carve_normals_workspace(nullptr, B, V, F, 3, true).bytes;
+}
+
+extern "C" int dirt_edge_terms_forward(int mode, const float* vertices, long long vertex_stride, const int32_t* faces,
+                                       float* out, void* workspace, size_t workspace_bytes, int B, long long V,
+                                       long long F, void* cuda_stream)
+{
+    launch_count() = 0;
+    if (!edge_terms_shape_ok(mode, B, V, F, vertex_stride)) return DIRT_ERR_BAD_SHAPE;
+    if ((long long)B * F == 0) return DIRT_OK;
+    if (V == 0) {
+        const int rc = required_check({out});
+        if (rc != DIRT_OK) return rc;
+        CUDA_TRY(cudaMemsetAsync(out, 0, sizeof(float) * 3 * (size_t)B * (size_t)F, (cudaStream_t)cuda_stream));
+        return DIRT_OK;
+    }
+    const int rc = mesh_check(vertices, faces, workspace, workspace_bytes, dirt_edge_terms_workspace_bytes(B, V, F), {},
+                              {out});
+    if (rc != DIRT_OK) return rc;
+    NormalsArgs a = make_normals_args(mode, vertices, vertex_stride, faces, B, V, F);
+    a.out = out;
+    CUDA_TRY(launch_edge_terms_forward(a, carve_normals_workspace(workspace, B, V, F, 3, true), (cudaStream_t)cuda_stream));
+    return DIRT_OK;
+}
+
+extern "C" int dirt_edge_terms_backward(int mode, const float* vertices, long long vertex_stride, const int32_t* faces,
+                                        const float* grad_out, float* grad_vertices, void* workspace,
+                                        size_t workspace_bytes, int B, long long V, long long F, void* cuda_stream)
+{
+    launch_count() = 0;
+    if (!edge_terms_shape_ok(mode, B, V, F, vertex_stride)) return DIRT_ERR_BAD_SHAPE;
+    if ((long long)B * V == 0) return DIRT_OK;
+    if (F == 0) {   // no edges: no gradient reaches the vertices
+        const int rc = required_check({grad_vertices});
+        if (rc != DIRT_OK) return rc;
+        CUDA_TRY(cudaMemsetAsync(grad_vertices, 0, sizeof(float) * 3 * (size_t)B * (size_t)V, (cudaStream_t)cuda_stream));
+        return DIRT_OK;
+    }
+    const int rc = mesh_check(vertices, faces, workspace, workspace_bytes, dirt_edge_terms_workspace_bytes(B, V, F), {},
+                              {grad_out, grad_vertices});
+    if (rc != DIRT_OK) return rc;
+    NormalsArgs a = make_normals_args(mode, vertices, vertex_stride, faces, B, V, F);
+    a.grad = grad_out;
+    a.g_vertices = grad_vertices;
+    CUDA_TRY(launch_edge_terms_backward(a, carve_normals_workspace(workspace, B, V, F, 3, true), (cudaStream_t)cuda_stream));
     return DIRT_OK;
 }
 

@@ -15,8 +15,9 @@
 // vertex does not hold up its warp's other 31 lanes.  Either way each sum has one fixed order for given faces, and two
 // calls give bit-identical results.
 //
-// The file also holds the vertex tangents (dirt_tangents_forward / _backward, DESIGN.md §7.14) and the mesh Laplacian
-// (dirt_laplacian_forward / _backward, DESIGN.md §7.16), which use the same adjacency, workspace and per-vertex passes.
+// The file also holds the vertex tangents (dirt_tangents_forward / _backward, DESIGN.md §7.14), the mesh Laplacian
+// (dirt_laplacian_forward / _backward, DESIGN.md §7.16) and the edge-length and normal-consistency terms
+// (dirt_edge_terms_forward / _backward, DESIGN.md §7.17), which use the same adjacency, workspace and per-vertex passes.
 #include <cub/block/block_scan.cuh>
 
 #include "../../include/dirt_b200.h"
@@ -678,9 +679,201 @@ __global__ void __launch_bounds__(NORMALS_THREADS) laplacian_cotangent_grad_kern
     }
 }
 
+// ---- edge lengths and normal consistency (DESIGN.md §7.17) ----------------------------------------------------------------
+//
+// One value per face edge, [B*F, 3]: edge k of face f joins v_k to v_{k+1 mod 3}.  Edge length: |p_{k+1} - p_k|.  Normal
+// consistency: 1 - u_f . (sum of u_g over P) / |P|, P the valid faces other than f that name both ends (each once), 0
+// when P is empty or the ends are one vertex.  The face passes are one thread per (item, face); the vertex passes are
+// the normals' gather.  a.grad is grad_out [B*F, 3]; a.gs the consistency backward's dL/dn_f [B*F, 3].
+
+__device__ __forceinline__ int next3(int k) { return k == 2 ? 0 : k + 1; }
+
+// u_g of item b for the face with vertices v
+__device__ __forceinline__ float3 unit_of(const NormalsArgs& a, long long b, const int v[3])
+{
+    const float* base = a.vertices + b * a.V * a.stride;
+    const float3 p0 = ld3(base + v[0] * a.stride);
+    return normalise(cross3(sub3(ld3(base + v[1] * a.stride), p0), sub3(ld3(base + v[2] * a.stride), p0)));
+}
+
+// Calls visit(g, v) for every valid face g != f that names both x and y (x != y), once per face, and returns how many.
+// It scans the shorter of the two rows (the row of the smaller vertex id when they are equally long) in row order, and
+// takes each face at its first corner in that row, so the order depends on the faces and the unordered pair alone.
+template <class Visit>
+__device__ __forceinline__ int for_each_partner(const NormalsArgs& a, int f, int x, int y, const Visit& visit)
+{
+    const int lx = __ldg(a.offsets + x + 1) - __ldg(a.offsets + x), ly = __ldg(a.offsets + y + 1) - __ldg(a.offsets + y);
+    const bool by_x = lx < ly || (lx == ly && x < y);
+    const int r = by_x ? x : y, o = by_x ? y : x;
+    const int hi = __ldg(a.offsets + r + 1);
+    int n = 0;
+    for (int j = __ldg(a.offsets + r); j < hi; ++j) {
+        const int i = __ldg(a.inc + j), k = i / a.F, g = i - k * a.F;
+        if (g == f) continue;
+        int v[3];
+#pragma unroll
+        for (int m = 0; m < 3; ++m) v[m] = __ldg(a.faces + 3ll * g + m);
+        if ((k > 0 && v[0] == r) || (k > 1 && v[1] == r)) continue;   // not the face's first corner naming r
+        if (v[0] != o && v[1] != o && v[2] != o) continue;
+        visit(g, v);
+        ++n;
+    }
+    return n;
+}
+
+__device__ __forceinline__ float3 div3(float3 a, float d)
+{
+    return make_float3(__fdiv_rn(a.x, d), __fdiv_rn(a.y, d), __fdiv_rn(a.z, d));
+}
+
+// whether edges j and k of the face with vertices v join the same unordered pair
+__device__ __forceinline__ bool same_pair(const int v[3], int j, int k)
+{
+    return (v[j] == v[k] && v[next3(j)] == v[next3(k)]) || (v[j] == v[next3(k)] && v[next3(j)] == v[k]);
+}
+
+// the sum of grad_out over the edges of face g (item b, vertices v) that join x and y, in edge order
+__device__ __forceinline__ float pair_grad(const NormalsArgs& a, long long b, int g, const int v[3], int x, int y)
+{
+    const float* G = a.grad + 3 * (b * a.F + g);
+    float s = 0.f;
+#pragma unroll
+    for (int k = 0; k < 3; ++k)
+        if ((v[k] == x && v[next3(k)] == y) || (v[k] == y && v[next3(k)] == x)) s = __fadd_rn(s, __ldg(G + k));
+    return s;
+}
+
+template <int MODE>
+__global__ void __launch_bounds__(NORMALS_THREADS) edge_terms_forward_kernel(NormalsArgs a, long long n)
+{
+    for (long long t = (long long)blockIdx.x * NORMALS_THREADS + threadIdx.x; t < n; t += (long long)gridDim.x * NORMALS_THREADS) {
+        const long long b = t / a.F;
+        const int f = (int)(t - b * a.F);
+        int v[3];
+        float o[3] = {0.f, 0.f, 0.f};
+        if (load_face(a.faces, f, a.V, v)) {
+            const float* base = a.vertices + b * a.V * a.stride;
+            if (MODE == DIRT_EDGE_LENGTH) {
+#pragma unroll
+                for (int k = 0; k < 3; ++k) {
+                    const float3 d = sub3(ld3(base + v[next3(k)] * a.stride), ld3(base + v[k] * a.stride));
+                    o[k] = __fsqrt_rn(dot3(d, d));
+                }
+            } else {
+                const float3 u = unit_of(a, b, v);
+#pragma unroll
+                for (int k = 0; k < 3; ++k) {
+                    if (v[k] == v[next3(k)]) continue;
+                    float3 s = make_float3(0.f, 0.f, 0.f);
+                    const int c = for_each_partner(a, f, v[k], v[next3(k)],
+                                                   [&](int, const int w[3]) { s = add3(s, unit_of(a, b, w)); });
+                    if (c) o[k] = __fsub_rn(1.f, __fdiv_rn(dot3(u, s), (float)c));
+                }
+            }
+        }
+#pragma unroll
+        for (int k = 0; k < 3; ++k) a.out[3 * t + k] = o[k];
+    }
+}
+
+// Edge length: the gradient to p_k of the corner k of the face of incidence i, from edge k (p_k its start) and edge k-1
+// (p_k its end): -(G_k e01 / |e01| + G_{k-1} e02 / |e02|) with the wedge's e01 = p_{k+1} - p_k, e02 = p_{k-1} - p_k;
+// none through a zero-length edge.
+struct EdgeLengthCornerGrad {
+    const NormalsArgs& a;
+    __device__ __forceinline__ float3 operator()(long long b, int i) const
+    {
+        const int k = i / a.F, f = i - k * a.F;
+        const Wedge w = wedge(a, b, i);
+        const float* G = a.grad + 3 * (b * a.F + f);
+        const float l1 = __fsqrt_rn(dot3(w.e01, w.e01)), l2 = __fsqrt_rn(dot3(w.e02, w.e02));
+        const float k1 = l1 == 0.f ? 0.f : __fdiv_rn(__ldg(G + k), l1);
+        const float k2 = l2 == 0.f ? 0.f : __fdiv_rn(__ldg(G + (k == 0 ? 2 : k - 1)), l2);
+        const float3 g = add3(scale3(w.e01, k1), scale3(w.e02, k2));
+        return make_float3(-g.x, -g.y, -g.z);
+    }
+};
+
+__global__ void __launch_bounds__(NORMALS_THREADS) edge_length_grad_kernel(NormalsArgs a)
+{
+    FOR_EACH_ROW(a) {
+        const Row r = row_of(a, t0);
+        const float3 g = row_sum(a.inc, r.lo, r.hi, r.b, EdgeLengthCornerGrad{a});
+        if (r.active) st3(a.g_vertices + 3 * r.t, g);
+    }
+}
+
+// Normal consistency, pass 1: dL/dn_f of each valid face into gs.  dL/du_f is, over each distinct unordered pair {x, y}
+// of f's edges with x != y and |P| > 0, -(G_f s + sum over P of G_g u_g) / |P|, where s = the sum of u_g over P and G_f,
+// G_g are the sums of grad_out over the edges of f and g that join x and y: f's own terms, and the terms in which f is
+// a partner of g.  Near a flat edge u_g is close to u_f, and the normalisation's gradient J removes nearly all of
+// dL/du_f, so the sums run over du = u_g - u_f instead: dL/du_f = g' - beta u_f with g' = -(G_f sum du + sum G_g du) / |P|
+// and beta = G_f + (sum G_g) / |P|, and J u_f = 1e-12 n / d^3 (d = |n| + 1e-12) is applied in closed form.
+__global__ void __launch_bounds__(NORMALS_THREADS) consistency_face_grad_kernel(NormalsArgs a, long long n)
+{
+    for (long long t = (long long)blockIdx.x * NORMALS_THREADS + threadIdx.x; t < n; t += (long long)gridDim.x * NORMALS_THREADS) {
+        const long long b = t / a.F;
+        const int f = (int)(t - b * a.F);
+        int v[3];
+        if (!load_face(a.faces, f, a.V, v)) continue;
+        const float* base = a.vertices + b * a.V * a.stride;
+        const float3 p0 = ld3(base + v[0] * a.stride);
+        const float3 nf = cross3(sub3(ld3(base + v[1] * a.stride), p0), sub3(ld3(base + v[2] * a.stride), p0));
+        const float3 uf = normalise(nf);
+        float3 gu = make_float3(0.f, 0.f, 0.f);
+        float beta = 0.f;
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            const int x = v[k], y = v[next3(k)];
+            if (x == y || (k > 0 && same_pair(v, 0, k)) || (k > 1 && same_pair(v, 1, k))) continue;
+            float3 s = make_float3(0.f, 0.f, 0.f), sg = s;
+            float gsum = 0.f;
+            const int c = for_each_partner(a, f, x, y, [&](int g, const int w[3]) {
+                const float3 du = sub3(unit_of(a, b, w), uf);
+                const float G = pair_grad(a, b, g, w, x, y);
+                s = add3(s, du);
+                sg = add3(sg, scale3(du, G));
+                gsum = __fadd_rn(gsum, G);
+            });
+            if (c) {
+                const float Gf = pair_grad(a, b, f, v, x, y);
+                gu = sub3(gu, div3(add3(scale3(s, Gf), sg), (float)c));
+                beta = __fadd_rn(beta, __fadd_rn(Gf, __fdiv_rn(gsum, (float)c)));
+            }
+        }
+        const float d = __fadd_rn(__fsqrt_rn(dot3(nf, nf)), 1.e-12f);
+        const float k = __fdiv_rn(__fmul_rn(beta, 1.e-12f), __fmul_rn(__fmul_rn(d, d), d));
+        st3(a.gs + 3 * t, sub3(normalise_grad(nf, gu), scale3(nf, k)));
+    }
+}
+
+// Normal consistency, pass 2: the gradient of corner k of the face of incidence i through n = e1 x e2, as CornerGrad.
+struct ConsistencyCornerGrad {
+    const NormalsArgs& a;
+    __device__ __forceinline__ float3 operator()(long long b, int i) const
+    {
+        const int k = i / a.F, f = i - k * a.F;
+        const Corners c = corners(a, b, f);
+        const float3 gn = ld3(a.gs + 3 * (b * a.F + f));
+        const float3 g1 = cross3(c.e2, gn), g2 = cross3(gn, c.e1);   // d/d e1, d/d e2
+        if (k == 1) return g1;
+        if (k == 2) return g2;
+        return make_float3(-__fadd_rn(g1.x, g2.x), -__fadd_rn(g1.y, g2.y), -__fadd_rn(g1.z, g2.z));
+    }
+};
+
+__global__ void __launch_bounds__(NORMALS_THREADS) consistency_vertex_grad_kernel(NormalsArgs a)
+{
+    FOR_EACH_ROW(a) {
+        const Row r = row_of(a, t0);
+        const float3 g = row_sum(a.inc, r.lo, r.hi, r.b, ConsistencyCornerGrad{a});
+        if (r.active) st3(a.g_vertices + 3 * r.t, g);
+    }
+}
+
 }  // namespace
 
-NormalsWorkspace carve_normals_workspace(void* base, int B, long long V, long long F, int grad_width)
+NormalsWorkspace carve_normals_workspace(void* base, int B, long long V, long long F, int grad_width, bool per_face)
 {
     NormalsWorkspace w = {};
     char* p = static_cast<char*>(base);
@@ -694,7 +887,7 @@ NormalsWorkspace carve_normals_workspace(void* base, int B, long long V, long lo
     w.inc = reinterpret_cast<int*>(take(sizeof(int) * (size_t)(3 * F)));
     // the build's scratch (counts, unsorted ids) and the backward's per-vertex gradients share one region
     const size_t build = ((sizeof(int) * (size_t)V + 255) & ~size_t(255)) + sizeof(int) * (size_t)(3 * F);
-    const size_t grads = sizeof(float) * grad_width * (size_t)B * (size_t)V;
+    const size_t grads = sizeof(float) * grad_width * (size_t)B * (size_t)(per_face ? F : V);
     char* scratch = take(build > grads ? build : grads);
     w.counts = reinterpret_cast<int*>(scratch);
     w.unsorted = scratch ? reinterpret_cast<int*>(scratch + ((sizeof(int) * (size_t)V + 255) & ~size_t(255))) : nullptr;
@@ -822,6 +1015,38 @@ cudaError_t launch_laplacian_backward(NormalsArgs a, const NormalsWorkspace& w, 
         laplacian_sum_grad_kernel<<<blocks_for(a.total), NORMALS_THREADS, 0, stream>>>(a);
         if ((e = launched()) != cudaSuccess) return e;
         laplacian_cotangent_grad_kernel<<<blocks_for(a.total), NORMALS_THREADS, 0, stream>>>(a);
+    }
+    return launched();
+}
+
+cudaError_t launch_edge_terms_forward(NormalsArgs a, const NormalsWorkspace& w, cudaStream_t stream)
+{
+    cudaError_t e;
+    const long long n = a.total / a.V * a.F;
+    if ((e = launch_corner_adjacency(a.faces, 0, 1, a.V, a.F, w.counts, w.offsets, w.unsorted, w.inc, stream)) != cudaSuccess)
+        return e;
+    a.offsets = w.offsets;
+    a.inc = w.inc;
+    if (a.mode == DIRT_EDGE_LENGTH)
+        edge_terms_forward_kernel<DIRT_EDGE_LENGTH><<<blocks_for(n), NORMALS_THREADS, 0, stream>>>(a, n);
+    else
+        edge_terms_forward_kernel<DIRT_NORMAL_CONSISTENCY><<<blocks_for(n), NORMALS_THREADS, 0, stream>>>(a, n);
+    return launched();
+}
+
+cudaError_t launch_edge_terms_backward(NormalsArgs a, const NormalsWorkspace& w, cudaStream_t stream)
+{
+    cudaError_t e;
+    a.offsets = w.offsets;
+    a.inc = w.inc;
+    a.gs = w.gs;
+    if (a.mode == DIRT_EDGE_LENGTH) {
+        edge_length_grad_kernel<<<blocks_for(a.total), NORMALS_THREADS, 0, stream>>>(a);
+    } else {
+        const long long n = a.total / a.V * a.F;
+        consistency_face_grad_kernel<<<blocks_for(n), NORMALS_THREADS, 0, stream>>>(a, n);
+        if ((e = launched()) != cudaSuccess) return e;
+        consistency_vertex_grad_kernel<<<blocks_for(a.total), NORMALS_THREADS, 0, stream>>>(a);
     }
     return launched();
 }

@@ -719,17 +719,19 @@ def _stride(rows, k):
     return rows.stride(0) if rows.shape[0] > 1 else k
 
 
-# A mesh op: vertex normals (either mode) or vertex tangents.  Its forward builds a corner-adjacency workspace of
-# workspace_bytes(B, V, F) bytes, where workspace_bytes is an entry point, and its backward reads that adjacency.
+# A mesh op: vertex normals (either mode), vertex tangents, the Laplacian or an edge term.  Its forward builds a
+# corner-adjacency workspace of workspace_bytes(B, V, F) bytes, where workspace_bytes is an entry point, and its
+# backward reads that adjacency.
 #   name: the op's name in errors (its backward's is name + 'Grad');
 #   forward, backward: its entry points in the library;
 #   inputs(route, faces, *inputs): their input arguments, in their order;
 #   width: the width of the output rows; input_widths: the width of each input's gradient rows, B*V of them;
 #   restate(route, faces, *inputs): the torch restatement on the op's own inputs and the faces the kernels use, in the
 #     output's shape;
-#   finish(route, grads): turns the backward's gradient rows into the inputs' gradients; None where they are the same.
-_MeshOp = namedtuple('_MeshOp', 'name forward backward workspace_bytes inputs width input_widths restate finish',
-                     defaults=(None,))
+#   finish(route, grads): turns the backward's gradient rows into the inputs' gradients; None where they are the same;
+#   rows: 'V' for one output row per (item, vertex), 'F' for one per (item, face).
+_MeshOp = namedtuple('_MeshOp', 'name forward backward workspace_bytes inputs width input_widths restate finish rows',
+                     defaults=(None, 'V'))
 
 
 class _MeshFunction(torch.autograd.Function):
@@ -741,7 +743,7 @@ class _MeshFunction(torch.autograd.Function):
     def forward(ctx, op, route, faces, *inputs):
         dev = inputs[0].device
         lib = _lib.lib()
-        out = torch.empty((route.B * route.V, op.width), dtype=torch.float32, device=dev)
+        out = torch.empty((route.B * getattr(route, op.rows), op.width), dtype=torch.float32, device=dev)
         ws_bytes = int(getattr(lib, op.workspace_bytes)(route.B, route.V, route.F))
         workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=dev) if ws_bytes else None
         with torch.cuda.device(dev):
@@ -760,8 +762,12 @@ class _MeshFunction(torch.autograd.Function):
             return (None,) * (3 + len(want))
         faces, *inputs = ctx.saved_tensors
         if torch.is_grad_enabled():
-            # create_graph=True: differentiable gradients through the restatement, on the faces the kernels used
-            out = op.restate(route, faces[((faces >= 0) & (faces < route.V)).all(1)], *inputs)
+            # create_graph=True: differentiable gradients through the restatement, on the faces the kernels used; a
+            # per-face output has the rows of the faces left out back as zeros
+            valid = ((faces >= 0) & (faces < route.V)).all(1)
+            out = op.restate(route, faces[valid], *inputs)
+            if op.rows == 'F':
+                out = out.new_zeros(route.lead + (route.F, op.width)).index_copy(-2, valid.nonzero()[:, 0], out)
             wanted = [t for t, w in zip(inputs, want) if w]
             grads = iter(torch.autograd.grad(out, wanted, grad_out.reshape(out.shape), create_graph=True))
             return (None,) * 3 + tuple(next(grads) if w else None for w in want)
@@ -783,7 +789,7 @@ def _mesh(op, route, faces, *inputs):
     if faces.dtype == torch.int64:
         faces = faces.clamp(-1, (1 << 31) - 1)   # above int32: >= V, so left out like any other invalid index
     out = _MeshFunction.apply(op, route, faces.to(torch.int32).contiguous(), *inputs)
-    return out.reshape(route.lead + (route.V, op.width))
+    return out.reshape(route.lead + (getattr(route, op.rows), op.width))
 
 
 def _normals_inputs(mode, route, faces, rows):

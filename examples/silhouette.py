@@ -1,17 +1,20 @@
 """Shape from silhouettes: deform a sphere into a cube through per-vertex offsets, with and without a mesh-Laplacian
-smoothness term.
+smoothness term, and optionally with a normal-consistency term.
 
-    python examples/silhouette.py [--steps N] [--weight LAMBDA]
+    python examples/silhouette.py [--steps N] [--weight LAMBDA] [--consistency MU]
 
 The target's silhouettes are rendered with `rasterise_batch` from 8 cameras around it (two rings of four, above and
 below the equator).  The source is `scenes.icosphere(3)` (642 vertices) plus an offset per vertex, fitted by Adam to
-    silhouette MSE + lambda * mean |laplacian|^2
-with `mesh.laplacian(..., mode='uniform')`.  `main` runs the fit twice, at lambda = --weight and at lambda = 0, and
-prints for each: the silhouette IoU on 6 held-out views (other azimuths and elevations) before and after, the final
-mean |uniform laplacian| of the mesh, and how many faces' normals turned against their starting normals (folds).
+    silhouette MSE + lambda * mean |laplacian|^2 + mu * mean normal_consistency
+with `mesh.laplacian(..., mode='uniform')` and `mesh.normal_consistency`.  `main` runs the fit twice, at
+(lambda, mu) = (--weight, 0) and (0, 0), and a third time at (--weight, --consistency) when that is given.  It prints for
+each: the silhouette IoU on 6 held-out views (other azimuths and elevations) before and after, the final mean
+|uniform laplacian| and mean normal consistency of the mesh, and how many faces' normals turned against their starting
+normals (folds).
 On an H100 at the defaults (DESIGN.md §7.16) the term leaves a 5x smoother mesh with a fifth of the folds (82 of 1280
 faces against 447), at about the same held-out IoU (0.908 against 0.912, from 0.652); the figures move a little from
-run to run, as the rasteriser sums vertex gradients with float atomics.
+run to run, as the rasteriser sums vertex gradients with float atomics.  DESIGN.md §7.17 records what the
+normal-consistency term changes.
 """
 import argparse
 import math
@@ -26,6 +29,7 @@ from examples.shadow import camera   # noqa: E402
 
 SIZE = 96           # silhouette width and height
 DISTANCE = 3.5      # of every camera from the origin
+CONSISTENCY = 0.3   # a normal-consistency weight mu for --consistency, from the sweep of DESIGN.md §7.17
 
 
 def cameras(azimuths, elevations, device):
@@ -59,8 +63,9 @@ def face_normals(vertices, faces):
     return torch.linalg.cross(p[:, 1] - p[:, 0], p[:, 2] - p[:, 0], dim=-1)
 
 
-def fit(weight, steps, lr=0.005, device=None, verbose=True):
-    """One fit at Laplacian weight `weight`.  Returns a dict of what `main` prints."""
+def fit(weight, steps, lr=0.005, device=None, verbose=True, consistency=0.):
+    """One fit at Laplacian weight `weight` and normal-consistency weight `consistency`.  Returns a dict of what `main`
+    prints."""
     from dirt_b200 import mesh, scenes
     dev = device or torch.device('cuda')
     v, f = scenes.icosphere(3)
@@ -83,6 +88,8 @@ def fit(weight, steps, lr=0.005, device=None, verbose=True):
         data = ((silhouettes(vertices, faces, train) - target) ** 2).mean()
         smooth = mesh.laplacian(vertices, faces, 'uniform').square().sum(-1).mean()
         loss = data + weight * smooth
+        if consistency:
+            loss = loss + consistency * mesh.normal_consistency(vertices, faces).mean()
         loss.backward()
         opt.step()
         if verbose and (step == 0 or (step + 1) % max(steps // 4, 1) == 0):
@@ -93,19 +100,24 @@ def fit(weight, steps, lr=0.005, device=None, verbose=True):
         end_iou = iou(silhouettes(vertices, faces, held_out), target_held)
         mean_l = mesh.laplacian(vertices, faces, 'uniform').norm(dim=-1).mean().item()
         start_l = mesh.laplacian(source, faces, 'uniform').norm(dim=-1).mean().item()
+        mean_c = mesh.normal_consistency(vertices, faces).mean().item()
+        start_c = mesh.normal_consistency(source, faces).mean().item()
         flipped = int(((face_normals(vertices, faces) * face_normals(source, faces)).sum(-1) < 0).sum())
-    return {'weight': weight, 'held_out_iou_start': start_iou, 'held_out_iou_end': end_iou,
-            'mean_laplacian_start': start_l, 'mean_laplacian_end': mean_l, 'flipped_faces': flipped,
-            'faces': int(faces.shape[0])}
+    return {'weight': weight, 'consistency': consistency, 'held_out_iou_start': start_iou, 'held_out_iou_end': end_iou,
+            'mean_laplacian_start': start_l, 'mean_laplacian_end': mean_l, 'mean_consistency_start': start_c,
+            'mean_consistency_end': mean_c, 'flipped_faces': flipped, 'faces': int(faces.shape[0])}
 
 
-def main(steps=300, weight=10.):
+def main(steps=300, weight=10., consistency=None):
     results = []
-    for w in (weight, 0.):
-        r = fit(w, steps)
-        print('lambda %g: held-out IoU %.4f -> %.4f, mean |uniform laplacian| %.5f (sphere %.5f), faces flipped %d of %d'
-              % (w, r['held_out_iou_start'], r['held_out_iou_end'], r['mean_laplacian_end'], r['mean_laplacian_start'],
-                 r['flipped_faces'], r['faces']))
+    runs = [(weight, 0.), (0., 0.)] + ([(weight, consistency)] if consistency is not None else [])
+    for w, mu in runs:
+        r = fit(w, steps, consistency=mu)
+        print('lambda %g, mu %g: held-out IoU %.4f -> %.4f, mean |uniform laplacian| %.5f (sphere %.5f), mean normal '
+              'consistency %.5f (sphere %.5f), faces flipped %d of %d'
+              % (w, mu, r['held_out_iou_start'], r['held_out_iou_end'], r['mean_laplacian_end'],
+                 r['mean_laplacian_start'], r['mean_consistency_end'], r['mean_consistency_start'], r['flipped_faces'],
+                 r['faces']))
         results.append(r)
     return results
 
@@ -114,5 +126,6 @@ if __name__ == '__main__':
     parser = argparse.ArgumentParser()
     parser.add_argument('--steps', type=int, default=300)
     parser.add_argument('--weight', type=float, default=10.)
+    parser.add_argument('--consistency', type=float, default=None, metavar='MU')
     args = parser.parse_args()
-    main(args.steps, args.weight)
+    main(args.steps, args.weight, args.consistency)

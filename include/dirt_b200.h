@@ -610,6 +610,40 @@ int dirt_laplacian_backward(int mode, const float* vertices, long long vertex_st
                             const float* grad_out, float* grad_vertices, void* workspace, size_t workspace_bytes,
                             int B, long long V, long long F, void* cuda_stream);
 
+/* Edge terms for fitting shapes, one value per face edge, for B items of V vertices sharing the faces:
+ *   vertices             float32 [B*V, 3], row stride vertex_stride >= 3 floats, unit stride along the row
+ *   faces                int32 [F, 3], shared by the batch
+ *   out, grad_out        float32 [B*F, 3], contiguous: entry k of face f is its edge k, from v_k to v_{k+1 mod 3}
+ *   grad_vertices        float32 [B*V, 3], contiguous
+ * With corners p0, p1, p2 of face f, u_f = n_f / (|n_f| + 1e-12) and n_f = (p1 - p0) x (p2 - p0):
+ *   DIRT_EDGE_LENGTH         |p_{k+1} - p_k|
+ *   DIRT_NORMAL_CONSISTENCY  1 - u_f . (sum of u_g over P) / |P|, where P holds the valid faces other than f that name
+ *                            both ends of the edge, each once; 0 when P is empty (a boundary edge) or the two ends are
+ *                            one vertex.  A flat edge gives 0, a right angle 1, a reversed neighbour about 2.
+ * An interior edge of a manifold mesh appears twice, once from each face, with equal values.  A face with an index
+ * outside [0, V) is left out: its three entries are 0, it receives no gradient and it is nobody's partner.
+ * Backward: grad_vertices = the gradient torch autograd gives the same expressions (none through a zero-length edge;
+ * a zero-area face passes the 1e12-scale values of its normal's division, as for the normals).
+ * Workspace: at least dirt_edge_terms_workspace_bytes(B, V, F) bytes (0 when B, V or F is 0), a function of the sizes
+ * alone, for both modes; the forward call writes the vertex -> face-corner adjacency into it and the backward call
+ * reads it there, as for the normals, and uses the rest as scratch.
+ * Every sum has one fixed order (no float atomics): repeated calls give bit-identical values and gradients.
+ * Forward: B = 0 or F = 0: nothing is launched; V = 0 with F > 0: every face is invalid, and out is zeroed without
+ * reading vertices, faces or the workspace.  Backward: B = 0 or V = 0: nothing is written; F = 0: grad_vertices is
+ * zeroed.  V < 2^31, 3F < 2^31; all pointers, the
+ * workspace included, 4-byte aligned.  These entries were added without a signature change to any other, so
+ * dirt_abi_version() stays 4. */
+enum {
+    DIRT_EDGE_LENGTH = 0,
+    DIRT_NORMAL_CONSISTENCY = 1
+};
+size_t dirt_edge_terms_workspace_bytes(int B, long long V, long long F);
+int dirt_edge_terms_forward(int mode, const float* vertices, long long vertex_stride, const int32_t* faces, float* out,
+                            void* workspace, size_t workspace_bytes, int B, long long V, long long F, void* cuda_stream);
+int dirt_edge_terms_backward(int mode, const float* vertices, long long vertex_stride, const int32_t* faces,
+                             const float* grad_out, float* grad_vertices, void* workspace, size_t workspace_bytes,
+                             int B, long long V, long long F, void* cuda_stream);
+
 /* Vertex tangents for tangent-space normal mapping, for B items of V vertices sharing the faces:
  *   vertices             float32 [B*V, 3], row stride vertex_stride >= 3 floats, unit stride along the row
  *   uvs                  float32, the uv of vertex v of item b at uvs + b*uv_item_stride + v*uv_stride, uv_stride >= 2,
