@@ -1207,30 +1207,60 @@ extern "C" int dirt_shadow_backward_deterministic(const float* positions, long l
 }
 
 // element offsets of the vertex rows stay below 2^62; vertex ids and incidence ids (k*F + f) are int32
-static bool normals_shape_ok(int mode, int B, long long V, long long F, long long stride)
+static bool mesh_shape_ok(int B, long long V, long long F, long long stride)
 {
-    if (mode != DIRT_NORMALS_AVERAGE && mode != DIRT_NORMALS_PRE_SPLIT) return false;
     if (B < 0 || V < 0 || F < 0 || stride < 3) return false;
     if (V >= (1ll << 31) || 3 * F >= (1ll << 31)) return false;
     return (double)B * V * stride <= 4.0e18;
 }
 
-extern "C" size_t dirt_normals_workspace_bytes(int B, long long V, long long F)
+// The mesh ops whose only input is the vertex rows: the vertex normals (DESIGN.md §7.3), the mesh Laplacian (§7.16) and
+// the edge lengths and normal consistency (§7.17).  Each accepts two modes, and sizes its workspace's gradient region
+// as grad_width floats per (item, vertex), or per (item, face) with per_face.  A per-face op's output is [B*F, 3].
+struct MeshOp {
+    int modes[2];
+    int grad_width;
+    bool per_face;
+    MeshPasses forward, backward;
+};
+static const MeshOp NORMALS_OP = {{DIRT_NORMALS_AVERAGE, DIRT_NORMALS_PRE_SPLIT}, 3, false, normals_forward_passes,
+                                  normals_backward_passes};
+static const MeshOp LAPLACIAN_OP = {{DIRT_LAPLACIAN_UNIFORM, DIRT_LAPLACIAN_COTANGENT}, 4, false,
+                                    laplacian_forward_passes, laplacian_backward_passes};
+static const MeshOp EDGE_TERMS_OP = {{DIRT_EDGE_LENGTH, DIRT_NORMAL_CONSISTENCY}, 3, true, edge_terms_forward_passes,
+                                     edge_terms_backward_passes};
+
+static bool mesh_op_shape_ok(const MeshOp& op, int mode, int B, long long V, long long F, long long stride)
 {
-    if (!normals_shape_ok(DIRT_NORMALS_AVERAGE, B, V, F, 3) || B == 0 || V == 0 || F == 0) return 0;
-    return carve_normals_workspace(nullptr, B, V, F).bytes;
+    return (mode == op.modes[0] || mode == op.modes[1]) && mesh_shape_ok(B, V, F, stride);
 }
 
-// The checks the eight mesh entries share, in order: the vertices, faces and workspace, NULL (the faces and workspace
-// only when a workspace is needed: `need`, the entry's workspace size, is 0 exactly when F = 0 once B*V > 0) then
-// 4-byte alignment (the workspace holds int32 adjacency and float gradients, read and written one element at a time, so
-// not scratch_check's 256 bytes); the workspace's size; the other inputs and then `outs` (the output, or the incoming
-// gradient and the gradients a backward requires), each by required_check.  Before it each entry makes its shape check
-// and its early return, which differ:
-// - the forwards and the normals and Laplacian backwards return DIRT_OK for B*V == 0 before they check anything else;
-// - the tangents backward first checks the alignment of its gradients, which may be NULL, then returns DIRT_OK for
-//   B*V == 0 or when no gradient is wanted;
-// - the edge-term entries return DIRT_OK for B*F == 0, and handle V == 0 themselves (see below).
+// grad_width 3 and per vertex: the vertex normals' and tangents' workspace
+static size_t mesh_workspace_bytes(int B, long long V, long long F, int grad_width = 3, bool per_face = false)
+{
+    if (!mesh_shape_ok(B, V, F, 3) || B == 0 || V == 0 || F == 0) return 0;
+    return carve_normals_workspace(nullptr, B, V, F, grad_width, per_face).bytes;
+}
+
+extern "C" size_t dirt_normals_workspace_bytes(int B, long long V, long long F) { return mesh_workspace_bytes(B, V, F); }
+
+extern "C" size_t dirt_laplacian_workspace_bytes(int B, long long V, long long F)
+{
+    return mesh_workspace_bytes(B, V, F, LAPLACIAN_OP.grad_width);
+}
+
+extern "C" size_t dirt_edge_terms_workspace_bytes(int B, long long V, long long F)
+{
+    return mesh_workspace_bytes(B, V, F, EDGE_TERMS_OP.grad_width, EDGE_TERMS_OP.per_face);
+}
+
+// The checks after an entry's shape check and early return, in order: the vertices, faces and workspace, NULL (the
+// faces and workspace only when a workspace is needed: `need`, the entry's workspace size, is 0 exactly when F = 0 once
+// B*V > 0) then 4-byte alignment (the workspace holds int32 adjacency and float gradients, read and written one element
+// at a time, so not scratch_check's 256 bytes); the workspace's size; the other inputs and then `outs` (the output, or
+// the incoming gradient and the gradients a backward requires), each by required_check.  The early returns are
+// mesh_forward's and mesh_backward's, and the tangents entries' own: they first check the alignment of their gradients,
+// which may be NULL, then return DIRT_OK for B*V == 0 or when no gradient is wanted.
 static int mesh_check(const float* vertices, const int32_t* faces, const void* workspace, size_t workspace_bytes,
                       size_t need, std::initializer_list<const void*> inputs, std::initializer_list<const void*> outs)
 {
@@ -1250,166 +1280,118 @@ static NormalsArgs make_normals_args(int mode, const float* vertices, long long 
     return a;
 }
 
+// Zeroes `rows` rows of 3 floats at out, which must not be NULL: a per-face op's call that has nothing to look at.
+static int zero_rows(float* out, long long rows, void* cuda_stream)
+{
+    const int rc = required_check({out});
+    if (rc != DIRT_OK) return rc;
+    CUDA_TRY(cudaMemsetAsync(out, 0, sizeof(float) * 3 * (size_t)rows, (cudaStream_t)cuda_stream));
+    return DIRT_OK;
+}
+
+// A forward returns DIRT_OK for no output rows (B*V, or B*F per face) before it checks anything else.  Per face, V == 0
+// with F > 0 makes every face invalid, so it zeroes out, checking only that pointer, before mesh_check (which requires a
+// workspace whenever F > 0).
+static int mesh_forward(const MeshOp& op, int mode, const float* vertices, long long vertex_stride,
+                        const int32_t* faces, float* out, void* workspace, size_t workspace_bytes, int B, long long V,
+                        long long F, void* cuda_stream)
+{
+    launch_count() = 0;
+    if (!mesh_op_shape_ok(op, mode, B, V, F, vertex_stride)) return DIRT_ERR_BAD_SHAPE;
+    if ((long long)B * (op.per_face ? F : V) == 0) return DIRT_OK;
+    if (op.per_face && V == 0) return zero_rows(out, (long long)B * F, cuda_stream);
+    const int rc = mesh_check(vertices, faces, workspace, workspace_bytes,
+                              mesh_workspace_bytes(B, V, F, op.grad_width, op.per_face), {}, {out});
+    if (rc != DIRT_OK) return rc;
+    NormalsArgs a = make_normals_args(mode, vertices, vertex_stride, faces, B, V, F);
+    a.out = out;
+    CUDA_TRY(launch_mesh_forward(op.forward, a,
+                                 carve_normals_workspace(F > 0 ? workspace : nullptr, B, V, F, op.grad_width, op.per_face),
+                                 (cudaStream_t)cuda_stream));
+    return DIRT_OK;
+}
+
+// A backward returns DIRT_OK for B*V == 0 before it checks anything else.  Per face, F == 0 leaves no edges, so it zeroes
+// grad_vertices, checking only that pointer, before mesh_check.
+static int mesh_backward(const MeshOp& op, int mode, const float* vertices, long long vertex_stride,
+                         const int32_t* faces, const float* grad_out, float* grad_vertices, void* workspace,
+                         size_t workspace_bytes, int B, long long V, long long F, void* cuda_stream)
+{
+    launch_count() = 0;
+    if (!mesh_op_shape_ok(op, mode, B, V, F, vertex_stride)) return DIRT_ERR_BAD_SHAPE;
+    if ((long long)B * V == 0) return DIRT_OK;
+    if (op.per_face && F == 0) return zero_rows(grad_vertices, (long long)B * V, cuda_stream);
+    const int rc = mesh_check(vertices, faces, workspace, workspace_bytes,
+                              mesh_workspace_bytes(B, V, F, op.grad_width, op.per_face), {}, {grad_out, grad_vertices});
+    if (rc != DIRT_OK) return rc;
+    NormalsArgs a = make_normals_args(mode, vertices, vertex_stride, faces, B, V, F);
+    a.grad = grad_out;
+    a.g_vertices = grad_vertices;
+    CUDA_TRY(launch_mesh_backward(op.backward, a,
+                                  carve_normals_workspace(F > 0 ? workspace : nullptr, B, V, F, op.grad_width, op.per_face),
+                                  (cudaStream_t)cuda_stream));
+    return DIRT_OK;
+}
+
 extern "C" int dirt_normals_forward(int mode, const float* vertices, long long vertex_stride, const int32_t* faces,
                                     float* normals, void* workspace, size_t workspace_bytes, int B, long long V, long long F,
                                     void* cuda_stream)
 {
-    launch_count() = 0;
-    if (!normals_shape_ok(mode, B, V, F, vertex_stride)) return DIRT_ERR_BAD_SHAPE;
-    if ((long long)B * V == 0) return DIRT_OK;
-    const int rc = mesh_check(vertices, faces, workspace, workspace_bytes, dirt_normals_workspace_bytes(B, V, F), {},
-                              {normals});
-    if (rc != DIRT_OK) return rc;
-    NormalsArgs a = make_normals_args(mode, vertices, vertex_stride, faces, B, V, F);
-    a.out = normals;
-    CUDA_TRY(launch_normals_forward(a, carve_normals_workspace(F > 0 ? workspace : nullptr, B, V, F),
-                                    (cudaStream_t)cuda_stream));
-    return DIRT_OK;
+    return mesh_forward(NORMALS_OP, mode, vertices, vertex_stride, faces, normals, workspace, workspace_bytes, B, V, F,
+                        cuda_stream);
 }
 
 extern "C" int dirt_normals_backward(int mode, const float* vertices, long long vertex_stride, const int32_t* faces,
                                      const float* grad_normals, float* grad_vertices, void* workspace,
                                      size_t workspace_bytes, int B, long long V, long long F, void* cuda_stream)
 {
-    launch_count() = 0;
-    if (!normals_shape_ok(mode, B, V, F, vertex_stride)) return DIRT_ERR_BAD_SHAPE;
-    if ((long long)B * V == 0) return DIRT_OK;
-    const int rc = mesh_check(vertices, faces, workspace, workspace_bytes, dirt_normals_workspace_bytes(B, V, F), {},
-                              {grad_normals, grad_vertices});
-    if (rc != DIRT_OK) return rc;
-    NormalsArgs a = make_normals_args(mode, vertices, vertex_stride, faces, B, V, F);
-    a.grad = grad_normals;
-    a.g_vertices = grad_vertices;
-    CUDA_TRY(launch_normals_backward(a, carve_normals_workspace(F > 0 ? workspace : nullptr, B, V, F),
-                                     (cudaStream_t)cuda_stream));
-    return DIRT_OK;
-}
-
-// ---- the mesh Laplacian (DESIGN.md §7.16): the normals' arguments, checks and early returns ------------------------
-
-static bool laplacian_shape_ok(int mode, int B, long long V, long long F, long long stride)
-{
-    return (mode == DIRT_LAPLACIAN_UNIFORM || mode == DIRT_LAPLACIAN_COTANGENT) &&
-           normals_shape_ok(DIRT_NORMALS_AVERAGE, B, V, F, stride);
-}
-
-extern "C" size_t dirt_laplacian_workspace_bytes(int B, long long V, long long F)
-{
-    if (!normals_shape_ok(DIRT_NORMALS_AVERAGE, B, V, F, 3) || B == 0 || V == 0 || F == 0) return 0;
-    return carve_normals_workspace(nullptr, B, V, F, 4).bytes;
+    return mesh_backward(NORMALS_OP, mode, vertices, vertex_stride, faces, grad_normals, grad_vertices, workspace,
+                         workspace_bytes, B, V, F, cuda_stream);
 }
 
 extern "C" int dirt_laplacian_forward(int mode, const float* vertices, long long vertex_stride, const int32_t* faces,
                                       float* out, void* workspace, size_t workspace_bytes, int B, long long V, long long F,
                                       void* cuda_stream)
 {
-    launch_count() = 0;
-    if (!laplacian_shape_ok(mode, B, V, F, vertex_stride)) return DIRT_ERR_BAD_SHAPE;
-    if ((long long)B * V == 0) return DIRT_OK;
-    const int rc = mesh_check(vertices, faces, workspace, workspace_bytes, dirt_laplacian_workspace_bytes(B, V, F), {},
-                              {out});
-    if (rc != DIRT_OK) return rc;
-    NormalsArgs a = make_normals_args(mode, vertices, vertex_stride, faces, B, V, F);
-    a.out = out;
-    CUDA_TRY(launch_laplacian_forward(a, carve_normals_workspace(F > 0 ? workspace : nullptr, B, V, F, 4),
-                                      (cudaStream_t)cuda_stream));
-    return DIRT_OK;
+    return mesh_forward(LAPLACIAN_OP, mode, vertices, vertex_stride, faces, out, workspace, workspace_bytes, B, V, F,
+                        cuda_stream);
 }
 
 extern "C" int dirt_laplacian_backward(int mode, const float* vertices, long long vertex_stride, const int32_t* faces,
                                        const float* grad_out, float* grad_vertices, void* workspace,
                                        size_t workspace_bytes, int B, long long V, long long F, void* cuda_stream)
 {
-    launch_count() = 0;
-    if (!laplacian_shape_ok(mode, B, V, F, vertex_stride)) return DIRT_ERR_BAD_SHAPE;
-    if ((long long)B * V == 0) return DIRT_OK;
-    const int rc = mesh_check(vertices, faces, workspace, workspace_bytes, dirt_laplacian_workspace_bytes(B, V, F), {},
-                              {grad_out, grad_vertices});
-    if (rc != DIRT_OK) return rc;
-    NormalsArgs a = make_normals_args(mode, vertices, vertex_stride, faces, B, V, F);
-    a.grad = grad_out;
-    a.g_vertices = grad_vertices;
-    CUDA_TRY(launch_laplacian_backward(a, carve_normals_workspace(F > 0 ? workspace : nullptr, B, V, F, 4),
-                                       (cudaStream_t)cuda_stream));
-    return DIRT_OK;
-}
-
-// ---- edge lengths and normal consistency (DESIGN.md §7.17): the Laplacian's arguments and checks ---------------------
-// The output is per face, so the early returns differ: the forward launches nothing for B*F == 0, and V == 0 with
-// F > 0 makes every face invalid, so it zeroes out.  The backward writes nothing for B*V == 0 and zeroes grad_vertices
-// for F == 0.  All are decided before mesh_check, which requires a workspace whenever F > 0.
-
-static bool edge_terms_shape_ok(int mode, int B, long long V, long long F, long long stride)
-{
-    return (mode == DIRT_EDGE_LENGTH || mode == DIRT_NORMAL_CONSISTENCY) &&
-           normals_shape_ok(DIRT_NORMALS_AVERAGE, B, V, F, stride);
-}
-
-extern "C" size_t dirt_edge_terms_workspace_bytes(int B, long long V, long long F)
-{
-    if (!normals_shape_ok(DIRT_NORMALS_AVERAGE, B, V, F, 3) || B == 0 || V == 0 || F == 0) return 0;
-    return carve_normals_workspace(nullptr, B, V, F, 3, true).bytes;
+    return mesh_backward(LAPLACIAN_OP, mode, vertices, vertex_stride, faces, grad_out, grad_vertices, workspace,
+                         workspace_bytes, B, V, F, cuda_stream);
 }
 
 extern "C" int dirt_edge_terms_forward(int mode, const float* vertices, long long vertex_stride, const int32_t* faces,
                                        float* out, void* workspace, size_t workspace_bytes, int B, long long V,
                                        long long F, void* cuda_stream)
 {
-    launch_count() = 0;
-    if (!edge_terms_shape_ok(mode, B, V, F, vertex_stride)) return DIRT_ERR_BAD_SHAPE;
-    if ((long long)B * F == 0) return DIRT_OK;
-    if (V == 0) {
-        const int rc = required_check({out});
-        if (rc != DIRT_OK) return rc;
-        CUDA_TRY(cudaMemsetAsync(out, 0, sizeof(float) * 3 * (size_t)B * (size_t)F, (cudaStream_t)cuda_stream));
-        return DIRT_OK;
-    }
-    const int rc = mesh_check(vertices, faces, workspace, workspace_bytes, dirt_edge_terms_workspace_bytes(B, V, F), {},
-                              {out});
-    if (rc != DIRT_OK) return rc;
-    NormalsArgs a = make_normals_args(mode, vertices, vertex_stride, faces, B, V, F);
-    a.out = out;
-    CUDA_TRY(launch_edge_terms_forward(a, carve_normals_workspace(workspace, B, V, F, 3, true), (cudaStream_t)cuda_stream));
-    return DIRT_OK;
+    return mesh_forward(EDGE_TERMS_OP, mode, vertices, vertex_stride, faces, out, workspace, workspace_bytes, B, V, F,
+                        cuda_stream);
 }
 
 extern "C" int dirt_edge_terms_backward(int mode, const float* vertices, long long vertex_stride, const int32_t* faces,
                                         const float* grad_out, float* grad_vertices, void* workspace,
                                         size_t workspace_bytes, int B, long long V, long long F, void* cuda_stream)
 {
-    launch_count() = 0;
-    if (!edge_terms_shape_ok(mode, B, V, F, vertex_stride)) return DIRT_ERR_BAD_SHAPE;
-    if ((long long)B * V == 0) return DIRT_OK;
-    if (F == 0) {   // no edges: no gradient reaches the vertices
-        const int rc = required_check({grad_vertices});
-        if (rc != DIRT_OK) return rc;
-        CUDA_TRY(cudaMemsetAsync(grad_vertices, 0, sizeof(float) * 3 * (size_t)B * (size_t)V, (cudaStream_t)cuda_stream));
-        return DIRT_OK;
-    }
-    const int rc = mesh_check(vertices, faces, workspace, workspace_bytes, dirt_edge_terms_workspace_bytes(B, V, F), {},
-                              {grad_out, grad_vertices});
-    if (rc != DIRT_OK) return rc;
-    NormalsArgs a = make_normals_args(mode, vertices, vertex_stride, faces, B, V, F);
-    a.grad = grad_out;
-    a.g_vertices = grad_vertices;
-    CUDA_TRY(launch_edge_terms_backward(a, carve_normals_workspace(workspace, B, V, F, 3, true), (cudaStream_t)cuda_stream));
-    return DIRT_OK;
+    return mesh_backward(EDGE_TERMS_OP, mode, vertices, vertex_stride, faces, grad_out, grad_vertices, workspace,
+                         workspace_bytes, B, V, F, cuda_stream);
 }
 
 // ---- vertex tangents and normal mapping (DESIGN.md §7.14) ----------------------------------------------------------
 
-// as normals_shape_ok, with the uv and normal rows' strides and the uvs' item stride
+// as mesh_shape_ok, with the uv and normal rows' strides and the uvs' item stride
 static bool tangents_shape_ok(int B, long long V, long long F, long long vs, long long us, long long uis, long long ns)
 {
-    if (!normals_shape_ok(DIRT_NORMALS_AVERAGE, B, V, F, vs) || us < 2 || uis < 0 || ns < 3) return false;
+    if (!mesh_shape_ok(B, V, F, vs) || us < 2 || uis < 0 || ns < 3) return false;
     const double rows = (double)B * V;
     return rows * us + (double)B * uis <= 4.0e18 && rows * ns <= 4.0e18 && rows * 4 <= 4.0e18;
 }
 
-extern "C" size_t dirt_tangents_workspace_bytes(int B, long long V, long long F)
-{
-    return dirt_normals_workspace_bytes(B, V, F);
-}
+extern "C" size_t dirt_tangents_workspace_bytes(int B, long long V, long long F) { return mesh_workspace_bytes(B, V, F); }
 
 static TangentArgs make_tangent_args(const float* vertices, long long vertex_stride, const float* uvs, long long uv_stride,
                                      long long uv_item_stride, const float* normals, long long normals_stride,

@@ -13,11 +13,14 @@
 // (its unit normal, or its corner gradients) from the positions: no per-face buffer, and no float atomics.  A row longer
 // than LONG_ROW is summed by the whole warp instead (lane-strided partial sums, then a butterfly), so that a high-valence
 // vertex does not hold up its warp's other 31 lanes.  Either way each sum has one fixed order for given faces, and two
-// calls give bit-identical results.
+// calls give bit-identical results.  Every such pass is an instance of row_pass_kernel<Term, Finish>: Term is what one
+// incidence adds to its row, Finish what the row's sum becomes.
 //
 // The file also holds the vertex tangents (dirt_tangents_forward / _backward, DESIGN.md §7.14), the mesh Laplacian
 // (dirt_laplacian_forward / _backward, DESIGN.md §7.16) and the edge-length and normal-consistency terms
 // (dirt_edge_terms_forward / _backward, DESIGN.md §7.17), which use the same adjacency, workspace and per-vertex passes.
+// The normals, the Laplacian and the edge terms also share one launch path (launch_mesh_forward / _backward), where
+// each op keeps only its mode dispatch (*_passes).
 #include <cub/block/block_scan.cuh>
 
 #include "../../include/dirt_b200.h"
@@ -110,6 +113,15 @@ __device__ __forceinline__ float3 normalise_grad(float3 x, float3 g)
                        __fmaf_rn(x.z, k, __fdiv_rn(g.z, d)));
 }
 
+__device__ __forceinline__ float3 div3(float3 a, float d)
+{
+    return make_float3(__fdiv_rn(a.x, d), __fdiv_rn(a.y, d), __fdiv_rn(a.z, d));
+}
+
+// the corner after and before corner k of a face
+__device__ __forceinline__ int next3(int k) { return k == 2 ? 0 : k + 1; }
+__device__ __forceinline__ int prev3(int k) { return k == 0 ? 2 : k - 1; }
+
 __device__ __forceinline__ bool load_face(const int* __restrict__ faces, long long f, int V, int v[3])
 {
 #pragma unroll
@@ -117,21 +129,63 @@ __device__ __forceinline__ bool load_face(const int* __restrict__ faces, long lo
     return v[0] >= 0 && v[0] < V && v[1] >= 0 && v[1] < V && v[2] >= 0 && v[2] < V;
 }
 
-// The positions of the corners of face f of item b, and its edges from corner 0.
+// The position of vertex v of item b.
+__device__ __forceinline__ float3 position(const NormalsArgs& a, long long b, int v)
+{
+    return ld3(a.vertices + b * a.V * a.stride + v * a.stride);
+}
+
+// The corners of a face of item b, and its edges from corner 0.
 struct Corners {
     int v[3];
     float3 e1, e2;
 };
 
-__device__ __forceinline__ Corners corners(const NormalsArgs& a, long long b, int f)
+// The edges of the face c.v of item b.
+__device__ __forceinline__ void edges_of(const NormalsArgs& a, long long b, Corners& c)
 {
-    Corners c;
-    load_face(a.faces, f, a.V, c.v);
     const float* base = a.vertices + b * a.V * a.stride;
     const float3 p0 = ld3(base + c.v[0] * a.stride);
     c.e1 = sub3(ld3(base + c.v[1] * a.stride), p0);
     c.e2 = sub3(ld3(base + c.v[2] * a.stride), p0);
+}
+
+__device__ __forceinline__ Corners corners_of(const NormalsArgs& a, long long b, const int v[3])
+{
+    Corners c;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) c.v[k] = v[k];
+    edges_of(a, b, c);
     return c;
+}
+
+__device__ __forceinline__ Corners corners(const NormalsArgs& a, long long b, int f)
+{
+    Corners c;
+    load_face(a.faces, f, a.V, c.v);
+    edges_of(a, b, c);
+    return c;
+}
+
+// u = unit(e1 x e2)
+__device__ __forceinline__ float3 unit_of(const Corners& c) { return normalise(cross3(c.e1, c.e2)); }
+
+// Corner k's share of g1 and g2, the gradients to e1 = p1 - p0 and e2 = p2 - p0: corner 0 gets -(g1 + g2).
+__device__ __forceinline__ float3 corner_share(int k, float3 g1, float3 g2)
+{
+    if (k == 1) return g1;
+    if (k == 2) return g2;
+    return make_float3(-__fadd_rn(g1.x, g2.x), -__fadd_rn(g1.y, g2.y), -__fadd_rn(g1.z, g2.z));
+}
+__device__ __forceinline__ float corner_share(int k, float g1, float g2)
+{
+    return k == 1 ? g1 : (k == 2 ? g2 : -__fadd_rn(g1, g2));
+}
+
+// The gradient to corner k of the face c of the gradient gn to its n = e1 x e2.
+__device__ __forceinline__ float3 cross_grad(const Corners& c, float3 gn, int k)
+{
+    return corner_share(k, cross3(c.e2, gn), cross3(gn, c.e1));   // d/d e1, d/d e2
 }
 
 // ---- the adjacency ----------------------------------------------------------------------------------------------------
@@ -236,14 +290,87 @@ __device__ __forceinline__ auto row_sum(const int* __restrict__ inc, int lo, int
     return s;
 }
 
+// The rows t = b*V + v of the batch.  A row is empty when it is past the batch or there are no faces.
+struct Row {
+    long long t, b;
+    int lo, hi;
+    bool active;
+};
+
+__device__ __forceinline__ Row row_of(const NormalsArgs& a, long long t0)
+{
+    Row r;
+    r.t = t0 + (threadIdx.x & 31);
+    r.active = r.t < a.total;
+    r.b = 0;
+    r.lo = r.hi = 0;
+    if (a.F == 0) return r;   // no adjacency to read
+    r.b = r.active ? r.t / a.V : 0;
+    const long long v = r.t - r.b * a.V;
+    if (r.active) {
+        r.lo = __ldg(a.offsets + v);
+        r.hi = __ldg(a.offsets + v + 1);
+    }
+    return r;
+}
+
+// The tangents' passes run on the rows of their mesh part.
+__host__ __device__ __forceinline__ long long total_of(const NormalsArgs& a) { return a.total; }
+__host__ __device__ __forceinline__ long long total_of(const TangentArgs& a) { return a.m.total; }
+__device__ __forceinline__ const int* inc_of(const NormalsArgs& a) { return a.inc; }
+__device__ __forceinline__ const int* inc_of(const TangentArgs& a) { return a.m.inc; }
+__device__ __forceinline__ Row row_of(const TangentArgs& a, long long t0) { return row_of(a.m, t0); }
+
+// Every per-vertex pass: one thread per row, each warp taking 32 consecutive rows (the loop is warp-uniform, as row_sum
+// needs).  Each row sums Term{a} over its incidences, and Finish{a}(r, sum) writes the row's result.
+template <class Term, class Finish, class Args>
+__global__ void __launch_bounds__(NORMALS_THREADS) row_pass_kernel(Args a)
+{
+    for (long long t0 = (long long)blockIdx.x * NORMALS_THREADS + (threadIdx.x & ~31); t0 < total_of(a);
+         t0 += (long long)gridDim.x * NORMALS_THREADS) {
+        const Row r = row_of(a, t0);
+        const auto s = row_sum(inc_of(a), r.lo, r.hi, r.b, Term{a});
+        if (r.active) Finish{a}(r, s);
+    }
+}
+
+// The passes whose row result is a vertex gradient.
+struct StoreGrad {
+    const NormalsArgs& a;
+    __device__ __forceinline__ void operator()(const Row& r, float3 g) const { st3(a.g_vertices + 3 * r.t, g); }
+};
+
+// ---- the vertex normals (DESIGN.md §7.3) ------------------------------------------------------------------------------
+
 // u_f of the face of incidence i
 struct FaceUnit {
     const NormalsArgs& a;
-    __device__ __forceinline__ float3 operator()(long long b, int i) const
+    __device__ __forceinline__ float3 operator()(long long b, int i) const { return unit_of(corners(a, b, i % a.F)); }
+};
+
+// average mode: the normalised sum
+struct StoreNormal {
+    const NormalsArgs& a;
+    __device__ __forceinline__ void operator()(const Row& r, float3 s) const { st3(a.out + 3 * r.t, normalise(s)); }
+};
+
+// pre-split mode: u_f of the last incidence of the row, or 0
+__global__ void __launch_bounds__(NORMALS_THREADS) normals_pre_split_kernel(NormalsArgs a)
+{
+    for (long long t0 = (long long)blockIdx.x * NORMALS_THREADS + (threadIdx.x & ~31); t0 < a.total;
+         t0 += (long long)gridDim.x * NORMALS_THREADS) {
+        const Row r = row_of(a, t0);
+        const float3 n = r.hi > r.lo ? FaceUnit{a}(r.b, __ldg(a.inc + r.hi - 1)) : make_float3(0.f, 0.f, 0.f);
+        if (r.active) st3(a.out + 3 * r.t, n);
+    }
+}
+
+// average mode: gs = the gradient of the vertex's sum of face normals
+struct StoreSumGrad {
+    const NormalsArgs& a;
+    __device__ __forceinline__ void operator()(const Row& r, float3 s) const
     {
-        const int f = i % a.F;
-        const Corners c = corners(a, b, f);
-        return normalise(cross3(c.e1, c.e2));
+        st3(a.gs + 3 * r.t, normalise_grad(s, ld3(a.grad + 3 * r.t)));
     }
 };
 
@@ -266,79 +393,12 @@ struct CornerGrad {
                 gu = add3(gu, ld3(a.grad + 3 * row));
         }
         const float3 gn = normalise_grad(cross3(c.e1, c.e2), gu);
-        const float3 g1 = cross3(c.e2, gn), g2 = cross3(gn, c.e1);   // d/d e1, d/d e2
+        const float3 g1 = cross3(c.e2, gn), g2 = cross3(gn, c.e1);
         if (k == 1) return g1;
         if (k == 2) return g2;
         return make_float3(-__fadd_rn(g1.x, g2.x), -__fadd_rn(g1.y, g2.y), -__fadd_rn(g1.z, g2.z));
     }
 };
-
-// The threads of a warp take consecutive (item, vertex) rows t = b*V + v; the loop is warp-uniform.
-#define FOR_EACH_ROW(a)                                                                                                \
-    for (long long t0 = (long long)blockIdx.x * NORMALS_THREADS + (threadIdx.x & ~31); t0 < (a).total;               \
-         t0 += (long long)gridDim.x * NORMALS_THREADS)
-
-struct Row {
-    long long t, b;
-    int lo, hi;
-    bool active;
-};
-
-__device__ __forceinline__ Row row_of(const NormalsArgs& a, long long t0)
-{
-    Row r;
-    r.t = t0 + (threadIdx.x & 31);
-    r.active = r.t < a.total;
-    r.b = r.active ? r.t / a.V : 0;
-    const long long v = r.t - r.b * a.V;
-    r.lo = r.hi = 0;
-    if (r.active) {
-        r.lo = __ldg(a.offsets + v);
-        r.hi = __ldg(a.offsets + v + 1);
-    }
-    return r;
-}
-
-template <int MODE>
-__global__ void __launch_bounds__(NORMALS_THREADS) normals_forward_kernel(NormalsArgs a)
-{
-    FOR_EACH_ROW(a) {
-        const Row r = row_of(a, t0);
-        float3 n;
-        if (MODE == DIRT_NORMALS_AVERAGE) {
-            n = normalise(row_sum(a.inc, r.lo, r.hi, r.b, FaceUnit{a}));
-        } else {
-            n = r.hi > r.lo ? FaceUnit{a}(r.b, __ldg(a.inc + r.hi - 1)) : make_float3(0.f, 0.f, 0.f);
-        }
-        if (r.active) st3(a.out + 3 * r.t, n);
-    }
-}
-
-// average mode: gs = the gradient of the vertex's sum of face normals
-__global__ void __launch_bounds__(NORMALS_THREADS) normals_sum_grad_kernel(NormalsArgs a)
-{
-    FOR_EACH_ROW(a) {
-        const Row r = row_of(a, t0);
-        const float3 s = row_sum(a.inc, r.lo, r.hi, r.b, FaceUnit{a});
-        if (r.active) st3(a.gs + 3 * r.t, normalise_grad(s, ld3(a.grad + 3 * r.t)));
-    }
-}
-
-template <int MODE>
-__global__ void __launch_bounds__(NORMALS_THREADS) normals_position_grad_kernel(NormalsArgs a)
-{
-    FOR_EACH_ROW(a) {
-        const Row r = row_of(a, t0);
-        const float3 g = row_sum(a.inc, r.lo, r.hi, r.b, CornerGrad<MODE>{a});
-        if (r.active) st3(a.g_vertices + 3 * r.t, g);
-    }
-}
-
-inline unsigned blocks_for(long long n)
-{
-    const long long b = (n + NORMALS_THREADS - 1) / NORMALS_THREADS;
-    return (unsigned)(b < 1 ? 1 : (b < MAX_BLOCKS ? b : MAX_BLOCKS));
-}
 
 // ---- the vertex tangents (DESIGN.md §7.14) ------------------------------------------------------------------------------
 //
@@ -422,31 +482,11 @@ struct TangentCornerGrad {
         const float3 g1 = scale3(gy, u.dv2), g2 = scale3(gy, -u.dv1);   // d/d e1, d/d e2
         const float gdv2 = dot3(gy, u.c.e1), gdv1 = -dot3(gy, u.c.e2);
         Frame g = zero_of(Frame());
-        if (k == 1) {
-            g.t = g1;
-            g.b.y = gdv1;
-        } else if (k == 2) {
-            g.t = g2;
-            g.b.y = gdv2;
-        } else {
-            g.t = make_float3(-__fadd_rn(g1.x, g2.x), -__fadd_rn(g1.y, g2.y), -__fadd_rn(g1.z, g2.z));
-            g.b.y = -__fadd_rn(gdv1, gdv2);
-        }
+        g.t = corner_share(k, g1, g2);
+        g.b.y = corner_share(k, gdv1, gdv2);
         return g;
     }
 };
-
-// A row with no incidences (F = 0: there is no adjacency to read)
-__device__ __forceinline__ Row tangent_row(const TangentArgs& a, long long t0)
-{
-    if (a.m.F) return row_of(a.m, t0);
-    Row r;
-    r.t = t0 + (threadIdx.x & 31);
-    r.active = r.t < a.m.total;
-    r.b = 0;
-    r.lo = r.hi = 0;
-    return r;
-}
 
 // n = unit(normal), x = t - (n . t) n: the vector T normalises
 struct Gram {
@@ -457,34 +497,29 @@ struct Gram {
 __device__ __forceinline__ Gram gram(const TangentArgs& a, const Row& r, float3 t)
 {
     Gram g;
-    g.n = r.active ? normalise(ld3(a.normals + r.t * a.normal_stride)) : make_float3(0.f, 0.f, 0.f);
+    g.n = normalise(ld3(a.normals + r.t * a.normal_stride));
     g.d = dot3(g.n, t);
     g.x = sub3(t, scale3(g.n, g.d));
     return g;
 }
 
-__global__ void __launch_bounds__(NORMALS_THREADS) tangents_forward_kernel(TangentArgs a)
-{
-    FOR_EACH_ROW(a.m) {
-        const Row r = tangent_row(a, t0);
-        const Frame s = row_sum(a.m.inc, r.lo, r.hi, r.b, FaceFrame{a});
+struct StoreTangent {
+    const TangentArgs& a;
+    __device__ __forceinline__ void operator()(const Row& r, Frame s) const
+    {
         const Gram g = gram(a, r, s.t);
         const float3 T = normalise(g.x);
         const float w = dot3(cross3(g.n, T), s.b) < 0.f ? -1.f : 1.f;
-        if (r.active) {
-            st3(a.out + 4 * r.t, T);
-            a.out[4 * r.t + 3] = w;
-        }
+        st3(a.out + 4 * r.t, T);
+        a.out[4 * r.t + 3] = w;
     }
-}
+};
 
 // gt = the gradient of the vertex's sum of face tangents; grad_normals, which is local to the vertex
-__global__ void __launch_bounds__(NORMALS_THREADS) tangents_vertex_grad_kernel(TangentArgs a)
-{
-    FOR_EACH_ROW(a.m) {
-        const Row r = tangent_row(a, t0);
-        const float3 t = row_sum(a.m.inc, r.lo, r.hi, r.b, FaceTangent{a});
-        if (!r.active) continue;
+struct TangentVertexGrad {
+    const TangentArgs& a;
+    __device__ __forceinline__ void operator()(const Row& r, float3 t) const
+    {
         const Gram g = gram(a, r, t);
         const float3 gx = normalise_grad(g.x, ld3(a.grad + 4 * r.t));
         const float gxn = dot3(gx, g.n);
@@ -495,21 +530,19 @@ __global__ void __launch_bounds__(NORMALS_THREADS) tangents_vertex_grad_kernel(T
             st3(a.g_normals + 3 * r.t, normalise_grad(ld3(a.normals + r.t * a.normal_stride), gn));
         }
     }
-}
+};
 
-__global__ void __launch_bounds__(NORMALS_THREADS) tangents_corner_grad_kernel(TangentArgs a)
-{
-    FOR_EACH_ROW(a.m) {
-        const Row r = tangent_row(a, t0);
-        const Frame g = row_sum(a.m.inc, r.lo, r.hi, r.b, TangentCornerGrad{a});
-        if (!r.active) continue;
+struct StoreTangentCornerGrad {
+    const TangentArgs& a;
+    __device__ __forceinline__ void operator()(const Row& r, Frame g) const
+    {
         if (a.g_vertices) st3(a.g_vertices + 3 * r.t, g.t);
         if (a.g_uvs) {
             a.g_uvs[2 * r.t] = 0.f;
             a.g_uvs[2 * r.t + 1] = g.b.y;
         }
     }
-}
+};
 
 // ---- the mesh Laplacian (DESIGN.md §7.16) ---------------------------------------------------------------------------------
 //
@@ -529,11 +562,9 @@ __device__ __forceinline__ Wedge wedge(const NormalsArgs& a, long long b, int i)
     const int k = i / a.F, f = i - k * a.F;
     Wedge w;
     w.v[0] = __ldg(a.faces + 3ll * f + k);
-    w.v[1] = __ldg(a.faces + 3ll * f + (k == 2 ? 0 : k + 1));
-    w.v[2] = __ldg(a.faces + 3ll * f + (k == 0 ? 2 : k - 1));
-    const float* base = a.vertices + b * a.V * a.stride;
-    const float3 q0 = ld3(base + w.v[0] * a.stride), q1 = ld3(base + w.v[1] * a.stride);
-    const float3 q2 = ld3(base + w.v[2] * a.stride);
+    w.v[1] = __ldg(a.faces + 3ll * f + next3(k));
+    w.v[2] = __ldg(a.faces + 3ll * f + prev3(k));
+    const float3 q0 = position(a, b, w.v[0]), q1 = position(a, b, w.v[1]), q2 = position(a, b, w.v[2]);
     w.e01 = sub3(q1, q0);
     w.e02 = sub3(q2, q0);
     w.e12 = sub3(q2, q1);
@@ -577,19 +608,13 @@ struct LaplacianTerm {
 
 __device__ __forceinline__ float3 xyz(float4 a) { return make_float3(a.x, a.y, a.z); }
 
-// The workspace's gradient region holds (g_S, g_D) of row t at gs + 4t, four floats read and written one at a time:
-// the C ABI asks the workspace for 4-byte alignment only.
-
-template <int MODE>
-__global__ void __launch_bounds__(NORMALS_THREADS) laplacian_forward_kernel(NormalsArgs a)
-{
-    FOR_EACH_ROW(a) {
-        const Row r = row_of(a, t0);
-        const float4 s = row_sum(a.inc, r.lo, r.hi, r.b, LaplacianTerm<MODE>{a});
-        const float d = __fadd_rn(s.w, 1.e-12f);
-        if (r.active) st3(a.out + 3 * r.t, make_float3(__fdiv_rn(s.x, d), __fdiv_rn(s.y, d), __fdiv_rn(s.z, d)));
+struct StoreLaplacian {
+    const NormalsArgs& a;
+    __device__ __forceinline__ void operator()(const Row& r, float4 s) const
+    {
+        st3(a.out + 3 * r.t, div3(xyz(s), __fadd_rn(s.w, 1.e-12f)));
     }
-}
+};
 
 // D_u + 1e-12 of the uniform mode, from the length of u's row
 __device__ __forceinline__ float uniform_den(const NormalsArgs& a, int u)
@@ -609,42 +634,38 @@ struct UniformNeighbourGrad {
         for (int j = 0; j < 3; ++j) {
             if (j == k) continue;
             const int u = __ldg(a.faces + 3ll * f + j);
-            const float3 gu = ld3(a.grad + 3 * (b * a.V + u));
-            const float d = uniform_den(a, u);
-            g = add3(g, make_float3(__fdiv_rn(gu.x, d), __fdiv_rn(gu.y, d), __fdiv_rn(gu.z, d)));
+            g = add3(g, div3(ld3(a.grad + 3 * (b * a.V + u)), uniform_den(a, u)));
         }
         return g;
     }
 };
 
 // uniform: the neighbours' terms, then vertex j's own -D_j p_j in S_j
-__global__ void __launch_bounds__(NORMALS_THREADS) laplacian_uniform_grad_kernel(NormalsArgs a)
-{
-    FOR_EACH_ROW(a) {
-        const Row r = row_of(a, t0);
-        const float3 s = row_sum(a.inc, r.lo, r.hi, r.b, UniformNeighbourGrad{a});
-        if (!r.active) continue;
-        const float D = 2.f * (float)(r.hi - r.lo), d = __fadd_rn(D, 1.e-12f);
-        const float3 g = ld3(a.grad + 3 * r.t);
-        const float3 gs = make_float3(__fdiv_rn(g.x, d), __fdiv_rn(g.y, d), __fdiv_rn(g.z, d));
+struct UniformGrad {
+    const NormalsArgs& a;
+    __device__ __forceinline__ void operator()(const Row& r, float3 s) const
+    {
+        const float D = 2.f * (float)(r.hi - r.lo);
+        const float3 gs = div3(ld3(a.grad + 3 * r.t), __fadd_rn(D, 1.e-12f));
         st3(a.g_vertices + 3 * r.t, sub3(s, scale3(gs, D)));
     }
-}
+};
+
+// The workspace's gradient region holds (g_S, g_D) of row t at gs + 4t, four floats read and written one at a time:
+// the C ABI asks the workspace for 4-byte alignment only.
 
 // cotangent, pass 1: gs[t] = (g_S, g_D) of vertex t, g_S = g / (D + 1e-12) and g_D = -(g . S) / (D + 1e-12)^2
-__global__ void __launch_bounds__(NORMALS_THREADS) laplacian_sum_grad_kernel(NormalsArgs a)
-{
-    FOR_EACH_ROW(a) {
-        const Row r = row_of(a, t0);
-        const float4 s = row_sum(a.inc, r.lo, r.hi, r.b, LaplacianTerm<DIRT_LAPLACIAN_COTANGENT>{a});
-        if (!r.active) continue;
+struct LaplacianSumGrad {
+    const NormalsArgs& a;
+    __device__ __forceinline__ void operator()(const Row& r, float4 s) const
+    {
         const float3 g = ld3(a.grad + 3 * r.t);
         const float d = __fadd_rn(s.w, 1.e-12f);
         const float gd = -__fdiv_rn(dot3(g, xyz(s)), __fmul_rn(d, d));
-        st3(a.gs + 4 * r.t, make_float3(__fdiv_rn(g.x, d), __fdiv_rn(g.y, d), __fdiv_rn(g.z, d)));
+        st3(a.gs + 4 * r.t, div3(g, d));
         a.gs[4 * r.t + 3] = gd;
     }
-}
+};
 
 // cotangent, pass 2: the gradient to q0 of the face's sum over its corners m of g_S(m) . S_m + g_D(m) |n| / 3, where
 // S_m is corner m's term.  Grouped by cotangent, that sum is sum_j c_j w_j + (sum_m g_D(m)) |n| / 3 with
@@ -670,31 +691,12 @@ struct CotangentCornerGrad {
     }
 };
 
-__global__ void __launch_bounds__(NORMALS_THREADS) laplacian_cotangent_grad_kernel(NormalsArgs a)
-{
-    FOR_EACH_ROW(a) {
-        const Row r = row_of(a, t0);
-        const float3 g = row_sum(a.inc, r.lo, r.hi, r.b, CotangentCornerGrad{a});
-        if (r.active) st3(a.g_vertices + 3 * r.t, g);
-    }
-}
-
 // ---- edge lengths and normal consistency (DESIGN.md §7.17) ----------------------------------------------------------------
 //
 // One value per face edge, [B*F, 3]: edge k of face f joins v_k to v_{k+1 mod 3}.  Edge length: |p_{k+1} - p_k|.  Normal
 // consistency: 1 - u_f . (sum of u_g over P) / |P|, P the valid faces other than f that name both ends (each once), 0
 // when P is empty or the ends are one vertex.  The face passes are one thread per (item, face); the vertex passes are
-// the normals' gather.  a.grad is grad_out [B*F, 3]; a.gs the consistency backward's dL/dn_f [B*F, 3].
-
-__device__ __forceinline__ int next3(int k) { return k == 2 ? 0 : k + 1; }
-
-// u_g of item b for the face with vertices v
-__device__ __forceinline__ float3 unit_of(const NormalsArgs& a, long long b, const int v[3])
-{
-    const float* base = a.vertices + b * a.V * a.stride;
-    const float3 p0 = ld3(base + v[0] * a.stride);
-    return normalise(cross3(sub3(ld3(base + v[1] * a.stride), p0), sub3(ld3(base + v[2] * a.stride), p0)));
-}
+// row passes.  a.grad is grad_out [B*F, 3]; a.gs the consistency backward's dL/dn_f [B*F, 3].
 
 // Calls visit(g, v) for every valid face g != f that names both x and y (x != y), once per face, and returns how many.
 // It scans the shorter of the two rows (the row of the smaller vertex id when they are equally long) in row order, and
@@ -719,11 +721,6 @@ __device__ __forceinline__ int for_each_partner(const NormalsArgs& a, int f, int
         ++n;
     }
     return n;
-}
-
-__device__ __forceinline__ float3 div3(float3 a, float d)
-{
-    return make_float3(__fdiv_rn(a.x, d), __fdiv_rn(a.y, d), __fdiv_rn(a.z, d));
 }
 
 // whether edges j and k of the face with vertices v join the same unordered pair
@@ -752,21 +749,20 @@ __global__ void __launch_bounds__(NORMALS_THREADS) edge_terms_forward_kernel(Nor
         int v[3];
         float o[3] = {0.f, 0.f, 0.f};
         if (load_face(a.faces, f, a.V, v)) {
-            const float* base = a.vertices + b * a.V * a.stride;
             if (MODE == DIRT_EDGE_LENGTH) {
 #pragma unroll
                 for (int k = 0; k < 3; ++k) {
-                    const float3 d = sub3(ld3(base + v[next3(k)] * a.stride), ld3(base + v[k] * a.stride));
+                    const float3 d = sub3(position(a, b, v[next3(k)]), position(a, b, v[k]));
                     o[k] = __fsqrt_rn(dot3(d, d));
                 }
             } else {
-                const float3 u = unit_of(a, b, v);
+                const float3 u = unit_of(corners_of(a, b, v));
 #pragma unroll
                 for (int k = 0; k < 3; ++k) {
                     if (v[k] == v[next3(k)]) continue;
                     float3 s = make_float3(0.f, 0.f, 0.f);
                     const int c = for_each_partner(a, f, v[k], v[next3(k)],
-                                                   [&](int, const int w[3]) { s = add3(s, unit_of(a, b, w)); });
+                                                   [&](int, const int w[3]) { s = add3(s, unit_of(corners_of(a, b, w))); });
                     if (c) o[k] = __fsub_rn(1.f, __fdiv_rn(dot3(u, s), (float)c));
                 }
             }
@@ -788,20 +784,11 @@ struct EdgeLengthCornerGrad {
         const float* G = a.grad + 3 * (b * a.F + f);
         const float l1 = __fsqrt_rn(dot3(w.e01, w.e01)), l2 = __fsqrt_rn(dot3(w.e02, w.e02));
         const float k1 = l1 == 0.f ? 0.f : __fdiv_rn(__ldg(G + k), l1);
-        const float k2 = l2 == 0.f ? 0.f : __fdiv_rn(__ldg(G + (k == 0 ? 2 : k - 1)), l2);
+        const float k2 = l2 == 0.f ? 0.f : __fdiv_rn(__ldg(G + prev3(k)), l2);
         const float3 g = add3(scale3(w.e01, k1), scale3(w.e02, k2));
         return make_float3(-g.x, -g.y, -g.z);
     }
 };
-
-__global__ void __launch_bounds__(NORMALS_THREADS) edge_length_grad_kernel(NormalsArgs a)
-{
-    FOR_EACH_ROW(a) {
-        const Row r = row_of(a, t0);
-        const float3 g = row_sum(a.inc, r.lo, r.hi, r.b, EdgeLengthCornerGrad{a});
-        if (r.active) st3(a.g_vertices + 3 * r.t, g);
-    }
-}
 
 // Normal consistency, pass 1: dL/dn_f of each valid face into gs.  dL/du_f is, over each distinct unordered pair {x, y}
 // of f's edges with x != y and |P| > 0, -(G_f s + sum over P of G_g u_g) / |P|, where s = the sum of u_g over P and G_f,
@@ -816,9 +803,8 @@ __global__ void __launch_bounds__(NORMALS_THREADS) consistency_face_grad_kernel(
         const int f = (int)(t - b * a.F);
         int v[3];
         if (!load_face(a.faces, f, a.V, v)) continue;
-        const float* base = a.vertices + b * a.V * a.stride;
-        const float3 p0 = ld3(base + v[0] * a.stride);
-        const float3 nf = cross3(sub3(ld3(base + v[1] * a.stride), p0), sub3(ld3(base + v[2] * a.stride), p0));
+        const Corners fc = corners_of(a, b, v);
+        const float3 nf = cross3(fc.e1, fc.e2);
         const float3 uf = normalise(nf);
         float3 gu = make_float3(0.f, 0.f, 0.f);
         float beta = 0.f;
@@ -829,7 +815,7 @@ __global__ void __launch_bounds__(NORMALS_THREADS) consistency_face_grad_kernel(
             float3 s = make_float3(0.f, 0.f, 0.f), sg = s;
             float gsum = 0.f;
             const int c = for_each_partner(a, f, x, y, [&](int g, const int w[3]) {
-                const float3 du = sub3(unit_of(a, b, w), uf);
+                const float3 du = sub3(unit_of(corners_of(a, b, w)), uf);
                 const float G = pair_grad(a, b, g, w, x, y);
                 s = add3(s, du);
                 sg = add3(sg, scale3(du, G));
@@ -847,28 +833,48 @@ __global__ void __launch_bounds__(NORMALS_THREADS) consistency_face_grad_kernel(
     }
 }
 
-// Normal consistency, pass 2: the gradient of corner k of the face of incidence i through n = e1 x e2, as CornerGrad.
+// Normal consistency, pass 2: the gradient of corner k of the face of incidence i through n = e1 x e2.
 struct ConsistencyCornerGrad {
     const NormalsArgs& a;
     __device__ __forceinline__ float3 operator()(long long b, int i) const
     {
         const int k = i / a.F, f = i - k * a.F;
-        const Corners c = corners(a, b, f);
-        const float3 gn = ld3(a.gs + 3 * (b * a.F + f));
-        const float3 g1 = cross3(c.e2, gn), g2 = cross3(gn, c.e1);   // d/d e1, d/d e2
-        if (k == 1) return g1;
-        if (k == 2) return g2;
-        return make_float3(-__fadd_rn(g1.x, g2.x), -__fadd_rn(g1.y, g2.y), -__fadd_rn(g1.z, g2.z));
+        return cross_grad(corners(a, b, f), ld3(a.gs + 3 * (b * a.F + f)), k);
     }
 };
 
-__global__ void __launch_bounds__(NORMALS_THREADS) consistency_vertex_grad_kernel(NormalsArgs a)
+inline unsigned blocks_for(long long n)
 {
-    FOR_EACH_ROW(a) {
-        const Row r = row_of(a, t0);
-        const float3 g = row_sum(a.inc, r.lo, r.hi, r.b, ConsistencyCornerGrad{a});
-        if (r.active) st3(a.g_vertices + 3 * r.t, g);
-    }
+    const long long b = (n + NORMALS_THREADS - 1) / NORMALS_THREADS;
+    return (unsigned)(b < 1 ? 1 : (b < MAX_BLOCKS ? b : MAX_BLOCKS));
+}
+
+// A grid-stride kernel over n threads' worth of work, and its launch check.
+template <class... P, class... A>
+cudaError_t launch(void (*kernel)(P...), long long n, cudaStream_t stream, const A&... args)
+{
+    kernel<<<blocks_for(n), NORMALS_THREADS, 0, stream>>>(args...);
+    return launched();
+}
+
+template <class Term, class Finish, class Args>
+cudaError_t launch_rows(const Args& a, cudaStream_t stream)
+{
+    return launch(row_pass_kernel<Term, Finish, Args>, total_of(a), stream, a);
+}
+
+// The workspace's adjacency and gradient region, attached to the passes' arguments.
+NormalsArgs attach(NormalsArgs a, const NormalsWorkspace& w)
+{
+    a.offsets = w.offsets;
+    a.inc = w.inc;
+    a.gs = w.gs;
+    return a;
+}
+
+cudaError_t build_adjacency(const NormalsArgs& a, const NormalsWorkspace& w, cudaStream_t stream)
+{
+    return launch_corner_adjacency(a.faces, 0, 1, a.V, a.F, w.counts, w.offsets, w.unsorted, w.inc, stream);
 }
 
 }  // namespace
@@ -902,61 +908,85 @@ cudaError_t launch_corner_adjacency(const int* faces, long long face_stride, int
     cudaError_t e;
     const long long rows = (long long)items * V, corners = 3ll * items * F;
     if ((e = cudaMemsetAsync(counts, 0, sizeof(int) * (size_t)rows, stream)) != cudaSuccess) return e;
-    count_kernel<<<blocks_for(corners / 3), NORMALS_THREADS, 0, stream>>>(faces, face_stride, items, F, V, counts);
-    if ((e = launched()) != cudaSuccess) return e;
+    if ((e = launch(count_kernel, corners / 3, stream, faces, face_stride, items, F, V, counts)) != cudaSuccess) return e;
     scan_kernel<<<1, SCAN_THREADS, 0, stream>>>(counts, rows, offsets);
     if ((e = launched()) != cudaSuccess) return e;
-    fill_kernel<<<blocks_for(corners / 3), NORMALS_THREADS, 0, stream>>>(faces, face_stride, items, F, V, offsets, counts, unsorted);
-    if ((e = launched()) != cudaSuccess) return e;
-    rank_kernel<<<blocks_for(corners), NORMALS_THREADS, 0, stream>>>(faces, face_stride, items, F, offsets, unsorted, inc, V);
-    return launched();
+    if ((e = launch(fill_kernel, corners / 3, stream, faces, face_stride, items, F, V, offsets, counts, unsorted)) != cudaSuccess)
+        return e;
+    return launch(rank_kernel, corners, stream, faces, face_stride, items, F, offsets, unsorted, inc, V);
 }
 
-cudaError_t launch_normals_forward(NormalsArgs a, const NormalsWorkspace& w, cudaStream_t stream)
+// ---- the mesh ops on NormalsArgs --------------------------------------------------------------------------------------
+
+cudaError_t launch_mesh_forward(MeshPasses passes, NormalsArgs a, const NormalsWorkspace& w, cudaStream_t stream)
 {
     cudaError_t e;
     if (a.total == 0) return cudaSuccess;
     if (a.F == 0) return cudaMemsetAsync(a.out, 0, sizeof(float) * 3 * (size_t)a.total, stream);
-    if ((e = launch_corner_adjacency(a.faces, 0, 1, a.V, a.F, w.counts, w.offsets, w.unsorted, w.inc, stream)) != cudaSuccess)
-        return e;
-    a.offsets = w.offsets;
-    a.inc = w.inc;
-    if (a.mode == DIRT_NORMALS_AVERAGE)
-        normals_forward_kernel<DIRT_NORMALS_AVERAGE><<<blocks_for(a.total), NORMALS_THREADS, 0, stream>>>(a);
-    else
-        normals_forward_kernel<DIRT_NORMALS_PRE_SPLIT><<<blocks_for(a.total), NORMALS_THREADS, 0, stream>>>(a);
-    return launched();
+    if ((e = build_adjacency(a, w, stream)) != cudaSuccess) return e;
+    return passes(attach(a, w), stream);
 }
 
-cudaError_t launch_normals_backward(NormalsArgs a, const NormalsWorkspace& w, cudaStream_t stream)
+cudaError_t launch_mesh_backward(MeshPasses passes, NormalsArgs a, const NormalsWorkspace& w, cudaStream_t stream)
 {
-    cudaError_t e;
     if (a.total == 0) return cudaSuccess;
     if (a.F == 0) return cudaMemsetAsync(a.g_vertices, 0, sizeof(float) * 3 * (size_t)a.total, stream);
-    a.offsets = w.offsets;
-    a.inc = w.inc;
-    a.gs = w.gs;
-    if (a.mode == DIRT_NORMALS_AVERAGE) {
-        normals_sum_grad_kernel<<<blocks_for(a.total), NORMALS_THREADS, 0, stream>>>(a);
-        if ((e = launched()) != cudaSuccess) return e;
-        normals_position_grad_kernel<DIRT_NORMALS_AVERAGE><<<blocks_for(a.total), NORMALS_THREADS, 0, stream>>>(a);
-    } else {
-        normals_position_grad_kernel<DIRT_NORMALS_PRE_SPLIT><<<blocks_for(a.total), NORMALS_THREADS, 0, stream>>>(a);
-    }
-    return launched();
+    return passes(attach(a, w), stream);
 }
+
+cudaError_t normals_forward_passes(const NormalsArgs& a, cudaStream_t stream)
+{
+    if (a.mode == DIRT_NORMALS_AVERAGE) return launch_rows<FaceUnit, StoreNormal>(a, stream);
+    return launch(normals_pre_split_kernel, a.total, stream, a);
+}
+
+cudaError_t normals_backward_passes(const NormalsArgs& a, cudaStream_t stream)
+{
+    cudaError_t e;
+    if (a.mode == DIRT_NORMALS_PRE_SPLIT) return launch_rows<CornerGrad<DIRT_NORMALS_PRE_SPLIT>, StoreGrad>(a, stream);
+    if ((e = launch_rows<FaceUnit, StoreSumGrad>(a, stream)) != cudaSuccess) return e;
+    return launch_rows<CornerGrad<DIRT_NORMALS_AVERAGE>, StoreGrad>(a, stream);
+}
+
+cudaError_t laplacian_forward_passes(const NormalsArgs& a, cudaStream_t stream)
+{
+    if (a.mode == DIRT_LAPLACIAN_UNIFORM) return launch_rows<LaplacianTerm<DIRT_LAPLACIAN_UNIFORM>, StoreLaplacian>(a, stream);
+    return launch_rows<LaplacianTerm<DIRT_LAPLACIAN_COTANGENT>, StoreLaplacian>(a, stream);
+}
+
+cudaError_t laplacian_backward_passes(const NormalsArgs& a, cudaStream_t stream)
+{
+    cudaError_t e;
+    if (a.mode == DIRT_LAPLACIAN_UNIFORM) return launch_rows<UniformNeighbourGrad, UniformGrad>(a, stream);
+    if ((e = launch_rows<LaplacianTerm<DIRT_LAPLACIAN_COTANGENT>, LaplacianSumGrad>(a, stream)) != cudaSuccess) return e;
+    return launch_rows<CotangentCornerGrad, StoreGrad>(a, stream);
+}
+
+cudaError_t edge_terms_forward_passes(const NormalsArgs& a, cudaStream_t stream)
+{
+    const long long n = a.total / a.V * a.F;
+    if (a.mode == DIRT_EDGE_LENGTH) return launch(edge_terms_forward_kernel<DIRT_EDGE_LENGTH>, n, stream, a, n);
+    return launch(edge_terms_forward_kernel<DIRT_NORMAL_CONSISTENCY>, n, stream, a, n);
+}
+
+cudaError_t edge_terms_backward_passes(const NormalsArgs& a, cudaStream_t stream)
+{
+    cudaError_t e;
+    const long long n = a.total / a.V * a.F;
+    if (a.mode == DIRT_EDGE_LENGTH) return launch_rows<EdgeLengthCornerGrad, StoreGrad>(a, stream);
+    if ((e = launch(consistency_face_grad_kernel, n, stream, a, n)) != cudaSuccess) return e;
+    return launch_rows<ConsistencyCornerGrad, StoreGrad>(a, stream);
+}
+
+// ---- the vertex tangents ------------------------------------------------------------------------------------------------
 
 cudaError_t launch_tangents_forward(TangentArgs a, const NormalsWorkspace& w, cudaStream_t stream)
 {
     cudaError_t e;
     if (a.m.total == 0) return cudaSuccess;
-    if (a.m.F > 0 &&
-        (e = launch_corner_adjacency(a.m.faces, 0, 1, a.m.V, a.m.F, w.counts, w.offsets, w.unsorted, w.inc, stream)) != cudaSuccess)
-        return e;
-    a.m.offsets = w.offsets;
-    a.m.inc = w.inc;
-    tangents_forward_kernel<<<blocks_for(a.m.total), NORMALS_THREADS, 0, stream>>>(a);
-    return launched();
+    if (a.m.F > 0 && (e = build_adjacency(a.m, w, stream)) != cudaSuccess) return e;
+    a.m = attach(a.m, w);
+    return launch_rows<FaceFrame, StoreTangent>(a, stream);   // with no faces every row is empty
 }
 
 cudaError_t launch_tangents_backward(TangentArgs a, const NormalsWorkspace& w, cudaStream_t stream)
@@ -973,82 +1003,10 @@ cudaError_t launch_tangents_backward(TangentArgs a, const NormalsWorkspace& w, c
     }
     const bool corner = a.g_vertices || a.g_uvs;
     if (!corner && !a.g_normals) return cudaSuccess;
-    a.m.offsets = w.offsets;
-    a.m.inc = w.inc;
+    a.m = attach(a.m, w);
     a.gt = corner ? w.gs : nullptr;
-    tangents_vertex_grad_kernel<<<blocks_for(a.m.total), NORMALS_THREADS, 0, stream>>>(a);
-    if ((e = launched()) != cudaSuccess) return e;
-    if (corner) {
-        tangents_corner_grad_kernel<<<blocks_for(a.m.total), NORMALS_THREADS, 0, stream>>>(a);
-        if ((e = launched()) != cudaSuccess) return e;
-    }
-    return cudaSuccess;
-}
-
-cudaError_t launch_laplacian_forward(NormalsArgs a, const NormalsWorkspace& w, cudaStream_t stream)
-{
-    cudaError_t e;
-    if (a.total == 0) return cudaSuccess;
-    if (a.F == 0) return cudaMemsetAsync(a.out, 0, sizeof(float) * 3 * (size_t)a.total, stream);
-    if ((e = launch_corner_adjacency(a.faces, 0, 1, a.V, a.F, w.counts, w.offsets, w.unsorted, w.inc, stream)) != cudaSuccess)
-        return e;
-    a.offsets = w.offsets;
-    a.inc = w.inc;
-    if (a.mode == DIRT_LAPLACIAN_UNIFORM)
-        laplacian_forward_kernel<DIRT_LAPLACIAN_UNIFORM><<<blocks_for(a.total), NORMALS_THREADS, 0, stream>>>(a);
-    else
-        laplacian_forward_kernel<DIRT_LAPLACIAN_COTANGENT><<<blocks_for(a.total), NORMALS_THREADS, 0, stream>>>(a);
-    return launched();
-}
-
-cudaError_t launch_laplacian_backward(NormalsArgs a, const NormalsWorkspace& w, cudaStream_t stream)
-{
-    cudaError_t e;
-    if (a.total == 0) return cudaSuccess;
-    if (a.F == 0) return cudaMemsetAsync(a.g_vertices, 0, sizeof(float) * 3 * (size_t)a.total, stream);
-    a.offsets = w.offsets;
-    a.inc = w.inc;
-    a.gs = w.gs;
-    if (a.mode == DIRT_LAPLACIAN_UNIFORM) {
-        laplacian_uniform_grad_kernel<<<blocks_for(a.total), NORMALS_THREADS, 0, stream>>>(a);
-    } else {
-        laplacian_sum_grad_kernel<<<blocks_for(a.total), NORMALS_THREADS, 0, stream>>>(a);
-        if ((e = launched()) != cudaSuccess) return e;
-        laplacian_cotangent_grad_kernel<<<blocks_for(a.total), NORMALS_THREADS, 0, stream>>>(a);
-    }
-    return launched();
-}
-
-cudaError_t launch_edge_terms_forward(NormalsArgs a, const NormalsWorkspace& w, cudaStream_t stream)
-{
-    cudaError_t e;
-    const long long n = a.total / a.V * a.F;
-    if ((e = launch_corner_adjacency(a.faces, 0, 1, a.V, a.F, w.counts, w.offsets, w.unsorted, w.inc, stream)) != cudaSuccess)
-        return e;
-    a.offsets = w.offsets;
-    a.inc = w.inc;
-    if (a.mode == DIRT_EDGE_LENGTH)
-        edge_terms_forward_kernel<DIRT_EDGE_LENGTH><<<blocks_for(n), NORMALS_THREADS, 0, stream>>>(a, n);
-    else
-        edge_terms_forward_kernel<DIRT_NORMAL_CONSISTENCY><<<blocks_for(n), NORMALS_THREADS, 0, stream>>>(a, n);
-    return launched();
-}
-
-cudaError_t launch_edge_terms_backward(NormalsArgs a, const NormalsWorkspace& w, cudaStream_t stream)
-{
-    cudaError_t e;
-    a.offsets = w.offsets;
-    a.inc = w.inc;
-    a.gs = w.gs;
-    if (a.mode == DIRT_EDGE_LENGTH) {
-        edge_length_grad_kernel<<<blocks_for(a.total), NORMALS_THREADS, 0, stream>>>(a);
-    } else {
-        const long long n = a.total / a.V * a.F;
-        consistency_face_grad_kernel<<<blocks_for(n), NORMALS_THREADS, 0, stream>>>(a, n);
-        if ((e = launched()) != cudaSuccess) return e;
-        consistency_vertex_grad_kernel<<<blocks_for(a.total), NORMALS_THREADS, 0, stream>>>(a);
-    }
-    return launched();
+    if ((e = launch_rows<FaceTangent, TangentVertexGrad>(a, stream)) != cudaSuccess) return e;
+    return corner ? launch_rows<TangentCornerGrad, StoreTangentCornerGrad>(a, stream) : cudaSuccess;
 }
 
 }  // namespace dirt

@@ -66,20 +66,14 @@ def vertex_normals(vertices, faces, name=None):
     (dirt/lighting.py:34-93).  vertices [*,V,3|4], faces [F,3] -> [*,V,3].  On CUDA in the shapes `normals_route`
     accepts, kernels compute it (a face with an index outside [0, V) is then left out); any other call runs the torch
     restatement."""
-    route = _normals_route(vertices, faces)
-    if route is None:
-        return _vertex_normals(vertices, faces)
-    return _mesh(_NORMALS, route, faces, _point_rows(vertices[..., :3], 3))
+    return _routed(_NORMALS, _vertex_normals, vertices, faces, _normals_route, _mesh)
 
 
 def vertex_normals_pre_split(vertices, faces, name=None, static=False):
     """As `vertex_normals` for meshes where every vertex belongs to exactly one face
     (dirt/lighting.py:101-133): each vertex takes the unit normal of its face (of its last face corner, corner-major,
     when there are several).  Routed as `vertex_normals`."""
-    route = _normals_route(vertices, faces)
-    if route is None:
-        return _vertex_normals_pre_split(vertices, faces)
-    return _mesh(_NORMALS_PRE_SPLIT, route, faces, _point_rows(vertices[..., :3], 3))
+    return _routed(_NORMALS_PRE_SPLIT, _vertex_normals_pre_split, vertices, faces, _normals_route, _mesh)
 
 
 def split_vertices_by_face(vertices, faces, name=None):
@@ -792,20 +786,32 @@ def _mesh(op, route, faces, *inputs):
     return out.reshape(route.lead + (getattr(route, op.rows), op.width))
 
 
-def _normals_inputs(mode, route, faces, rows):
-    """The input arguments of dirt_normals_forward / _backward, in their order."""
+# The ops whose only input is the vertex rows: the vertex normals, the Laplacian and the edge terms.
+
+def _rows_inputs(mode, route, faces, rows):
+    """The input arguments of their entry points (mode, vertices, vertex_stride, faces), in their order."""
     return [mode, _ptr(rows), _stride(rows, 3), _ptr(faces)]
 
 
-def _restate_normals(restate, route, faces, rows):
+def _restate_rows(restate, route, faces, rows):
+    """`restate(vertices, faces)` on the op's rows"""
     return restate(_unflat_points(rows, route), faces)
 
 
+def _routed(op, restate, vertices, faces, route_of, mesh):
+    """A call of op through `mesh` when `route_of` (`_normals_route`) accepts it, else of its torch restatement
+    `restate(vertices, faces)`.  Each public function passes the `_normals_route` and `_mesh` of its own module."""
+    route = route_of(vertices, faces)
+    if route is None:
+        return restate(vertices, faces)
+    return mesh(op, route, faces, _point_rows(vertices[..., :3], 3))
+
+
 _NORMALS = _MeshOp('VertexNormals', 'dirt_normals_forward', 'dirt_normals_backward', 'dirt_normals_workspace_bytes',
-                   partial(_normals_inputs, _lib.NORMALS_AVERAGE), 3, (3,), partial(_restate_normals, _vertex_normals))
+                   partial(_rows_inputs, _lib.NORMALS_AVERAGE), 3, (3,), partial(_restate_rows, _vertex_normals))
 _NORMALS_PRE_SPLIT = _NORMALS._replace(name='VertexNormalsPreSplit',
-                                       inputs=partial(_normals_inputs, _lib.NORMALS_PRE_SPLIT),
-                                       restate=partial(_restate_normals, _vertex_normals_pre_split))
+                                       inputs=partial(_rows_inputs, _lib.NORMALS_PRE_SPLIT),
+                                       restate=partial(_restate_rows, _vertex_normals_pre_split))
 
 
 # ---- tangent-space normal mapping (DESIGN.md §7.14) -------------------------------------------------------------------

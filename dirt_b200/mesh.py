@@ -13,7 +13,7 @@ from functools import partial
 import torch
 
 from . import _lib
-from .lighting import _MeshOp, _face_normals, _mesh, _normals_route, _point_rows, _prepare, _stride, _ptr, _unflat_points
+from .lighting import _MeshOp, _face_normals, _mesh, _normals_route, _prepare, _restate_rows, _routed, _rows_inputs
 
 MODES = {'uniform': _lib.LAPLACIAN_UNIFORM, 'cotangent': _lib.LAPLACIAN_COTANGENT}
 
@@ -49,18 +49,9 @@ def _check_mode(mode):
         raise ValueError("laplacian: mode must be 'uniform' or 'cotangent', not %r" % (mode,))
 
 
-def _laplacian_inputs(mode, route, faces, rows):
-    """The input arguments of dirt_laplacian_forward / _backward, in their order."""
-    return [MODES[mode], _ptr(rows), _stride(rows, 3), _ptr(faces)]
-
-
-def _restate_laplacian(mode, route, faces, rows):
-    return _vertex_laplacian(_unflat_points(rows, route), faces, mode)
-
-
 _LAPLACIAN = {mode: _MeshOp('Laplacian', 'dirt_laplacian_forward', 'dirt_laplacian_backward',
-                            'dirt_laplacian_workspace_bytes', partial(_laplacian_inputs, mode), 3, (3,),
-                            partial(_restate_laplacian, mode))
+                            'dirt_laplacian_workspace_bytes', partial(_rows_inputs, MODES[mode]), 3, (3,),
+                            partial(_restate_rows, partial(_vertex_laplacian, mode=mode)))
               for mode in MODES}
 
 
@@ -82,10 +73,7 @@ def laplacian(vertices, faces, mode='uniform', name=None):
     On CUDA in the shapes `lighting.normals_route` accepts, deterministic kernels compute it (a face with an index
     outside [0, V) is then left out); any other call runs the torch restatement `_vertex_laplacian` (DESIGN.md §7.16)."""
     _check_mode(mode)
-    route = _normals_route(vertices, faces)
-    if route is None:
-        return _vertex_laplacian(vertices, faces, mode)
-    return _mesh(_LAPLACIAN[mode], route, faces, _point_rows(vertices[..., :3], 3))
+    return _routed(_LAPLACIAN[mode], partial(_vertex_laplacian, mode=mode), vertices, faces, _normals_route, _mesh)
 
 
 # ---- edge lengths and normal consistency (DESIGN.md §7.17) -------------------------------------------------------------
@@ -124,21 +112,12 @@ def _normal_consistency(vertices, faces):
 EDGE_MODES = {'edge_lengths': _lib.EDGE_LENGTH, 'normal_consistency': _lib.NORMAL_CONSISTENCY}
 
 
-def _edge_inputs(mode, route, faces, rows):
-    """The input arguments of dirt_edge_terms_forward / _backward, in their order."""
-    return [mode, _ptr(rows), _stride(rows, 3), _ptr(faces)]
-
-
-def _restate_edges(restate, route, faces, rows):
-    return restate(_unflat_points(rows, route), faces)
-
-
 _EDGE_LENGTHS = _MeshOp('EdgeLengths', 'dirt_edge_terms_forward', 'dirt_edge_terms_backward',
-                        'dirt_edge_terms_workspace_bytes', partial(_edge_inputs, _lib.EDGE_LENGTH), 3, (3,),
-                        partial(_restate_edges, _edge_lengths), rows='F')
+                        'dirt_edge_terms_workspace_bytes', partial(_rows_inputs, _lib.EDGE_LENGTH), 3, (3,),
+                        partial(_restate_rows, _edge_lengths), rows='F')
 _NORMAL_CONSISTENCY = _EDGE_LENGTHS._replace(name='NormalConsistency',
-                                             inputs=partial(_edge_inputs, _lib.NORMAL_CONSISTENCY),
-                                             restate=partial(_restate_edges, _normal_consistency))
+                                             inputs=partial(_rows_inputs, _lib.NORMAL_CONSISTENCY),
+                                             restate=partial(_restate_rows, _normal_consistency))
 
 
 def edge_lengths(vertices, faces, name=None):
@@ -152,10 +131,7 @@ def edge_lengths(vertices, faces, name=None):
     On CUDA in the shapes `lighting.normals_route` accepts, deterministic kernels compute it (a face with an index
     outside [0, V) then gets 0 and receives no gradient); any other call runs the torch restatement `_edge_lengths`
     (DESIGN.md §7.17)."""
-    route = _normals_route(vertices, faces)
-    if route is None:
-        return _edge_lengths(vertices, faces)
-    return _mesh(_EDGE_LENGTHS, route, faces, _point_rows(vertices[..., :3], 3))
+    return _routed(_EDGE_LENGTHS, _edge_lengths, vertices, faces, _normals_route, _mesh)
 
 
 def normal_consistency(vertices, faces, name=None):
@@ -175,7 +151,4 @@ def normal_consistency(vertices, faces, name=None):
     On CUDA in the shapes `lighting.normals_route` accepts, deterministic kernels compute it (a face with an index
     outside [0, V) then gets 0, receives no gradient and is nobody's partner); any other call runs the torch
     restatement `_normal_consistency` (DESIGN.md §7.17)."""
-    route = _normals_route(vertices, faces)
-    if route is None:
-        return _normal_consistency(vertices, faces)
-    return _mesh(_NORMAL_CONSISTENCY, route, faces, _point_rows(vertices[..., :3], 3))
+    return _routed(_NORMAL_CONSISTENCY, _normal_consistency, vertices, faces, _normals_route, _mesh)

@@ -372,6 +372,165 @@ def laplacian_backward(P, faces, grad, mode):
     return _t(row_sum(c.offsets, cotangent_corner_grad(c, Pt, laplacian_sum_grad(c, Pt, Gt))))
 
 
+# ---- edge lengths and normal consistency (DESIGN.md §7.17) ------------------------------------------------------------
+#
+# One value per face edge, [B, F, 3]: edge k of face f runs from v_k to v_{k+1 mod 3}.  The face passes are one thread
+# per (item, face); the vertex passes are the row sums above.
+
+LENGTH, CONSISTENCY = 0, 1
+
+
+class Partners:
+    """for_each_partner of every edge (f, k) of every valid face with v_k != v_{k+1}: the other valid faces g that name
+    both ends, each once, in the kernel's order.  It scans the shorter of the two rows (the smaller vertex id's when they
+    are equally long) in row order and takes each face at its first corner naming that row's vertex.  Arrays per edge:
+    f, k, x = v_k, y = v_{k+1}, count; per partner, in order: edge (its index), slot (its place in the edge's order)
+    and g."""
+
+    def __init__(self, c):
+        F, faces = c.F, c.faces
+        ok = ((faces >= 0) & (faces < c.V)).all(1) if F else np.zeros(0, bool)
+        self.valid = ok
+        f, k = np.nonzero(np.repeat(ok[:, None], 3, 1))
+        x, y = faces[f, k], faces[f, (k + 1) % 3]
+        keep = x != y
+        self.f, self.k, self.x, self.y = f[keep], k[keep], x[keep], y[keep]
+        n = c.count
+        lx, ly = n[self.x], n[self.y]
+        by_x = (lx < ly) | ((lx == ly) & (self.x < self.y))
+        r, o = np.where(by_x, self.x, self.y), np.where(by_x, self.y, self.x)
+        length = n[r]
+        edge = np.repeat(np.arange(len(r)), length)
+        j = c.offsets[r][edge] + np.arange(len(edge)) - np.repeat(np.cumsum(length) - length, length)
+        i = c.inc[j]
+        kk, g = i // max(F, 1), i % max(F, 1)
+        w = faces[g]
+        first = ~(((kk > 0) & (w[:, 0] == r[edge])) | ((kk > 1) & (w[:, 1] == r[edge])))
+        named = (w == o[edge, None]).any(1)
+        take = (g != self.f[edge]) & first & named
+        self.edge, self.g = edge[take], g[take]
+        self.count = np.bincount(self.edge, minlength=len(r))
+        start = np.cumsum(self.count) - self.count
+        self.slot = np.arange(len(self.edge)) - start[self.edge]
+
+    def ordered_sum(self, terms, zero):
+        """[edges, ...] float32: the sum per edge of terms [partners, ...] in partner order, from `zero`."""
+        s = np.broadcast_to(zero, (len(self.f),) + zero.shape).copy()
+        for m in range(int(self.slot.max()) + 1 if len(self.slot) else 0):
+            at = self.slot == m
+            s[self.edge[at]] = s[self.edge[at]] + terms[at]
+        return s
+
+
+def face_units(faces, Pt):
+    """unit_of: u_g [F, B, 3] of every face from its own corners (only the valid faces' are used)"""
+    f = np.clip(np.asarray(faces, np.int64).reshape(-1, 3), 0, max(len(Pt) - 1, 0))
+    p0 = Pt[f[:, 0]]
+    return normalise(cross3(Pt[f[:, 1]] - p0, Pt[f[:, 2]] - p0))
+
+
+def edge_terms_forward(P, faces, mode):
+    """edge_terms_forward_kernel: [B, F, 3]; 0 for a face with an invalid index"""
+    P = np.asarray(P, np.float32)
+    c, Pt = Corners(faces, P.shape[1]), _t(P)
+    out = np.zeros((c.F, P.shape[0], 3), np.float32)
+    if c.F == 0 or c.V == 0:
+        return _t(out)
+    ok = ((c.faces >= 0) & (c.faces < c.V)).all(1)
+    if mode == LENGTH:
+        f = np.flatnonzero(ok)
+        for k in range(3):
+            d = Pt[c.faces[f, (k + 1) % 3]] - Pt[c.faces[f, k]]
+            out[f, :, k] = np.sqrt(dot3(d, d))
+        return _t(out)
+    p = Partners(c)
+    u = face_units(c.faces, Pt)
+    s = p.ordered_sum(u[p.g], np.zeros(u.shape[1:], np.float32))
+    e = np.flatnonzero(p.count > 0)
+    uf = u[p.f[e]]
+    out[p.f[e], :, p.k[e]] = np.float32(1) - dot3(uf, s[e]) / p.count[e].astype(np.float32)[:, None]
+    return _t(out)
+
+
+def edge_length_corner_grad(c, Pt, Gt):
+    """EdgeLengthCornerGrad: each position's gradient [n, B, 3] for grad_out Gt [F, B, 3]"""
+    w = Wedge(c, Pt)
+    l1, l2 = np.sqrt(dot3(w.e01, w.e01)), np.sqrt(dot3(w.e02, w.e02))
+    G1, G2 = Gt[c.f, :, c.k], Gt[c.f, :, (c.k + 2) % 3]
+    k1 = np.where(l1 == 0, F0, G1 / np.where(l1 == 0, np.float32(1), l1))
+    k2 = np.where(l2 == 0, F0, G2 / np.where(l2 == 0, np.float32(1), l2))
+    return -(w.e01 * k1[..., None] + w.e02 * k2[..., None])
+
+
+def pair_grad(faces, Gt, g, x, y):
+    """pair_grad: [n, B] the sum of grad_out over the edges of faces g that join x and y, in edge order from +0"""
+    w = faces[g]
+    s = np.zeros((len(g),) + Gt.shape[1:-1], np.float32)
+    for k in range(3):
+        a, b = w[:, k], w[:, (k + 1) % 3]
+        s = np.where((((a == x) & (b == y)) | ((a == y) & (b == x)))[:, None], s + Gt[g, :, k], s)
+    return s
+
+
+def same_pair(v, j, k):
+    """whether edges j and k [n] of faces v [n, 3] join the same unordered pair"""
+    n = np.arange(len(v))
+    a, b, c, d = v[:, j], v[:, (j + 1) % 3], v[n, k], v[n, (k + 1) % 3]
+    return ((a == c) & (b == d)) | ((a == d) & (b == c))
+
+
+def consistency_face_grad(c, Pt, Gt):
+    """consistency_face_grad_kernel: dL/dn_f [F, B, 3] of every valid face (0 for the others) for grad_out Gt
+    [F, B, 3].  Each distinct unordered pair of f's edges, in edge order, adds -(G_f sum du + sum G_g du) / |P| to
+    dL/du_f and G_f + (sum G_g) / |P| to beta, du = u_g - u_f."""
+    p = Partners(c)
+    u = face_units(c.faces, Pt)
+    B = Pt.shape[1]
+    zero3, zero = np.zeros((B, 3), np.float32), np.zeros(B, np.float32)
+    du = u[p.g] - u[p.f[p.edge]]
+    G = pair_grad(c.faces, Gt, p.g, p.x[p.edge], p.y[p.edge])
+    s = p.ordered_sum(du, zero3)
+    sg = p.ordered_sum(du * G[..., None], zero3)
+    gsum = p.ordered_sum(G, zero)
+    n = np.maximum(p.count, 1).astype(np.float32)[:, None]
+    Gf = pair_grad(c.faces, Gt, p.f, p.x, p.y)
+    dgu = (s * Gf[..., None] + sg) / n[..., None]
+    dbeta = Gf + gsum / n
+    v = c.faces[p.f]
+    counted = (p.count > 0) & ~((p.k > 0) & same_pair(v, 0, p.k)) & ~((p.k > 1) & same_pair(v, 1, p.k))
+    gu, beta = np.zeros((c.F, B, 3), np.float32), np.zeros((c.F, B), np.float32)
+    for k in range(3):   # f's edges in order; at most one per (f, k)
+        e = np.flatnonzero(counted & (p.k == k))
+        gu[p.f[e]] = gu[p.f[e]] - dgu[e]
+        beta[p.f[e]] = beta[p.f[e]] + dbeta[e]
+    f = c.faces.clip(0, max(c.V - 1, 0))
+    p0 = Pt[f[:, 0]]
+    nf = cross3(Pt[f[:, 1]] - p0, Pt[f[:, 2]] - p0)
+    d = np.sqrt(dot3(nf, nf)) + EPS
+    k = (beta * np.float32(1e-12)) / ((d * d) * d)
+    out = normalise_grad(nf, gu) - nf * k[..., None]
+    return np.where(p.valid[:, None, None], out, F0)
+
+
+def consistency_corner_grad(c, Pt, gs):
+    """ConsistencyCornerGrad: each position's gradient [n, B, 3] through n = e1 x e2 from dL/dn_f gs [F, B, 3]"""
+    e1, e2 = c.edges(Pt)
+    gn = gs[c.f]
+    g1, g2 = cross3(e2, gn), cross3(gn, e1)
+    return c.pick(_negsum(g1, g2), g1, g2)
+
+
+def edge_terms_backward(P, faces, grad, mode):
+    """grad_vertices [B, V, 3] for grad_out [B, F, 3]"""
+    P = np.asarray(P, np.float32)
+    c, Pt, Gt = Corners(faces, P.shape[1]), _t(P), _t(grad)
+    if c.F == 0:
+        return np.zeros(P.shape, np.float32)
+    if mode == LENGTH:
+        return _t(row_sum(c.offsets, edge_length_corner_grad(c, Pt, Gt)))
+    return _t(row_sum(c.offsets, consistency_corner_grad(c, Pt, consistency_face_grad(c, Pt, Gt))))
+
+
 # ---- bit-for-bit comparison -------------------------------------------------------------------------------------------
 
 def first_difference(got, want):

@@ -11,7 +11,10 @@
    uvs, a tangent along the normal, a zero normal, and each gradient asked for alone.
 3. The row-sum boundary: rows of exactly 32 and 33 corners, a warp of 32 long rows, warps straddling two items with long
    rows on both sides and a partly empty last warp; each item alone gives the bits it gets inside a batch.
-4. The same against the small-grid build, whose launches run many grid-stride rounds."""
+4. The edge lengths and normal consistency (both face passes, both vertex passes) on the same meshes, on
+   test_gpu_edge_terms.py's degenerate mesh (duplicated, reversed, non-manifold, repeated-index and zero-area faces)
+   and on a fan of 5000 faces, whose partner search scans the rim rows and never the hub's.
+5. The same against the small-grid build, whose launches run many grid-stride rounds."""
 import ctypes
 
 import numpy as np
@@ -344,7 +347,43 @@ def check_tangents(name, want):
         _same(shared, mo.tangents_forward(P, uv, N, f), '%s tangents forward, shared uvs' % name)
 
 
-# ---- 4. the small-grid build ------------------------------------------------------------------------------------------------
+# ---- 4. the edge terms -----------------------------------------------------------------------------------------------------
+
+def _edge_meshes():
+    from test_gpu_edge_terms import _degenerate
+    out = dict(MESHES)
+    out['edge_degenerate'] = (_degenerate, 2)
+    out['fan_5000'] = (lambda: mo.fan(5000), 3)
+    return out
+
+
+EDGE_MESHES = sorted(MESHES) + ['edge_degenerate', 'fan_5000']
+
+
+def check_edge_terms(v, f, B, seed, what):
+    """Forward and backward of both edge terms on B strided items [B, V, 4]."""
+    from dirt_b200 import mesh
+    x = _items(v, B, seed)
+    P = x[..., :3].cpu().numpy()
+    faces = torch.tensor(f, device=DEV)
+    g = _grad((B, len(f), 3), seed + 1)
+    for name, m in (('edge_lengths', mo.LENGTH), ('normal_consistency', mo.CONSISTENCY)):
+        leaf = x.detach().clone().requires_grad_(True)
+        out = getattr(mesh, name)(leaf, faces)
+        out.backward(g)
+        _same(out, mo.edge_terms_forward(P, f, m), '%s %s forward' % (what, name))
+        _same(leaf.grad[..., :3], mo.edge_terms_backward(P, f, g.cpu().numpy(), m), '%s %s grad_vertices' % (what, name))
+        assert not leaf.grad[..., 3].any()
+
+
+@pytest.mark.parametrize('name', EDGE_MESHES)
+def test_edge_terms_bit_for_bit(cuda_lib, name):
+    fixture, B = _edge_meshes()[name]
+    v, f = fixture()
+    check_edge_terms(v, f, B, 50, name)
+
+
+# ---- 5. the small-grid build ------------------------------------------------------------------------------------------------
 
 @pytest.fixture(scope='module')
 def small(cuda_lib, tmp_path_factory):
@@ -361,3 +400,14 @@ def test_small_grid_build_bit_for_bit(cuda_lib, small, name):
         m.setattr(_lib, 'lib', lambda: small)
         check_normals_and_laplacian(v, f, max(B, 3), 40, name + ' (small grid)')
         check_tangents('degenerate' if name == 'degenerate' else 'straddle', 'all')
+
+
+@pytest.mark.parametrize('name', ['edge_degenerate', 'straddle', 'fan_5000', 'uv_sphere'])
+def test_small_grid_build_edge_terms_bit_for_bit(cuda_lib, small, name):
+    """DIRT_NORMALS_MAX_BLOCKS = 3: the edge terms' face and vertex passes run many grid-stride rounds."""
+    from dirt_b200 import _lib
+    fixture, B = _edge_meshes()[name]
+    v, f = fixture()
+    with pytest.MonkeyPatch.context() as m:
+        m.setattr(_lib, 'lib', lambda: small)
+        check_edge_terms(v, f, max(B, 3), 60, name + ' (small grid)')

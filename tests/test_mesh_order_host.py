@@ -15,8 +15,10 @@ from conftest import rel_close
 MESHES = {'icosphere': mo.icosphere, 'grid': mo.grid, 'uv_sphere': mo.uv_sphere, 'fan': lambda: mo.fan(3000)}
 
 
-def _check(got, want, name, rel=1e-4):
-    ok, ratio = rel_close(np.asarray(got, np.float64), np.asarray(want, np.float64), rel=rel)
+def _check(got, want, name, rel=1e-4, atol=0.):
+    """rel_close, with entries within atol of float64 counted as equal"""
+    got, want = np.asarray(got, np.float64), np.asarray(want, np.float64)
+    ok, ratio = rel_close(np.where(np.abs(got - want) <= atol, want, got), want, rel=rel)
     assert ok, '%s: worst error / tolerance %.3f' % (name, ratio)
 
 
@@ -88,6 +90,22 @@ def test_laplacian_agrees_with_the_torch_restatement(name, mode):
     m = mo.UNIFORM if mode == 'uniform' else mo.COTANGENT
     _check(mo.laplacian_forward(P, f, m), want, 'laplacian')
     _check(mo.laplacian_backward(P, f, g, m), gw, 'laplacian grad')
+
+
+@pytest.mark.parametrize('mode', ['edge_lengths', 'normal_consistency'])
+@pytest.mark.parametrize('name', sorted(MESHES))
+def test_edge_terms_agree_with_the_torch_restatement(name, mode):
+    from dirt_b200 import mesh
+    v, f = MESHES[name]()
+    P = _batch(v, 2, 10)
+    g = np.random.default_rng(11).standard_normal(P.shape[:1] + f.shape).astype(np.float32)
+    want, (gw,) = _autograd(lambda x: getattr(mesh, '_' + mode)(x, torch.tensor(f)), [P], [0], g)
+    m = mo.LENGTH if mode == 'edge_lengths' else mo.CONSISTENCY
+    # values within 1e-6 of float64 count as equal, as in test_gpu_edge_terms.py: 1 - u_f . mean(u_g) cancels
+    _check(mo.edge_terms_forward(P, f, m), want, mode, atol=1e-6)
+    # the uv-sphere's pole vertices sum the consistency terms of 224 sliver faces that nearly cancel (DESIGN.md §7.17)
+    _check(mo.edge_terms_backward(P, f, g, m), gw, mode + ' grad',
+           5e-4 if (name, m) == ('uv_sphere', mo.CONSISTENCY) else 1e-4)
 
 
 def _signs_and_zeros(got, want, zeros=True):
